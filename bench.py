@@ -70,12 +70,12 @@ def peaks():
         d = json.load(open(p))
         return {"bf16_tflops": d["bf16_tflops"], "bf16_tflops_sustained": d.get("bf16_tflops_sustained"),
                 "hbm_gbs": d["hbm_gbs"], "source": "measured (MEASURED_PEAKS.json)"}
-    return {"bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "hbm_gbs": 6650.0,
-            "source": "fallback (B200_PROFILING.md)"}
+    return {"bf16_tflops": 989.0, "bf16_tflops_sustained": None, "hbm_gbs": 3350.0,
+            "source": "NVIDIA H100 SXM data sheet, dense, 700 W (not measured)"}
 
 
 class ClockSampler:
-    """nvidia-smi sampled DURING the timed region (B200_PROFILING.md clocks line)."""
+    """nvidia-smi sampled DURING the timed region: SM clock, power draw and throttle reasons."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -215,6 +215,8 @@ def main():
     ap.add_argument("--no-extras", action="store_true", help="skip sweep / modes / configs34 / cpu_baseline (quick runs)")
     ap.add_argument("--no-c5", action="store_true", help="skip the BASELINE configs[4] record (16384^3)")
     ap.add_argument("--slices", default="", help="K-slices of the B exchange, e.g. '512,1536,2048' (default: the plan's)")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="after the timed steps, write what the last timed step computed (a fixed row sample of C) to DIR/*.npy")
     args = ap.parse_args()
     _claim_stdout()
     if args.impl == "reference":
@@ -329,6 +331,14 @@ def main():
     value = flops_step / (ms * 1e-3) / 1e9
     kernel_name = g.last_kernel()
     _phase("timed region done")
+    if args.dump_outputs and rank == 0:
+        # C of the last timed step (rank 0's panel), every 8th row: 512 x 4096 float32 = 8 MiB.  The inputs come
+        # from the seeded generator above, so two builds given the same arguments can be compared element by element.
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        Cl = sets[(args.steps - 1) % R][2]
+        rows = torch.arange(0, Mloc, 8, device=dev)
+        np.save(os.path.join(args.dump_outputs, "C_rows.npy"), Cl[rows].float().cpu().numpy())
+        np.save(os.path.join(args.dump_outputs, "C_row_index.npy"), rows.cpu().numpy().astype(np.float64))
 
     # ---- verification of the timed path (every rank, after the timed loop) --------------------------
     step(0)
@@ -465,7 +475,7 @@ def main():
                                 f"{[k1 - k0 for k0, k1 in plan.chunks]} (ncclBroadcast, in place) pipelined with the K-sliced GEMM "
                                 "through the C ABI (b200_gemm_f32_rowpanel)") if world > 1 else "single GPU (b200_gemm_f32)",
                    "precision_mode": MODE_NAMES.get(mode, str(mode)), "kernel": kernel_name,
-                   "l2": f"{R} rotating input/output sets of {3 * N0 * N0 * 4 / 1e6:.0f} MB each (> 126 MB L2 between reuses)",
+                   "l2": f"{R} rotating input/output sets of {3 * N0 * N0 * 4 / 1e6:.0f} MB each (> 50 MB L2 between reuses)",
                    "inputs": "uniform(-1,1), row-major, lda=k ldb=n ldc=n (cuda/test_MMult.cpp:62)",
                    "verification": "64 rows of every rank's C panel vs the fp64-accumulated oracle after the timed loop "
                                    f"(tolerance {MODE_TOL.get(mode, 1e-5)} * max|C|), B bit-compared across ranks"},
@@ -498,7 +508,7 @@ def main():
         if os.path.exists(tp):
             try:
                 # bytes per launch (dram read+write) of this kernel at this size from the committed
-                # `ncu --set full` capture (profiles/, tools/summarize_ncu.py); null if not captured
+                # DRAM capture committed as profiles/traffic.json; null when none is committed
                 tj = json.load(open(tp))
                 out["roofline"]["traffic"] = tj.get(f"{kernel_name}@{N0}")
                 out["roofline"]["traffic_source"] = tj.get("_source", "profiles/ ncu capture (not measured in this run)")
@@ -540,7 +550,7 @@ def main():
                            "bit_exact_vs_REF_MMult_naive": bool(np.array_equal(got, ref_naive)),
                            "frac_of_bf16_peak": 2.0 * N0 ** 3 / t_ms / 1e9 / pk["bf16_tflops"]}
         out["modes"] = modes
-        fp32_peak = 2 * 128 * torch.cuda.get_device_properties(dev).multi_processor_count * (clocks["sm_max_mhz"] or 1965.0) * 1e6 / 1e12
+        fp32_peak = 2 * 128 * torch.cuda.get_device_properties(dev).multi_processor_count * (clocks["sm_max_mhz"] or 1980.0) * 1e6 / 1e12
         out["fp32_cuda_core_peak_tflops"] = fp32_peak
         if "strict_ffma" in modes:
             modes["strict_ffma"]["frac_of_fp32_cuda_core_peak"] = modes["strict_ffma"]["gflops"] / 1e3 / fp32_peak

@@ -3,7 +3,7 @@
 The product is the CUDA library; this module only loads it and forwards pointers.  PyTorch is
 plumbing (device memory, streams, torch.distributed) and is imported lazily, only by the helpers
 that take tensors.  There is NO CPU fallback: if the shared library is missing, import fails
-loudly; if no sm_100 GPU is present, every compute call raises B200GemmError(-2).
+loudly; if no sm_90 GPU is present, every compute call raises B200GemmError(-2).
 
 Interface mirrored from the reference (file:line in /root/reference):
   MY_MMult(m, n, k, a, lda, b, ldb, c, ldc)                 aarch64/MMult0.cpp:3   (host, C += A*B)
@@ -44,7 +44,7 @@ class B200GemmError(RuntimeError):
 if not os.path.exists(LIB_PATH):
     raise ImportError(
         f"{LIB_PATH} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-        "(nvcc, sm_100a). There is no CPU or PyTorch fallback for this path.")
+        "(nvcc, sm_90a). There is no CPU or PyTorch fallback for this path.")
 
 lib = C.CDLL(LIB_PATH)
 _vp, _i = C.c_void_p, C.c_int

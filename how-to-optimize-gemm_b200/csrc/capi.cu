@@ -2,7 +2,7 @@
 // construction and caching, kernel selection and launch.  Host-side counterpart of the reference's
 // MY_MMult wrappers (cuda/MMult_cuda_12.cu:228-235; aarch64-int8/MMult_4x8_21.c:81-143).
 //
-// No cuBLAS, no CUTLASS, no CPU fallback: if no sm_100 device is usable every compute entry point
+// No cuBLAS, no CUTLASS, no CPU fallback: if no sm_90 device is usable every compute entry point
 // fails with B200_ERR_NO_DEVICE.
 #include "../../include/b200gemm.h"
 
@@ -53,12 +53,8 @@ struct EpiOpts { int axpby = 0; float alpha = 1.f, beta = 0.f; };
 thread_local EpiOpts t_epi;
 // SMs the tensor-core launches of the current call leave free (the row-panel plan sets it while a later K-slice
 // of B is still being broadcast: a persistent GEMM holding every SM would starve NCCL's copy kernels and
-// serialise the exchange behind the math — measured on 2 x B200, DESIGN §7).
+// serialise the exchange behind the math, DESIGN §7).
 thread_local int t_sm_reserve = 0;
-// The row-panel plan sets this for GEMMs that run while NCCL's copy kernels hold some SMs: CTAs that start late then
-// draw fewer tiles instead of delaying a statically scheduled grid (measured on 2 x B200: a K = 1024 slice took 137 us
-// instead of ~80 under the static schedule).
-thread_local int t_dynamic_sched = 0;
 int g_dbg_b_lbo = 0, g_dbg_b_sbo = 0;
 
 // ---- per-device state ------------------------------------------------------------------------------
@@ -92,8 +88,6 @@ struct DevCtx {
   int dev = -1;
   int* flags = nullptr;      // tail-split ordering flags (zero between launches), 16 rotating slots of 1024 ints
   unsigned flag_slot = 0;
-  int* sched_counters = nullptr;   // dynamic tile scheduler: 64 rotating work counters, zero between launches
-  unsigned sched_slot = 0;
   // split-precision workspace (planes of A and B, row / column maxima): cached, grow-only
   std::mutex ws_mu;
   Scratch ws;
@@ -135,7 +129,7 @@ int ensure_device() {
   if (c->ok == 1) return 0;
   cudaDeviceProp prop;
   if (cudaGetDeviceProperties(&prop, dev) != cudaSuccess) { cudaGetLastError(); c->ok = -1; return B200_ERR_NO_DEVICE; }
-  if (prop.major != 10) { c->ok = -1; return B200_ERR_NO_DEVICE; }
+  if (prop.major != 9) { c->ok = -1; return B200_ERR_NO_DEVICE; }
   if (!g_encode) {
     void* fn = nullptr;
     cudaDriverEntryPointQueryResult qres;
@@ -150,11 +144,6 @@ int ensure_device() {
   if (!c->flags) {
     if (cudaMalloc(&c->flags, 16 * 1024 * sizeof(int)) != cudaSuccess || cudaMemset(c->flags, 0, 16 * 1024 * sizeof(int)) != cudaSuccess) {
       cudaGetLastError(); c->flags = nullptr; c->ok = -1; return B200_ERR_NO_DEVICE;
-    }
-  }
-  if (!c->sched_counters) {
-    if (cudaMalloc(&c->sched_counters, 64 * sizeof(int)) != cudaSuccess || cudaMemset(c->sched_counters, 0, 64 * sizeof(int)) != cudaSuccess) {
-      cudaGetLastError(); c->sched_counters = nullptr; c->ok = -1; return B200_ERR_NO_DEVICE;
     }
   }
   if (!c->ws_event && cudaEventCreateWithFlags(&c->ws_event, cudaEventDisableTiming) != cudaSuccess) {
@@ -242,8 +231,6 @@ int last_launch_status() {
 // the stream drains; every kernel launched through here calls griddep_wait before it touches global memory.
 int g_pdl = 1;                // tuning hook (b200_gemm_debug_set_pdl)
 int g_prepass_fork = 1;       // F16X2: B's pre-pass chain on an auxiliary stream beside A's (b200_gemm_debug_set_pdl bit 1 = off)
-int g_dynamic_sched = 0;      // 1: every tensor-core launch draws its tiles from an atomic counter (b200_gemm_debug_set_dynamic_sched).  Default: static
-                              // round robin (measured 0-8 % faster when the GPU is ours alone) except where t_dynamic_sched asks for it
 template <typename... KArgs, typename... Args>
 cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, int cluster, Args&&... args) {
   cudaLaunchConfig_t cfg = {};
@@ -295,21 +282,19 @@ int launch_generic_requant(int m, int n, int k, const int8_t* A, int lda, const 
 // ---- tensor-core launch -------------------------------------------------------------------
 int g_force_bn = 0;          // test/tuning hook (b200_gemm_debug_set_bn): 0 = heuristic
 int g_group_rows = 0;         // tuning hook: rows per raster group of the tensor-core kernels (0 = 2048)
-int g_force_cg = 0;           // test/tuning hook (b200_gemm_debug_set_cta_group): 0 = auto, 1, 2
-int g_epi8 = 1;               // pair kernels of the plain kinds drain with 8 epilogue warps (tuning hook b200_gemm_debug_set_epilogue bit 1 = back to 4):
-                              // measured int8 4096^3 2.07 -> 2.32 POP/s, bf16->fp32 2304^3 692 -> 823 TFLOP/s, bit-identical results
 constexpr int kStreamCDefault = 0;
 int g_stream_c = -1;          // split modes: streaming stores for C (-1 = unresolved: B200GEMM_STREAM_C or the default above)
-int g_epi_direct = 0;         // tuning hook (b200_gemm_debug_set_epilogue): 1 = direct register stores for non-folding passes
 int g_ffma_fat = -1;          // strict kernel: 1 = 128x256 fat-thread variant, 0 = 128x128, -1 = by size
 int g_ffma_halves = 1;        // strict kernel: split the tail round into half tiles (tuning hook)
 
-template <int KIND, int BN, int STAGES, typename OutT, class Prod = ProdSingle, int A_ROW_BYTES = 128, int CG = 1, int EPIW = 4>
+// B: row-major k x n (b_rows_total rows, pitch ldb) for the 16-bit kinds; for tf32 / int8 it is B^T, n x k
+// (pitch ldb), which wgmma needs K-major (launch_tc_kmajor builds it).
+template <int KIND, int BN, int STAGES, typename OutT, class Prod = ProdSingle, int A_ROW_BYTES = 128>
 int launch_tc(int m, int n, int k, const void* A, long long lda, int a_rows_total, int a_plane_rows,
               const void* B, long long ldb, int b_rows_total, int b_plane_rows, void* C, int ldc,
               cudaStream_t st, const char* name, int chunk_k = 0, const float* row_max = nullptr,
               const float* col_max = nullptr, int accumulate = 0) {
-  using Cfg = TcConfig<KIND, BN, STAGES, Prod, A_ROW_BYTES, CG, EPIW>;
+  using Cfg = TcConfig<KIND, BN, STAGES, Prod, A_ROW_BYTES>;
   using T = KindTraits<KIND>;
   constexpr CUtensorMapDataType dt = KIND == KIND_F16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
                                    : KIND == KIND_FP16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16
@@ -319,8 +304,10 @@ int launch_tc(int m, int n, int k, const void* A, long long lda, int a_rows_tota
   int rc = get_map(&tmA, A, dt, T::ELEM, k, a_rows_total, (unsigned long long)lda * T::ELEM, Cfg::BK, Cfg::BM,
                    A_ROW_BYTES == 128 ? 1 : 3);
   if (rc) return rc;
-  rc = get_map(&tmB, B, dt, T::ELEM, n, b_rows_total, (unsigned long long)ldb * T::ELEM, Cfg::B_BOX_COLS, Cfg::BK,
-               T::B_LAYOUT == 1 ? 2 : 1);
+  if constexpr (T::B_KMAJOR)
+    rc = get_map(&tmB, B, dt, T::ELEM, k, n, (unsigned long long)ldb * T::ELEM, Cfg::BK, Cfg::B_BOX_ROWS, 1);
+  else
+    rc = get_map(&tmB, B, dt, T::ELEM, n, b_rows_total, (unsigned long long)ldb * T::ELEM, Cfg::B_BOX_COLS, Cfg::BK, 1);
   if (rc) return rc;
   TcParams p;
   p.C = C; p.ldc = ldc; p.M = m; p.N = n; p.K = k;
@@ -337,14 +324,13 @@ int launch_tc(int m, int n, int k, const void* A, long long lda, int a_rows_tota
   p.row_max = row_max; p.col_max = col_max;
   p.accumulate = accumulate;
   p.axpby = t_epi.axpby; p.alpha = t_epi.alpha; p.beta = t_epi.beta;
-  p.epi_direct = g_epi_direct;
   p.stream_c = g_stream_c < 0 ? (g_stream_c = (getenv("B200GEMM_STREAM_C") ? atoi(getenv("B200GEMM_STREAM_C")) : kStreamCDefault)) : g_stream_c;
-  auto kern = gemm_tc_kernel<KIND, BN, STAGES, OutT, Prod, A_ROW_BYTES, CG, EPIW>;
+  auto kern = gemm_tc_kernel<KIND, BN, STAGES, OutT, Prod, A_ROW_BYTES>;
   if (int arc = ensure_smem_attr(kern, Cfg::SMEM_BYTES)) return arc;
   int tiles = p.tiles_m * p.tiles_n;
-  const int units_max = (t_ctx->sms - t_sm_reserve > 2 * CG ? t_ctx->sms - t_sm_reserve : t_ctx->sms) / CG;   // CTAs, or CTA pairs (one per TPC)
+  const int units_max = t_ctx->sms - t_sm_reserve > 2 ? t_ctx->sms - t_sm_reserve : t_ctx->sms;   // one CTA per SM
   // Wave quantisation: the last, partial round of tiles (or the only round of a small problem) is
-  // cut along K so that every CTA/pair has work: rem tiles x split parts <= units.
+  // cut along K so that every CTA has work: rem tiles x split parts <= units.
   const int num_kb = (k + Cfg::BK - 1) / Cfg::BK;
   const int rem = tiles % units_max;
   int split = 1;
@@ -353,30 +339,20 @@ int launch_tc(int m, int n, int k, const void* A, long long lda, int a_rows_tota
     if (split > 4) split = 4;
     if (split > num_kb / 8) split = num_kb / 8;       // keep >= 8 k-blocks per part
     if (split < 1) split = 1;
-    if (rem * CG * Cfg::EPI_WARPS > 1024) split = 1;  // flag slot capacity
-  }
-  // When at least one full round exists, the partial last round is better served by half-width tiles
-  // (no K split, no fold): 2*rem items of half the duration.  Needs BN/2 to be a whole number of
-  // B column blocks per CTA.
-  p.halfn = 0;
-  if (g_split_tail == 1 && tiles >= units_max && rem > 0 && 2 * rem <= units_max &&
-      ((BN / 2 / CG) % Cfg::B_BOX_COLS) == 0 && (BN / 2) % 16 == 0 && (BN / 2) % OutPack<OutT>::COLS == 0) {
-    p.halfn = 1;
-    split = 1;
+    if (rem * Cfg::EPI_WARPS > 1024) split = 1;       // flag slot capacity
   }
   p.split = split;
-  p.full_tiles = (split > 1 || p.halfn) ? tiles - rem : tiles;
+  p.full_tiles = split > 1 ? tiles - rem : tiles;
   p.flags = t_ctx->flags + (t_ctx->flag_slot++ % 16) * 1024;
-  p.sched_counter = (g_dynamic_sched || t_dynamic_sched) ? t_ctx->sched_counters + (t_ctx->sched_slot++ % 64) : nullptr;
   if (split > 1) {          // the ordering flags start from zero whatever an aborted earlier launch left behind
     cudaError_t e = cudaMemsetAsync(p.flags, 0, 1024 * sizeof(int), st);
     if (e != cudaSuccess) { cudaGetLastError(); return (int)e; }
   }
-  const int items = p.full_tiles + (tiles - p.full_tiles) * (p.halfn ? 2 : split);
+  const int items = p.full_tiles + (tiles - p.full_tiles) * split;
   const int units = items < units_max ? items : units_max;
   g_ktimer.begin(st);
   {
-    cudaError_t e = launch_pdl(kern, dim3(units * CG), dim3(Cfg::THREADS), Cfg::SMEM_BYTES, st, CG, tmA, tmB, p);
+    cudaError_t e = launch_pdl(kern, dim3(units), dim3(Cfg::THREADS), Cfg::SMEM_BYTES, st, 1, tmA, tmB, p);
     if (e != cudaSuccess) { cudaGetLastError(); return (int)e; }
   }
   g_ktimer.end(st);
@@ -390,8 +366,8 @@ int launch_tc(int m, int n, int k, const void* A, long long lda, int a_rows_tota
 int pick_bn(int m, int n, bool allow256, bool allow192 = true) {
   if (g_force_bn == 128 || (g_force_bn == 192 && allow192) || (g_force_bn == 256 && allow256)) return g_force_bn;
   const int cands[3] = {256, 192, 128};
-  // relative efficiency of the 1-CTA kernels, measured on B200 at N=4096 (bf16: 1347 / 1317 / 1058
-  // TFLOP/s; the CTA-pair kernel: 1538): narrower tiles amortise shared-memory operand reads worse
+  // relative per-tile efficiency assumed for the three widths: narrower tiles re-read A from shared memory
+  // more often per output column
   const double eff[3] = {1.00, 0.97, 0.80};
   int best = 128;
   double best_cost = 1e300;
@@ -407,67 +383,18 @@ int pick_bn(int m, int n, bool allow256, bool allow192 = true) {
   return best;
 }
 
-// CTA pairs (tcgen05 cta_group::2, 256 x BN per pair): each CTA stages only its half of B, halving the
-// shared-memory operand traffic per MMA that bounds the 1-CTA kernel (1538 vs 1347 TFLOP/s, bf16 4096^3).
-// Used once the 256 x 256 pair tiles fill most of the 74 pairs; below that the 1-CTA tiles fill the
-// machine better (N = 1536, BF16X3: 128x128 tiles 143 TFLOP/s, pair tiles 95).
-bool use_pair(int m, int n) {
-  if (g_force_cg == 1) return false;
-  if (g_force_cg == 2) return m > 128 && n > 128;
-  if (m <= 128 || n <= 128) return false;
-  const long long tiles = (long long)((m + 255) / 256) * ((n + 255) / 256);
-  return tiles * 5 >= (long long)(t_ctx->sms / 2) * 4;
-}
-
 #define TC_PLAIN(KIND, OUT, NAME)                                                                     \
-  if (use_pair(m, n) && g_epi8)                                                                       \
-    return launch_tc<KIND, 256, 6, OUT, ProdSingle, 128, 2, 8>(m, n, k, A, lda, m, 0, B, ldb, k, 0, C, ldc, st, NAME "_2cta_256x256_e8"); \
-  if (use_pair(m, n))                                                                                 \
-    return launch_tc<KIND, 256, 6, OUT, ProdSingle, 128, 2>(m, n, k, A, lda, m, 0, B, ldb, k, 0, C, ldc, st, NAME "_2cta_256x256"); \
   switch (pick_bn(m, n, true)) {                                                                      \
     case 256: return launch_tc<KIND, 256, 4, OUT>(m, n, k, A, lda, m, 0, B, ldb, k, 0, C, ldc, st, NAME "_128x256"); \
     case 192: return launch_tc<KIND, 192, 5, OUT>(m, n, k, A, lda, m, 0, B, ldb, k, 0, C, ldc, st, NAME "_128x192"); \
     default:  return launch_tc<KIND, 128, 6, OUT>(m, n, k, A, lda, m, 0, B, ldb, k, 0, C, ldc, st, NAME "_128x128"); \
   }
 
-int tc_tf32(int m, int n, int k, const float* A, int lda, const float* B, int ldb, float* C, int ldc, cudaStream_t st, int acc = 0) {
-  if (use_pair(m, n) && g_epi8)
-    return launch_tc<KIND_TF32, 256, 6, float, ProdSingle, 128, 2, 8>(m, n, k, A, lda, m, 0, B, ldb, k, 0, C, ldc, st, "tc_tf32_2cta_256x256_e8", 0, nullptr, nullptr, acc);
-  if (use_pair(m, n))
-    return launch_tc<KIND_TF32, 256, 6, float, ProdSingle, 128, 2>(m, n, k, A, lda, m, 0, B, ldb, k, 0, C, ldc, st, "tc_tf32_2cta_256x256", 0, nullptr, nullptr, acc);
-  switch (pick_bn(m, n, true)) {
-    case 256: return launch_tc<KIND_TF32, 256, 4, float>(m, n, k, A, lda, m, 0, B, ldb, k, 0, C, ldc, st, "tc_tf32_128x256", 0, nullptr, nullptr, acc);
-    case 192: return launch_tc<KIND_TF32, 192, 5, float>(m, n, k, A, lda, m, 0, B, ldb, k, 0, C, ldc, st, "tc_tf32_128x192", 0, nullptr, nullptr, acc);
-    default:  return launch_tc<KIND_TF32, 128, 6, float>(m, n, k, A, lda, m, 0, B, ldb, k, 0, C, ldc, st, "tc_tf32_128x128", 0, nullptr, nullptr, acc);
-  }
-}
 int tc_bf16_f32(int m, int n, int k, const void* A, int lda, const void* B, int ldb, void* C, int ldc, cudaStream_t st) {
   TC_PLAIN(KIND_F16, float, "tc_bf16")
 }
 int tc_bf16_bf16(int m, int n, int k, const void* A, int lda, const void* B, int ldb, void* C, int ldc, cudaStream_t st) {
   TC_PLAIN(KIND_F16, bf16_out, "tc_bf16_obf16")
-}
-int tc_s8(int m, int n, int k, const void* A, int lda, const void* B, int ldb, void* C, int ldc, cudaStream_t st) {
-  // int8 column blocks are 128 elements wide (128 B): BN = 192 is not a whole number of them
-  if (use_pair(m, n) && g_epi8)
-    return launch_tc<KIND_I8, 256, 6, int32_t, ProdSingle, 128, 2, 8>(m, n, k, A, lda, m, 0, B, ldb, k, 0, C, ldc, st, "tc_s8_2cta_256x256_e8");
-  if (use_pair(m, n))
-    return launch_tc<KIND_I8, 256, 6, int32_t, ProdSingle, 128, 2>(m, n, k, A, lda, m, 0, B, ldb, k, 0, C, ldc, st, "tc_s8_2cta_256x256");
-  if (pick_bn(m, n, true, false) == 256)
-    return launch_tc<KIND_I8, 256, 4, int32_t>(m, n, k, A, lda, m, 0, B, ldb, k, 0, C, ldc, st, "tc_s8_128x256");
-  return launch_tc<KIND_I8, 128, 6, int32_t>(m, n, k, A, lda, m, 0, B, ldb, k, 0, C, ldc, st, "tc_s8_128x128");
-}
-
-// int8 in, int8 out through the requantising epilogue (scales / bias ride in the row_max / col_max slots)
-int tc_s8_requant(int m, int n, int k, const void* A, int lda, const void* B, int ldb, void* C, int ldc,
-                  const float* scales, const float* bias, cudaStream_t st) {
-  if (use_pair(m, n) && g_epi8)
-    return launch_tc<KIND_I8, 256, 6, s8_out, ProdSingle, 128, 2, 8>(m, n, k, A, lda, m, 0, B, ldb, k, 0, C, ldc, st, "tc_s8_requant_2cta_256x256_e8", 0, scales, bias);
-  if (use_pair(m, n))
-    return launch_tc<KIND_I8, 256, 6, s8_out, ProdSingle, 128, 2>(m, n, k, A, lda, m, 0, B, ldb, k, 0, C, ldc, st, "tc_s8_requant_2cta_256x256", 0, scales, bias);
-  if (pick_bn(m, n, true, false) == 256)
-    return launch_tc<KIND_I8, 256, 4, s8_out>(m, n, k, A, lda, m, 0, B, ldb, k, 0, C, ldc, st, "tc_s8_requant_128x256", 0, scales, bias);
-  return launch_tc<KIND_I8, 128, 6, s8_out>(m, n, k, A, lda, m, 0, B, ldb, k, 0, C, ldc, st, "tc_s8_requant_128x128", 0, scales, bias);
 }
 
 // ---- split-precision fp32 on the tensor cores ---------------------------------------------------
@@ -503,6 +430,46 @@ void ws_release(cudaStream_t st) {
   cudaEventRecord(c->ws_event, st);
   c->ws_stream = st;
   c->ws_busy = true;
+}
+
+// tf32 / int8: wgmma reads these operand types only K-major, so B (k x n) is first transposed into the device
+// workspace (B^T, n rows of 16-byte-aligned pitch), then the GEMM reads it.
+template <int KIND, int BN, int STAGES, typename OutT>
+int launch_tc_kmajor(int m, int n, int k, const void* A, int lda, const void* B, int ldb, void* C, int ldc,
+                     cudaStream_t st, const char* name, const float* row_max = nullptr, const float* col_max = nullptr,
+                     int acc = 0) {
+  using E = typename std::conditional<KIND == KIND_TF32, float, uint8_t>::type;
+  const long long kp = (((long long)k * (long long)sizeof(E) + 15) & ~15LL) / (long long)sizeof(E);
+  std::lock_guard<std::mutex> wlk(t_ctx->ws_mu);
+  if (int rc = split_ws_reserve((size_t)n * kp * sizeof(E))) return rc;
+  ws_acquire(st);
+  struct Release { cudaStream_t s; ~Release() { ws_release(s); } } rel{st};
+  E* bt = reinterpret_cast<E*>(t_ctx->ws.p);
+  launch_pdl(transpose_kernel<E>, dim3((n + 31) / 32, (k + 31) / 32), dim3(256), 0, st, 1, reinterpret_cast<const E*>(B),
+             (long long)ldb, k, n, bt, kp);
+  g_launches++;
+  if (int rc = last_launch_status()) return rc;
+  return launch_tc<KIND, BN, STAGES, OutT>(m, n, k, A, lda, m, 0, bt, kp, n, 0, C, ldc, st, name, 0, row_max, col_max, acc);
+}
+
+int tc_tf32(int m, int n, int k, const float* A, int lda, const float* B, int ldb, float* C, int ldc, cudaStream_t st, int acc = 0) {
+  switch (pick_bn(m, n, true)) {
+    case 256: return launch_tc_kmajor<KIND_TF32, 256, 4, float>(m, n, k, A, lda, B, ldb, C, ldc, st, "tc_tf32_128x256", nullptr, nullptr, acc);
+    case 192: return launch_tc_kmajor<KIND_TF32, 192, 5, float>(m, n, k, A, lda, B, ldb, C, ldc, st, "tc_tf32_128x192", nullptr, nullptr, acc);
+    default:  return launch_tc_kmajor<KIND_TF32, 128, 6, float>(m, n, k, A, lda, B, ldb, C, ldc, st, "tc_tf32_128x128", nullptr, nullptr, acc);
+  }
+}
+int tc_s8(int m, int n, int k, const void* A, int lda, const void* B, int ldb, void* C, int ldc, cudaStream_t st) {
+  if (pick_bn(m, n, true, false) == 256)
+    return launch_tc_kmajor<KIND_I8, 256, 4, int32_t>(m, n, k, A, lda, B, ldb, C, ldc, st, "tc_s8_128x256");
+  return launch_tc_kmajor<KIND_I8, 128, 6, int32_t>(m, n, k, A, lda, B, ldb, C, ldc, st, "tc_s8_128x128");
+}
+// int8 in, int8 out through the requantising epilogue (scales / bias ride in the row_max / col_max slots)
+int tc_s8_requant(int m, int n, int k, const void* A, int lda, const void* B, int ldb, void* C, int ldc,
+                  const float* scales, const float* bias, cudaStream_t st) {
+  if (pick_bn(m, n, true, false) == 256)
+    return launch_tc_kmajor<KIND_I8, 256, 4, s8_out>(m, n, k, A, lda, B, ldb, C, ldc, st, "tc_s8_requant_128x256", scales, bias);
+  return launch_tc_kmajor<KIND_I8, 128, 6, s8_out>(m, n, k, A, lda, B, ldb, C, ldc, st, "tc_s8_requant_128x128", scales, bias);
 }
 
 // Plane geometry shared by the per-call pre-pass and the pre-split B handle (b200_gemm_f32_pack_b).
@@ -541,24 +508,11 @@ int gemm_f32_split(int m, int n, int k, const float* A, int lda, const float* B,
   const SplitJob ja{A, lda, m, k, pA, pka, m}, jb{B, ldb, k, n, const_cast<uint16_t*>(pB), pnb, kp};
   int rc = launch_split<NP>(ja, jb, prepB ? 1 : 2, st);
   if (rc) return rc;
-  if (use_pair(m, n)) {
-    if constexpr (NP == 3)
-      return launch_tc<KIND_F16, 256, 4, float, ProdX3, 64, 2>(m, n, k, pA, pka, NP * m, m, pB, pnb, NP * kp, kp, C, ldc, st, "tc_bf16x3_2cta_256x256", g_split_chunk_k[0], nullptr, nullptr, acc);
-    else
-      return launch_tc<KIND_F16, 256, 6, float, ProdX2, 64, 2>(m, n, k, pA, pka, NP * m, m, pB, pnb, NP * kp, kp, C, ldc, st, "tc_bf16x2_2cta_256x256", g_split_chunk_k[1], nullptr, nullptr, acc);
-  }
-  const int bn = pick_bn(m, n, NP == 2);
-  if constexpr (NP == 3) {
-    if (bn == 192)
-      return launch_tc<KIND_F16, 192, 3, float, ProdX3, 64>(m, n, k, pA, pka, NP * m, m, pB, pnb, NP * kp, kp, C, ldc, st, "tc_bf16x3_128x192", g_split_chunk_k[0], nullptr, nullptr, acc);
+  // the running sum and the chunk accumulator of a 64 x 128 tile both live in a consumer's registers
+  if constexpr (NP == 3)
     return launch_tc<KIND_F16, 128, 4, float, ProdX3, 64>(m, n, k, pA, pka, NP * m, m, pB, pnb, NP * kp, kp, C, ldc, st, "tc_bf16x3_128x128", g_split_chunk_k[0], nullptr, nullptr, acc);
-  } else {
-    if (bn == 256)
-      return launch_tc<KIND_F16, 256, 4, float, ProdX2, 64>(m, n, k, pA, pka, NP * m, m, pB, pnb, NP * kp, kp, C, ldc, st, "tc_bf16x2_128x256", g_split_chunk_k[1], nullptr, nullptr, acc);
-    if (bn == 192)
-      return launch_tc<KIND_F16, 192, 4, float, ProdX2, 64>(m, n, k, pA, pka, NP * m, m, pB, pnb, NP * kp, kp, C, ldc, st, "tc_bf16x2_128x192", g_split_chunk_k[1], nullptr, nullptr, acc);
+  else
     return launch_tc<KIND_F16, 128, 6, float, ProdX2, 64>(m, n, k, pA, pka, NP * m, m, pB, pnb, NP * kp, kp, C, ldc, st, "tc_bf16x2_128x128", g_split_chunk_k[1], nullptr, nullptr, acc);
-  }
 }
 
 // B200_F32_F16X2: scaled fp16 split, 3 products.  Row maxima of A and column maxima of B give exact
@@ -611,19 +565,6 @@ int launch_f16_split_cols(const float* B, long long ldb, int rows, int cols, flo
 int gemm_f16x2_core(int m, int n, int k, const F16Operand& a, const F16Operand& b, float* C, int ldc, int acc,
                     cudaStream_t st) {
   constexpr int NP = 2;
-  if (use_pair(m, n))
-    return launch_tc<KIND_FP16, 256, 6, float, ProdX2, 64, 2>(m, n, k, a.planes, a.pitch, NP * a.plane_rows, a.plane_rows,
-                                                              b.planes, b.pitch, NP * b.plane_rows, b.plane_rows, C, ldc, st,
-                                                              "tc_f16x2_2cta_256x256", g_split_chunk_k[2], a.maxv, b.maxv, acc);
-  const int bn = pick_bn(m, n, true);
-  if (bn == 256)
-    return launch_tc<KIND_FP16, 256, 4, float, ProdX2, 64>(m, n, k, a.planes, a.pitch, NP * a.plane_rows, a.plane_rows,
-                                                           b.planes, b.pitch, NP * b.plane_rows, b.plane_rows, C, ldc, st,
-                                                           "tc_f16x2_128x256", g_split_chunk_k[2], a.maxv, b.maxv, acc);
-  if (bn == 192)
-    return launch_tc<KIND_FP16, 192, 4, float, ProdX2, 64>(m, n, k, a.planes, a.pitch, NP * a.plane_rows, a.plane_rows,
-                                                           b.planes, b.pitch, NP * b.plane_rows, b.plane_rows, C, ldc, st,
-                                                           "tc_f16x2_128x192", g_split_chunk_k[2], a.maxv, b.maxv, acc);
   return launch_tc<KIND_FP16, 128, 6, float, ProdX2, 64>(m, n, k, a.planes, a.pitch, NP * a.plane_rows, a.plane_rows,
                                                          b.planes, b.pitch, NP * b.plane_rows, b.plane_rows, C, ldc, st,
                                                          "tc_f16x2_128x128", g_split_chunk_k[2], a.maxv, b.maxv, acc);
@@ -799,18 +740,18 @@ int gemm_f32_impl(int m, int n, int k, const float* dA, int lda, const float* dB
   mode = resolve_f32_mode(mode);
   const bool tma = tma_ok(dA, lda, dB, ldb, 4);
   // AUTO on a small problem: the split path costs two launches (pre-pass + GEMM); up to 512^3 the
-  // single-launch strict FFMA2 kernel is within 15 % of it (measured, tools/probe_small.py: 9.3 vs 10.6
-  // TFLOP/s at 512^3, 2.0 vs 2.0 at 256^3) and bit-exact against the reference oracle.  From 640^3 the
-  // tensor-core path pulls away (19.2 vs 15.0; 63.0 vs 41.0 at 1024^3).
+  // single-launch strict FFMA kernel keeps up with it and is bit-exact against the reference oracle (measured on
+  // H100 with tools/probe_crossover.py, TFLOP/s strict : BF16X3 — 256^3 1.9 : 2.0, 512^3 8.6 : 8.4); from 640^3
+  // the tensor-core path pulls away (13.6 : 14.9, 1024^3 36.4 : 51.4).
   if (was_auto && (mode == B200_F32_BF16X3 || mode == B200_F32_F16X2) && tma && (double)m * n * k <= 2.0e8) mode = B200_F32_STRICT;
   // AUTO between ~640^3 and ~1100^3: the two-launch BF16X3 path (one fused split + GEMM) beats the four-launch
-  // F16X2 path while launches, not tensor work, dominate (tools/probe_crossover.py, TFLOP/s BF16X3 : F16X2 —
-  // 768^3 23.6 : 20.1, 1024^3 61.5 : 53.4, 1152^3 98.5 : 98.7, 1536^3 170 : 193, 2048^3 201 : 252).  Both are fp32-class.
+  // F16X2 path while launches, not tensor work, dominate (H100, TFLOP/s BF16X3 : F16X2 — 768^3 20.3 : 15.3,
+  // 1024^3 51.4 : 42.6, 1152^3 65.8 : 72.3, 2048^3 109 : 146).  Both are fp32-class.
   else if (was_auto && mode == B200_F32_F16X2 && (double)m * n * k < 1.3e9) mode = B200_F32_BF16X3;
   switch (mode) {
     case B200_F32_STRICT:
-      // 128x256 fat-thread tiles once they fill most of the machine (measured at N = 4096 / 3072 / 2048:
-      // 58.9 / 57.7 / 50.8 TFLOP/s against 58.5 / 57.2 / 49.3 for 128x128; at 1024 the small tile wins 40.6 : 24.1)
+      // 128x256 fat-thread tiles from 96 of them (measured on H100, fat : 128x128 TFLOP/s — 4096^3 45.6 : 43.8,
+      // 3072^3 40.4 : 43.1, 2048^3 43.5 : 42.8, 1536^3 25.2 : 24.0; at 1024^3, 32 fat tiles, the small tile wins 36.2 : 20.1)
       if (tma && (g_ffma_fat == 1 || (g_ffma_fat < 0 && (long long)((m + 127) / 128) * ((n + 255) / 256) >= 96)))
         return launch_ffma_fat(m, n, k, dA, lda, dB, ldb, dC, ldc, accumulate, st);
       if (tma) return launch_ffma(m, n, k, dA, lda, dB, ldb, dC, ldc, accumulate, st);
@@ -833,7 +774,7 @@ int gemm_f32_impl(int m, int n, int k, const float* dA, int lda, const float* dB
 
 extern "C" {
 
-const char* b200_gemm_version(void) { return "b200gemm 0.2 (sm_100a; tcgen05+TMA; round 2)"; }
+const char* b200_gemm_version(void) { return "b200gemm 0.3 (sm_90a; wgmma+TMA)"; }
 
 int b200_gemm_device_ok(void) { return ensure_device(); }
 
@@ -841,7 +782,7 @@ const char* b200_gemm_strerror(int code) {
   switch (code) {
     case B200_OK: return "ok";
     case B200_ERR_BAD_ARG: return "bad argument";
-    case B200_ERR_NO_DEVICE: return "no usable sm_100 CUDA device (there is no CPU fallback)";
+    case B200_ERR_NO_DEVICE: return "no usable sm_90 CUDA device (there is no CPU fallback)";
     case B200_ERR_UNSUPPORTED: return "mode not supported for these operands";
     case B200_ERR_TENSORMAP: return "cuTensorMapEncodeTiled failed";
     case B200_ERR_NCCL: return "NCCL failure (b200_nccl_last_error has the text)";
@@ -858,10 +799,12 @@ void b200_gemm_set_default_f32_mode(int mode) {
 void b200_gemm_debug_set_b_desc(int lbo_bytes, int sbo_bytes) { g_dbg_b_lbo = lbo_bytes; g_dbg_b_sbo = sbo_bytes; }
 void b200_gemm_debug_set_bn(int bn) { g_force_bn = bn; }
 void b200_gemm_debug_set_pdl(int v) { g_pdl = (v & 1) != 0; g_prepass_fork = (v & 2) == 0; }
-void b200_gemm_debug_set_dynamic_sched(int on) { g_dynamic_sched = on != 0; }
-void b200_gemm_debug_set_cta_group(int cg) { g_force_cg = cg; }
+// The sm_90 kernels have one static tile schedule, no CTA pairs and one epilogue form: these hooks of the
+// ABI are accepted and have no effect.
+void b200_gemm_debug_set_dynamic_sched(int) {}
+void b200_gemm_debug_set_cta_group(int) {}
 void b200_gemm_debug_set_split_tail(int on) { g_split_tail = on; }
-void b200_gemm_debug_set_epilogue(int v) { g_epi_direct = v & 1; g_epi8 = ((v >> 1) & 1) ^ 1; }
+void b200_gemm_debug_set_epilogue(int) {}
 void b200_gemm_debug_set_group_rows(int rows) { g_group_rows = rows; }
 void b200_gemm_debug_set_ffma_variant(int v) { g_ffma_halves = v & 1; g_ffma_fat = v < 0 ? -1 : (v >> 1) & 1; }
 void b200_gemm_debug_set_split_chunk(int x3_k, int x2_k) { g_split_chunk_k[0] = x3_k; g_split_chunk_k[1] = x2_k; g_split_chunk_k[2] = x2_k; }
@@ -891,8 +834,10 @@ int b200_gemm_reserve_workspace(size_t bytes) {
 // Bytes b200_gemm_f32 needs for an m x n x k product in `precision_mode` (0 for modes without a split).
 size_t b200_gemm_workspace_bytes(int m, int n, int k, int precision_mode) {
   const int mode = resolve_f32_mode(precision_mode);
+  if (m <= 0 || n <= 0 || k <= 0) return 0;
+  if (mode == B200_F32_TF32) return (size_t)n * (size_t)(((long long)k + 3) & ~3LL) * 4;   // B^T (launch_tc_kmajor)
   const int np = mode == B200_F32_BF16X3 ? 3 : (mode == B200_F32_BF16X2 || mode == B200_F32_F16X2) ? 2 : 0;
-  if (!np || m <= 0 || n <= 0 || k <= 0) return 0;
+  if (!np) return 0;
   const size_t a = ((size_t)np * m * plane_pitch(k) * 2 + 1023) & ~(size_t)1023;
   const size_t b = ((size_t)np * b_plane_rows(k) * plane_pitch(n) * 2 + 1023) & ~(size_t)1023;
   return a + b + (size_t)m * 4 + 1024;
@@ -1159,27 +1104,23 @@ int b200_gemm_mxf4(int m, int n, int k, const uint8_t* dAq, const uint8_t* dSFA,
   cudaStream_t st = (cudaStream_t)stream;
   if (k == 0) return launch_zero<float>(m, n, dC, ldc, st);
   if (!dAq || !dSFA || !dBq || !dSFB || !aligned16(dAq) || !aligned16(dBq) || !aligned16(dSFA) || !aligned16(dSFB)) return B200_ERR_BAD_ARG;
-  using Cfg = Mxf4Cfg<128>;
+  // both operands expanded (exactly) to bf16 in the workspace, then the bf16 tensor-core GEMM (gemm_mxf4.cuh)
   const int kpad = (k + 127) & ~127;
-  CUtensorMap tmA, tmB;
-  rc = get_map(&tmA, dAq, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, kpad / 2, m, kpad / 2, 128, Cfg::BM, 1);
-  if (rc) return rc;
-  rc = get_map(&tmB, dBq, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, kpad / 2, n, kpad / 2, 128, 128, 1);
-  if (rc) return rc;
-  Mxf4Params p;
-  p.C = dC; p.ldc = ldc; p.M = m; p.N = n; p.K = kpad;
-  p.sfa = dSFA; p.sfb = dSFB;
-  p.tiles_m = (m + 127) / 128; p.tiles_n = (n + 127) / 128;
-  p.vec_ok = aligned16(dC) && (ldc % 4) == 0;
-  auto kern = gemm_mxf4_kernel<128>;
-  if (int arc = ensure_smem_attr(kern, Cfg::SMEM_BYTES)) return arc;
-  const int tiles = p.tiles_m * p.tiles_n;
-  g_ktimer.begin(st);
-  kern<<<tiles < t_ctx->sms ? tiles : t_ctx->sms, Cfg::THREADS, Cfg::SMEM_BYTES, st>>>(tmA, tmB, p);
-  g_ktimer.end(st);
-  g_launches++;
-  t_last_kernel = "tc_mxf4_128x128";
-  return last_launch_status();
+  const long long npitch = ((long long)n + 7) & ~7LL;
+  const size_t a_bytes = ((size_t)m * kpad * 2 + 1023) & ~(size_t)1023;
+  std::lock_guard<std::mutex> wlk(t_ctx->ws_mu);
+  if (int wrc = split_ws_reserve(a_bytes + (size_t)kpad * npitch * 2)) return wrc;
+  ws_acquire(st);
+  struct Release { cudaStream_t s; ~Release() { ws_release(s); } } rel{st};
+  uint16_t* a16 = reinterpret_cast<uint16_t*>(t_ctx->ws.p);
+  uint16_t* b16 = reinterpret_cast<uint16_t*>(reinterpret_cast<uint8_t*>(t_ctx->ws.p) + a_bytes);
+  long long blocks = ((long long)m * (kpad / 32) + 255) / 256;
+  if (blocks > t_ctx->sms * 16) blocks = t_ctx->sms * 16;
+  launch_pdl(mxf4_expand_rows_kernel, dim3((unsigned)blocks), dim3(256), 0, st, 1, dAq, dSFA, m, kpad, a16);
+  launch_pdl(mxf4_expand_cols_t_kernel, dim3((n + 255) / 256, kpad / 32), dim3(256), 0, st, 1, dBq, dSFB, n, kpad, b16, npitch);
+  g_launches += 2;
+  if ((rc = last_launch_status())) return rc;
+  return launch_tc<KIND_F16, 128, 6, float>(m, n, kpad, a16, kpad, m, 0, b16, npitch, kpad, 0, dC, ldc, st, "tc_mxf4_128x128");
 }
 
 int b200_convert_f32_to_bf16(const float* dSrc, uint16_t* dDst, size_t count, void* stream) {
@@ -1188,7 +1129,7 @@ int b200_convert_f32_to_bf16(const float* dSrc, uint16_t* dDst, size_t count, vo
   int rc = ensure_device();
   if (rc) return rc;
   size_t blocks = (count + 255) / 256;
-  if (blocks > 148 * 32) blocks = 148 * 32;
+  if (blocks > (size_t)t_ctx->sms * 32) blocks = (size_t)t_ctx->sms * 32;
   convert_f32_to_bf16_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(dSrc, dDst, count);
   g_launches++;
   t_last_kernel = "convert_f32_to_bf16";
@@ -1284,7 +1225,7 @@ int b200_gemm_s8s32_host(int m, int n, int k, const int8_t* A, int lda, const in
   std::lock_guard<std::mutex> lk(t_ctx->host_mu);
   int8_t *dA = nullptr, *dB = nullptr;
   int32_t* dC = nullptr;
-  // device images padded to 16-byte pitches so the tcgen05 path is taken for any m,n,k
+  // device images padded to 16-byte pitches so the tensor-core path is taken for any m,n,k
   const size_t pa = ((size_t)k + 15) & ~(size_t)15, pb = ((size_t)n + 15) & ~(size_t)15;
   const size_t pc = (size_t)n * 4;
   cudaStream_t st = 0;

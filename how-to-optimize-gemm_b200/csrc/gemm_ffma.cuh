@@ -1,4 +1,4 @@
-// gemm_ffma.cuh — the strict-fp32 path: CUDA-core SGEMM for sm_100a, fed by TMA, packed FFMA2 math.
+// gemm_ffma.cuh — the strict-fp32 path: CUDA-core SGEMM for sm_90a, fed by TMA, FFMA math.
 //
 // Arithmetic contract (what makes this the drop-in for cuda/MMult_cuda_12.cu:200-206 and bit-exact
 // against the reference's naive oracle as its own makefile builds it, aarch64/REF_MMult.cpp:24 with
@@ -12,12 +12,10 @@
 // slots are spent on staging.  A lands K-contiguous with SWIZZLE_128B so four consecutive rows read
 // by a warp hit distinct banks; B lands N-contiguous (512-byte rows).
 //
-// Math: Blackwell's packed FFMA2 (fma.rn.f32x2) performs two fused multiply-adds per lane per
-// instruction; ptxas folds the scalar A operand into the instruction's broadcast form
-// (FFMA2 Rd, Ra.F32, Rb.F32x2, Rc.F32x2), so one k-step is 32 FFMA2 instead of 64 FFMA — half the issue
-// slots and register-port reads, same rounding (each lane is an IEEE fma).
+// Math: the accumulators are kept as float2 pairs (two adjacent columns); each pair is updated by two
+// IEEE fmas (ffma2 below), so every element is one fused multiply-add chain.
 //
-// Wave quantisation: 2 CTAs/SM x 148 SMs = 296 slots.  Tiles beyond the last full round are issued as
+// Wave quantisation: 2 CTAs/SM x 132 SMs = 264 slots.  Tiles beyond the last full round are issued as
 // two HALF tiles (rows ty+16*i for i in [0,4) or [4,8)) when that fills the machine better — each
 // half is still a complete sequential-k chain per element, so the contract above is untouched.
 #pragma once
@@ -35,6 +33,11 @@ __device__ __forceinline__ float2 lds64(uint32_t addr) {
   float2 v;
   asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(addr));
   return v;
+}
+
+// d = a * b + c on both halves of a float2 pair, each a single-rounding fma
+__device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) {
+  return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
 }
 
 struct FfmaParams {
@@ -116,9 +119,7 @@ __device__ __forceinline__ void ffma_tile(const CUtensorMap& tmA, const CUtensor
     mbar_wait(bar_full + 8 * s, use & 1);
     const uint32_t a_st = a_thr + s * Cfg::A_STAGE;
     const uint32_t b_st = b_thr + s * Cfg::B_STAGE;
-    // Fully unrolled over the stage (8 x [8 LDS.128 of A + 4 x (2 LDS.128 of B + 32 FFMA2)]).  Measured
-    // alternatives on B200 at N=4096: unroll 2 -> 57.2, unroll 4 -> 57.6, full -> 58.5 TFLOP/s; an
-    // LDS.64 software-pipelined form (operands fetched one k-step ahead) -> 57.6.
+    // Fully unrolled over the stage (8 x [8 LDS.128 of A + 4 x (2 LDS.128 of B + 64 FFMA)]).
 #pragma unroll
     for (int kc = 0; kc < Cfg::BK / 4; kc++) {
       float4 a4[NI];
@@ -136,7 +137,7 @@ __device__ __forceinline__ void ffma_tile(const CUtensorMap& tmA, const CUtensor
           const float av = kk == 0 ? a4[i].x : kk == 1 ? a4[i].y : kk == 2 ? a4[i].z : a4[i].w;
           const float2 aa = make_float2(av, av);
 #pragma unroll
-          for (int j = 0; j < 4; j++) acc[i][j] = __ffma2_rn(aa, bv[j], acc[i][j]);
+          for (int j = 0; j < 4; j++) acc[i][j] = ffma2(aa, bv[j], acc[i][j]);
         }
       }
     }
@@ -214,8 +215,8 @@ gemm_ffma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 // "Fat-thread" variant: 128 x 256 CTA tile, 256 threads, 8 x 16 outputs per thread (128 accumulators,
 // 1 CTA per SM, up to 255 registers).  Same arithmetic contract.  The larger register budget allows
 // what the 128-register 8x8 kernel cannot: both operand streams are fetched one step ahead (A for the
-// next 4 k-steps, B for the next k-step) while the current 64 FFMA2 issue, so no shared-memory latency
-// is exposed at k-chunk boundaries, and each k-step needs 6 LDS.128 per 64 FFMA2 instead of 4 per 32.
+// next 4 k-steps, B for the next k-step) while the current 128 FFMA issue, so no shared-memory latency
+// is exposed at k-chunk boundaries, and each k-step needs 6 LDS.128 per 128 FFMA instead of 4 per 64.
 struct FfmaFatCfg {
   static constexpr int BM = 128, BN = 256, BK = 32, STAGES = 3;
   static constexpr int A_STAGE = BM * BK * 4;     // 16 KB, swizzled 128 B rows
@@ -312,7 +313,7 @@ __device__ __forceinline__ void ffma_fat_tile(const CUtensorMap& tmA, const CUte
           const float av = kk == 0 ? a4[ac][i].x : kk == 1 ? a4[ac][i].y : kk == 2 ? a4[ac][i].z : a4[ac][i].w;
           const float2 aa = make_float2(av, av);
 #pragma unroll
-          for (int j = 0; j < 8; j++) acc[i][j] = __ffma2_rn(aa, bv[j], acc[i][j]);
+          for (int j = 0; j < 8; j++) acc[i][j] = ffma2(aa, bv[j], acc[i][j]);
         }
       }
     }

@@ -1,20 +1,21 @@
-// gemm_mxf4.cuh — the 4-bit path (SURVEY §8 f-4): block-scaled MXFP4 GEMM on tcgen05.mma.kind::mxf4.
+// gemm_mxf4.cuh — the 4-bit path (SURVEY §8 f-4): block-scaled MXFP4 operands.
 //
 // The reference lists a `cuda-int4` back-end and ships only the word "WIP" (cuda-int4/README.md:1,
-// README.md:13-15,118-120).  Blackwell has no integer 4-bit tensor path; its 4-bit operand type is
-// OCP MXFP4: E2M1 elements (+-{0, .5, 1, 1.5, 2, 3, 4, 6}) with one shared UE8M0 scale (a power of two)
-// per 32 consecutive K elements.  This file holds
+// README.md:13-15,118-120).  The 4-bit operand type here is OCP MXFP4: E2M1 elements
+// (+-{0, .5, 1, 1.5, 2, 3, 4, 6}) with one shared UE8M0 scale (a power of two) per 32 consecutive K elements.
+// This file holds
 //   * the quantisers: fp32 rows -> packed E2M1 + scales (A as stored), and the transposing variant for a
-//     row-major B (4-bit operands must be K-major for the tensor core — the one place where the reorder_b /
-//     trans_w role of aarch64-int8/MMult_4x8_21.c:45-71 does come back as a real pass);
-//   * gemm_mxf4_kernel: C[m x n] (fp32) = A_q[m x k] * B_q^T[n x k], scales applied by the tensor core.
+//     row-major B (4-bit operands are stored K-major — the one place where the reorder_b / trans_w role of
+//     aarch64-int8/MMult_4x8_21.c:45-71 does come back as a real pass);
+//   * the expansion of quantised operands to bf16 for the GEMM (see "the GEMM on sm_90" below).
 //
 // Layouts in HBM
 //   elements  rows x (k/2) bytes, two E2M1 per byte (element 2i in the low nibble), K contiguous;
 //   scales    512-byte atoms [rows/128][k/128]: byte (r % 32) * 16 + ((r / 32) % 4) * 4 + (kblock % 4) of the
-//             atom holds the UE8M0 scale of row r, K-block kblock — the tile one tcgen05.cp.32x128b.warpx4 moves
-//             into TMEM (32 lanes x 4 columns, each 32-bit column = the 4 scales of one row).
+//             atom holds the UE8M0 scale of row r, K-block kblock.
 #pragma once
+#include <cuda_bf16.h>
+
 #include "ptx.cuh"
 
 namespace b200 {
@@ -42,6 +43,7 @@ __device__ __forceinline__ float ue8m0_inv(uint32_t e) {         // 2^-(e - 127)
   x = x < 1 ? 1 : (x > 254 ? 254 : x);
   return __uint_as_float((uint32_t)x << 23);
 }
+__device__ __forceinline__ float exp2i_small(int e) { return __uint_as_float((uint32_t)(127 + e) << 23); }
 __host__ __device__ __forceinline__ size_t mxf4_sf_offset(int r, int kblock, int katoms) {
   return ((size_t)(r >> 7) * katoms + (kblock >> 2)) * 512 + (size_t)(r & 31) * 16 + ((r >> 5) & 3) * 4 + (kblock & 3);
 }
@@ -117,204 +119,67 @@ __global__ void __launch_bounds__(256) mxf4_quantize_cols_t_kernel(const float* 
   }
 }
 
-// ---- the GEMM -------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tc_mma_mxf4(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                            uint32_t sfa_tmem, uint32_t sfb_tmem, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::mxf4.block_scale.block32 [%0], %1, %2, %3, [%5], [%6], p;\n\t}"
-      ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate), "r"(sfa_tmem), "r"(sfb_tmem)
-      : "memory");
+// ---- the GEMM on sm_90 -------------------------------------------------------------------------------------
+// Hopper's tensor cores take no 4-bit operand.  An E2M1 element times its UE8M0 block scale is exactly a bf16
+// (one mantissa bit; the scale only moves the exponent), so both operands are expanded to bf16 — A as m x kpad
+// row-major, B^T back to row-major kpad x n — and multiplied by the bf16 wgmma kernel (gemm_tc.cuh) with fp32
+// accumulation: every product is exact, as in a block-scaled MMA.
+__device__ __forceinline__ float e2m1_decode(uint32_t c) {
+  const uint32_t m = c & 7u;
+  const float mag = m < 2 ? 0.5f * (float)m : (float)(2 + (m & 1)) * exp2i_small((int)(m >> 1) - 2);
+  return (c & 8u) ? -mag : mag;
 }
-// 32 rows x 16 bytes of shared memory -> TMEM lanes 0..31 (replicated into all four lane quadrants), 4 columns
-__device__ __forceinline__ void tc_cp_32x128b_warpx4(uint32_t taddr, uint64_t sdesc) {
-  asm volatile("tcgen05.cp.cta_group::1.32x128b.warpx4 [%0], %1;" ::"r"(taddr), "l"(sdesc) : "memory");
+__device__ __forceinline__ float ue8m0_value(uint32_t e) {       // 2^(e - 127); 255 is NaN
+  if (e == 255u) return __uint_as_float(0x7FC00000u);
+  return e == 0u ? __uint_as_float(0x00400000u) : __uint_as_float(e << 23);
 }
-// 1-D bulk copy global -> shared, completion counted in bytes on `bar`
-__device__ __forceinline__ void bulk_load(uint32_t dst_smem, const void* src, uint32_t bytes, uint32_t bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-               ::"r"(dst_smem), "l"(src), "r"(bytes), "r"(bar) : "memory");
-}
-// Block-scaled instruction descriptor (E2M1 x E2M1, UE8M0 scales, K-major operands, dense K = 64):
-//   [4,6) b_sf_id  [7,10) a_format  [10,13) b_format  [15] a_major  [16] b_major  [17,23) N>>3
-//   [23] scale_format (1 = UE8M0)  [24,29) M>>4  [29,31) a_sf_id  [31] k_size (0 = K64)
-__host__ __device__ constexpr uint32_t make_idesc_mxf4(uint32_t M, uint32_t N, uint32_t a_sf_id, uint32_t b_sf_id) {
-  return (b_sf_id << 4) | (1u << 7) | (1u << 10) | ((N >> 3) << 17) | (1u << 23) | ((M >> 4) << 24) | (a_sf_id << 29);
-}
-
-struct Mxf4Params {
-  float* C;
-  long long ldc;
-  int M, N, K;              // K padded to a multiple of 128 by the quantisers (zero elements)
-  const uint8_t* sfa;       // scale atoms of A [M/128][K/128][512]
-  const uint8_t* sfb;       // scale atoms of B [N/128][K/128][512]
-  int tiles_m, tiles_n;
-  int vec_ok;
-};
-
-template <int BN>
-struct Mxf4Cfg {
-  static constexpr int BM = 128, STAGES = 4;
-  static constexpr int BK = 256;                        // elements per stage: one 128-byte swizzled row
-  static constexpr int A_STAGE = BM * 128, B_STAGE = BN * 128;
-  static constexpr int SF_A = 2 * 512, SF_B = (BN / 128) * 2 * 512;     // two K-atoms (2 x 128 elements) per stage
-  static constexpr int STAGE_BYTES = A_STAGE + B_STAGE + SF_A + SF_B;
-  static constexpr int SMEM_BYTES = 1024 + STAGES * STAGE_BYTES + (2 * STAGES + 2) * 8 + 16;
-  static constexpr int THREADS = 192;
-  static constexpr int TMEM_COLS = 512;
-  static constexpr int SF_COL0 = 2 * BN;                // after the two accumulators
-  static constexpr int SF_COLS_PER_SLOT = 8 + (BN / 128) * 8;            // SFA: 2 atoms x 4 columns, SFB likewise per 128 columns
-  static_assert(BN == 128, "tile width (two 256-column accumulators would leave no TMEM for the scales)");
-  static_assert(SF_COL0 + 2 * SF_COLS_PER_SLOT <= 512, "TMEM budget");
-};
-
-// Persistent, warp-specialised like gemm_tc_kernel: warp 0 = producer (TMA for elements, bulk copies for
-// scale atoms), warp 1 = tcgen05.cp of the scales + MMA issue, warps 2..5 = epilogue (direct 16-byte stores:
-// lane = row holds 128 contiguous bytes per pass).  Two TMEM accumulators, scale slots double-buffered.
-template <int BN>
-__global__ void __launch_bounds__(192, 1)
-gemm_mxf4_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const Mxf4Params p) {
-  using Cfg = Mxf4Cfg<BN>;
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t sA = smem_base;
-  const uint32_t sB = sA + Cfg::STAGES * Cfg::A_STAGE;
-  const uint32_t sSF = sB + Cfg::STAGES * Cfg::B_STAGE;            // per stage: SFA atoms then SFB atoms
-  const uint32_t sBar = sSF + Cfg::STAGES * (Cfg::SF_A + Cfg::SF_B);
-  const uint32_t bar_full = sBar, bar_empty = sBar + 8 * Cfg::STAGES;
-  const uint32_t bar_tfull = sBar + 16 * Cfg::STAGES, bar_tempty = bar_tfull + 16;
-  const uint32_t s_tmem_ptr = bar_tempty + 16;
-  uint8_t* smem_gen = smem_raw + (smem_base - smem_u32(smem_raw));
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmA);
-    tma_prefetch_desc(&tmB);
-    for (int i = 0; i < Cfg::STAGES; i++) { mbar_init(bar_full + 8 * i, 1); mbar_init(bar_empty + 8 * i, 1); }
-    for (int i = 0; i < 2; i++) { mbar_init(bar_tfull + 8 * i, 1); mbar_init(bar_tempty + 8 * i, 4); }
-    fence_barrier_init();
-  }
-  if (warp == 1) tmem_alloc<Cfg::TMEM_COLS>(s_tmem_ptr);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *reinterpret_cast<volatile uint32_t*>(smem_gen + (s_tmem_ptr - smem_base));
-  const int num_tiles = p.tiles_m * p.tiles_n;
-  const int num_kb = p.K / Cfg::BK + ((p.K % Cfg::BK) ? 1 : 0);
-  const int katoms = p.K >> 7;
-
-  if (warp == 0) {
-    int s = 0;
-    uint32_t ph = 0;
-    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-      const int mb = t % p.tiles_m, nb = t / p.tiles_m;
-      for (int kb = 0; kb < num_kb; kb++) {
-        mbar_wait(bar_empty + 8 * s, ph ^ 1);
-        if (elect_one()) {
-          const int ka = kb * 2;                                  // first K-atom of this stage
-          const int na = min(2, katoms - ka);                     // a K tail of 128 elements has one atom
-          const uint32_t sf_bytes = (uint32_t)na * 512u * (1 + BN / 128);
-          mbar_arrive_expect_tx(bar_full + 8 * s, Cfg::A_STAGE + Cfg::B_STAGE + sf_bytes);
-          tma_load_2d(sA + s * Cfg::A_STAGE, &tmA, bar_full + 8 * s, kb * 128, mb * Cfg::BM);
-          tma_load_2d(sB + s * Cfg::B_STAGE, &tmB, bar_full + 8 * s, kb * 128, nb * BN);
-          const uint32_t sf0 = sSF + s * (Cfg::SF_A + Cfg::SF_B);
-          bulk_load(sf0, p.sfa + ((size_t)mb * katoms + ka) * 512, na * 512, bar_full + 8 * s);
+// 32 consecutive K elements of one row -> bf16 (RNE of an exact value: no rounding happens)
+__device__ __forceinline__ void mxf4_expand32(const uint8_t* q, uint32_t se, float (&x)[32]) {
+  const uint4 v = *reinterpret_cast<const uint4*>(q);
+  const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+  const float s = ue8m0_value(se);
 #pragma unroll
-          for (int h = 0; h < BN / 128; h++)
-            bulk_load(sf0 + Cfg::SF_A + h * 1024, p.sfb + ((size_t)(nb * (BN / 128) + h) * katoms + ka) * 512, na * 512,
-                      bar_full + 8 * s);
-        }
-        __syncwarp();
-        if (++s == Cfg::STAGES) { s = 0; ph ^= 1; }
+  for (int e = 0; e < 32; e++) x[e] = e2m1_decode((w[e >> 3] >> (4 * (e & 7))) & 15u) * s;
+}
+
+// A: rows x kpad/2 bytes -> rows x kpad bf16 (pitch kpad).  Thread = one 32-element block.
+__global__ void __launch_bounds__(256) mxf4_expand_rows_kernel(const uint8_t* __restrict__ q, const uint8_t* __restrict__ sf,
+                                                               int rows, int kpad, uint16_t* __restrict__ dst) {
+  griddep_launch();
+  griddep_wait();
+  const int kblocks = kpad >> 5, katoms = kpad >> 7;
+  const long long total = (long long)rows * kblocks;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const int r = (int)(i / kblocks), kb = (int)(i - (long long)r * kblocks);
+    float x[32];
+    mxf4_expand32(q + (long long)r * (kpad >> 1) + kb * 16, sf[mxf4_sf_offset(r, kb, katoms)], x);
+    uint4* d = reinterpret_cast<uint4*>(dst + (long long)r * kpad + kb * 32);
+#pragma unroll
+    for (int j = 0; j < 4; j++) {
+      uint32_t w[4];
+#pragma unroll
+      for (int e = 0; e < 4; e++) {
+        uint32_t r2;
+        asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(r2) : "f"(x[8 * j + 2 * e + 1]), "f"(x[8 * j + 2 * e]));
+        w[e] = r2;
       }
-    }
-  } else if (warp == 1) {
-    int s = 0, as = 0, slot = 0;
-    uint32_t ph = 0, aph = 0;
-    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-      mbar_wait(bar_tempty + 8 * as, aph ^ 1);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + as * BN;
-      for (int kb = 0; kb < num_kb; kb++) {
-        mbar_wait(bar_full + 8 * s, ph);
-        tc_fence_after();
-        if (elect_one()) {
-          const uint32_t sf0 = sSF + s * (Cfg::SF_A + Cfg::SF_B);
-          const uint32_t t_sf = tmem_base + Cfg::SF_COL0 + slot * Cfg::SF_COLS_PER_SLOT;
-          const int na = min(2, katoms - kb * 2);
-          // scale atoms -> TMEM: a 512-byte atom is 32 rows x 16 B, no swizzle (8-row core matrices 128 B apart)
-          // TMEM slot: SFA atom a at columns [4a, 4a+4); SFB of atom a at [8 + a*NB4, ...), 4 columns per 128 tile columns
-          constexpr int NB4 = (BN / 128) * 4;
-          for (int a = 0; a < na; a++) {
-            tc_cp_32x128b_warpx4(t_sf + a * 4, make_sdesc(sf0 + a * 512, 16, 128, 0));
-#pragma unroll
-            for (int h = 0; h < BN / 128; h++)
-              tc_cp_32x128b_warpx4(t_sf + 8 + a * NB4 + h * 4, make_sdesc(sf0 + Cfg::SF_A + h * 1024 + a * 512, 16, 128, 0));
-          }
-          const uint32_t a0 = sA + s * Cfg::A_STAGE, b0 = sB + s * Cfg::B_STAGE;
-#pragma unroll
-          for (int k = 0; k < 4; k++) {                           // four K = 64 MMAs per 256-element stage
-            if (k < 2 * na) {
-              const uint32_t sfid = (k & 1) * 2;                  // which pair of the atom's four scales
-              const uint32_t idesc = make_idesc_mxf4(128, BN, sfid, sfid);
-              const uint64_t ad = make_sdesc(a0 + k * 32, 16, 1024, 2);
-              const uint64_t bd = make_sdesc(b0 + k * 32, 16, 1024, 2);
-              tc_mma_mxf4(d_tmem, ad, bd, idesc, t_sf + (k >> 1) * 4, t_sf + 8 + (k >> 1) * NB4, (kb | k) != 0 ? 1u : 0u);
-            }
-          }
-          tc_commit(bar_empty + 8 * s);
-        }
-        __syncwarp();
-        slot ^= 1;
-        if (++s == Cfg::STAGES) { s = 0; ph ^= 1; }
-      }
-      if (elect_one()) tc_commit(bar_tfull + 8 * as);
-      __syncwarp();
-      if (++as == 2) { as = 0; aph ^= 1; }
-    }
-  } else {
-    const int q = warp & 3;
-    int as = 0;
-    uint32_t aph = 0;
-    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-      const int mb = t % p.tiles_m, nb = t / p.tiles_m;
-      const int gm = mb * Cfg::BM + q * 32 + lane;
-      mbar_wait(bar_tfull + 8 * as, aph);
-      tc_fence_after();
-      const uint32_t t_addr = tmem_base + ((uint32_t)(q * 32) << 16) + as * BN;
-#pragma unroll 1
-      for (int ps = 0; ps < BN / 32; ps++) {
-        uint32_t r[32];
-        tmem_ld_32x32b_x32(t_addr + ps * 32, r);
-        tmem_ld_wait();
-        if (ps == BN / 32 - 1) {
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(bar_tempty + 8 * as);
-        }
-        const int col0 = nb * BN + ps * 32;
-        if (gm < p.M && col0 < p.N) {
-          float* dst = p.C + (long long)gm * p.ldc + col0;
-          if (p.vec_ok && col0 + 32 <= p.N) {
-#pragma unroll
-            for (int j = 0; j < 8; j++)
-              reinterpret_cast<uint4*>(dst)[j] = make_uint4(r[4 * j], r[4 * j + 1], r[4 * j + 2], r[4 * j + 3]);
-          } else {
-#pragma unroll
-            for (int e = 0; e < 32; e++)
-              if (col0 + e < p.N) dst[e] = __uint_as_float(r[e]);
-          }
-        }
-      }
-      if (++as == 2) { as = 0; aph ^= 1; }
+      d[j] = make_uint4(w[0], w[1], w[2], w[3]);
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<Cfg::TMEM_COLS>(tmem_base);
-  }
+}
+
+// B^T: n x kpad/2 bytes -> row-major kpad x n bf16 (pitch dld).  Thread = one column n and one 32-row K-block;
+// neighbouring threads write neighbouring columns.
+__global__ void __launch_bounds__(256) mxf4_expand_cols_t_kernel(const uint8_t* __restrict__ q, const uint8_t* __restrict__ sf,
+                                                                 int n, int kpad, uint16_t* __restrict__ dst, long long dld) {
+  griddep_launch();
+  griddep_wait();
+  const int c = blockIdx.x * blockDim.x + threadIdx.x, kb = blockIdx.y, katoms = kpad >> 7;
+  if (c >= n) return;
+  float x[32];
+  mxf4_expand32(q + (long long)c * (kpad >> 1) + kb * 16, sf[mxf4_sf_offset(c, kb, katoms)], x);
+#pragma unroll
+  for (int e = 0; e < 32; e++) dst[(long long)(kb * 32 + e) * dld + c] = __bfloat16_as_ushort(__float2bfloat16_rn(x[e]));
 }
 
 }  // namespace b200

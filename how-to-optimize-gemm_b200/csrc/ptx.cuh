@@ -1,5 +1,5 @@
-// ptx.cuh — thin inline-PTX wrappers for sm_100a: mbarrier, TMA (cp.async.bulk.tensor),
-// tcgen05 (alloc / mma / commit / ld), descriptor builders.  No CUTLASS, no libraries.
+// ptx.cuh — thin inline-PTX wrappers for sm_90a: mbarrier, TMA (cp.async.bulk.tensor), wgmma shared-memory
+// descriptors, register re-balancing, programmatic dependent launch.  No CUTLASS, no libraries.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -50,30 +50,6 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   }
 }
 
-// cluster-scope variants: the barrier is signalled by the peer CTA of a pair and guards data the peer wrote
-// into this CTA's shared memory (the dynamic tile scheduler's work-item slots)
-__device__ __forceinline__ bool mbar_try_wait_cluster(uint32_t bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(ok)
-      : "r"(bar), "r"(parity)
-      : "memory");
-  return ok != 0;
-}
-__device__ __forceinline__ void mbar_wait_cluster(uint32_t bar, uint32_t parity) {
-  if (mbar_try_wait_cluster(bar, parity)) return;
-  const long long t0 = clock64();
-  while (!mbar_try_wait_cluster(bar, parity)) {
-    if (clock64() - t0 > 4000000000LL) { asm volatile("trap;"); }
-  }
-}
-__device__ __forceinline__ void st_shared_cluster_u32(uint32_t cluster_addr, uint32_t v) {
-  asm volatile("st.shared::cluster.u32 [%0], %1;" ::"r"(cluster_addr), "r"(v) : "memory");
-}
-
 // ---------------------------------------------------------------- TMA
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* m) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(m)) : "memory");
@@ -96,166 +72,23 @@ __device__ __forceinline__ void tma_load_2d_hint(uint32_t dst_smem, const CUtens
       : "memory");
 }
 
-// ---------------------------------------------------------------- tcgen05 / TMEM
-template <int NCOLS>
-__device__ __forceinline__ void tmem_alloc(uint32_t smem_dst) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst),
-               "n"(NCOLS)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <int NCOLS>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(NCOLS)
-               : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// tcgen05.commit: arrive on `bar` when all previously issued MMAs of this thread completed.
-__device__ __forceinline__ void tc_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                   bar)
-               : "memory");
+// ---------------------------------------------------------------- wgmma descriptors
+// Shared-memory matrix descriptor of wgmma (64 bit):
+//   [0,14) start>>4  [16,30) LBO>>4  [32,46) SBO>>4  [49,52) base offset (0: atoms 1 KB aligned)  [62,64) swizzle
+// swizzle: 1 = 128B, 2 = 64B, 3 = 32B.  K-major operands: SBO = stride between 8-row groups, LBO unused.
+// MN-major operands: LBO = stride between 64-element (128-byte) column blocks, SBO = stride between 8-row k groups.
+enum MmaKind { KIND_F16 = 0 /*bf16 operands*/, KIND_TF32 = 1, KIND_I8 = 2, KIND_FP16 = 3 /*fp16 operands*/ };
+enum Swz { SWZ_128B = 1, SWZ_64B = 2 };
+
+__device__ __forceinline__ uint64_t make_sdesc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes, uint32_t swz) {
+  uint64_t d = 0;
+  d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
+  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
+  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
+  d |= (uint64_t)swz << 62;
+  return d;
 }
 
-enum MmaKind { KIND_F16 = 0 /*bf16 operands*/, KIND_TF32 = 1, KIND_I8 = 2, KIND_FP16 = 3 /*fp16 operands, kind::f16*/ };
-
-// D[tmem] (+)= A[smem desc] * B[smem desc]; single-thread issue.
-template <int KIND>
-__device__ __forceinline__ void tc_mma(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc,
-                                       uint32_t idesc, uint32_t accumulate) {
-  if constexpr (KIND == KIND_F16 || KIND == KIND_FP16) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-  } else if constexpr (KIND == KIND_TF32) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-  } else {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-  }
-}
-
-// TMEM -> registers: this warp's 32 lanes x 32 consecutive 32-bit columns.
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-        "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// ---------------------------------------------------------------- CTA pairs (cta_group::2)
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// shared::cta address -> shared::cluster address of the same offset in CTA `rank` of the cluster
-__device__ __forceinline__ uint32_t mapa(uint32_t addr, uint32_t rank) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank));
-  return r;
-}
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-// TMA load issued by either CTA of a pair into ITS OWN shared memory, completing bytes on a barrier
-// that may live in the peer (leader) CTA: `bar_cluster` is a shared::cluster address.
-__device__ __forceinline__ void tma_load_2d_cg2(uint32_t dst_smem, const CUtensorMap* m,
-                                                uint32_t bar_cluster, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes "
-      "[%0], [%1, {%3, %4}], [%2];"
-      ::"r"(dst_smem), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_cluster), "r"(c0), "r"(c1)
-      : "memory");
-}
-template <int NCOLS>
-__device__ __forceinline__ void tmem_alloc_cg2(uint32_t smem_dst) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst),
-               "n"(NCOLS)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-template <int NCOLS>
-__device__ __forceinline__ void tmem_dealloc_cg2(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(NCOLS)
-               : "memory");
-}
-// commit of the pair's MMAs, arriving on the barrier at this offset in every CTA of `cta_mask`
-__device__ __forceinline__ void tc_commit_cg2(uint32_t bar, uint16_t cta_mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-      ::"r"(bar), "h"(cta_mask)
-      : "memory");
-}
-// 2-CTA MMA: M = 256 (128 rows per CTA), B split in halves of N/2 columns across the pair; issued by
-// one thread of the leader CTA only.
-template <int KIND>
-__device__ __forceinline__ void tc_mma_cg2(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc,
-                                           uint32_t idesc, uint32_t accumulate) {
-  if constexpr (KIND == KIND_F16 || KIND == KIND_FP16) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-  } else if constexpr (KIND == KIND_TF32) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-  } else {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::i8 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-  }
-}
-
-// ---------------------------------------------------------------- descriptors
-// UMMA instruction descriptor (32 bit), fields per the sm_100 layout:
-//   [4,6) c_format (1=F32, 2=S32)  [7,10) a_format  [10,13) b_format
-//   [15] a_major (0=K)  [16] b_major (1=MN)  [17,23) N>>3  [24,29) M>>4
-// formats: kind::f16 {0=F16,1=BF16}; kind::tf32 {2=TF32}; kind::i8 {0=U8,1=S8}.
-__host__ __device__ constexpr uint32_t make_idesc(uint32_t c_fmt, uint32_t ab_fmt, uint32_t a_mn,
-                                                  uint32_t b_mn, uint32_t M, uint32_t N) {
-  return (c_fmt << 4) | (ab_fmt << 7) | (ab_fmt << 10) | (a_mn << 15) | (b_mn << 16) |
-         ((N >> 3) << 17) | ((M >> 4) << 24);
-}
-
-// UMMA shared-memory matrix descriptor (64 bit):
-//   [0,14) start>>4  [16,30) LBO>>4  [32,46) SBO>>4  [46,48) version=1  [61,64) layout type
-// layout_type: 2 = SWIZZLE_128B (16-byte atoms), 1 = SWIZZLE_128B_BASE32B (32-byte atoms; the only
-// layout the hardware accepts for an MN-major tf32 operand).
 // int32 accumulator -> int8, the arithmetic of chgemm's requant tail (aarch64-int8/int8kernel_m4.S:386-426):
 // scvtf (int32 -> fp32, RNE), fmul by the row's scale, optional fadd of the row's bias (two roundings, not
 // fused), fcvtas (to nearest, ties AWAY from zero, saturating, NaN -> 0), sqxtn x2 (saturate to int8).
@@ -291,17 +124,6 @@ __device__ __forceinline__ bool elect_one() {
   uint32_t pred;
   asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.b32 %0, 1, 0, p;\n\t}" : "=r"(pred));
   return pred != 0;
-}
-
-__device__ __forceinline__ uint64_t make_sdesc(uint32_t smem_addr, uint32_t lbo_bytes,
-                                               uint32_t sbo_bytes, uint32_t layout_type = 2) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)layout_type << 61;
-  return d;
 }
 
 }  // namespace b200

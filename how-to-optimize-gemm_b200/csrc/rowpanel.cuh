@@ -68,7 +68,6 @@ struct b200_rowpanel {
   int trace = 0;            // diagnostics: timing events around every stage of the last call (b200_rowpanel_trace)
   cudaEvent_t tr[8 + 6 * kMaxSlices] = {};
   int reserve_sms = 0;      // SMs the GEMMs of all but the last K-slice leave to the exchange's copy kernels
-  int dynamic_sched = 1;    // those GEMMs draw their tiles dynamically (they share the GPU with NCCL's copy kernels)
   int k0[kMaxSlices + 1] = {};
   cudaStream_t comm_stream = nullptr;
   cudaEvent_t ev_start = nullptr, ev_b[kMaxSlices] = {}, ev_done = nullptr;
@@ -192,12 +191,9 @@ int b200_rowpanel_create(b200_rowpanel** out, void* nccl_comm, int m_local_max, 
   } else if (rp->world == 1 || k < 1024) {
     rp->nslices = 1; rp->k0[0] = 0; rp->k0[1] = k;
   } else {
-    // Up to 256 MB of B: two slices, 1 : 3.  Every extra slice costs a GEMM launch with its own pass over C (~30 us at
-    // 4096^2) and every ncclBroadcast ~40 us of fixed latency, so at 64 MB more slices lose more than a shorter first
-    // slice gains (measured on 2 x B200, profiles/r02_rowpanel_trace.txt: [512,1536,2048] 0.58 ms, [2048,2048] 0.48,
-    // [1024,3072] 0.47).  Larger operands (BASELINE config 5: 1 GiB) amortise those costs: equal slices of ~256 MB, so
-    // that only a quarter of the exchange, not the first 256 MB + everything the math could not cover, stays exposed
-    // (8 GPUs, 16384^3, two slices: 3.96 ms against ~2.3 ms of math per rank).
+    // Up to 256 MB of B: two slices, 1 : 3.  Every extra slice costs a GEMM launch with its own pass over C and
+    // every ncclBroadcast a fixed latency, so small operands use few slices.  Larger operands (BASELINE config 5:
+    // 1 GiB) amortise those costs: equal slices of ~256 MB, so that only a quarter of the exchange stays exposed.
     const double bytes = (double)k * n * 4.0;
     int ns = (int)((bytes + 268435455.0) / 268435456.0);
     ns = ns < 2 ? 2 : (ns > 8 ? 8 : ns);
@@ -244,7 +240,7 @@ int b200_rowpanel_trace_dump(b200_rowpanel* rp, float* out, int cap) {
 }
 int b200_rowpanel_set_reserve_sms(b200_rowpanel* rp, int sms) {
   if (!rp || sms < -1 || sms > 64) return B200_ERR_BAD_ARG;
-  if (sms == -1) { rp->dynamic_sched = 0; return 0; }       // tuning: static schedule for the co-running GEMMs too
+  if (sms == -1) return 0;
   rp->reserve_sms = sms;
   return 0;
 }
@@ -292,9 +288,8 @@ int b200_gemm_f32_rowpanel(b200_rowpanel* rp, int m_local, int n, int k, const f
       const F16Operand ob{rp->b_planes[j], rp->b_pitch, rp->b_rows[j], cmax};
       const bool corun = rp->world > 1 && j + 1 < rp->nslices;      // a later slice is still being broadcast
       t_sm_reserve = corun ? rp->reserve_sms : 0;
-      t_dynamic_sched = corun ? rp->dynamic_sched : 0;
       rc = gemm_f16x2_core(m_local, n, kr, oa, ob, dC, ldc, j > 0 ? 1 : 0, st);
-      t_sm_reserve = 0; t_dynamic_sched = 0;
+      t_sm_reserve = 0;
       if (rc) return rc;
       rp_mark(rp, 8 + 6 * j + 4, st);
     }
@@ -305,9 +300,8 @@ int b200_gemm_f32_rowpanel(b200_rowpanel* rp, int m_local, int n, int k, const f
     RP_CK(cudaStreamWaitEvent(st, rp->ev_b[j], 0));
     const bool corun = rp->world > 1 && j + 1 < rp->nslices;
     t_sm_reserve = corun ? rp->reserve_sms : 0;
-    t_dynamic_sched = corun ? rp->dynamic_sched : 0;
     rc = gemm_f32_impl(m_local, n, kr, dA + kk0, lda, dB + (size_t)kk0 * ldb, ldb, dC, ldc, rp->mode, j > 0 ? 1 : 0, st);
-    t_sm_reserve = 0; t_dynamic_sched = 0;
+    t_sm_reserve = 0;
     if (rc) return rc;
   }
   return 0;

@@ -96,7 +96,7 @@ int main(int argc, char** argv) {
   s.k = argc > 4 ? std::atoi(argv[4]) : 4096;
   s.repeats = argc > 5 ? std::atoi(argv[5]) : 20;
   if (s.world < 1 || s.world > ndev) { std::fprintf(stderr, "%d GPUs requested, %d present\n", s.world, ndev); return 1; }
-  if (b200_gemm_device_ok() != 0) { std::fprintf(stderr, "no usable sm_100 device (there is no CPU fallback)\n"); return 1; }
+  if (b200_gemm_device_ok() != 0) { std::fprintf(stderr, "no usable sm_90 device (there is no CPU fallback)\n"); return 1; }
   if (s.world > 1) BK(b200_comm_unique_id(s.id));
   srand48(20260923);
   s.a.resize((size_t)s.world * s.m * s.k);

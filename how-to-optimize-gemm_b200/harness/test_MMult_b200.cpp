@@ -1,4 +1,4 @@
-// test_MMult_b200.cpp — sweep driver for libb200gemm, the B200 counterpart of the reference's
+// test_MMult_b200.cpp — sweep driver for libb200gemm, the GPU counterpart of the reference's
 // benchmark/verify harness (cuda/test_MMult.cpp:21-146).  Same protocol, same output:
 //
 //   version = '<name>';                                   (cuda/makefile:43)

@@ -3,7 +3,7 @@
  *                 double* packZ_cost, double* packN_cost, double* kernel_cost)
  *   aarch64-int8/test_MMult.c:9,98; reference definition aarch64-int8/MMult_4x8_21.c:81-86.
  * C = A*B, int8 x int8 -> int32, any m,n,k; the three cost out-params are zeroed exactly as the
- * reference does (MMult_4x8_21.c:88) — there is no packZ/packN pass on B200 (TMA does it). */
+ * reference does (MMult_4x8_21.c:88) — there is no packZ/packN pass here (TMA stages A; the library transposes B once per call for the tensor core). */
 #include <stdint.h>
 #include <stdio.h>
 #include <stdlib.h>

@@ -1,5 +1,5 @@
 /*
- * b200gemm.h — C ABI of the B200-native row-major GEMM (libb200gemm.so).
+ * b200gemm.h — C ABI of the H100-native (sm_90a) row-major GEMM (libb200gemm.so).
  *
  * This header is the drop-in boundary for the hot path of
  * tpoisonooo/how-to-optimize-gemm: the free function MY_MMult that the
@@ -28,9 +28,9 @@
  * as void*; NULL = the legacy default stream the reference harness uses,
  * cuda/test_MMult.cpp:98-110), never synchronise or allocate in steady state (see
  * b200_gemm_reserve_workspace for the first call) and may be called on any stream of any
- * sm_100 device (per-device state; make the device current on the calling thread).  They return 0 on success or a cudaError_t /
+ * sm_90 device (per-device state; make the device current on the calling thread).  They return 0 on success or a cudaError_t /
  * negative B200_ERR_* code.  There is NO CPU fallback: without a CUDA device of
- * compute capability 10.x every compute entry point returns
+ * compute capability 9.x every compute entry point returns
  * B200_ERR_NO_DEVICE.
  */
 #ifndef B200GEMM_H_
@@ -46,7 +46,7 @@ extern "C" {
 /* ---- status codes (negative; positive values are cudaError_t) ------------ */
 #define B200_OK                 0
 #define B200_ERR_BAD_ARG       -1   /* null pointer, negative size, ld too small */
-#define B200_ERR_NO_DEVICE     -2   /* no sm_100 device / driver entry point missing */
+#define B200_ERR_NO_DEVICE     -2   /* no sm_90 device / driver entry point missing */
 #define B200_ERR_UNSUPPORTED   -3   /* mode not available for this dtype */
 #define B200_ERR_TENSORMAP     -4   /* cuTensorMapEncodeTiled rejected the operand */
 #define B200_ERR_NCCL          -5   /* libnccl missing or an NCCL call failed: b200_nccl_last_error() */
@@ -55,11 +55,11 @@ extern "C" {
 enum b200_f32_mode {
   B200_F32_STRICT = 0,   /* CUDA-core FFMA, fp32 multiply-add, k ascending: the
                             arithmetic of cuda/MMult_cuda_12.cu:200-206          */
-  B200_F32_TF32   = 1,   /* one tcgen05 kind::tf32 pass (10-bit mantissa inputs,
-                            fp32 accumulate in TMEM)                              */
-  B200_F32_BF16X3 = 2,   /* split-bf16: a=a1+a2+a3, 6 tcgen05 kind::f16 products per
+  B200_F32_TF32   = 1,   /* one tf32 wgmma pass (10-bit mantissa inputs, fp32
+                            accumulate)                                           */
+  B200_F32_BF16X3 = 2,   /* split-bf16: a=a1+a2+a3, 6 bf16 wgmma products per
                             k-step, two-level accumulation (K chunks of 512, each a
-                            fresh TMEM accumulator added with a rounded fp32 add to a
+                            fresh accumulator added with a rounded fp32 add to a
                             running sum held in registers): fp32-class error on the
                             tensor cores, elementwise.  The round-1 default.      */
   B200_F32_BF16X2 = 3,   /* split-bf16: a=a1+a2, 3 products, ~2^-17 relative       */
@@ -70,7 +70,7 @@ enum b200_f32_mode {
                             up to ~1100^3 the two-launch BF16X3 path               */
   B200_F32_F16X2  = 5    /* scaled split-fp16: rows of A / columns of B are scaled by
                             exact powers of two into [-1,1], a'=h1+h2 in fp16 (22
-                            bits), 3 tcgen05 kind::f16 products, two-level
+                            bits), 3 fp16 wgmma products, two-level
                             accumulation, epilogue unscales.  fp32-class NORMWISE
                             error (elements far below their row/column maximum keep
                             absolute, not relative, precision): half the tensor-core
@@ -86,7 +86,7 @@ enum b200_out_type {
 
 /* Library / device ---------------------------------------------------------- */
 const char* b200_gemm_version(void);
-/* 0 if a usable sm_100 device is current, else B200_ERR_NO_DEVICE. */
+/* 0 if a usable sm_90 device is current, else B200_ERR_NO_DEVICE. */
 int  b200_gemm_device_ok(void);
 /* Human-readable text for a code returned by this library. */
 const char* b200_gemm_strerror(int code);
@@ -103,7 +103,11 @@ void b200_gemm_set_default_f32_mode(int mode);
  * — b200_gemm_reserve_workspace(b200_gemm_workspace_bytes(m, n, k, mode)) on the device that will run the
  * calls — to keep even the first call allocation-free (e.g. ahead of CUDA-graph capture).  State is per device:
  * one process may drive several GPUs (make the device current on the calling thread); calls on different
- * streams of one device are serialised on the workspace by an event, not by the host. */
+ * streams of one device are serialised on the workspace by an event, not by the host.
+ * The same workspace holds B^T for B200_F32_TF32 (counted by b200_gemm_workspace_bytes) and for the int8 entry
+ * points (n * k16 bytes, k16 = k rounded up to 16), and the bf16 expansions of both operands for b200_gemm_mxf4
+ * (round1024(2 * m * kpad) + 2 * kpad * n8 bytes, kpad = k rounded up to 128, n8 = n rounded up to 8): reserve
+ * that much before the first such call to keep it allocation-free too. */
 size_t b200_gemm_workspace_bytes(int m, int n, int k, int precision_mode);
 int    b200_gemm_reserve_workspace(size_t bytes);
 
@@ -249,8 +253,9 @@ int  b200_gemm_f32_rowpanel_host(b200_rowpanel* plan, int m_local, int n, int k,
 /* ---- the 4-bit path (SURVEY §8 f-4) ------------------------------------------------------------------
  * The reference lists a cuda-int4 back-end and ships only the word "WIP" (cuda-int4/README.md:1;
  * README.md:13-15,118-120), so there is no interface to mirror: this is the chgemm idea (quantised operands,
- * wide accumulate) on Blackwell's only 4-bit tensor type, OCP MXFP4 — E2M1 elements with one power-of-two
- * UE8M0 scale per 32 consecutive K elements (tcgen05.mma.kind::mxf4.block_scale), fp32 accumulate and output.
+ * wide accumulate) on OCP MXFP4 — E2M1 elements with one power-of-two UE8M0 scale per 32 consecutive K
+ * elements, fp32 accumulate and output.  sm_90 has no 4-bit tensor-core operand: the GEMM expands both operands
+ * exactly to bf16 (workspace) and runs the bf16 tensor-core kernel.
  *   quantize_a   A (m x k fp32, row-major)  -> dQ (m rows of kpad/2 bytes, two elements per byte, low nibble
  *                first; kpad = k rounded up to 128) + dSF (scale atoms, b200_mxf4_sf_bytes(m, k) bytes)
  *   quantize_b   B (k x n fp32, row-major)  -> B^T quantised along K: dQ has n rows (4-bit operands must be
@@ -270,20 +275,18 @@ int b200_gemm_mxf4(int m, int n, int k, const uint8_t* dAq, const uint8_t* dSFA,
 int b200_convert_f32_to_bf16(const float* dSrc, uint16_t* dDst, size_t count,
                              void* stream);
 
-/* Test/diagnostic hook: overrides for the UMMA shared-memory descriptor of the
- * MN-major B operand (bytes; 0 = library default).  Used only by the probe in
- * tests/ to pin the descriptor semantics on real hardware. */
+/* Test/diagnostic hook: overrides for the wgmma shared-memory descriptor (LBO, SBO) of the
+ * MN-major B operand of the 16-bit kinds (bytes; 0 = library default). */
 void b200_gemm_debug_set_b_desc(int lbo_bytes, int sbo_bytes);
 /* Tuning hook: 0 = launch without programmatic dependent launch (default 1: the library's tensor-core and
  * pre-pass kernels are launched with the programmatic-serialisation attribute and order themselves with
  * griddepcontrol.wait, so a kernel's prologue overlaps the tail of its predecessor in the stream). */
 void b200_gemm_debug_set_pdl(int mask);   /* bit 0: PDL on; bit 1: keep the F16X2 pre-pass of B on the caller's stream (default: auxiliary stream beside A's) */
-/* Tuning hook: 0 = static round-robin tile schedule (default 1: a scheduler warp hands tiles out from an atomic
- * counter, so CTAs that start late because a co-running kernel holds their SM draw fewer tiles). */
+/* Accepted for ABI compatibility; no effect (the sm_90 kernels use one static round-robin tile schedule). */
 void b200_gemm_debug_set_dynamic_sched(int on);
 /* Tuning hook: force the tensor-core tile width (128, 192 or 256; 0 = built-in heuristic). */
 void b200_gemm_debug_set_bn(int bn);
-/* Tuning hook: 1 = single-CTA tiles only, 2 = CTA pairs (tcgen05 cta_group::2) always, 0 = auto. */
+/* Accepted for ABI compatibility; no effect (the sm_90 kernels have no CTA pairs). */
 void b200_gemm_debug_set_cta_group(int cg);
 /* Tuning hook: 1 (default) = the last partial round of tiles is split along K across the idle
  * CTAs and folded into C in order; 0 = whole tiles only. */
@@ -296,10 +299,7 @@ void b200_gemm_debug_set_group_rows(int rows);
 /* Tuning hook for the strict fp32 kernels: bit 0 = half tiles in the last partial round (default on),
  * bit 1 = force the 128x256 fat-thread kernel; a negative value restores selection by size. */
 void b200_gemm_debug_set_ffma_variant(int v);
-/* Tuning hook, bit mask: bit 0 = non-folding epilogue passes store straight from registers instead of through
- * the shared-memory transpose (measured no faster on B200; default off); bit 1 = drain the CTA-pair kernels of
- * the plain kinds (bf16, tf32, int8) with 4 epilogue warps instead of the default 8 (two warps per TMEM lane
- * quadrant, half the column passes each; results are bit-identical). */
+/* Accepted for ABI compatibility; no effect (the sm_90 kernels have one epilogue form). */
 void b200_gemm_debug_set_epilogue(int mask);
 /* Measurement hook: while enabled, a CUDA-event pair is recorded on the launching stream around
  * every dominant GEMM kernel launch (not the split pre-pass).  b200_gemm_debug_kernel_time_ms

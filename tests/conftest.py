@@ -7,7 +7,7 @@ sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs an sm_90 GPU (H100); run with -m gpu")
 
 
 @pytest.fixture(scope="session")
@@ -20,7 +20,7 @@ def oracle():
 def ref():
     import _libs
     if not _libs.have_ref():
-        pytest.skip("oracle/_ref/libref.so not built (needs /root/reference; run `make -C oracle ref`)")
+        pytest.skip("oracle/_ref/libref.so not built (needs the reference sources; run `make -C oracle ref`)")
     return _libs.load_ref()
 
 

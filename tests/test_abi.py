@@ -1,5 +1,5 @@
 """The drop-in boundary without a GPU: the C-ABI library loads, exports exactly what
-include/b200gemm.h declares, and refuses to compute (loudly) when there is no sm_100 device."""
+include/b200gemm.h declares, and refuses to compute (loudly) when there is no sm_90 device."""
 import ctypes as C
 import os
 import re

@@ -4,6 +4,7 @@ import json
 import os
 import subprocess
 import sys
+import pytest
 
 import _libs
 
@@ -28,6 +29,8 @@ def test_reference_arm_survives_the_torchrun_environment():
     828 s at N=2/4 and crashed at N=8 — growing OpenBLAS-0.2.20's thread pool after load dead-locks.  The arm now
     runs the CPU path in a fresh process whose pool is sized by OPENBLAS_NUM_THREADS at load; same workload string
     as our arm (the driver's same_config check)."""
+    if not _libs.have_ref():
+        pytest.skip("oracle/_ref/libref.so (the reference's OpenBLAS) not built")
     env = dict(os.environ, OMP_NUM_THREADS="1", RANK="0", WORLD_SIZE="2", LOCAL_RANK="0", B200_REF_THREADS="128")
     r = subprocess.run([sys.executable, os.path.join(_libs.ROOT, "bench.py"), "--impl", "reference", "--gpus", "2",
                         "--steps", "1", "--warmup", "1"], capture_output=True, text=True, timeout=300, env=env)

@@ -1,6 +1,6 @@
 """Resource budget of the compiled kernels, from the `-Xptxas -v` log the in-tree build writes
 (how-to-optimize-gemm_b200/build_ptxas.log): the occupancy each kernel is designed for (DESIGN §4) only holds
-while these stay true.  CPU only (ptxas cross-compiles sm_100a without a GPU)."""
+while these stay true.  CPU only (ptxas cross-compiles sm_90a without a GPU)."""
 import os
 import re
 
@@ -15,7 +15,7 @@ def kernels():
         subprocess.check_call(["make", "-B", "-C", os.path.join(_libs.ROOT, _libs.PKG), "libb200gemm.so"])
     out, name = {}, None
     for line in open(LOG):
-        m = re.search(r"Compiling entry function '(\w+)' for 'sm_100a'", line)
+        m = re.search(r"Compiling entry function '(\w+)' for 'sm_90a'", line)
         if m:
             name = m.group(1)
             out[name] = {"regs": None, "spill": None}
@@ -34,9 +34,9 @@ def test_log_covers_every_kernel_family():
 
 
 def test_tensor_core_kernels_do_not_spill():
-    # one CTA per SM.  192 threads (4 epilogue warps): up to 255 registers; 320 threads (8 epilogue warps): 204;
-    # split-precision kernels (384 threads, setmaxnreg 88 / 208 after a 168-register launch): the running sum of a
-    # tile lives in the epilogue warps' registers — a spill there would sit in the per-chunk add loop
+    # one CTA of 384 threads per SM (168 registers at launch; setmaxnreg 40 for the producer warpgroup, 232 for
+    # the two consumers): the running sum of a split-precision tile lives in the consumers' registers — a spill
+    # there would sit in the per-chunk add loop
     for n, v in kernels().items():
         if "gemm_tc_kernel" in n:
             # <= 48 bytes: a few split kernels keep the mbarrier watchdog's clock value in one stack slot

@@ -156,7 +156,7 @@ def test_s8s32_bit_exact(gemm, oracle, m, n, k):
 
 def test_s8_extremes_and_alignment(gemm, oracle):
     """[-127,127] extremes (chgemm input contract, /root/reference/README.md:82); 16-byte aligned
-    pitches go through tcgen05 kind::i8, everything else through the CUDA-core kernel: same bits."""
+    pitches go through the int8 wgmma kernel, everything else through the CUDA-core kernel: same bits."""
     m, n, k = 160, 272, 512
     for fill_a, fill_b in [(127, 127), (-127, 127), (-127, -127)]:
         a = np.full((m, k), fill_a, np.int8)
@@ -236,7 +236,7 @@ def test_full_size_s8_requant_4096(gemm, oracle):
     a, b, scales, bias = _rq_case(oracle, N, N, N, 81, "layer")
     A, B, S, Bi = cuda(a), cuda(b), cuda(scales), cuda(bias)
     out = gemm.gemm_s8s8_requant(A, B, S, Bi)
-    assert gemm.last_kernel().startswith("tc_s8_requant_2cta_256x256")
+    assert gemm.last_kernel().startswith("tc_s8_requant_128x256")
     rows = np.arange(0, N, 31)[:128]
     ref = _libs.requant_s8(oracle, _libs.ref_s8(oracle, a[rows], b), scales[rows], bias[rows])
     assert np.array_equal(out[torch.from_numpy(rows).cuda()].cpu().numpy(), ref)

@@ -1,4 +1,4 @@
-"""Small-N crossover between the strict FFMA2 kernel and the BF16X3 tensor-core path (what AUTO should pick)."""
+"""Small-N crossover between the strict FFMA kernel and the BF16X3 tensor-core path (what AUTO should pick)."""
 import os
 import sys
 
