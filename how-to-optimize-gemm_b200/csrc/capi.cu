@@ -264,7 +264,8 @@ template <typename InT, typename OutT>
 int launch_generic(int m, int n, int k, const InT* A, int lda, const InT* B, int ldb, OutT* C, int ldc,
                    int accumulate, cudaStream_t st, const char* name) {
   dim3 grid((n + 63) / 64, (m + 63) / 64);
-  gemm_generic_kernel<InT, OutT><<<grid, 256, 0, st>>>(m, n, k, A, lda, B, ldb, C, ldc, accumulate);
+  gemm_generic_kernel<InT, OutT><<<grid, 256, 0, st>>>(m, n, k, A, lda, B, ldb, C, ldc, accumulate, nullptr, nullptr,
+                                                       t_epi.axpby, t_epi.alpha, t_epi.beta);
   g_launches++;
   t_last_kernel = name;
   return last_launch_status();
@@ -401,7 +402,8 @@ int tc_bf16_bf16(int m, int n, int k, const void* A, int lda, const void* B, int
 // Workspace for the bf16 planes: cached, grow-only (no per-call cudaMalloc in steady state).  Calls
 // in split modes are serialised on this buffer by stream order; use one stream per library instance.
 // K extent accumulated inside the tensor core before folding into C (0 = whole K): [0] BF16X3, [1] BF16X2
-int g_split_chunk_k[3] = {512, 512, 1024};   // BF16X3, BF16X2, F16X2
+constexpr int kSplitChunkDefault[3] = {512, 512, 1024};   // BF16X3, BF16X2, F16X2
+int g_split_chunk_k[3] = {kSplitChunkDefault[0], kSplitChunkDefault[1], kSplitChunkDefault[2]};
 // Grows the device's split workspace to `need` bytes.  Starts at 256 MiB (every size of the reference's
 // 256..4096 sweep fits: its harness averages the first, cold call into each row, and a cudaFree +
 // cudaMalloc there costs tens of ms) and at least doubles.  Growth synchronises the device (other
@@ -662,6 +664,7 @@ int launch_ffma(int m, int n, int k, const float* A, int lda, const float* B, in
   p.C = C; p.ldc = ldc; p.M = m; p.N = n; p.K = k;
   p.vec_ok = aligned16(C) && (ldc % 4) == 0;
   p.accumulate = accumulate;
+  p.axpby = t_epi.axpby; p.alpha = t_epi.alpha; p.beta = t_epi.beta;
   p.tiles_m = (m + Cfg::BM - 1) / Cfg::BM;
   p.tiles_n = (n + Cfg::BN - 1) / Cfg::BN;
   p.group_m = 8;
@@ -692,6 +695,7 @@ int launch_ffma_fat(int m, int n, int k, const float* A, int lda, const float* B
   p.C = C; p.ldc = ldc; p.M = m; p.N = n; p.K = k;
   p.vec_ok = aligned16(C) && (ldc % 4) == 0;
   p.accumulate = accumulate;
+  p.axpby = t_epi.axpby; p.alpha = t_epi.alpha; p.beta = t_epi.beta;
   p.tiles_m = (m + Cfg::BM - 1) / Cfg::BM;
   p.tiles_n = (n + Cfg::BN - 1) / Cfg::BN;
   p.group_m = 8;
@@ -807,7 +811,11 @@ void b200_gemm_debug_set_split_tail(int on) { g_split_tail = on; }
 void b200_gemm_debug_set_epilogue(int) {}
 void b200_gemm_debug_set_group_rows(int rows) { g_group_rows = rows; }
 void b200_gemm_debug_set_ffma_variant(int v) { g_ffma_halves = v & 1; g_ffma_fat = v < 0 ? -1 : (v >> 1) & 1; }
-void b200_gemm_debug_set_split_chunk(int x3_k, int x2_k) { g_split_chunk_k[0] = x3_k; g_split_chunk_k[1] = x2_k; g_split_chunk_k[2] = x2_k; }
+void b200_gemm_debug_set_split_chunk(int x3_k, int x2_k) {
+  g_split_chunk_k[0] = x3_k < 0 ? kSplitChunkDefault[0] : x3_k;
+  g_split_chunk_k[1] = x2_k < 0 ? kSplitChunkDefault[1] : x2_k;
+  g_split_chunk_k[2] = x2_k < 0 ? kSplitChunkDefault[2] : x2_k;
+}
 void b200_gemm_debug_kernel_timing(int enable) { g_ktimer.on = enable != 0; g_ktimer.n = 0; }
 int b200_gemm_debug_kernel_time_ms(double* sum_ms) {
   double sum = 0;
@@ -859,28 +867,19 @@ int b200_gemm_f32_ex(int m, int n, int k, float alpha, const float* dA, int lda,
   if (rc) return rc;
   rc = ensure_device();
   if (rc) return rc;
-  const int mode = resolve_f32_mode(precision_mode);
-  const bool cuda_core = mode == B200_F32_STRICT || !tma_ok(dA, lda, dB, ldb, 4) || k == 0 ||
-                         (precision_mode == B200_F32_AUTO && (double)m * n * k <= 2.0e8);
-  const dim3 sg((n + 255) / 256, m < 4096 ? m : 4096);
-  if (alpha == 0.f || cuda_core) {
-    // CUDA-core paths (strict FFMA chain, generic kernels): C <- (beta/alpha) C, C += A*B, C <- alpha C.
-    // beta == 0 must not read C (NaN-safe, as cuBLAS): start from C = A*B instead.
-    if (alpha == 0.f || k == 0) {
-      if (beta == 0.f) return launch_zero<float>(m, n, dC, ldc, st);
-      scale_inplace_kernel<<<sg, 256, 0, st>>>(m, n, dC, ldc, beta);
-      g_launches++;
-      return last_launch_status();
-    }
-    if (beta != 0.f && beta != alpha) { scale_inplace_kernel<<<sg, 256, 0, st>>>(m, n, dC, ldc, beta / alpha); g_launches++; }
-    rc = gemm_f32_impl(m, n, k, dA, lda, dB, ldb, dC, ldc, cuda_core && mode != B200_F32_STRICT && tma_ok(dA, lda, dB, ldb, 4) ? B200_F32_STRICT : mode,
-                       beta != 0.f ? 1 : 0, st);
-    if (rc) return rc;
-    scale_inplace_kernel<<<sg, 256, 0, st>>>(m, n, dC, ldc, alpha);
+  if (alpha == 0.f || k == 0) {           // C = beta * C: A and B are not read; beta == 0 does not read C either
+    if (beta == 0.f) return launch_zero<float>(m, n, dC, ldc, st);
+    const dim3 sg((n + 255) / 256, m < 4096 ? m : 4096);
+    scale_inplace_kernel<<<sg, 256, 0, st>>>(m, n, dC, ldc, beta);
     g_launches++;
     return last_launch_status();
   }
-  t_epi.axpby = 1; t_epi.alpha = alpha; t_epi.beta = beta;      // tensor-core modes: fused into the epilogue
+  int mode = resolve_f32_mode(precision_mode);
+  // AUTO on a small problem with TMA-able operands: the single-launch strict kernel, whatever the default mode
+  if (precision_mode == B200_F32_AUTO && (double)m * n * k <= 2.0e8 && tma_ok(dA, lda, dB, ldb, 4)) mode = B200_F32_STRICT;
+  // every kernel applies alpha and beta in its epilogue (alpha * AB, then + beta * C with C read only when
+  // beta != 0): no pre-scaled C, so beta / alpha never has to be representable
+  t_epi.axpby = 1; t_epi.alpha = alpha; t_epi.beta = beta;
   rc = gemm_f32_impl(m, n, k, dA, lda, dB, ldb, dC, ldc, mode, 0, st);
   t_epi = EpiOpts();
   return rc;

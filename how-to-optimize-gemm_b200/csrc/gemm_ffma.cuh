@@ -48,7 +48,28 @@ struct FfmaParams {
   int accumulate;   // 1: accumulator chains start from C(i,j) (C += A*B), 0: from zero (C = A*B)
   int tiles_m, tiles_n, group_m;
   int full_tiles;   // CTAs [0, full_tiles) own whole tiles; later CTAs own half tiles, two per tile
+  // General epilogue C = alpha * (A*B) + beta * C (b200_gemm_f32_ex), axpby == 1 only; the chains then start
+  // from zero and C is read only when beta != 0.
+  int axpby;
+  float alpha, beta;
 };
+
+// Four adjacent outputs ev (columns gn..gn+3 of one row, dst = &C(row, gn)) through the general epilogue, with
+// the arithmetic of the tensor-core epilogue: alpha * v rounded, then fma(beta, C, .).
+__device__ __forceinline__ void ffma_axpby4(const FfmaParams& p, const float* dst, int gn, bool vec, float (&ev)[4]) {
+#pragma unroll
+  for (int e = 0; e < 4; e++) ev[e] *= p.alpha;
+  if (p.beta == 0.f) return;
+  if (vec) {
+    const float4 o = *reinterpret_cast<const float4*>(dst);
+    ev[0] = fmaf(p.beta, o.x, ev[0]); ev[1] = fmaf(p.beta, o.y, ev[1]);
+    ev[2] = fmaf(p.beta, o.z, ev[2]); ev[3] = fmaf(p.beta, o.w, ev[3]);
+  } else {
+#pragma unroll
+    for (int e = 0; e < 4; e++)
+      if (gn + e < p.N) ev[e] = fmaf(p.beta, dst[e], ev[e]);
+  }
+}
 
 struct FfmaCfg {
   static constexpr int BM = 128, BN = 128, BK = 32, STAGES = 3;
@@ -154,11 +175,12 @@ __device__ __forceinline__ void ffma_tile(const CUtensorMap& tmA, const CUtensor
     for (int j = 0; j < 2; j++) {
       const int gn = n0 + tx * 4 + 64 * j;
       float* dst = p.C + (long long)gm * p.ldc + gn;
-      if (p.vec_ok && gn + 4 <= p.N) {
-        *reinterpret_cast<float4*>(dst) =
-            make_float4(acc[i][2 * j].x, acc[i][2 * j].y, acc[i][2 * j + 1].x, acc[i][2 * j + 1].y);
+      const bool vec = p.vec_ok && gn + 4 <= p.N;
+      float ev[4] = {acc[i][2 * j].x, acc[i][2 * j].y, acc[i][2 * j + 1].x, acc[i][2 * j + 1].y};
+      if (p.axpby) ffma_axpby4(p, dst, gn, vec, ev);
+      if (vec) {
+        *reinterpret_cast<float4*>(dst) = make_float4(ev[0], ev[1], ev[2], ev[3]);
       } else {
-        const float ev[4] = {acc[i][2 * j].x, acc[i][2 * j].y, acc[i][2 * j + 1].x, acc[i][2 * j + 1].y};
 #pragma unroll
         for (int e = 0; e < 4; e++)
           if (gn + e < p.N) dst[e] = ev[e];
@@ -329,11 +351,12 @@ __device__ __forceinline__ void ffma_fat_tile(const CUtensorMap& tmA, const CUte
     for (int j = 0; j < 4; j++) {
       const int gn = n0 + tx * 4 + 64 * j;
       float* dst = p.C + (long long)gm * p.ldc + gn;
-      if (p.vec_ok && gn + 4 <= p.N) {
-        *reinterpret_cast<float4*>(dst) =
-            make_float4(acc[i][2 * j].x, acc[i][2 * j].y, acc[i][2 * j + 1].x, acc[i][2 * j + 1].y);
+      const bool vec = p.vec_ok && gn + 4 <= p.N;
+      float ev[4] = {acc[i][2 * j].x, acc[i][2 * j].y, acc[i][2 * j + 1].x, acc[i][2 * j + 1].y};
+      if (p.axpby) ffma_axpby4(p, dst, gn, vec, ev);
+      if (vec) {
+        *reinterpret_cast<float4*>(dst) = make_float4(ev[0], ev[1], ev[2], ev[3]);
       } else {
-        const float ev[4] = {acc[i][2 * j].x, acc[i][2 * j].y, acc[i][2 * j + 1].x, acc[i][2 * j + 1].y};
 #pragma unroll
         for (int e = 0; e < 4; e++)
           if (gn + e < p.N) dst[e] = ev[e];

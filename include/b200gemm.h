@@ -127,9 +127,10 @@ int b200_gemm_f32_acc(int m, int n, int k,
 
 /* fp32: C = alpha * A*B + beta * C on DEVICE pointers — the contract of the reference's cuBLAS comparator
  * (cublasSgemm, cuda/MMult_cuBLAS_1.cpp:11-19; the harness only ever passes alpha = 1, beta = 0).  beta == 0
- * never reads C.  (1, 0) and (1, 1) are b200_gemm_f32 / b200_gemm_f32_acc exactly; any other pair is fused
- * into the epilogue of the tensor-core modes, and costs two element-wise passes over C around the kernel in
- * STRICT mode and on the generic (unaligned-operand) path. */
+ * never reads C; alpha == 0 never reads A or B (one element-wise pass C = beta * C).  (1, 0) and (1, 1) are
+ * b200_gemm_f32 / b200_gemm_f32_acc exactly; any other pair is fused into the epilogue of every kernel
+ * (tensor-core, strict FFMA and generic): the product is accumulated from zero and stored as
+ * fma(beta, C, alpha * AB), so no intermediate such as beta / alpha can overflow. */
 int b200_gemm_f32_ex(int m, int n, int k, float alpha,
                      const float* dA, int lda, const float* dB, int ldb, float beta,
                      float* dC, int ldc, int precision_mode, void* stream);
@@ -292,7 +293,9 @@ void b200_gemm_debug_set_cta_group(int cg);
  * CTAs and folded into C in order; 0 = whole tiles only. */
 void b200_gemm_debug_set_split_tail(int on);
 /* Tuning hook: K extent the tensor core accumulates before the epilogue folds the partial sum
- * into C with a rounded fp32 add (two-level accumulation of the split modes); 0 = whole K. */
+ * into C with a rounded fp32 add (two-level accumulation of the split modes); 0 = whole K.
+ * bf16x2_k sets both BF16X2 and F16X2.  A negative value restores the built-in default of its
+ * mode(s): 512 for BF16X3 and BF16X2, 1024 for F16X2. */
 void b200_gemm_debug_set_split_chunk(int bf16x3_k, int bf16x2_k);
 /* Tuning hook: rows of A per raster group of the persistent tile schedule (0 = 2048). */
 void b200_gemm_debug_set_group_rows(int rows);

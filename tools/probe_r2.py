@@ -77,7 +77,7 @@ for grp in (2048, 4096):
         sweep.append({"group_rows": grp, "chunk_k": ck, "ms": ms, "tflops": flops / ms / 1e9, "rel_err": err(Cm)})
         print(sweep[-1], flush=True)
 g.lib.b200_gemm_debug_set_group_rows(0)
-g.lib.b200_gemm_debug_set_split_chunk(512, 512)
+g.lib.b200_gemm_debug_set_split_chunk(-1, -1)      # the built-in chunks of every split mode
 out["f16x2_sweep"] = sweep
 os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
 json.dump(out, open(os.path.join(ROOT, "gpurun_out", f"probe_r2_{N}.json"), "w"), indent=1)
