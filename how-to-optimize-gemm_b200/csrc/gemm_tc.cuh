@@ -137,8 +137,9 @@ __device__ __forceinline__ void tile_coords(int t, int tiles_m, int tiles_n, int
   nb = r / rows;
 }
 
-// Scaled split mode (B200_F32_F16X2): exponent e with maxv * 2^-e in [0.5, 1); 0 for zero, denormal,
-// inf or NaN maxima.  Range [-125, 128].
+// Scaled split mode (B200_F32_F16X2): exponent e with maxv * 2^-e in [0.5, 1) for every finite nonzero
+// maxv (a subnormal maximum takes the exponent of its leading bit); 0 for zero, inf or NaN maxima.
+// Range [-148, 128].
 __host__ __device__ __forceinline__ int pow2_exp(float maxv) {
   uint32_t bits;
 #ifdef __CUDA_ARCH__
@@ -147,15 +148,32 @@ __host__ __device__ __forceinline__ int pow2_exp(float maxv) {
   memcpy(&bits, &maxv, 4);
 #endif
   const int ef = (int)((bits >> 23) & 0xFF);
-  return (ef == 0 || ef == 255) ? 0 : ef - 126;
+  const uint32_t mant = bits & 0x7FFFFFu;          // a subnormal is mant * 2^-149
+#ifdef __CUDA_ARCH__
+  const int sub = (31 - __clz(mant | 1u)) - 148;
+#else
+  const int sub = (31 - __builtin_clz(mant | 1u)) - 148;
+#endif
+  return ef == 255 ? 0 : ef != 0 ? ef - 126 : mant != 0 ? sub : 0;
 }
 // 2^e as a float, e in [-126, 127]
 __device__ __forceinline__ float exp2i(int e) { return __uint_as_float((uint32_t)(127 + e) << 23); }
-// x * 2^e for any e in [-256, 256] through two normal power-of-two factors (exact unless the result
-// itself leaves the fp32 range)
-__device__ __forceinline__ float mul_pow2(float x, int e) {
+// Pre-pass scaling x * 2^e, e in [-128, 148] (= -pow2_exp): two normal power-of-two factors.  Exact whenever
+// the result is normal; a result below 2^-126 may be rounded twice, but every such value is below half the
+// smallest fp16 subnormal and splits into zero planes either way.
+__device__ __forceinline__ float scale_pow2(float x, int e) {
   const int h = e >> 1;
-  return x * exp2i(h) * exp2i(min(e - h, 127));
+  return x * exp2i(h) * exp2i(e - h);
+}
+// F16X2 epilogue unscale: x * 2^e rounded once, for e in [-296, 256] (= e_row + e_col) and an accumulator x
+// that is 0 or 2^-48 <= |x| < 2^32 (a sum of products of fp16 values below 1, each a multiple of 2^-48).
+// x * 2^a with a = clamp(e, -78, 95) is exact and normal; the second factor 2^b, b = clamp(e - a, -126, 127),
+// then rounds once.  b is clamped only where the result is below 2^-172 (rounds to 0 either way) or above
+// 2^174 (overflows either way).  No factor is ever inf, so 0 stays 0.
+__device__ __forceinline__ float mul_pow2(float x, int e) {
+  const int a = max(min(e, 95), -78);
+  const int b = max(min(e - a, 127), -126);
+  return x * exp2i(a) * exp2i(b);
 }
 
 struct WorkItem { int tile, part, kb0, kb1; };
@@ -453,10 +471,25 @@ __global__ void __launch_bounds__(256) transpose_kernel(const E* __restrict__ sr
 // pitch dld (elements, multiple of 8).  x = p1 + p2 + p3 with p1 = bf16(x), p2 = bf16(x - p1),
 // p3 = bf16(x - p1 - p2); the subtractions are exact in fp32.  Rows [rows, plane_rows) and columns
 // [cols, dld) of every plane are written as zero (K padding of B must contribute nothing).
+// Range edges: a finite x never gets an infinite plane (|x| >= 0x7f7f8000 rounds to bf16 inf; its plane
+// is clamped to +-0x7f7f, and the residual x - p1 stays exact), and a non-finite x gives p1 = x and
+// zero lower planes.
 struct SplitJob {
   const float* src; long long ld; int rows, cols;
   uint16_t* dst; long long dld; int plane_rows;
 };
+
+// One round-to-nearest-even bf16 plane of the pair (lo, hi), packed {hi, lo}; lo and hi become the residuals.
+__device__ __forceinline__ uint32_t bf16_plane2(float& lo, float& hi) {
+  uint32_t w;
+  asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(w) : "f"(hi), "f"(lo));
+  const bool fin_lo = fabsf(lo) <= 3.40282347e38f, fin_hi = fabsf(hi) <= 3.40282347e38f;   // false for inf, NaN
+  if (fin_lo && (w & 0x7FFFu) == 0x7F80u) w -= 1u;                    // +-inf -> +-0x7f7f
+  if (fin_hi && (w & 0x7FFF0000u) == 0x7F800000u) w -= 0x10000u;
+  lo = fin_lo ? lo - __uint_as_float(w << 16) : 0.f;
+  hi = fin_hi ? hi - __uint_as_float(w & 0xFFFF0000u) : 0.f;
+  return w;
+}
 
 // One launch splits both operands (blockIdx.z picks A or B).  A thread owns 8 consecutive columns
 // (two 16-byte loads, one 16-byte store per plane) and walks rows blockIdx.y, +gridDim.y, ... two at
@@ -502,12 +535,7 @@ __global__ void __launch_bounds__(256) split_planes_kernel(const SplitJob ja, co
       for (int pl = 0; pl < NP; pl++) {
         uint32_t w[4];
 #pragma unroll
-        for (int e = 0; e < 4; e++) {
-          // packs {hi half <- x[2e+1], lo half <- x[2e]}, round-to-nearest-even
-          asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(w[e]) : "f"(x[u][2 * e + 1]), "f"(x[u][2 * e]));
-          x[u][2 * e] -= __uint_as_float(w[e] << 16);
-          x[u][2 * e + 1] -= __uint_as_float(w[e] & 0xFFFF0000u);
-        }
+        for (int e = 0; e < 4; e++) w[e] = bf16_plane2(x[u][2 * e], x[u][2 * e + 1]);
         *reinterpret_cast<uint4*>(dst + ((long long)pl * plane_rows + r) * dld + c) = make_uint4(w[0], w[1], w[2], w[3]);
       }
     }
@@ -592,7 +620,7 @@ __global__ void __launch_bounds__(256) split_f16_rows_kernel(const float* __rest
         const int c = (j * 32 + lane) * 8;
         if (c < dld) {
 #pragma unroll
-          for (int e = 0; e < 8; e++) x[j][e] = mul_pow2(x[j][e], ex);
+          for (int e = 0; e < 8; e++) x[j][e] = scale_pow2(x[j][e], ex);
           uint4 h1, h2;
           split_f16x8(x[j], h1, h2);
           *reinterpret_cast<uint4*>(d1 + c) = h1;
@@ -630,7 +658,7 @@ __global__ void __launch_bounds__(256) split_f16_rows_kernel(const float* __rest
           const int c = c0 + u * 256;
           if (c < dld) {
 #pragma unroll
-            for (int e = 0; e < 8; e++) x[u][e] = mul_pow2(x[u][e], ex);
+            for (int e = 0; e < 8; e++) x[u][e] = scale_pow2(x[u][e], ex);
             uint4 h1, h2;
             split_f16x8(x[u], h1, h2);
             *reinterpret_cast<uint4*>(d1 + c) = h1;
@@ -715,7 +743,7 @@ __global__ void __launch_bounds__(256) split_f16_cols_kernel(const float* __rest
       const int r = r0 + u;
       if (r >= plane_rows) break;
 #pragma unroll
-      for (int e = 0; e < 8; e++) x[u][e] = mul_pow2(x[u][e], ex[e]);
+      for (int e = 0; e < 8; e++) x[u][e] = scale_pow2(x[u][e], ex[e]);
       uint4 h1, h2;
       split_f16x8(x[u], h1, h2);
       *reinterpret_cast<uint4*>(dst + (long long)r * dld + c) = h1;

@@ -77,6 +77,20 @@ enum b200_f32_mode {
                             work of BF16X3 at the same measured error.
                             THE LIBRARY DEFAULT.                                   */
 };
+/* Range contract of the fp32 modes (tests/test_fp32_range_gpu.py), over the whole fp32
+ * range including subnormals, FLT_MAX, inf and NaN:
+ *  - C(i,j) is non-finite exactly where the IEEE result is: an inf or NaN in row i of A or
+ *    column j of B, or a result beyond FLT_MAX.  No other element is contaminated.  The split
+ *    modes may return NaN where IEEE gives +-inf: they form inf*(b1 + b2) as inf*b1 + inf*b2.
+ *  - Finite results: STRICT is one fused multiply-add chain per element (bit-exact against the
+ *    naive reference); BF16X3 within 2^-22 (|A||B|)ij, BF16X2 within 2^-14 (|A||B|)ij, TF32
+ *    within 2^-9 (|A||B|)ij, elementwise; F16X2 within 2^-20 K max|A(i,:)| max|B(:,j)|
+ *    (normwise per row and column, subnormal and near-FLT_MAX maxima included); each plus
+ *    its fp32 accumulation error.  In the bf16 and tf32 modes an operand below about 2^-110
+ *    loses bits absolutely (its lower planes fall under the bf16 subnormal quantum 2^-133):
+ *    add 2^-133 (sum_k |A(i,k)| + sum_k |B(k,j)|).
+ *  - The H100 tensor cores keep subnormal bf16, tf32 and fp16 inputs and subnormal fp32
+ *    products and sums (observed on an H100 80GB HBM3): nothing is flushed to zero.        */
 
 /* ---- bf16 output selector -------------------------------------------------- */
 enum b200_out_type {
