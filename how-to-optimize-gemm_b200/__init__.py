@@ -18,6 +18,7 @@ LIB_PATH = os.path.join(_HERE, "libb200gemm.so")
 
 F32_STRICT, F32_TF32, F32_BF16X3, F32_BF16X2, F32_AUTO, F32_F16X2 = 0, 1, 2, 3, 4, 5
 OUT_F32, OUT_BF16 = 0, 1
+OP_N, OP_T = 0, 1
 
 EXPORTS = [
     "b200_gemm_version", "b200_gemm_device_ok", "b200_gemm_strerror", "b200_gemm_last_kernel",
@@ -25,7 +26,8 @@ EXPORTS = [
     "b200_gemm_f32", "b200_gemm_f32_acc", "b200_gemm_f32_ex", "b200_gemm_workspace_bytes", "b200_gemm_reserve_workspace", "b200_mxf4_q_bytes", "b200_mxf4_sf_bytes",
     "b200_mxf4_quantize_a", "b200_mxf4_quantize_b", "b200_gemm_mxf4", "b200_gemm_f32_host", "b200_gemm_bf16", "b200_gemm_s8s32",
     "b200_gemm_s8s32_host", "b200_gemm_s8s8_requant", "b200_gemm_f32_pack_b", "b200_gemm_f32_packed",
-    "b200_gemm_f32_pack_free", "b200_nccl_load", "b200_nccl_last_error", "b200_comm_unique_id", "b200_comm_init_rank",
+    "b200_gemm_f32_pack_free", "b200_gemm_f32_op", "b200_gemm_bf16_op", "b200_gemm_s8s32_op", "b200_gemm_workspace_bytes_op",
+    "b200_nccl_load", "b200_nccl_last_error", "b200_comm_unique_id", "b200_comm_init_rank",
     "b200_comm_destroy", "b200_rowpanel_create", "b200_rowpanel_destroy", "b200_rowpanel_slices", "b200_rowpanel_set_reserve_sms", "b200_rowpanel_trace", "b200_rowpanel_trace_dump", "b200_gemm_f32_rowpanel",
     "b200_gemm_f32_rowpanel_host", "b200_gemm_f32_pack_a", "b200_gemm_f32_packed_ab", "b200_gemm_f32_pack_free_a",
     "b200_convert_f32_to_bf16", "b200_gemm_debug_set_b_desc", "b200_gemm_debug_set_bn",
@@ -70,6 +72,11 @@ lib.b200_gemm_f32_host.argtypes = [_i, _i, _i, _vp, _i, _vp, _i, _vp, _i, _i]
 lib.b200_gemm_bf16.argtypes = [_i, _i, _i, _vp, _i, _vp, _i, _vp, _i, _i, _vp]
 lib.b200_gemm_s8s32.argtypes = [_i, _i, _i, _vp, _i, _vp, _i, _vp, _i, _vp]
 lib.b200_gemm_s8s32_host.argtypes = [_i, _i, _i, _vp, _i, _vp, _i, _vp, _i]
+lib.b200_gemm_f32_op.argtypes = [_i, _i, _i, _i, _i, C.c_float, _vp, _i, _vp, _i, C.c_float, _vp, _i, _i, _vp]
+lib.b200_gemm_bf16_op.argtypes = [_i, _i, _i, _i, _i, _vp, _i, _vp, _i, _vp, _i, _i, _vp]
+lib.b200_gemm_s8s32_op.argtypes = [_i, _i, _i, _i, _i, _vp, _i, _vp, _i, _vp, _i, _vp]
+lib.b200_gemm_workspace_bytes_op.argtypes = [_i, _i, _i, _i, _i, _i]
+lib.b200_gemm_workspace_bytes_op.restype = C.c_size_t
 lib.b200_gemm_f32_pack_b.argtypes = [_i, _i, _vp, _i, _i, C.POINTER(_vp), _vp]
 lib.b200_gemm_f32_packed.argtypes = [_i, _i, _i, _vp, _i, _vp, _vp, _i, _i, _vp]
 lib.b200_gemm_f32_pack_free.argtypes = [_vp]
@@ -164,6 +171,66 @@ def _ld(t):
     if t.shape[1] <= 1:              # a single column: any stride is reported for the size-1 dimension
         return max(1, t.stride(0)) if t.shape[0] > 1 else 1
     return t.stride(0) if t.shape[0] > 1 else max(t.shape[1], t.stride(0))
+
+
+def operand_layout(shape, strides):
+    """(op, ld) under which the C ABI reads a 2-D operand of this shape and these strides (elements) in place.
+
+    Row-major (unit stride along dim 1): OP_N, ld = stride(0).  Transposed view of a row-major matrix (unit stride
+    along dim 0, e.g. W.t()): OP_T, ld = stride(1).  A dimension of size 1 may have any stride; a tensor that is both
+    (a single row or column) is taken as row-major.  Any other stride pattern raises ValueError: the library never
+    copies an operand."""
+    r, c = shape
+    s0, s1 = strides
+    if c <= 1:                       # a single column: row-major with any row stride
+        return OP_N, (max(1, s0) if r > 1 else 1)
+    if s1 == 1:
+        return OP_N, (s0 if r > 1 else max(c, s0))
+    if s0 == 1 or r <= 1:            # column c of the view is row c of the stored (c x r) matrix
+        return OP_T, s1
+    raise ValueError(f"operand of shape {tuple(shape)} and strides {tuple(strides)} is neither row-major nor the "
+                     "transpose of a row-major matrix")
+
+
+def gemm(A, B, out=None, *, alpha=1.0, beta=0.0, mode=F32_AUTO, out_dtype=None, stream=None):
+    """C = alpha * A @ B + beta * C for fp32 (any precision mode), bf16 (fp32 or bf16 C) and int8 (int32 C) CUDA
+    tensors.  Each operand may be row-major or the transpose of a row-major matrix (x @ W.t() passes W as stored):
+    it is read in place (b200_gemm_f32_op / _bf16_op / _s8s32_op), never copied.  out must be row-major; it is
+    read only when beta != 0.  bf16 and int8 take alpha = 1, beta = 0 only."""
+    import torch
+    assert A.dim() == 2 and B.dim() == 2 and A.is_cuda and B.is_cuda and A.dtype == B.dtype
+    m, k = A.shape
+    k2, n = B.shape
+    assert k == k2, (A.shape, B.shape)
+    op_a, lda = operand_layout(tuple(A.shape), A.stride())
+    op_b, ldb = operand_layout(tuple(B.shape), B.stride())
+    if A.dtype == torch.float32:
+        cdt = torch.float32
+    elif A.dtype == torch.bfloat16:
+        cdt = out_dtype or (out.dtype if out is not None else torch.float32)
+        assert cdt in (torch.float32, torch.bfloat16)
+    elif A.dtype == torch.int8:
+        cdt = torch.int32
+    else:
+        raise TypeError(f"unsupported operand dtype {A.dtype}")
+    if A.dtype != torch.float32 and (alpha != 1.0 or beta != 0.0):
+        raise ValueError("bf16 and int8 GEMMs take alpha = 1, beta = 0 only")
+    if out is None:
+        assert beta == 0.0, "beta != 0 reads C: pass out"
+        out = torch.empty((m, n), dtype=cdt, device=A.device)
+    assert out.dtype == cdt and tuple(out.shape) == (m, n)
+    if n > 1:
+        assert out.stride(1) == 1, "out must be row-major"
+    st = _stream_ptr(stream)
+    if A.dtype == torch.float32:
+        _check(lib.b200_gemm_f32_op(op_a, op_b, m, n, k, alpha, A.data_ptr(), lda, B.data_ptr(), ldb, beta, out.data_ptr(),
+                                    _ld(out), mode, st))
+    elif A.dtype == torch.bfloat16:
+        _check(lib.b200_gemm_bf16_op(op_a, op_b, m, n, k, A.data_ptr(), lda, B.data_ptr(), ldb, out.data_ptr(), _ld(out),
+                                     OUT_F32 if cdt == torch.float32 else OUT_BF16, st))
+    else:
+        _check(lib.b200_gemm_s8s32_op(op_a, op_b, m, n, k, A.data_ptr(), lda, B.data_ptr(), ldb, out.data_ptr(), _ld(out), st))
+    return out
 
 
 def gemm_f32(A, B, out=None, mode=F32_AUTO, stream=None, accumulate=False):

@@ -27,12 +27,15 @@ template <> __device__ __forceinline__ void store_out<float, uint16_t>(uint16_t*
 }
 
 // 64x64 tile, 256 threads, 4x4 per thread, BK = 16.
+// Element strides per index: A(i, p) = A[i * a_rs + p * a_cs], B(p, j) = B[p * b_rs + j * b_cs].  Row-major A is
+// (lda, 1), a transposed one (A^T stored k x m, pitch lda) is (1, lda); likewise B.  The arithmetic does not
+// depend on the strides.
 // axpby (fp32 in / fp32 out only): C = alpha * (A*B) + beta * C (b200_gemm_f32_ex); the chains start from zero,
 // alpha * chain is rounded, then fma(beta, C, .), and C is read only when beta != 0.
 template <typename InT, typename OutT>
 __global__ void __launch_bounds__(256)
-gemm_generic_kernel(int M, int N, int K, const InT* __restrict__ A, long long lda,
-                    const InT* __restrict__ B, long long ldb, OutT* __restrict__ C, long long ldc,
+gemm_generic_kernel(int M, int N, int K, const InT* __restrict__ A, long long a_rs, long long a_cs,
+                    const InT* __restrict__ B, long long b_rs, long long b_cs, OutT* __restrict__ C, long long ldc,
                     int accumulate, const float* __restrict__ rq_scale = nullptr,
                     const float* __restrict__ rq_bias = nullptr, int axpby = 0, float alpha = 1.f, float beta = 0.f) {
   using Acc = typename LoadAs<InT>::Acc;
@@ -63,10 +66,10 @@ gemm_generic_kernel(int M, int N, int K, const InT* __restrict__ A, long long ld
       const int idx = threadIdx.x + r * 256;          // 0..1023
       const int am = idx >> 4, ak = idx & 15;          // A tile 64 x 16, k fastest
       const int gm = m0 + am, gk = k0 + ak;
-      As[ak][am] = (gm < M && gk < K) ? LoadAs<InT>::ld(A + (long long)gm * lda + gk) : (Acc)0;
+      As[ak][am] = (gm < M && gk < K) ? LoadAs<InT>::ld(A + (long long)gm * a_rs + (long long)gk * a_cs) : (Acc)0;
       const int bk = idx >> 6, bn = idx & 63;          // B tile 16 x 64, n fastest
       const int gk2 = k0 + bk, gn = n0 + bn;
-      Bs[bk][bn] = (gk2 < K && gn < N) ? LoadAs<InT>::ld(B + (long long)gk2 * ldb + gn) : (Acc)0;
+      Bs[bk][bn] = (gk2 < K && gn < N) ? LoadAs<InT>::ld(B + (long long)gk2 * b_rs + (long long)gn * b_cs) : (Acc)0;
     }
     __syncthreads();
 #pragma unroll

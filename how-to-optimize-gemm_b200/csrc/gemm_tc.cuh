@@ -1,6 +1,6 @@
 // gemm_tc.cuh — the tensor-core path: persistent, warp-specialised wgmma GEMM for sm_90a.
 //
-//   C[m x n] = A[m x k] * B[k x n],  all row-major.
+//   C[m x n] = op(A) * op(B),  C row-major; each operand stored row-major as given (N) or as its transpose (T).
 //
 // Mapping of the reference's roles (SURVEY §8a) onto Hopper:
 //   packA / packB  (aarch64/MMult_4x4_21.cpp:459-572; the gmem->smem staging of
@@ -11,10 +11,14 @@
 //                                                          wgmma 64 x BN x K into register accumulators
 //   stg128 epilogue (cuda/MMult_cuda_12.cu:210-222)     -> stores straight from the accumulator registers
 //
-// 16-bit operands: row-major B is the MMA's "MN-major" operand; TMA drops [BK x 128B] column blocks of B
-// into the canonical MN-major swizzled layout and wgmma transposes it on the fly (no transpose pass).
-// tf32 and int8: wgmma takes only K-major B for 32- and 8-bit types, so the caller passes B^T (n x k),
-// produced by transpose_kernel (the job of reorder_b / trans_w in aarch64-int8/MMult_4x8_21.c:45-71).
+// Operand layouts in shared memory (template parameters AL / BL of the kernel, LAYOUT_K or LAYOUT_MN):
+//   K-major:  rows of one operand's M (or N) index, BK elements of K per 128- or 64-byte swizzled row.  Row-major
+//             A (m x k) and B^T (n x k) are K-major as stored.
+//   MN-major: [BK k-rows x 128 B] column blocks of a k x m or k x n row-major matrix, SWIZZLE_128B, 8 k-rows per
+//             1 KB atom; wgmma transposes them on the fly.  Row-major B (k x n) and A^T (k x m) are MN-major as
+//             stored.  16-bit kinds only: the tile of A^T is the tile of row-major B, one 64-column box per consumer.
+// tf32 and int8: wgmma takes only K-major operands for 32- and 8-bit types, so a row-major B or a transposed A
+// is first transposed by transpose_kernel (the job of reorder_b / trans_w in aarch64-int8/MMult_4x8_21.c:45-71).
 //
 // Split-precision fp32 (B200_F32_BF16X3 / _BF16X2 / _F16X2): A and B arrive as NPA / NPB stacked 16-bit
 // "planes" (a = a1 + a2 + a3, produced by split_planes_kernel); each k-block stage holds every plane once
@@ -34,13 +38,15 @@
 
 namespace b200 {
 
+enum Layout { LAYOUT_K = 0, LAYOUT_MN = 1 };   // shared-memory layout of one operand (see above)
+
 template <int KIND> struct KindTraits;
-// B_KMAJOR: B is staged as B^T (n x k rows of 128 B, SWIZZLE_128B), else as 128-byte column blocks of
-// row-major B (MN-major, SWIZZLE_128B, 8 k-rows per 1 KB atom).
-template <> struct KindTraits<KIND_F16>  { static constexpr int ELEM = 2; static constexpr bool B_KMAJOR = false; };
-template <> struct KindTraits<KIND_FP16> { static constexpr int ELEM = 2; static constexpr bool B_KMAJOR = false; };
-template <> struct KindTraits<KIND_TF32> { static constexpr int ELEM = 4; static constexpr bool B_KMAJOR = true; };
-template <> struct KindTraits<KIND_I8>   { static constexpr int ELEM = 1; static constexpr bool B_KMAJOR = true; };
+// B_LAYOUT: the layout of B for a row-major B, the default of the kernel's BL parameter (16-bit kinds: MN-major
+// as stored; tf32 / int8: K-major, i.e. B^T).
+template <> struct KindTraits<KIND_F16>  { static constexpr int ELEM = 2; static constexpr int B_LAYOUT = LAYOUT_MN; };
+template <> struct KindTraits<KIND_FP16> { static constexpr int ELEM = 2; static constexpr int B_LAYOUT = LAYOUT_MN; };
+template <> struct KindTraits<KIND_TF32> { static constexpr int ELEM = 4; static constexpr int B_LAYOUT = LAYOUT_K; };
+template <> struct KindTraits<KIND_I8>   { static constexpr int ELEM = 1; static constexpr int B_LAYOUT = LAYOUT_K; };
 
 // Plane products issued per k-step.  Single: plain GEMM.  X3: a=a1+a2+a3, b likewise, all terms down
 // to 2^-16 relative (a1b3, a3b1, a2b2, a1b2, a2b1, a1b1) — dropped terms are <= 2^-24.  X2: two planes,
@@ -92,9 +98,13 @@ struct TcParams {
 // REGACC (split-precision fp32 modes): the tensor core adds into its fp32 accumulator with truncation,
 // so a long K chain drifts (error grows ~K).  K is cut into chunks of chunk_kb k-blocks; each chunk starts a
 // fresh wgmma accumulator that is added, with a rounded fp32 add, to the tile's running sum in registers.
-template <int KIND, int BN, int STAGES, class Prod, int A_ROW_BYTES>
+// AL / BL: layouts of A and B.  K-major A and MN-major B tiles are staged exactly as before this choice existed;
+// an MN-major A tile is staged like an MN-major B tile (BM / 64 boxes of [BK rows x 128 B]) and a K-major B tile
+// like a K-major A tile (BN rows of A_ROW_BYTES, SWIZZLE_128B or _64B), so byte counts are the same either way.
+template <int KIND, int BN, int STAGES, class Prod, int A_ROW_BYTES, int AL = LAYOUT_K, int BL = KindTraits<KIND>::B_LAYOUT>
 struct TcConfig {
   using T = KindTraits<KIND>;
+  static constexpr bool A_MN = AL == LAYOUT_MN, B_MN = BL == LAYOUT_MN;
   static constexpr bool REGACC = Prod::N > 1;
   static constexpr int BM = 128;
   static constexpr int TILE_M = BM;                         // rows of C per work unit
@@ -103,27 +113,36 @@ struct TcConfig {
   static constexpr int BK = A_ROW_BYTES / T::ELEM;          // one swizzled row of K per stage
   static constexpr int A_PLANE = BM * A_ROW_BYTES;          // 16 KB (SW128) or 8 KB (SW64)
   static constexpr int A_SWZ = A_ROW_BYTES == 128 ? SWZ_128B : SWZ_64B;
-  static constexpr int A_SBO = 8 * A_ROW_BYTES;             // 8-row core-matrix group stride
-  static constexpr int A_WG = 64 * A_ROW_BYTES;             // offset of the second consumer's rows
-  static constexpr int B_BOX_COLS = T::B_KMAJOR ? BN : 128 / T::ELEM;   // B columns per TMA box
-  static constexpr int B_BOX_ROWS = T::B_KMAJOR ? BN : BK;
+  static constexpr int A_SBO = 8 * A_ROW_BYTES;             // K-major: 8-row core-matrix group stride
+  static constexpr int MN_BOX_COLS = 128 / T::ELEM;         // MN-major: columns per 128-byte TMA box
+  static constexpr int MN_BOX_BYTES = BK * 128;             // MN-major: one [BK rows x 128 B] box
+  static constexpr int A_BOXES = A_MN ? BM / MN_BOX_COLS : 1;                // TMA boxes per A plane
+  static constexpr int A_WG = A_MN ? MN_BOX_BYTES : 64 * A_ROW_BYTES;      // offset of the second consumer's rows
+  static constexpr int B_BOX_COLS = B_MN ? MN_BOX_COLS : BN;               // B columns per TMA box
+  static constexpr int B_BOX_ROWS = B_MN ? BK : BN;
   static constexpr int B_BOXES = BN / B_BOX_COLS;
-  static constexpr int B_BOX_BYTES = T::B_KMAJOR ? BN * 128 : BK * 128;
+  static constexpr int B_BOX_BYTES = B_MN ? MN_BOX_BYTES : BN * A_ROW_BYTES;
   static constexpr int B_PLANE = B_BOXES * B_BOX_BYTES;
   static constexpr int A_STAGE = Prod::NPA * A_PLANE;
   static constexpr int B_STAGE = Prod::NPB * B_PLANE;
   static constexpr int STAGE_BYTES = A_STAGE + B_STAGE;
-  static constexpr int MMA_K = Wgmma<KIND, BN>::K;
+  using MMA = Wgmma<KIND, BN, A_MN ? 1 : 0, B_MN ? 1 : 0>;
+  static constexpr int MMA_K = MMA::K;
   static constexpr int MMAS_PER_STAGE = BK / MMA_K;
-  static constexpr int A_KADV = MMA_K * T::ELEM;            // bytes inside the swizzled row
-  static constexpr int B_KADV = T::B_KMAJOR ? MMA_K * T::ELEM : MMA_K * 128;   // K-major: bytes in the row; MN-major: k-rows of 128 B
+  // k advance per MMA: K-major: bytes inside the swizzled row; MN-major: k-rows of 128 B
+  static constexpr int A_KADV = A_MN ? MMA_K * 128 : MMA_K * T::ELEM;
+  static constexpr int B_KADV = B_MN ? MMA_K * 128 : MMA_K * T::ELEM;
   static constexpr int ACC = BN / 2;                        // accumulator registers per consumer thread
   static constexpr int SMEM_BYTES = 1024 /*align slack*/ + STAGES * STAGE_BYTES + 2 * STAGES * 8;
   static constexpr int THREADS = 128 * (1 + CONSUMERS);
   static_assert(SMEM_BYTES <= 232448, "exceeds the 227 KB dynamic shared memory of sm_90");
   static_assert(!REGACC || BN <= 128, "register accumulation keeps two 64 x BN fp32 tiles per consumer in registers");
-  static_assert(!T::B_KMAJOR || (Prod::NPB == 1 && A_ROW_BYTES == 128), "K-major B: single plane, 128-byte rows");
-  static_assert(BN % 64 == 0 || T::B_KMAJOR, "MN-major B is staged in 64-column blocks");
+  static_assert(T::ELEM == 2 || (!A_MN && !B_MN && Prod::NPA == 1 && Prod::NPB == 1 && A_ROW_BYTES == 128),
+                "tf32 / int8: K-major A and B, single plane, 128-byte rows");
+  static_assert(!B_MN || BN % MN_BOX_COLS == 0, "MN-major B is staged in 128-byte column blocks");
+  static_assert(!A_MN || (A_BOXES == CONSUMERS && A_BOXES * MN_BOX_BYTES == A_PLANE),
+                "MN-major A: one 64-column box per consumer warpgroup, the bytes of a K-major A plane");
+  static_assert(B_PLANE == BN * A_ROW_BYTES, "a B plane holds BN x BK elements in either layout");
 };
 
 __device__ __forceinline__ void tile_coords(int t, int tiles_m, int tiles_n, int group_m, int& mb,
@@ -257,13 +276,13 @@ __device__ __forceinline__ void store_pair(const TcParams& p, int row, int col, 
   }
 }
 
-template <int KIND, int BN, int STAGES, typename OutT, class Prod, int A_ROW_BYTES>
-__global__ void __launch_bounds__((TcConfig<KIND, BN, STAGES, Prod, A_ROW_BYTES>::THREADS), 1)
+template <int KIND, int BN, int STAGES, typename OutT, class Prod, int A_ROW_BYTES, int AL = LAYOUT_K,
+          int BL = KindTraits<KIND>::B_LAYOUT>
+__global__ void __launch_bounds__((TcConfig<KIND, BN, STAGES, Prod, A_ROW_BYTES, AL, BL>::THREADS), 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                const TcParams p) {
-  using Cfg = TcConfig<KIND, BN, STAGES, Prod, A_ROW_BYTES>;
-  using T = KindTraits<KIND>;
-  using MMA = Wgmma<KIND, BN>;
+  using Cfg = TcConfig<KIND, BN, STAGES, Prod, A_ROW_BYTES, AL, BL>;
+  using MMA = typename Cfg::MMA;
   using Acc = typename MMA::Acc;
 
   extern __shared__ uint8_t smem_raw[];
@@ -309,11 +328,26 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           mbar_wait(bar_empty + 8 * s, ph ^ 1);
           const uint32_t full = bar_full + 8 * s;
           mbar_arrive_expect_tx(full, Cfg::STAGE_BYTES);
+          if constexpr (Cfg::A_MN) {                  // A^T (k x m): one 64-column box per consumer
 #pragma unroll
-          for (int pa = 0; pa < Prod::NPA; pa++)
-            tma_load_2d(sA + s * Cfg::A_STAGE + pa * Cfg::A_PLANE, &tmA, full, kb * Cfg::BK, pa * p.a_plane_rows + m0);
-          if constexpr (T::B_KMAJOR) {
-            tma_load_2d(sB + s * Cfg::B_STAGE, &tmB, full, kb * Cfg::BK, n0);
+            for (int pa = 0; pa < Prod::NPA; pa++)
+#pragma unroll
+              for (int j = 0; j < Cfg::A_BOXES; j++)
+                tma_load_2d(sA + s * Cfg::A_STAGE + pa * Cfg::A_PLANE + j * Cfg::MN_BOX_BYTES, &tmA, full,
+                            m0 + j * Cfg::MN_BOX_COLS, pa * p.a_plane_rows + kb * Cfg::BK);
+          } else {
+#pragma unroll
+            for (int pa = 0; pa < Prod::NPA; pa++)
+              tma_load_2d(sA + s * Cfg::A_STAGE + pa * Cfg::A_PLANE, &tmA, full, kb * Cfg::BK, pa * p.a_plane_rows + m0);
+          }
+          if constexpr (!Cfg::B_MN) {                 // B^T (n x k): one box of BN rows per plane
+            if constexpr (Prod::NPB == 1) {
+              tma_load_2d(sB + s * Cfg::B_STAGE, &tmB, full, kb * Cfg::BK, n0);
+            } else {
+#pragma unroll
+              for (int pb = 0; pb < Prod::NPB; pb++)
+                tma_load_2d(sB + s * Cfg::B_STAGE + pb * Cfg::B_PLANE, &tmB, full, kb * Cfg::BK, pb * p.b_plane_rows + n0);
+            }
           } else {
 #pragma unroll
             for (int pb = 0; pb < Prod::NPB; pb++)
@@ -356,10 +390,18 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           for (int pr = 0; pr < Prod::N; pr++) {
 #pragma unroll
             for (int k = 0; k < Cfg::MMAS_PER_STAGE; k++) {
-              const uint64_t ad = make_sdesc(a0 + Prod::ia(pr) * Cfg::A_PLANE + k * Cfg::A_KADV, 16, Cfg::A_SBO, Cfg::A_SWZ);
-              const uint64_t bd = T::B_KMAJOR
-                                      ? make_sdesc(b0 + k * Cfg::B_KADV, 16, 1024, SWZ_128B)
-                                      : make_sdesc(b0 + Prod::ib(pr) * Cfg::B_PLANE + k * Cfg::B_KADV, b_lbo, b_sbo, SWZ_128B);
+              // K-major: SBO = 8-row group stride, LBO unused; MN-major: LBO = column-block stride, SBO = 8 k-rows
+              uint64_t ad, bd;
+              if constexpr (Cfg::A_MN)
+                ad = make_sdesc(a0 + Prod::ia(pr) * Cfg::A_PLANE + k * Cfg::A_KADV, Cfg::MN_BOX_BYTES, 1024, SWZ_128B);
+              else
+                ad = make_sdesc(a0 + Prod::ia(pr) * Cfg::A_PLANE + k * Cfg::A_KADV, 16, Cfg::A_SBO, Cfg::A_SWZ);
+              if constexpr (Cfg::B_MN)
+                bd = make_sdesc(b0 + Prod::ib(pr) * Cfg::B_PLANE + k * Cfg::B_KADV, b_lbo, b_sbo, SWZ_128B);
+              else if constexpr (Prod::NPB == 1)
+                bd = make_sdesc(b0 + k * Cfg::B_KADV, 16, Cfg::A_SBO, Cfg::A_SWZ);
+              else
+                bd = make_sdesc(b0 + Prod::ib(pr) * Cfg::B_PLANE + k * Cfg::B_KADV, 16, Cfg::A_SBO, Cfg::A_SWZ);
               MMA::mma(acc, ad, bd, ((kb - c0) | k | pr) != 0 ? 1u : 0u);
             }
           }

@@ -174,6 +174,53 @@ int b200_gemm_s8s32_host(int m, int n, int k,
                          const int8_t* A, int lda, const int8_t* B, int ldb,
                          int32_t* C, int ldc);
 
+/* ---- transposed operands (cuBLAS transa / transb; chgemm's trans / trans_w, aarch64-int8/MMult_4x8_21.c:45-71) ----
+ * C = alpha * op(A) * op(B) + beta * C, C row-major m x n (ldc >= n), each operand stored row-major either as is or
+ * transposed:
+ *   op_a = B200_OP_N: A is m x k, lda >= k;   B200_OP_T: A is stored as A^T, k x m, lda >= m
+ *   op_b = B200_OP_N: B is k x n, ldb >= n;   B200_OP_T: B is stored as B^T, n x k, ldb >= k
+ * (a PyTorch caller's x @ W.t() with W of shape n x k is op_b = B200_OP_T, ldb = W.stride(0)).  An op other than 0 or 1
+ * is B200_ERR_BAD_ARG.  (N, N) is b200_gemm_f32_ex / b200_gemm_bf16 / b200_gemm_s8s32 exactly: same kernels, kernel
+ * names, launches and bits.  The (alpha, beta) rules of b200_gemm_f32_ex hold for every layout; AUTO picks its route
+ * from m, n, k and the TMA-ability of the operands as stored, as for NN.  DEVICE pointers, asynchronous on `stream`.
+ *
+ * No operand is copied to row-major first where the tensor cores can read it as stored: wgmma reads 16-bit operands
+ * K-major or MN-major, so A^T is staged as MN-major A and B^T as K-major B.  tf32 and int8 read only K-major
+ * operands, so B^T is read in place and a transposed A (or, as for NN, a row-major B) goes through transpose_kernel
+ * into the workspace.  Kernel launches per call (TMA-able operands):
+ *
+ *   path                    NN   NT (B^T given)   TN (A^T given)   TT
+ *   bf16 -> fp32 / bf16      1   1                1                1     operands read in place
+ *   TF32, int8               2   1                3                2     transposes into the workspace
+ *   BF16X3, BF16X2           2   2                2                2     one split launch for both operands
+ *   F16X2                    4   3                5                4     B^T's column maxima are its row maxima (the
+ *                                                                        row pre-pass); A^T's row maxima are column
+ *                                                                        maxima (column maxima + column split)
+ *   STRICT                   1   2                2                3     A^T / B^T transposed into the workspace,
+ *                                                                        then the unchanged FFMA kernel
+ *   not TMA-able (generic)   1   1                1                1
+ *
+ * Every transposed result is bit-identical to the NN call on row-major copies of the operands: the planes, maxima and
+ * transposes hold the same values and the MMAs take the same K order.  A new wgmma kernel is named with the layout
+ * after the kind ("tc_bf16_nt_128x256", "tc_f16x2_tn_128x128"); a route that runs an NN kernel keeps its name.
+ * Workspace: b200_gemm_workspace_bytes_op gives what the fp32 route uses (transposes and plane padding included; for
+ * AUTO the largest of the routes AUTO may take at this size), equal to b200_gemm_workspace_bytes for (N, N).  bf16
+ * uses none; int8 uses n * k16 bytes for a row-major B and m * k16 (at a 1 KB-aligned offset after B's) for a
+ * transposed A, k16 = k rounded up to 16.  The packed handles, the row-panel plan, the requantising int8 GEMM and the
+ * host-pointer entry points take row-major operands only. */
+#define B200_OP_N 0   /* operand stored as is: op(A) = A (m x k, lda >= k); op(B) = B (k x n, ldb >= n)      */
+#define B200_OP_T 1   /* operand stored transposed: A as k x m (lda >= m); B as n x k (ldb >= k), row-major */
+int b200_gemm_f32_op(int op_a, int op_b, int m, int n, int k, float alpha,
+                     const float* dA, int lda, const float* dB, int ldb, float beta,
+                     float* dC, int ldc, int precision_mode, void* stream);
+int b200_gemm_bf16_op(int op_a, int op_b, int m, int n, int k,
+                      const uint16_t* dA, int lda, const uint16_t* dB, int ldb,
+                      void* dC, int ldc, int out_type, void* stream);
+int b200_gemm_s8s32_op(int op_a, int op_b, int m, int n, int k,
+                       const int8_t* dA, int lda, const int8_t* dB, int ldb,
+                       int32_t* dC, int ldc, void* stream);
+size_t b200_gemm_workspace_bytes_op(int op_a, int op_b, int m, int n, int k, int precision_mode);
+
 /* Pre-split operands for the split-precision modes (AUTO = the library default): the reference
  * leaves its "packAB interface open" for callers that reuse one operand (README.md:85; PackMatrixA/B,
  * aarch64/MMult_4x4_13.cpp:259,361).  TMA needs no repacking of row-major operands, but the fp32 ->
