@@ -17,16 +17,17 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libb200gemm.so")
 
 F32_STRICT, F32_TF32, F32_BF16X3, F32_BF16X2, F32_AUTO, F32_F16X2 = 0, 1, 2, 3, 4, 5
-OUT_F32, OUT_BF16 = 0, 1
+OUT_F32, OUT_BF16, OUT_F16 = 0, 1, 2
 OP_N, OP_T = 0, 1
 
 EXPORTS = [
     "b200_gemm_version", "b200_gemm_device_ok", "b200_gemm_strerror", "b200_gemm_last_kernel",
     "b200_gemm_launch_count", "b200_gemm_default_f32_mode", "b200_gemm_set_default_f32_mode",
     "b200_gemm_f32", "b200_gemm_f32_acc", "b200_gemm_f32_ex", "b200_gemm_workspace_bytes", "b200_gemm_reserve_workspace", "b200_mxf4_q_bytes", "b200_mxf4_sf_bytes",
-    "b200_mxf4_quantize_a", "b200_mxf4_quantize_b", "b200_gemm_mxf4", "b200_gemm_f32_host", "b200_gemm_bf16", "b200_gemm_s8s32",
+    "b200_mxf4_quantize_a", "b200_mxf4_quantize_b", "b200_gemm_mxf4", "b200_gemm_f32_host", "b200_gemm_bf16", "b200_gemm_f16", "b200_gemm_s8s32",
     "b200_gemm_s8s32_host", "b200_gemm_s8s8_requant", "b200_gemm_f32_pack_b", "b200_gemm_f32_packed",
-    "b200_gemm_f32_pack_free", "b200_gemm_f32_op", "b200_gemm_bf16_op", "b200_gemm_s8s32_op", "b200_gemm_workspace_bytes_op",
+    "b200_gemm_f32_pack_free", "b200_gemm_f32_op", "b200_gemm_bf16_op", "b200_gemm_bf16_ex", "b200_gemm_f16_ex",
+    "b200_gemm_s8s32_op", "b200_gemm_workspace_bytes_op",
     "b200_nccl_load", "b200_nccl_last_error", "b200_comm_unique_id", "b200_comm_init_rank",
     "b200_comm_destroy", "b200_rowpanel_create", "b200_rowpanel_destroy", "b200_rowpanel_slices", "b200_rowpanel_set_reserve_sms", "b200_rowpanel_trace", "b200_rowpanel_trace_dump", "b200_gemm_f32_rowpanel",
     "b200_gemm_f32_rowpanel_host", "b200_gemm_f32_pack_a", "b200_gemm_f32_packed_ab", "b200_gemm_f32_pack_free_a",
@@ -70,10 +71,13 @@ lib.b200_mxf4_quantize_b.argtypes = [_i, _i, _vp, _i, _vp, _vp, _vp]
 lib.b200_gemm_mxf4.argtypes = [_i, _i, _i, _vp, _vp, _vp, _vp, _vp, _i, _vp]
 lib.b200_gemm_f32_host.argtypes = [_i, _i, _i, _vp, _i, _vp, _i, _vp, _i, _i]
 lib.b200_gemm_bf16.argtypes = [_i, _i, _i, _vp, _i, _vp, _i, _vp, _i, _i, _vp]
+lib.b200_gemm_f16.argtypes = [_i, _i, _i, _vp, _i, _vp, _i, _vp, _i, _i, _vp]
 lib.b200_gemm_s8s32.argtypes = [_i, _i, _i, _vp, _i, _vp, _i, _vp, _i, _vp]
 lib.b200_gemm_s8s32_host.argtypes = [_i, _i, _i, _vp, _i, _vp, _i, _vp, _i]
 lib.b200_gemm_f32_op.argtypes = [_i, _i, _i, _i, _i, C.c_float, _vp, _i, _vp, _i, C.c_float, _vp, _i, _i, _vp]
 lib.b200_gemm_bf16_op.argtypes = [_i, _i, _i, _i, _i, _vp, _i, _vp, _i, _vp, _i, _i, _vp]
+lib.b200_gemm_bf16_ex.argtypes = [_i, _i, _i, _i, _i, C.c_float, _vp, _i, _vp, _i, C.c_float, _vp, _i, _i, _vp]
+lib.b200_gemm_f16_ex.argtypes = [_i, _i, _i, _i, _i, C.c_float, _vp, _i, _vp, _i, C.c_float, _vp, _i, _i, _vp]
 lib.b200_gemm_s8s32_op.argtypes = [_i, _i, _i, _i, _i, _vp, _i, _vp, _i, _vp, _i, _vp]
 lib.b200_gemm_workspace_bytes_op.argtypes = [_i, _i, _i, _i, _i, _i]
 lib.b200_gemm_workspace_bytes_op.restype = C.c_size_t
@@ -193,12 +197,14 @@ def operand_layout(shape, strides):
 
 
 def gemm(A, B, out=None, *, alpha=1.0, beta=0.0, mode=F32_AUTO, out_dtype=None, stream=None):
-    """C = alpha * A @ B + beta * C for fp32 (any precision mode), bf16 (fp32 or bf16 C) and int8 (int32 C) CUDA
-    tensors.  Each operand may be row-major or the transpose of a row-major matrix (x @ W.t() passes W as stored):
-    it is read in place (b200_gemm_f32_op / _bf16_op / _s8s32_op), never copied.  out must be row-major; it is
-    read only when beta != 0.  bf16 and int8 take alpha = 1, beta = 0 only."""
+    """C = alpha * A @ B + beta * C for fp32 (any precision mode), bf16 (fp32 or bf16 C), fp16 (fp32 or fp16 C) and
+    int8 (int32 C) CUDA tensors.  Each operand may be row-major or the transpose of a row-major matrix (x @ W.t()
+    passes W as stored): it is read in place (b200_gemm_f32_op / _bf16_op / _bf16_ex / _f16_ex / _s8s32_op), never
+    copied.  out must be row-major; it is read only when beta != 0.  int8 takes alpha = 1, beta = 0 only."""
     import torch
-    assert A.dim() == 2 and B.dim() == 2 and A.is_cuda and B.is_cuda and A.dtype == B.dtype
+    assert A.dim() == 2 and B.dim() == 2 and A.is_cuda and B.is_cuda
+    if A.dtype != B.dtype:
+        raise TypeError(f"operands of different dtypes: {A.dtype} and {B.dtype}")
     m, k = A.shape
     k2, n = B.shape
     assert k == k2, (A.shape, B.shape)
@@ -206,15 +212,15 @@ def gemm(A, B, out=None, *, alpha=1.0, beta=0.0, mode=F32_AUTO, out_dtype=None, 
     op_b, ldb = operand_layout(tuple(B.shape), B.stride())
     if A.dtype == torch.float32:
         cdt = torch.float32
-    elif A.dtype == torch.bfloat16:
+    elif A.dtype in (torch.bfloat16, torch.float16):
         cdt = out_dtype or (out.dtype if out is not None else torch.float32)
-        assert cdt in (torch.float32, torch.bfloat16)
+        assert cdt in (torch.float32, A.dtype), f"{A.dtype} operands write float32 or {A.dtype} C, not {cdt}"
     elif A.dtype == torch.int8:
         cdt = torch.int32
     else:
         raise TypeError(f"unsupported operand dtype {A.dtype}")
-    if A.dtype != torch.float32 and (alpha != 1.0 or beta != 0.0):
-        raise ValueError("bf16 and int8 GEMMs take alpha = 1, beta = 0 only")
+    if A.dtype == torch.int8 and (alpha != 1.0 or beta != 0.0):
+        raise ValueError("the int8 GEMM takes alpha = 1, beta = 0 only")
     if out is None:
         assert beta == 0.0, "beta != 0 reads C: pass out"
         out = torch.empty((m, n), dtype=cdt, device=A.device)
@@ -225,9 +231,13 @@ def gemm(A, B, out=None, *, alpha=1.0, beta=0.0, mode=F32_AUTO, out_dtype=None, 
     if A.dtype == torch.float32:
         _check(lib.b200_gemm_f32_op(op_a, op_b, m, n, k, alpha, A.data_ptr(), lda, B.data_ptr(), ldb, beta, out.data_ptr(),
                                     _ld(out), mode, st))
-    elif A.dtype == torch.bfloat16:
+    elif A.dtype == torch.bfloat16 and alpha == 1.0 and beta == 0.0:
         _check(lib.b200_gemm_bf16_op(op_a, op_b, m, n, k, A.data_ptr(), lda, B.data_ptr(), ldb, out.data_ptr(), _ld(out),
                                      OUT_F32 if cdt == torch.float32 else OUT_BF16, st))
+    elif A.dtype in (torch.bfloat16, torch.float16):
+        fn, ot = (lib.b200_gemm_bf16_ex, OUT_BF16) if A.dtype == torch.bfloat16 else (lib.b200_gemm_f16_ex, OUT_F16)
+        _check(fn(op_a, op_b, m, n, k, alpha, A.data_ptr(), lda, B.data_ptr(), ldb, beta, out.data_ptr(), _ld(out),
+                  OUT_F32 if cdt == torch.float32 else ot, st))
     else:
         _check(lib.b200_gemm_s8s32_op(op_a, op_b, m, n, k, A.data_ptr(), lda, B.data_ptr(), ldb, out.data_ptr(), _ld(out), st))
     return out

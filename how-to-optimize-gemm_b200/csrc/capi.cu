@@ -402,52 +402,40 @@ int pick_bn(int m, int n, bool allow256, bool allow192 = true) {
   return best;
 }
 
-#define TC_PLAIN(KIND, OUT, NAME)                                                                     \
-  switch (pick_bn(m, n, true)) {                                                                      \
-    case 256: return launch_tc<KIND, 256, 4, OUT>(m, n, k, A, lda, m, 0, B, ldb, k, 0, C, ldc, st, NAME "_128x256"); \
-    case 192: return launch_tc<KIND, 192, 5, OUT>(m, n, k, A, lda, m, 0, B, ldb, k, 0, C, ldc, st, NAME "_128x192"); \
-    default:  return launch_tc<KIND, 128, 6, OUT>(m, n, k, A, lda, m, 0, B, ldb, k, 0, C, ldc, st, NAME "_128x128"); \
-  }
-
-int tc_bf16_f32(int m, int n, int k, const void* A, int lda, const void* B, int ldb, void* C, int ldc, cudaStream_t st) {
-  TC_PLAIN(KIND_F16, float, "tc_bf16")
-}
-int tc_bf16_bf16(int m, int n, int k, const void* A, int lda, const void* B, int ldb, void* C, int ldc, cudaStream_t st) {
-  TC_PLAIN(KIND_F16, bf16_out, "tc_bf16_obf16")
-}
-
 // Layout index of a transposed-operand call: 0 = NT (B given as B^T), 1 = TN (A given as A^T), 2 = TT; NN has none.
 inline int op_index(int op_a, int op_b) { return op_a ? (op_b ? 2 : 1) : 0; }
 constexpr int kLayoutA[3] = {LAYOUT_K, LAYOUT_MN, LAYOUT_MN}, kLayoutB[3] = {LAYOUT_K, LAYOUT_MN, LAYOUT_K};
 
-// bf16 with at least one transposed operand, read in place: A^T is the MN-major A, B^T the K-major B.  names: the
-// three tile widths 256 / 192 / 128.
-template <typename OutT, int AL, int BL>
-int tc_bf16_layout(int m, int n, int k, const void* A, int lda, const void* B, int ldb, void* C, int ldc, cudaStream_t st,
-                   const char* const (&names)[3]) {
+// The plain 16-bit GEMM (KIND_F16 = bf16, KIND_FP16 = fp16; OutT float, bf16_out or f16_out) in one layout, read in
+// place: A^T is the MN-major A, B^T the K-major B.  names: the three tile widths 256 / 192 / 128.
+template <int KIND, typename OutT, int AL, int BL>
+int tc16_layout(int m, int n, int k, const void* A, int lda, const void* B, int ldb, void* C, int ldc, cudaStream_t st,
+                const char* const (&names)[3]) {
   const int ar = AL == LAYOUT_MN ? k : m, br = BL == LAYOUT_MN ? k : n;      // rows of the operands as stored
   switch (pick_bn(m, n, true)) {
-    case 256: return launch_tc<KIND_F16, 256, 4, OutT, ProdSingle, 128, AL, BL>(m, n, k, A, lda, ar, 0, B, ldb, br, 0, C, ldc, st, names[0]);
-    case 192: return launch_tc<KIND_F16, 192, 5, OutT, ProdSingle, 128, AL, BL>(m, n, k, A, lda, ar, 0, B, ldb, br, 0, C, ldc, st, names[1]);
-    default:  return launch_tc<KIND_F16, 128, 6, OutT, ProdSingle, 128, AL, BL>(m, n, k, A, lda, ar, 0, B, ldb, br, 0, C, ldc, st, names[2]);
+    case 256: return launch_tc<KIND, 256, 4, OutT, ProdSingle, 128, AL, BL>(m, n, k, A, lda, ar, 0, B, ldb, br, 0, C, ldc, st, names[0]);
+    case 192: return launch_tc<KIND, 192, 5, OutT, ProdSingle, 128, AL, BL>(m, n, k, A, lda, ar, 0, B, ldb, br, 0, C, ldc, st, names[1]);
+    default:  return launch_tc<KIND, 128, 6, OutT, ProdSingle, 128, AL, BL>(m, n, k, A, lda, ar, 0, B, ldb, br, 0, C, ldc, st, names[2]);
   }
 }
-template <typename OutT>
-int tc_bf16_op(int op_a, int op_b, int m, int n, int k, const void* A, int lda, const void* B, int ldb, void* C, int ldc,
-               cudaStream_t st, const char* const (&names)[3][3]) {
+// names[layout][width]: layout 0 = NN, 1 = NT, 2 = TN, 3 = TT.
+template <int KIND, typename OutT>
+int tc16_op(int op_a, int op_b, int m, int n, int k, const void* A, int lda, const void* B, int ldb, void* C, int ldc,
+            cudaStream_t st, const char* const (&names)[4][3]) {
+  if (!op_a && !op_b) return tc16_layout<KIND, OutT, LAYOUT_K, LAYOUT_MN>(m, n, k, A, lda, B, ldb, C, ldc, st, names[0]);
   switch (op_index(op_a, op_b)) {
-    case 0: return tc_bf16_layout<OutT, kLayoutA[0], kLayoutB[0]>(m, n, k, A, lda, B, ldb, C, ldc, st, names[0]);
-    case 1: return tc_bf16_layout<OutT, kLayoutA[1], kLayoutB[1]>(m, n, k, A, lda, B, ldb, C, ldc, st, names[1]);
-    default: return tc_bf16_layout<OutT, kLayoutA[2], kLayoutB[2]>(m, n, k, A, lda, B, ldb, C, ldc, st, names[2]);
+    case 0: return tc16_layout<KIND, OutT, kLayoutA[0], kLayoutB[0]>(m, n, k, A, lda, B, ldb, C, ldc, st, names[1]);
+    case 1: return tc16_layout<KIND, OutT, kLayoutA[1], kLayoutB[1]>(m, n, k, A, lda, B, ldb, C, ldc, st, names[2]);
+    default: return tc16_layout<KIND, OutT, kLayoutA[2], kLayoutB[2]>(m, n, k, A, lda, B, ldb, C, ldc, st, names[3]);
   }
 }
-const char* const kNamesBf16[3][3] = {{"tc_bf16_nt_128x256", "tc_bf16_nt_128x192", "tc_bf16_nt_128x128"},
-                                      {"tc_bf16_tn_128x256", "tc_bf16_tn_128x192", "tc_bf16_tn_128x128"},
-                                      {"tc_bf16_tt_128x256", "tc_bf16_tt_128x192", "tc_bf16_tt_128x128"}};
-const char* const kNamesBf16Obf16[3][3] = {
-    {"tc_bf16_obf16_nt_128x256", "tc_bf16_obf16_nt_128x192", "tc_bf16_obf16_nt_128x128"},
-    {"tc_bf16_obf16_tn_128x256", "tc_bf16_obf16_tn_128x192", "tc_bf16_obf16_tn_128x128"},
-    {"tc_bf16_obf16_tt_128x256", "tc_bf16_obf16_tt_128x192", "tc_bf16_obf16_tt_128x128"}};
+#define TC16_NAMES(P)                                                                               \
+  {{P "_128x256", P "_128x192", P "_128x128"}, {P "_nt_128x256", P "_nt_128x192", P "_nt_128x128"}, \
+   {P "_tn_128x256", P "_tn_128x192", P "_tn_128x128"}, {P "_tt_128x256", P "_tt_128x192", P "_tt_128x128"}}
+const char* const kNamesBf16[4][3] = TC16_NAMES("tc_bf16");
+const char* const kNamesBf16Obf16[4][3] = TC16_NAMES("tc_bf16_obf16");
+const char* const kNamesF16[4][3] = TC16_NAMES("tc_f16");
+const char* const kNamesF16Of16[4][3] = TC16_NAMES("tc_f16_of16");
 
 // ---- split-precision fp32 on the tensor cores ---------------------------------------------------
 // Workspace for the bf16 planes: cached, grow-only (no per-call cudaMalloc in steady state).  Calls
@@ -1124,7 +1112,7 @@ int gemm_f32_ex_impl(int op_a, int op_b, int m, int n, int k, float alpha, const
   if (alpha == 0.f || k == 0) {           // C = beta * C: A and B are not read; beta == 0 does not read C either
     if (beta == 0.f) return launch_zero<float>(m, n, dC, ldc, st);
     const dim3 sg((n + 255) / 256, m < 4096 ? m : 4096);
-    scale_inplace_kernel<<<sg, 256, 0, st>>>(m, n, dC, ldc, beta);
+    scale_inplace_kernel<float><<<sg, 256, 0, st>>>(m, n, dC, ldc, beta);
     g_launches++;
     return last_launch_status();
   }
@@ -1135,6 +1123,77 @@ int gemm_f32_ex_impl(int op_a, int op_b, int m, int n, int k, float alpha, const
   // beta != 0): no pre-scaled C, so beta / alpha never has to be representable
   t_epi.axpby = 1; t_epi.alpha = alpha; t_epi.beta = beta;
   rc = gemm_f32_impl(m, n, k, dA, lda, dB, ldb, dC, ldc, mode, 0, st, op_a, op_b);
+  t_epi = EpiOpts();
+  return rc;
+}
+
+// 16-bit operands: KIND_F16 (bf16, C fp32 or bf16) and KIND_FP16 (fp16, C fp32 or fp16).  E is the generic kernel's
+// element type of the kind (uint16_t holds bf16 bits).
+template <int KIND> struct Kind16;
+template <> struct Kind16<KIND_F16> {
+  using E = uint16_t;
+  static constexpr int OUT16 = B200_OUT_BF16;
+  using Out16 = bf16_out;
+  static constexpr const char* kGeneric = "generic_bf16_64x64";
+  static constexpr const char* const (&names)[4][3] = kNamesBf16;
+  static constexpr const char* const (&names16)[4][3] = kNamesBf16Obf16;
+};
+template <> struct Kind16<KIND_FP16> {
+  using E = __half;
+  static constexpr int OUT16 = B200_OUT_F16;
+  using Out16 = f16_out;
+  static constexpr const char* kGeneric = "generic_f16_64x64";
+  static constexpr const char* const (&names)[4][3] = kNamesF16;
+  static constexpr const char* const (&names16)[4][3] = kNamesF16Of16;
+};
+
+// C = op(A) op(B) (the general epilogue when t_epi asks for it): every layout is read in place by one launch.
+template <int KIND>
+int gemm16_impl(int op_a, int op_b, int m, int n, int k, const uint16_t* dA, int lda, const uint16_t* dB, int ldb,
+                void* dC, int ldc, int out_type, cudaStream_t st) {
+  using K16 = Kind16<KIND>;
+  using E = typename K16::E;
+  if (out_type != B200_OUT_F32 && out_type != K16::OUT16) return B200_ERR_BAD_ARG;
+  int rc = check_args(m, n, k, dA, lda, dB, ldb, dC, ldc, op_a, op_b);
+  if (rc == 1) return 0;
+  if (rc) return rc;
+  rc = ensure_device();
+  if (rc) return rc;
+  const bool c32 = out_type == B200_OUT_F32;
+  if (k == 0) return c32 ? launch_zero<float>(m, n, (float*)dC, ldc, st) : launch_zero<uint16_t>(m, n, (uint16_t*)dC, ldc, st);
+  if (!tma_ok(dA, lda, dB, ldb, 2)) {
+    const E* a = reinterpret_cast<const E*>(dA);
+    const E* b = reinterpret_cast<const E*>(dB);
+    if (c32) return launch_generic<E, float>(m, n, k, a, lda, b, ldb, (float*)dC, ldc, 0, st, K16::kGeneric, op_a, op_b);
+    return launch_generic<E, E>(m, n, k, a, lda, b, ldb, (E*)dC, ldc, 0, st, K16::kGeneric, op_a, op_b);
+  }
+  if (c32) return tc16_op<KIND, float>(op_a, op_b, m, n, k, dA, lda, dB, ldb, dC, ldc, st, K16::names);
+  return tc16_op<KIND, typename K16::Out16>(op_a, op_b, m, n, k, dA, lda, dB, ldb, dC, ldc, st, K16::names16);
+}
+
+// C = alpha op(A) op(B) + beta C with the rules of b200_gemm_f32_ex; (1, 0) is the plain call.
+template <int KIND>
+int gemm16_ex_impl(int op_a, int op_b, int m, int n, int k, float alpha, const uint16_t* dA, int lda, const uint16_t* dB,
+                   int ldb, float beta, void* dC, int ldc, int out_type, cudaStream_t st) {
+  if (alpha == 1.f && beta == 0.f) return gemm16_impl<KIND>(op_a, op_b, m, n, k, dA, lda, dB, ldb, dC, ldc, out_type, st);
+  using E = typename Kind16<KIND>::E;
+  if (out_type != B200_OUT_F32 && out_type != Kind16<KIND>::OUT16) return B200_ERR_BAD_ARG;
+  int rc = check_args(m, n, k, dA, lda, dB, ldb, dC, ldc, op_a, op_b);
+  if (rc == 1) return 0;
+  if (rc) return rc;
+  rc = ensure_device();
+  if (rc) return rc;
+  const bool c32 = out_type == B200_OUT_F32;
+  if (alpha == 0.f || k == 0) {           // C = beta * C: A and B are not read; beta == 0 does not read C either
+    if (beta == 0.f) return c32 ? launch_zero<float>(m, n, (float*)dC, ldc, st) : launch_zero<uint16_t>(m, n, (uint16_t*)dC, ldc, st);
+    const dim3 sg((n + 255) / 256, m < 4096 ? m : 4096);
+    if (c32) scale_inplace_kernel<float><<<sg, 256, 0, st>>>(m, n, (float*)dC, ldc, beta);
+    else scale_inplace_kernel<E><<<sg, 256, 0, st>>>(m, n, (E*)dC, ldc, beta);
+    g_launches++;
+    return last_launch_status();
+  }
+  t_epi.axpby = 1; t_epi.alpha = alpha; t_epi.beta = beta;
+  rc = gemm16_impl<KIND>(op_a, op_b, m, n, k, dA, lda, dB, ldb, dC, ldc, out_type, st);
   t_epi = EpiOpts();
   return rc;
 }
@@ -1160,23 +1219,22 @@ int b200_gemm_f32_acc(int m, int n, int k, const float* dA, int lda, const float
 
 int b200_gemm_bf16(int m, int n, int k, const uint16_t* dA, int lda, const uint16_t* dB, int ldb,
                    void* dC, int ldc, int out_type, void* stream) {
-  cudaStream_t st = (cudaStream_t)stream;
-  if (out_type != B200_OUT_F32 && out_type != B200_OUT_BF16) return B200_ERR_BAD_ARG;
-  int rc = check_args(m, n, k, dA, lda, dB, ldb, dC, ldc);
-  if (rc == 1) return 0;
-  if (rc) return rc;
-  rc = ensure_device();
-  if (rc) return rc;
-  if (k == 0)
-    return out_type == B200_OUT_F32 ? launch_zero<float>(m, n, (float*)dC, ldc, st)
-                                    : launch_zero<uint16_t>(m, n, (uint16_t*)dC, ldc, st);
-  if (!tma_ok(dA, lda, dB, ldb, 2)) {
-    if (out_type == B200_OUT_F32)
-      return launch_generic<uint16_t, float>(m, n, k, dA, lda, dB, ldb, (float*)dC, ldc, 0, st, "generic_bf16_64x64");
-    return launch_generic<uint16_t, uint16_t>(m, n, k, dA, lda, dB, ldb, (uint16_t*)dC, ldc, 0, st, "generic_bf16_64x64");
-  }
-  if (out_type == B200_OUT_F32) return tc_bf16_f32(m, n, k, dA, lda, dB, ldb, dC, ldc, st);
-  return tc_bf16_bf16(m, n, k, dA, lda, dB, ldb, dC, ldc, st);
+  return gemm16_impl<KIND_F16>(B200_OP_N, B200_OP_N, m, n, k, dA, lda, dB, ldb, dC, ldc, out_type, (cudaStream_t)stream);
+}
+
+int b200_gemm_f16(int m, int n, int k, const uint16_t* dA, int lda, const uint16_t* dB, int ldb,
+                  void* dC, int ldc, int out_type, void* stream) {
+  return gemm16_impl<KIND_FP16>(B200_OP_N, B200_OP_N, m, n, k, dA, lda, dB, ldb, dC, ldc, out_type, (cudaStream_t)stream);
+}
+
+int b200_gemm_bf16_ex(int op_a, int op_b, int m, int n, int k, float alpha, const uint16_t* dA, int lda,
+                      const uint16_t* dB, int ldb, float beta, void* dC, int ldc, int out_type, void* stream) {
+  return gemm16_ex_impl<KIND_F16>(op_a, op_b, m, n, k, alpha, dA, lda, dB, ldb, beta, dC, ldc, out_type, (cudaStream_t)stream);
+}
+
+int b200_gemm_f16_ex(int op_a, int op_b, int m, int n, int k, float alpha, const uint16_t* dA, int lda,
+                     const uint16_t* dB, int ldb, float beta, void* dC, int ldc, int out_type, void* stream) {
+  return gemm16_ex_impl<KIND_FP16>(op_a, op_b, m, n, k, alpha, dA, lda, dB, ldb, beta, dC, ldc, out_type, (cudaStream_t)stream);
 }
 
 int b200_gemm_s8s32(int m, int n, int k, const int8_t* dA, int lda, const int8_t* dB, int ldb,
@@ -1195,24 +1253,7 @@ int b200_gemm_s8s32(int m, int n, int k, const int8_t* dA, int lda, const int8_t
 
 int b200_gemm_bf16_op(int op_a, int op_b, int m, int n, int k, const uint16_t* dA, int lda, const uint16_t* dB, int ldb,
                       void* dC, int ldc, int out_type, void* stream) {
-  if (op_a == B200_OP_N && op_b == B200_OP_N) return b200_gemm_bf16(m, n, k, dA, lda, dB, ldb, dC, ldc, out_type, stream);
-  cudaStream_t st = (cudaStream_t)stream;
-  if (out_type != B200_OUT_F32 && out_type != B200_OUT_BF16) return B200_ERR_BAD_ARG;
-  int rc = check_args(m, n, k, dA, lda, dB, ldb, dC, ldc, op_a, op_b);
-  if (rc == 1) return 0;
-  if (rc) return rc;
-  rc = ensure_device();
-  if (rc) return rc;
-  if (k == 0)
-    return out_type == B200_OUT_F32 ? launch_zero<float>(m, n, (float*)dC, ldc, st)
-                                    : launch_zero<uint16_t>(m, n, (uint16_t*)dC, ldc, st);
-  if (!tma_ok(dA, lda, dB, ldb, 2)) {
-    if (out_type == B200_OUT_F32)
-      return launch_generic<uint16_t, float>(m, n, k, dA, lda, dB, ldb, (float*)dC, ldc, 0, st, "generic_bf16_64x64", op_a, op_b);
-    return launch_generic<uint16_t, uint16_t>(m, n, k, dA, lda, dB, ldb, (uint16_t*)dC, ldc, 0, st, "generic_bf16_64x64", op_a, op_b);
-  }
-  if (out_type == B200_OUT_F32) return tc_bf16_op<float>(op_a, op_b, m, n, k, dA, lda, dB, ldb, dC, ldc, st, kNamesBf16);
-  return tc_bf16_op<bf16_out>(op_a, op_b, m, n, k, dA, lda, dB, ldb, dC, ldc, st, kNamesBf16Obf16);
+  return gemm16_impl<KIND_F16>(op_a, op_b, m, n, k, dA, lda, dB, ldb, dC, ldc, out_type, (cudaStream_t)stream);
 }
 
 int b200_gemm_s8s32_op(int op_a, int op_b, int m, int n, int k, const int8_t* dA, int lda, const int8_t* dB, int ldb,

@@ -7,6 +7,7 @@
 // accumulation, so the fp32 instance keeps the strict contract of gemm_ffma.cuh.
 #pragma once
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <stdint.h>
 #include <type_traits>
 
@@ -14,24 +15,29 @@
 
 namespace b200 {
 
+// Element types: float, int8_t, uint16_t = bf16 bits, __half = fp16.  Every 16-bit load is exact in fp32.
 template <typename T> struct LoadAs;
 template <> struct LoadAs<float>   { using Acc = float;   __device__ static float   ld(const float* p)   { return *p; } };
 template <> struct LoadAs<int8_t>  { using Acc = int32_t; __device__ static int32_t ld(const int8_t* p)  { return (int32_t)*p; } };
 template <> struct LoadAs<uint16_t>{ using Acc = float;   __device__ static float   ld(const uint16_t* p){ return __uint_as_float((uint32_t)*p << 16); } };
+template <> struct LoadAs<__half>  { using Acc = float;   __device__ static float   ld(const __half* p)  { return __half2float(*p); } };
 
+// fp32 -> 16-bit stores round to nearest even (fp16: beyond 65504 to +-inf)
 template <typename Acc, typename OutT> __device__ __forceinline__ void store_out(OutT* p, Acc v);
 template <> __device__ __forceinline__ void store_out<float, float>(float* p, float v) { *p = v; }
 template <> __device__ __forceinline__ void store_out<int32_t, int32_t>(int32_t* p, int32_t v) { *p = v; }
 template <> __device__ __forceinline__ void store_out<float, uint16_t>(uint16_t* p, float v) {
   *p = __bfloat16_as_ushort(__float2bfloat16_rn(v));
 }
+template <> __device__ __forceinline__ void store_out<float, __half>(__half* p, float v) { *p = __float2half_rn(v); }
 
 // 64x64 tile, 256 threads, 4x4 per thread, BK = 16.
 // Element strides per index: A(i, p) = A[i * a_rs + p * a_cs], B(p, j) = B[p * b_rs + j * b_cs].  Row-major A is
 // (lda, 1), a transposed one (A^T stored k x m, pitch lda) is (1, lda); likewise B.  The arithmetic does not
 // depend on the strides.
-// axpby (fp32 in / fp32 out only): C = alpha * (A*B) + beta * C (b200_gemm_f32_ex); the chains start from zero,
-// alpha * chain is rounded, then fma(beta, C, .), and C is read only when beta != 0.
+// axpby (fp32, bf16 or fp16 in; fp32 or 16-bit out): C = alpha * (A*B) + beta * C (b200_gemm_f32_ex, _bf16_ex,
+// _f16_ex); the chains start from zero, alpha * chain is rounded, then fma(beta, float(C), .), rounded once more to
+// a 16-bit C, and C is read only when beta != 0.
 template <typename InT, typename OutT>
 __global__ void __launch_bounds__(256)
 gemm_generic_kernel(int M, int N, int K, const InT* __restrict__ A, long long a_rs, long long a_cs,
@@ -103,13 +109,13 @@ gemm_generic_kernel(int M, int N, int K, const InT* __restrict__ A, long long a_
           // requantising store (int8 C): per-row scale and optional per-row bias
           C[(long long)gm * ldc + gn] = (int8_t)requant_s8(acc[i][j], rq_scale[gm], rq_bias ? rq_bias[gm] : 0.0f,
                                                             rq_bias != nullptr);
-        } else if constexpr (std::is_same<Acc, float>::value && std::is_same<OutT, float>::value) {
+        } else if constexpr (std::is_same<Acc, float>::value) {        // fp32, bf16 or fp16 C
           float v = acc[i][j];
           if (axpby) {
             v *= alpha;
-            if (beta != 0.f) v = fmaf(beta, C[(long long)gm * ldc + gn], v);
+            if (beta != 0.f) v = fmaf(beta, LoadAs<OutT>::ld(C + (long long)gm * ldc + gn), v);
           }
-          C[(long long)gm * ldc + gn] = v;
+          store_out<float, OutT>(C + (long long)gm * ldc + gn, v);
         } else {
           store_out<Acc, OutT>(C + (long long)gm * ldc + gn, acc[i][j]);
         }
@@ -126,10 +132,15 @@ __global__ void convert_f32_to_bf16_kernel(const float* __restrict__ src, uint16
   for (; i < n; i += stride) dst[i] = __bfloat16_as_ushort(__float2bfloat16_rn(src[i]));
 }
 
-// C *= s over an m x n window (C = beta * C of the general epilogue when alpha == 0 or k == 0)
-__global__ void scale_inplace_kernel(int M, int N, float* __restrict__ C, long long ldc, float s) {
+// C = s * C over an m x n window (C = beta * C of the general epilogue when alpha == 0 or k == 0); 16-bit C is
+// read exactly and the product rounded once
+template <typename T>
+__global__ void scale_inplace_kernel(int M, int N, T* __restrict__ C, long long ldc, float s) {
   for (int r = blockIdx.y; r < M; r += gridDim.y)
-    for (int c = blockIdx.x * blockDim.x + threadIdx.x; c < N; c += gridDim.x * blockDim.x) C[(long long)r * ldc + c] *= s;
+    for (int c = blockIdx.x * blockDim.x + threadIdx.x; c < N; c += gridDim.x * blockDim.x) {
+      T* e = C + (long long)r * ldc + c;
+      store_out<float, T>(e, s * LoadAs<T>::ld(e));
+    }
 }
 
 template <typename T>

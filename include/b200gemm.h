@@ -92,10 +92,11 @@ enum b200_f32_mode {
  *  - The H100 tensor cores keep subnormal bf16, tf32 and fp16 inputs and subnormal fp32
  *    products and sums (observed on an H100 80GB HBM3): nothing is flushed to zero.        */
 
-/* ---- bf16 output selector -------------------------------------------------- */
+/* ---- output selector of the 16-bit GEMMs ----------------------------------- */
 enum b200_out_type {
-  B200_OUT_F32  = 0,     /* C written as float   (4 B/elem) */
-  B200_OUT_BF16 = 1      /* C written as bf16    (2 B/elem) */
+  B200_OUT_F32  = 0,     /* C written as float   (4 B/elem): bf16 and fp16 operands */
+  B200_OUT_BF16 = 1,     /* C written as bf16    (2 B/elem): bf16 operands only     */
+  B200_OUT_F16  = 2      /* C written as fp16    (2 B/elem): fp16 operands only     */
 };
 
 /* Library / device ---------------------------------------------------------- */
@@ -149,6 +150,28 @@ int b200_gemm_f32_ex(int m, int n, int k, float alpha,
                      const float* dA, int lda, const float* dB, int ldb, float beta,
                      float* dC, int ldc, int precision_mode, void* stream);
 
+/* 16-bit operands: C = alpha * op(A)*op(B) + beta * C on DEVICE pointers — cublasGemmEx's contract for bf16 and fp16
+ * (cuda/MMult_cuBLAS_2.cpp).  op_a / op_b and the leading dimensions are those of b200_gemm_f32_op (below).
+ *   b200_gemm_bf16_ex: bf16 operands, out_type B200_OUT_F32 or B200_OUT_BF16.
+ *   b200_gemm_f16_ex:  IEEE fp16 operands, out_type B200_OUT_F32 or B200_OUT_F16.
+ * Errors: an out_type that does not fit the operand type (F16 for bf16, BF16 for fp16, anything else), an op other
+ * than 0 or 1, an ld below its op's minimum or a null pointer is B200_ERR_BAD_ARG; m == 0 or n == 0 is a no-op.
+ * (alpha, beta) = (1, 0) is b200_gemm_bf16_op / b200_gemm_f16 exactly: same kernel, kernel name, launches and bits.
+ * Any other pair is fused into the epilogue of the tensor-core and the generic kernel: the fp32 accumulator x is
+ * stored as round_out(fma(beta, float(C), alpha * x)).  float(C) is exact for 16-bit C; round_out is the identity
+ * for fp32 C and one round-to-nearest-even to bf16 / fp16 otherwise.  beta == 0 never reads C (a NaN already in C
+ * stays out of the result); alpha == 0 or k == 0 never reads A or B: one element-wise pass C = round_out(beta *
+ * float(C)), zeros when beta == 0.  fp16 C rounds to nearest even and overflows to +-inf, as torch's .half() does.
+ * fp32 C may take the K-split tail (beta * C is folded by the first K part only); 16-bit C never does.  No workspace.
+ * Kernels: "tc_f16_128x{256,192,128}" (fp32 C) and "tc_f16_of16_128x..." (fp16 C), with the layout infix _nt / _tn
+ * / _tt as for bf16; operands that TMA cannot read take "generic_f16_64x64" (CUDA cores, sequential k). */
+int b200_gemm_bf16_ex(int op_a, int op_b, int m, int n, int k, float alpha,
+                      const uint16_t* dA, int lda, const uint16_t* dB, int ldb, float beta,
+                      void* dC, int ldc, int out_type, void* stream);
+int b200_gemm_f16_ex(int op_a, int op_b, int m, int n, int k, float alpha,
+                     const uint16_t* dA, int lda, const uint16_t* dB, int ldb, float beta,
+                     void* dC, int ldc, int out_type, void* stream);
+
 /* fp32 with HOST pointers and the CPU harness contract C += A*B
  * (aarch64/MMult0.cpp:11-19; harness zeroes C first, aarch64/test_MMult.cpp:107).
  * Stages H2D, runs b200_gemm_f32 on the device, adds into C on the device,
@@ -162,6 +185,13 @@ int b200_gemm_f32_host(int m, int n, int k,
 int b200_gemm_bf16(int m, int n, int k,
                    const uint16_t* dA, int lda, const uint16_t* dB, int ldb,
                    void* dC, int ldc, int out_type, void* stream);
+
+/* IEEE fp16 operands (raw uint16 bit patterns), fp32 accumulate; C is float (B200_OUT_F32) or fp16 (B200_OUT_F16,
+ * round to nearest even, overflow to +-inf).  The fp16 twin of b200_gemm_bf16: same tiles, schedule and routes.
+ * DEVICE pointers. */
+int b200_gemm_f16(int m, int n, int k,
+                  const uint16_t* dA, int lda, const uint16_t* dB, int ldb,
+                  void* dC, int ldc, int out_type, void* stream);
 
 /* int8 x int8 -> int32, exact: C = A*B (aarch64-int8/README.md:8; oracle
  * aarch64-int8/REF_MMult.c:10-23).  DEVICE pointers. */
@@ -191,6 +221,7 @@ int b200_gemm_s8s32_host(int m, int n, int k,
  *
  *   path                    NN   NT (B^T given)   TN (A^T given)   TT
  *   bf16 -> fp32 / bf16      1   1                1                1     operands read in place
+ *   fp16 -> fp32 / fp16      1   1                1                1     operands read in place (b200_gemm_f16_ex)
  *   TF32, int8               2   1                3                2     transposes into the workspace
  *   BF16X3, BF16X2           2   2                2                2     one split launch for both operands
  *   F16X2                    4   3                5                4     B^T's column maxima are its row maxima (the
