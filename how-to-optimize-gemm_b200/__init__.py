@@ -19,6 +19,8 @@ LIB_PATH = os.path.join(_HERE, "libb200gemm.so")
 F32_STRICT, F32_TF32, F32_BF16X3, F32_BF16X2, F32_AUTO, F32_F16X2 = 0, 1, 2, 3, 4, 5
 OUT_F32, OUT_BF16, OUT_F16 = 0, 1, 2
 OP_N, OP_T = 0, 1
+ACT_NONE, ACT_RELU, ACT_GELU, ACT_GELU_TANH = 0, 1, 2, 3
+ACTIVATIONS = {None: ACT_NONE, "relu": ACT_RELU, "gelu": ACT_GELU, "gelu_tanh": ACT_GELU_TANH}
 
 EXPORTS = [
     "b200_gemm_version", "b200_gemm_device_ok", "b200_gemm_strerror", "b200_gemm_last_kernel",
@@ -27,6 +29,7 @@ EXPORTS = [
     "b200_mxf4_quantize_a", "b200_mxf4_quantize_b", "b200_gemm_mxf4", "b200_gemm_f32_host", "b200_gemm_bf16", "b200_gemm_f16", "b200_gemm_s8s32",
     "b200_gemm_s8s32_host", "b200_gemm_s8s8_requant", "b200_gemm_f32_pack_b", "b200_gemm_f32_packed",
     "b200_gemm_f32_pack_free", "b200_gemm_f32_op", "b200_gemm_bf16_op", "b200_gemm_bf16_ex", "b200_gemm_f16_ex",
+    "b200_gemm_bf16_epi", "b200_gemm_f16_epi",
     "b200_gemm_s8s32_op", "b200_gemm_workspace_bytes_op",
     "b200_nccl_load", "b200_nccl_last_error", "b200_comm_unique_id", "b200_comm_init_rank",
     "b200_comm_destroy", "b200_rowpanel_create", "b200_rowpanel_destroy", "b200_rowpanel_slices", "b200_rowpanel_set_reserve_sms", "b200_rowpanel_trace", "b200_rowpanel_trace_dump", "b200_gemm_f32_rowpanel",
@@ -78,6 +81,8 @@ lib.b200_gemm_f32_op.argtypes = [_i, _i, _i, _i, _i, C.c_float, _vp, _i, _vp, _i
 lib.b200_gemm_bf16_op.argtypes = [_i, _i, _i, _i, _i, _vp, _i, _vp, _i, _vp, _i, _i, _vp]
 lib.b200_gemm_bf16_ex.argtypes = [_i, _i, _i, _i, _i, C.c_float, _vp, _i, _vp, _i, C.c_float, _vp, _i, _i, _vp]
 lib.b200_gemm_f16_ex.argtypes = [_i, _i, _i, _i, _i, C.c_float, _vp, _i, _vp, _i, C.c_float, _vp, _i, _i, _vp]
+lib.b200_gemm_bf16_epi.argtypes = [_i, _i, _i, _i, _i, C.c_float, _vp, _i, _vp, _i, C.c_float, _vp, _i, _i, _vp, _i, _vp]
+lib.b200_gemm_f16_epi.argtypes = [_i, _i, _i, _i, _i, C.c_float, _vp, _i, _vp, _i, C.c_float, _vp, _i, _i, _vp, _i, _vp]
 lib.b200_gemm_s8s32_op.argtypes = [_i, _i, _i, _i, _i, _vp, _i, _vp, _i, _vp, _i, _vp]
 lib.b200_gemm_workspace_bytes_op.argtypes = [_i, _i, _i, _i, _i, _i]
 lib.b200_gemm_workspace_bytes_op.restype = C.c_size_t
@@ -196,12 +201,38 @@ def operand_layout(shape, strides):
                      "transpose of a row-major matrix")
 
 
-def gemm(A, B, out=None, *, alpha=1.0, beta=0.0, mode=F32_AUTO, out_dtype=None, stream=None):
+def _epilogue_args(A, B, bias, activation):
+    """Checks a bias / activation request of gemm() (before anything touches the device); returns the ACT_* code."""
+    import torch
+    if activation not in ACTIVATIONS:
+        raise ValueError(f"activation must be one of {sorted(a for a in ACTIVATIONS if a)} or None, not {activation!r}")
+    if A.dtype not in (torch.bfloat16, torch.float16) or B.dtype != A.dtype:
+        raise TypeError(f"a bias or an activation needs bf16 or fp16 operands of one dtype, not {A.dtype} and {B.dtype}")
+    if bias is not None:
+        if bias.dtype != A.dtype:
+            raise ValueError(f"the bias must have the operands' dtype {A.dtype}, not {bias.dtype}")
+        if bias.dim() != 1 or bias.shape[0] != B.shape[1]:
+            raise ValueError(f"the bias must be 1-D with n = {B.shape[1]} elements, not of shape {tuple(bias.shape)}")
+        if not bias.is_contiguous() or not bias.is_cuda:
+            raise ValueError("the bias must be a contiguous CUDA tensor")
+    return ACTIVATIONS[activation]
+
+
+def gemm(A, B, out=None, *, alpha=1.0, beta=0.0, bias=None, activation=None, mode=F32_AUTO, out_dtype=None,
+         stream=None):
     """C = alpha * A @ B + beta * C for fp32 (any precision mode), bf16 (fp32 or bf16 C), fp16 (fp32 or fp16 C) and
     int8 (int32 C) CUDA tensors.  Each operand may be row-major or the transpose of a row-major matrix (x @ W.t()
     passes W as stored): it is read in place (b200_gemm_f32_op / _bf16_op / _bf16_ex / _f16_ex / _s8s32_op), never
-    copied.  out must be row-major; it is read only when beta != 0.  int8 takes alpha = 1, beta = 0 only."""
+    copied.  out must be row-major; it is read only when beta != 0.  int8 takes alpha = 1, beta = 0 only.
+
+    bf16 and fp16 also take a bias (1-D, contiguous, n elements of the operands' dtype) and an activation (None,
+    "relu", "gelu" or "gelu_tanh") fused into the epilogue (b200_gemm_bf16_epi / _f16_epi):
+    C = act(alpha * A @ B + beta * C + bias), so gemm(x, W.t(), bias=b, activation="gelu") is
+    F.gelu(F.linear(x, W, b)) in one launch.  Other operand dtypes refuse them with TypeError; a bias of another dtype
+    or length is a ValueError."""
     import torch
+    epi = bias is not None or activation is not None
+    act = _epilogue_args(A, B, bias, activation) if epi else ACT_NONE
     assert A.dim() == 2 and B.dim() == 2 and A.is_cuda and B.is_cuda
     if A.dtype != B.dtype:
         raise TypeError(f"operands of different dtypes: {A.dtype} and {B.dtype}")
@@ -228,7 +259,11 @@ def gemm(A, B, out=None, *, alpha=1.0, beta=0.0, mode=F32_AUTO, out_dtype=None, 
     if n > 1:
         assert out.stride(1) == 1, "out must be row-major"
     st = _stream_ptr(stream)
-    if A.dtype == torch.float32:
+    if epi:
+        fn, ot = (lib.b200_gemm_bf16_epi, OUT_BF16) if A.dtype == torch.bfloat16 else (lib.b200_gemm_f16_epi, OUT_F16)
+        _check(fn(op_a, op_b, m, n, k, alpha, A.data_ptr(), lda, B.data_ptr(), ldb, beta, out.data_ptr(), _ld(out),
+                  OUT_F32 if cdt == torch.float32 else ot, bias.data_ptr() if bias is not None else None, act, st))
+    elif A.dtype == torch.float32:
         _check(lib.b200_gemm_f32_op(op_a, op_b, m, n, k, alpha, A.data_ptr(), lda, B.data_ptr(), ldb, beta, out.data_ptr(),
                                     _ld(out), mode, st))
     elif A.dtype == torch.bfloat16 and alpha == 1.0 and beta == 0.0:

@@ -49,7 +49,8 @@ struct KernelTimer {
 std::atomic<int> g_default_f32_mode{-1};
 thread_local const char* t_last_kernel = "none";
 // General epilogue request of the current call (b200_gemm_f32_ex): read by launch_tc, reset by the entry point.
-struct EpiOpts { int axpby = 0; float alpha = 1.f, beta = 0.f; };
+// bias / act: the bias / activation epilogue of the 16-bit GEMMs (b200_gemm_bf16_epi / _f16_epi), act -1 = none.
+struct EpiOpts { int axpby = 0; float alpha = 1.f, beta = 0.f; const void* bias = nullptr; int act = -1; };
 thread_local EpiOpts t_epi;
 // SMs the tensor-core launches of the current call leave free (the row-panel plan sets it while a later K-slice
 // of B is still being broadcast: a persistent GEMM holding every SM would starve NCCL's copy kernels and
@@ -275,7 +276,8 @@ int launch_generic(int m, int n, int k, const InT* A, int lda, const InT* B, int
   dim3 grid((n + 63) / 64, (m + 63) / 64);
   const long long a_rs = op_a ? 1 : lda, a_cs = op_a ? lda : 1, b_rs = op_b ? 1 : ldb, b_cs = op_b ? ldb : 1;
   gemm_generic_kernel<InT, OutT><<<grid, 256, 0, st>>>(m, n, k, A, a_rs, a_cs, B, b_rs, b_cs, C, ldc, accumulate, nullptr,
-                                                       nullptr, t_epi.axpby, t_epi.alpha, t_epi.beta);
+                                                       nullptr, t_epi.axpby, t_epi.alpha, t_epi.beta,
+                                                       reinterpret_cast<const InT*>(t_epi.bias), t_epi.act);
   g_launches++;
   t_last_kernel = name;
   return last_launch_status();
@@ -303,8 +305,9 @@ int g_ffma_halves = 1;        // strict kernel: split the tail round into half t
 //   B MN-major: k x n (b_rows_total rows, pitch ldb);  B K-major: B^T, n x k (b_rows_total rows, pitch ldb)
 // Stacked planes (split modes) lie along the rows, plane p at row p * a_plane_rows / p * b_plane_rows.  tf32 and
 // int8 take K-major A and B only (launch_tc_kmajor builds them).
+// EPI: the bias / activation kernel (t_epi.bias / act), which never takes the K-split tail.
 template <int KIND, int BN, int STAGES, typename OutT, class Prod = ProdSingle, int A_ROW_BYTES = 128, int AL = LAYOUT_K,
-          int BL = KindTraits<KIND>::B_LAYOUT>
+          int BL = KindTraits<KIND>::B_LAYOUT, bool EPI = false>
 int launch_tc(int m, int n, int k, const void* A, long long lda, int a_rows_total, int a_plane_rows,
               const void* B, long long ldb, int b_rows_total, int b_plane_rows, void* C, int ldc,
               cudaStream_t st, const char* name, int chunk_k = 0, const float* row_max = nullptr,
@@ -343,8 +346,10 @@ int launch_tc(int m, int n, int k, const void* A, long long lda, int a_rows_tota
   p.row_max = row_max; p.col_max = col_max;
   p.accumulate = accumulate;
   p.axpby = t_epi.axpby; p.alpha = t_epi.alpha; p.beta = t_epi.beta;
+  p.act = t_epi.act;
+  if constexpr (EPI) p.bias = t_epi.bias;        // shares col_max's slot: EPI kernels are never scaled
   p.stream_c = g_stream_c < 0 ? (g_stream_c = (getenv("B200GEMM_STREAM_C") ? atoi(getenv("B200GEMM_STREAM_C")) : kStreamCDefault)) : g_stream_c;
-  auto kern = gemm_tc_kernel<KIND, BN, STAGES, OutT, Prod, A_ROW_BYTES, AL, BL>;
+  auto kern = gemm_tc_kernel<KIND, BN, STAGES, OutT, Prod, A_ROW_BYTES, AL, BL, EPI>;
   if (int arc = ensure_smem_attr(kern, Cfg::SMEM_BYTES)) return arc;
   int tiles = p.tiles_m * p.tiles_n;
   const int units_max = t_ctx->sms - t_sm_reserve > 2 ? t_ctx->sms - t_sm_reserve : t_ctx->sms;   // one CTA per SM
@@ -353,7 +358,7 @@ int launch_tc(int m, int n, int k, const void* A, long long lda, int a_rows_tota
   const int num_kb = (k + Cfg::BK - 1) / Cfg::BK;
   const int rem = tiles % units_max;
   int split = 1;
-  if (g_split_tail && OB == 4 && rem > 0) {
+  if (!EPI && g_split_tail && OB == 4 && rem > 0) {    // an activation must see the complete sum: no split
     split = units_max / rem;
     if (split > 4) split = 4;
     if (split > num_kb / 8) split = num_kb / 8;       // keep >= 8 k-blocks per part
@@ -407,26 +412,27 @@ inline int op_index(int op_a, int op_b) { return op_a ? (op_b ? 2 : 1) : 0; }
 constexpr int kLayoutA[3] = {LAYOUT_K, LAYOUT_MN, LAYOUT_MN}, kLayoutB[3] = {LAYOUT_K, LAYOUT_MN, LAYOUT_K};
 
 // The plain 16-bit GEMM (KIND_F16 = bf16, KIND_FP16 = fp16; OutT float, bf16_out or f16_out) in one layout, read in
-// place: A^T is the MN-major A, B^T the K-major B.  names: the three tile widths 256 / 192 / 128.
-template <int KIND, typename OutT, int AL, int BL>
+// place: A^T is the MN-major A, B^T the K-major B.  names: the three tile widths 256 / 192 / 128.  EPI: the bias /
+// activation kernels.
+template <int KIND, typename OutT, int AL, int BL, bool EPI = false>
 int tc16_layout(int m, int n, int k, const void* A, int lda, const void* B, int ldb, void* C, int ldc, cudaStream_t st,
                 const char* const (&names)[3]) {
   const int ar = AL == LAYOUT_MN ? k : m, br = BL == LAYOUT_MN ? k : n;      // rows of the operands as stored
   switch (pick_bn(m, n, true)) {
-    case 256: return launch_tc<KIND, 256, 4, OutT, ProdSingle, 128, AL, BL>(m, n, k, A, lda, ar, 0, B, ldb, br, 0, C, ldc, st, names[0]);
-    case 192: return launch_tc<KIND, 192, 5, OutT, ProdSingle, 128, AL, BL>(m, n, k, A, lda, ar, 0, B, ldb, br, 0, C, ldc, st, names[1]);
-    default:  return launch_tc<KIND, 128, 6, OutT, ProdSingle, 128, AL, BL>(m, n, k, A, lda, ar, 0, B, ldb, br, 0, C, ldc, st, names[2]);
+    case 256: return launch_tc<KIND, 256, 4, OutT, ProdSingle, 128, AL, BL, EPI>(m, n, k, A, lda, ar, 0, B, ldb, br, 0, C, ldc, st, names[0]);
+    case 192: return launch_tc<KIND, 192, 5, OutT, ProdSingle, 128, AL, BL, EPI>(m, n, k, A, lda, ar, 0, B, ldb, br, 0, C, ldc, st, names[1]);
+    default:  return launch_tc<KIND, 128, 6, OutT, ProdSingle, 128, AL, BL, EPI>(m, n, k, A, lda, ar, 0, B, ldb, br, 0, C, ldc, st, names[2]);
   }
 }
 // names[layout][width]: layout 0 = NN, 1 = NT, 2 = TN, 3 = TT.
-template <int KIND, typename OutT>
+template <int KIND, typename OutT, bool EPI = false>
 int tc16_op(int op_a, int op_b, int m, int n, int k, const void* A, int lda, const void* B, int ldb, void* C, int ldc,
             cudaStream_t st, const char* const (&names)[4][3]) {
-  if (!op_a && !op_b) return tc16_layout<KIND, OutT, LAYOUT_K, LAYOUT_MN>(m, n, k, A, lda, B, ldb, C, ldc, st, names[0]);
+  if (!op_a && !op_b) return tc16_layout<KIND, OutT, LAYOUT_K, LAYOUT_MN, EPI>(m, n, k, A, lda, B, ldb, C, ldc, st, names[0]);
   switch (op_index(op_a, op_b)) {
-    case 0: return tc16_layout<KIND, OutT, kLayoutA[0], kLayoutB[0]>(m, n, k, A, lda, B, ldb, C, ldc, st, names[1]);
-    case 1: return tc16_layout<KIND, OutT, kLayoutA[1], kLayoutB[1]>(m, n, k, A, lda, B, ldb, C, ldc, st, names[2]);
-    default: return tc16_layout<KIND, OutT, kLayoutA[2], kLayoutB[2]>(m, n, k, A, lda, B, ldb, C, ldc, st, names[3]);
+    case 0: return tc16_layout<KIND, OutT, kLayoutA[0], kLayoutB[0], EPI>(m, n, k, A, lda, B, ldb, C, ldc, st, names[1]);
+    case 1: return tc16_layout<KIND, OutT, kLayoutA[1], kLayoutB[1], EPI>(m, n, k, A, lda, B, ldb, C, ldc, st, names[2]);
+    default: return tc16_layout<KIND, OutT, kLayoutA[2], kLayoutB[2], EPI>(m, n, k, A, lda, B, ldb, C, ldc, st, names[3]);
   }
 }
 #define TC16_NAMES(P)                                                                               \
@@ -436,6 +442,10 @@ const char* const kNamesBf16[4][3] = TC16_NAMES("tc_bf16");
 const char* const kNamesBf16Obf16[4][3] = TC16_NAMES("tc_bf16_obf16");
 const char* const kNamesF16[4][3] = TC16_NAMES("tc_f16");
 const char* const kNamesF16Of16[4][3] = TC16_NAMES("tc_f16_of16");
+const char* const kNamesBf16Epi[4][3] = TC16_NAMES("tc_bf16_epi");
+const char* const kNamesBf16Obf16Epi[4][3] = TC16_NAMES("tc_bf16_obf16_epi");
+const char* const kNamesF16Epi[4][3] = TC16_NAMES("tc_f16_epi");
+const char* const kNamesF16Of16Epi[4][3] = TC16_NAMES("tc_f16_of16_epi");
 
 // ---- split-precision fp32 on the tensor cores ---------------------------------------------------
 // Workspace for the bf16 planes: cached, grow-only (no per-call cudaMalloc in steady state).  Calls
@@ -1137,6 +1147,8 @@ template <> struct Kind16<KIND_F16> {
   static constexpr const char* kGeneric = "generic_bf16_64x64";
   static constexpr const char* const (&names)[4][3] = kNamesBf16;
   static constexpr const char* const (&names16)[4][3] = kNamesBf16Obf16;
+  static constexpr const char* const (&names_epi)[4][3] = kNamesBf16Epi;
+  static constexpr const char* const (&names16_epi)[4][3] = kNamesBf16Obf16Epi;
 };
 template <> struct Kind16<KIND_FP16> {
   using E = __half;
@@ -1145,10 +1157,13 @@ template <> struct Kind16<KIND_FP16> {
   static constexpr const char* kGeneric = "generic_f16_64x64";
   static constexpr const char* const (&names)[4][3] = kNamesF16;
   static constexpr const char* const (&names16)[4][3] = kNamesF16Of16;
+  static constexpr const char* const (&names_epi)[4][3] = kNamesF16Epi;
+  static constexpr const char* const (&names16_epi)[4][3] = kNamesF16Of16Epi;
 };
 
 // C = op(A) op(B) (the general epilogue when t_epi asks for it): every layout is read in place by one launch.
-template <int KIND>
+// EPI: the bias / activation kernels (t_epi.bias / act; gemm16_epi_impl has handled k == 0).
+template <int KIND, bool EPI = false>
 int gemm16_impl(int op_a, int op_b, int m, int n, int k, const uint16_t* dA, int lda, const uint16_t* dB, int ldb,
                 void* dC, int ldc, int out_type, cudaStream_t st) {
   using K16 = Kind16<KIND>;
@@ -1167,8 +1182,9 @@ int gemm16_impl(int op_a, int op_b, int m, int n, int k, const uint16_t* dA, int
     if (c32) return launch_generic<E, float>(m, n, k, a, lda, b, ldb, (float*)dC, ldc, 0, st, K16::kGeneric, op_a, op_b);
     return launch_generic<E, E>(m, n, k, a, lda, b, ldb, (E*)dC, ldc, 0, st, K16::kGeneric, op_a, op_b);
   }
-  if (c32) return tc16_op<KIND, float>(op_a, op_b, m, n, k, dA, lda, dB, ldb, dC, ldc, st, K16::names);
-  return tc16_op<KIND, typename K16::Out16>(op_a, op_b, m, n, k, dA, lda, dB, ldb, dC, ldc, st, K16::names16);
+  if (c32) return tc16_op<KIND, float, EPI>(op_a, op_b, m, n, k, dA, lda, dB, ldb, dC, ldc, st, EPI ? K16::names_epi : K16::names);
+  return tc16_op<KIND, typename K16::Out16, EPI>(op_a, op_b, m, n, k, dA, lda, dB, ldb, dC, ldc, st,
+                                                 EPI ? K16::names16_epi : K16::names16);
 }
 
 // C = alpha op(A) op(B) + beta C with the rules of b200_gemm_f32_ex; (1, 0) is the plain call.
@@ -1194,6 +1210,40 @@ int gemm16_ex_impl(int op_a, int op_b, int m, int n, int k, float alpha, const u
   }
   t_epi.axpby = 1; t_epi.alpha = alpha; t_epi.beta = beta;
   rc = gemm16_impl<KIND>(op_a, op_b, m, n, k, dA, lda, dB, ldb, dC, ldc, out_type, st);
+  t_epi = EpiOpts();
+  return rc;
+}
+
+static_assert(ACT_NONE == B200_ACT_NONE && ACT_RELU == B200_ACT_RELU && ACT_GELU == B200_ACT_GELU &&
+              ACT_GELU_TANH == B200_ACT_GELU_TANH, "EpiAct follows the header's codes");
+
+// C = round_out(act(fma(beta, float(C), alpha * op(A) op(B)) + bias)): the _ex rules plus the bias / activation
+// epilogue.  No bias and B200_ACT_NONE is the _ex call; k == 0 or alpha == 0 is one element-wise pass.
+template <int KIND>
+int gemm16_epi_impl(int op_a, int op_b, int m, int n, int k, float alpha, const uint16_t* dA, int lda, const uint16_t* dB,
+                    int ldb, float beta, void* dC, int ldc, int out_type, const uint16_t* bias, int act, cudaStream_t st) {
+  if (act < B200_ACT_NONE || act > B200_ACT_GELU_TANH) return B200_ERR_BAD_ARG;
+  if (bias == nullptr && act == B200_ACT_NONE)
+    return gemm16_ex_impl<KIND>(op_a, op_b, m, n, k, alpha, dA, lda, dB, ldb, beta, dC, ldc, out_type, st);
+  using E = typename Kind16<KIND>::E;
+  if (out_type != B200_OUT_F32 && out_type != Kind16<KIND>::OUT16) return B200_ERR_BAD_ARG;
+  int rc = check_args(m, n, k, dA, lda, dB, ldb, dC, ldc, op_a, op_b);
+  if (rc == 1) return 0;
+  if (rc) return rc;
+  rc = ensure_device();
+  if (rc) return rc;
+  const bool c32 = out_type == B200_OUT_F32;
+  const E* b = reinterpret_cast<const E*>(bias);
+  if (alpha == 0.f || k == 0) {           // C = act(beta * C + bias): A and B are not read; beta == 0 does not read C
+    const dim3 sg((n + 255) / 256, m < 4096 ? m : 4096);
+    if (c32) bias_act_inplace_kernel<float, E><<<sg, 256, 0, st>>>(m, n, (float*)dC, ldc, beta, b, act);
+    else bias_act_inplace_kernel<E, E><<<sg, 256, 0, st>>>(m, n, (E*)dC, ldc, beta, b, act);
+    g_launches++;
+    t_last_kernel = "bias_act_inplace";
+    return last_launch_status();
+  }
+  t_epi.axpby = 1; t_epi.alpha = alpha; t_epi.beta = beta; t_epi.bias = bias; t_epi.act = act;
+  rc = gemm16_impl<KIND, true>(op_a, op_b, m, n, k, dA, lda, dB, ldb, dC, ldc, out_type, st);
   t_epi = EpiOpts();
   return rc;
 }
@@ -1235,6 +1285,20 @@ int b200_gemm_bf16_ex(int op_a, int op_b, int m, int n, int k, float alpha, cons
 int b200_gemm_f16_ex(int op_a, int op_b, int m, int n, int k, float alpha, const uint16_t* dA, int lda,
                      const uint16_t* dB, int ldb, float beta, void* dC, int ldc, int out_type, void* stream) {
   return gemm16_ex_impl<KIND_FP16>(op_a, op_b, m, n, k, alpha, dA, lda, dB, ldb, beta, dC, ldc, out_type, (cudaStream_t)stream);
+}
+
+int b200_gemm_bf16_epi(int op_a, int op_b, int m, int n, int k, float alpha, const uint16_t* dA, int lda,
+                       const uint16_t* dB, int ldb, float beta, void* dC, int ldc, int out_type, const uint16_t* dBias,
+                       int act, void* stream) {
+  return gemm16_epi_impl<KIND_F16>(op_a, op_b, m, n, k, alpha, dA, lda, dB, ldb, beta, dC, ldc, out_type, dBias, act,
+                                   (cudaStream_t)stream);
+}
+
+int b200_gemm_f16_epi(int op_a, int op_b, int m, int n, int k, float alpha, const uint16_t* dA, int lda,
+                      const uint16_t* dB, int ldb, float beta, void* dC, int ldc, int out_type, const uint16_t* dBias,
+                      int act, void* stream) {
+  return gemm16_epi_impl<KIND_FP16>(op_a, op_b, m, n, k, alpha, dA, lda, dB, ldb, beta, dC, ldc, out_type, dBias, act,
+                                    (cudaStream_t)stream);
 }
 
 int b200_gemm_s8s32(int m, int n, int k, const int8_t* dA, int lda, const int8_t* dB, int ldb,

@@ -31,6 +31,17 @@ template <> __device__ __forceinline__ void store_out<float, uint16_t>(uint16_t*
 }
 template <> __device__ __forceinline__ void store_out<float, __half>(__half* p, float v) { *p = __float2half_rn(v); }
 
+// act(t + b) with a runtime activation code (EpiAct); b = -0 stands for no bias (t + -0 is t, zeros included).
+__device__ __forceinline__ float act_bias(float t, float b, int act) {
+  t = __fadd_rn(t, b);
+  switch (act) {
+    case ACT_RELU: return epi_act<ACT_RELU>(t);
+    case ACT_GELU: return epi_act<ACT_GELU>(t);
+    case ACT_GELU_TANH: return epi_act<ACT_GELU_TANH>(t);
+    default: return t;
+  }
+}
+
 // 64x64 tile, 256 threads, 4x4 per thread, BK = 16.
 // Element strides per index: A(i, p) = A[i * a_rs + p * a_cs], B(p, j) = B[p * b_rs + j * b_cs].  Row-major A is
 // (lda, 1), a transposed one (A^T stored k x m, pitch lda) is (1, lda); likewise B.  The arithmetic does not
@@ -38,12 +49,15 @@ template <> __device__ __forceinline__ void store_out<float, __half>(__half* p, 
 // axpby (fp32, bf16 or fp16 in; fp32 or 16-bit out): C = alpha * (A*B) + beta * C (b200_gemm_f32_ex, _bf16_ex,
 // _f16_ex); the chains start from zero, alpha * chain is rounded, then fma(beta, float(C), .), rounded once more to
 // a 16-bit C, and C is read only when beta != 0.
+// bias / act (16-bit operands, b200_gemm_bf16_epi / _f16_epi; needs axpby): after the alpha / beta step, t + bias[j]
+// (skipped for a null bias) goes through epi_act (ptx.cuh), the tensor-core kernel's activation.  act = -1: none.
 template <typename InT, typename OutT>
 __global__ void __launch_bounds__(256)
 gemm_generic_kernel(int M, int N, int K, const InT* __restrict__ A, long long a_rs, long long a_cs,
                     const InT* __restrict__ B, long long b_rs, long long b_cs, OutT* __restrict__ C, long long ldc,
                     int accumulate, const float* __restrict__ rq_scale = nullptr,
-                    const float* __restrict__ rq_bias = nullptr, int axpby = 0, float alpha = 1.f, float beta = 0.f) {
+                    const float* __restrict__ rq_bias = nullptr, int axpby = 0, float alpha = 1.f, float beta = 0.f,
+                    const InT* __restrict__ bias = nullptr, int act = -1) {
   using Acc = typename LoadAs<InT>::Acc;
   __shared__ Acc As[16][64 + 4];
   __shared__ Acc Bs[16][64 + 4];
@@ -115,6 +129,9 @@ gemm_generic_kernel(int M, int N, int K, const InT* __restrict__ A, long long a_
             v *= alpha;
             if (beta != 0.f) v = fmaf(beta, LoadAs<OutT>::ld(C + (long long)gm * ldc + gn), v);
           }
+          if constexpr (sizeof(InT) == 2) {
+            if (act >= 0) v = act_bias(v, bias != nullptr ? LoadAs<InT>::ld(bias + gn) : -0.f, act);
+          }
           store_out<float, OutT>(C + (long long)gm * ldc + gn, v);
         } else {
           store_out<Acc, OutT>(C + (long long)gm * ldc + gn, acc[i][j]);
@@ -140,6 +157,19 @@ __global__ void scale_inplace_kernel(int M, int N, T* __restrict__ C, long long 
     for (int c = blockIdx.x * blockDim.x + threadIdx.x; c < N; c += gridDim.x * blockDim.x) {
       T* e = C + (long long)r * ldc + c;
       store_out<float, T>(e, s * LoadAs<T>::ld(e));
+    }
+}
+
+// C = act(beta * C + bias[c]) over an m x n window (the bias / activation epilogue when alpha == 0 or k == 0): beta == 0
+// contributes +0 and leaves C unread; a null bias adds nothing.  16-bit C is read exactly and the result rounded once.
+template <typename T, typename BiasT>
+__global__ void bias_act_inplace_kernel(int M, int N, T* __restrict__ C, long long ldc, float s,
+                                        const BiasT* __restrict__ bias, int act) {
+  for (int r = blockIdx.y; r < M; r += gridDim.y)
+    for (int c = blockIdx.x * blockDim.x + threadIdx.x; c < N; c += gridDim.x * blockDim.x) {
+      T* e = C + (long long)r * ldc + c;
+      const float t = s != 0.f ? s * LoadAs<T>::ld(e) : 0.f;
+      store_out<float, T>(e, act_bias(t, bias != nullptr ? LoadAs<BiasT>::ld(bias + c) : -0.f, act));
     }
 }
 

@@ -86,7 +86,12 @@ struct TcParams {
   // Scaled split mode (B200_F32_F16X2): operands were multiplied by 2^-e(row) / 2^-e(col) before the
   // fp16 split; the epilogue multiplies back by 2^e(row) * 2^e(col), exact.  Null = no scaling.
   const float* row_max;    // [M] max |A(i,:)|
-  const float* col_max;    // [N] max |B(:,j)|
+  union {
+    const float* col_max;  // [N] max |B(:,j)|
+    // EPI kernels (16-bit kinds, single plane, never scaled): the bias, n elements of the operand type (bf16 or fp16
+    // bits), null = none.  It shares the slot so that TcParams, and with it every other kernel's code, is unchanged.
+    const void* bias;
+  };
   // General epilogue C = alpha * (A*B) + beta * C (cuBLAS semantics, cuda/MMult_cuBLAS_1.cpp:11-19); fp32, bf16 or
   // fp16 output (16-bit C is read exactly as fp32 and the result rounded once).  axpby == 0: alpha = 1 and
   // beta = accumulate (the two contracts the reference's harnesses use).
@@ -95,6 +100,7 @@ struct TcParams {
   int accumulate;          // 1: C += A*B (every partial, including the first, is folded into C); fp32/int32 only
   int stream_c;            // 1: the split modes' single pass over C uses streaming (evict-first) stores
   int dbg_b_lbo, dbg_b_sbo;  // MN-major B descriptor strides, 0 = defaults (probe hook, see b200_gemm_debug_set_b_desc)
+  int act;                 // EPI kernels: y = act(t + bias[col]) after the alpha / beta step; an EpiAct (ptx.cuh)
 };
 
 // REGACC (split-precision fp32 modes): the tensor core adds into its fp32 accumulator with truncation,
@@ -235,9 +241,12 @@ template <typename OutT> __device__ __forceinline__ float c16_to_f32(uint32_t h)
 }
 
 // One consumer thread's pair of adjacent columns (col, col + 1) of row `row` into C.
-template <typename OutT, typename V>
+// ACT >= 0 (EPI kernels, fp32 / bf16 / fp16 C): after the alpha / beta step t = fma(beta, C, alpha * x), store
+// act(t + b[e]); b = -0 when there is no bias (t + -0 is t for every t, the sign of zero included).
+template <typename OutT, typename V, int ACT = -1>
 __device__ __forceinline__ void store_pair(const TcParams& p, int row, int col, V v0, V v1, bool fold, bool l2_read,
-                                           float al, float be, int re, const int (&ce)[2], float sc, float bi) {
+                                           float al, float be, int re, const int (&ce)[2], float sc, float bi,
+                                           float b0 = -0.f, float b1 = -0.f) {
   if (row >= p.M || col >= p.N) return;
   const bool both = col + 1 < p.N;
   if constexpr (std::is_same<OutT, float>::value) {
@@ -252,8 +261,16 @@ __device__ __forceinline__ void store_pair(const TcParams& p, int row, int col, 
         if (p.axpby) { x[0] = fmaf(be, o.x, x[0]); x[1] = fmaf(be, o.y, x[1]); }
         else { x[0] += o.x; x[1] += o.y; }
       }
+      if constexpr (ACT >= 0) { x[0] = epi_act<ACT>(__fadd_rn(x[0], b0)); x[1] = epi_act<ACT>(__fadd_rn(x[1], b1)); }
       if (p.stream_c) __stcs(reinterpret_cast<float2*>(dst), make_float2(x[0], x[1]));
       else *reinterpret_cast<float2*>(dst) = make_float2(x[0], x[1]);
+    } else if constexpr (ACT >= 0) {
+#pragma unroll
+      for (int e = 0; e < 2; e++)
+        if (e == 0 || both) {
+          const float t = !fold ? x[e] : p.axpby ? fmaf(be, __ldcg(dst + e), x[e]) : x[e] + __ldcg(dst + e);
+          dst[e] = epi_act<ACT>(__fadd_rn(t, e == 0 ? b0 : b1));
+        }
     } else {
 #pragma unroll
       for (int e = 0; e < 2; e++)
@@ -283,6 +300,7 @@ __device__ __forceinline__ void store_pair(const TcParams& p, int row, int col, 
         x[1] = fmaf(be, c16_to_f32<OutT>(o >> 16), x[1]);
       }
     }
+    if constexpr (ACT >= 0) { x[0] = epi_act<ACT>(__fadd_rn(x[0], b0)); x[1] = epi_act<ACT>(__fadd_rn(x[1], b1)); }
     const uint32_t w = std::is_same<OutT, f16_out>::value ? cvt_f16x2(x[0], x[1]) : cvt_bf16x2(x[0], x[1]);
     if (both && p.vec_ok) *reinterpret_cast<uint32_t*>(dst) = w;
     else {
@@ -301,14 +319,48 @@ __device__ __forceinline__ void store_pair(const TcParams& p, int row, int col, 
   }
 }
 
+// Bias + activation epilogue (EPI kernels) of one warp's 16 rows of a tile: the bias pair of each column pair is
+// loaded once (one 4-byte load where the bias address allows) and shared by the thread's two rows.  ACT is the
+// tile-uniform p.act, dispatched once per tile so that the unrolled store loop holds one activation only.
+template <int KIND, typename OutT, int ACT, int BN>
+__device__ __forceinline__ void epi_rows(const TcParams& p, const float (&acc)[BN / 2], int row0, int col0, bool fold,
+                                         float al, float be) {
+  using Bias16 = typename std::conditional<KIND == KIND_FP16, f16_out, bf16_out>::type;
+  const uint16_t* bias = reinterpret_cast<const uint16_t*>(p.bias);
+  const bool bias_vec = (reinterpret_cast<uintptr_t>(bias) & 3) == 0;
+  const int ce[2] = {0, 0};
+#pragma unroll
+  for (int j = 0; j < BN / 8; j++) {
+    const int col = col0 + 8 * j;
+    float b[2] = {-0.f, -0.f};
+    if (bias != nullptr && col < p.N) {
+      uint32_t h;
+      if (bias_vec && col + 1 < p.N) h = __ldg(reinterpret_cast<const unsigned int*>(bias + col));
+      else h = (uint32_t)__ldg(reinterpret_cast<const unsigned short*>(bias + col)) |
+               (col + 1 < p.N ? (uint32_t)__ldg(reinterpret_cast<const unsigned short*>(bias + col + 1)) << 16 : 0u);
+      b[0] = c16_to_f32<Bias16>(h & 0xFFFFu);
+      b[1] = c16_to_f32<Bias16>(h >> 16);
+    }
+#pragma unroll
+    for (int h = 0; h < 2; h++)
+      store_pair<OutT, float, ACT>(p, row0 + 8 * h, col, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], fold, false, al, be,
+                                   0, ce, 0.f, 0.f, b[0], b[1]);
+  }
+}
+
+// EPI: the bias / activation epilogue (16-bit kinds, single plane, float / bf16_out / f16_out C).  Its kernels never
+// take the K-split tail (launch_tc sets split = 1): the activation must see the complete sum.
 template <int KIND, int BN, int STAGES, typename OutT, class Prod, int A_ROW_BYTES, int AL = LAYOUT_K,
-          int BL = KindTraits<KIND>::B_LAYOUT>
+          int BL = KindTraits<KIND>::B_LAYOUT, bool EPI = false>
 __global__ void __launch_bounds__((TcConfig<KIND, BN, STAGES, Prod, A_ROW_BYTES, AL, BL>::THREADS), 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                const TcParams p) {
   using Cfg = TcConfig<KIND, BN, STAGES, Prod, A_ROW_BYTES, AL, BL>;
   using MMA = typename Cfg::MMA;
   using Acc = typename MMA::Acc;
+  static_assert(!EPI || (KindTraits<KIND>::ELEM == 2 && !Cfg::REGACC &&
+                         (std::is_same<OutT, float>::value || OutBytes<OutT>::V == 2)),
+                "bias / activation epilogue: 16-bit single-plane kinds with fp32 or 16-bit C");
 
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;   // swizzle atoms need 1 KB
@@ -479,23 +531,32 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           }
         }
       }
-#pragma unroll
-      for (int j = 0; j < BN / 8; j++) {
-        const int col = col0 + 8 * j;
-        int ce[2] = {0, 0};
-        if (!std::is_same<OutT, s8_out>::value && p.col_max != nullptr) {
-#pragma unroll
-          for (int e = 0; e < 2; e++)
-            if (col + e < p.N) ce[e] = pow2_exp(__ldg(p.col_max + col + e));
+      if constexpr (EPI) {
+        switch (p.act) {
+          case ACT_RELU: epi_rows<KIND, OutT, ACT_RELU, BN>(p, acc, row0, col0, fold, al, be); break;
+          case ACT_GELU: epi_rows<KIND, OutT, ACT_GELU, BN>(p, acc, row0, col0, fold, al, be); break;
+          case ACT_GELU_TANH: epi_rows<KIND, OutT, ACT_GELU_TANH, BN>(p, acc, row0, col0, fold, al, be); break;
+          default: epi_rows<KIND, OutT, ACT_NONE, BN>(p, acc, row0, col0, fold, al, be); break;
         }
+      } else {
 #pragma unroll
-        for (int h = 0; h < 2; h++) {
-          if constexpr (Cfg::REGACC)
-            store_pair<OutT>(p, row0 + 8 * h, col, sum[4 * j + 2 * h], sum[4 * j + 2 * h + 1], fold, it.part > 0, al, be,
-                             re[h], ce, sc[h], bi[h]);
-          else
-            store_pair<OutT>(p, row0 + 8 * h, col, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], fold, it.part > 0, al, be,
-                             re[h], ce, sc[h], bi[h]);
+        for (int j = 0; j < BN / 8; j++) {
+          const int col = col0 + 8 * j;
+          int ce[2] = {0, 0};
+          if (!std::is_same<OutT, s8_out>::value && p.col_max != nullptr) {
+#pragma unroll
+            for (int e = 0; e < 2; e++)
+              if (col + e < p.N) ce[e] = pow2_exp(__ldg(p.col_max + col + e));
+          }
+#pragma unroll
+          for (int h = 0; h < 2; h++) {
+            if constexpr (Cfg::REGACC)
+              store_pair<OutT>(p, row0 + 8 * h, col, sum[4 * j + 2 * h], sum[4 * j + 2 * h + 1], fold, it.part > 0, al, be,
+                               re[h], ce, sc[h], bi[h]);
+            else
+              store_pair<OutT>(p, row0 + 8 * h, col, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], fold, it.part > 0, al,
+                               be, re[h], ce, sc[h], bi[h]);
+          }
         }
       }
       if (w >= p.full_tiles && p.split > 1) {          // publish this part (the last one re-arms the flag)

@@ -3,6 +3,7 @@
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
+#include <math.h>
 #include <stdint.h>
 
 namespace b200 {
@@ -105,6 +106,30 @@ __device__ __forceinline__ int32_t requant_s8(int32_t acc, float scale, float bi
   r = fminf(fmaxf(r, -128.0f), 127.0f);
   const int32_t q = __float_as_int(__fadd_rn(r, magic)) - 0x4B400000;
   return f != f ? 0 : q;
+}
+
+// Epilogue activations of the 16-bit GEMMs (the B200_ACT_* codes of b200gemm.h), in fp32, shared by the tensor-core
+// and the generic kernel so that both routes give the same bits for the same t.  Every step is an explicit
+// round-to-nearest op, so no FMA contraction can make the two inlined copies differ.
+//   RELU:      t < 0 ? +0 : t (NaN and -0 pass through, as torch.relu does)
+//   GELU:      t * Phi(t) = 0.5 t erfc(-t / sqrt 2): erfc keeps relative accuracy for negative t, where 1 + erf cancels
+//   GELU_TANH: 0.5 t (1 + tanh(sqrt(2 / pi) (t + 0.044715 t^3)))
+// Both GELUs give +inf at +inf, -0 at -inf (the limits of the function) and NaN at NaN.
+enum EpiAct { ACT_NONE = 0, ACT_RELU = 1, ACT_GELU = 2, ACT_GELU_TANH = 3 };
+template <int ACT>
+__device__ __forceinline__ float epi_act(float t) {
+  if constexpr (ACT == ACT_RELU) {
+    return t < 0.f ? 0.f : t;
+  } else if constexpr (ACT == ACT_GELU) {
+    const float g = __fmul_rn(__fmul_rn(0.5f, t), erfcf(__fmul_rn(-0.707106781186547524f, t)));
+    return t == -INFINITY ? -0.f : g;
+  } else if constexpr (ACT == ACT_GELU_TANH) {
+    const float u = __fmul_rn(0.797884560802865356f, __fmaf_rn(__fmul_rn(0.044715f, t), __fmul_rn(t, t), t));
+    const float g = __fmul_rn(__fmul_rn(0.5f, t), __fadd_rn(1.f, tanhf(u)));
+    return t == -INFINITY ? -0.f : g;
+  } else {
+    return t;
+  }
 }
 
 // Register re-balancing between warpgroups (4 aligned warps): data-movement warps give registers back,

@@ -162,7 +162,8 @@ int b200_gemm_f32_ex(int m, int n, int k, float alpha,
  * for fp32 C and one round-to-nearest-even to bf16 / fp16 otherwise.  beta == 0 never reads C (a NaN already in C
  * stays out of the result); alpha == 0 or k == 0 never reads A or B: one element-wise pass C = round_out(beta *
  * float(C)), zeros when beta == 0.  fp16 C rounds to nearest even and overflows to +-inf, as torch's .half() does.
- * fp32 C may take the K-split tail (beta * C is folded by the first K part only); 16-bit C never does.  No workspace.
+ * fp32 C may take the K-split tail (beta * C is folded by the first K part only); 16-bit C never does, and neither does
+ * a call with a bias or an activation (b200_gemm_bf16_epi / _f16_epi, below).  No workspace.
  * Kernels: "tc_f16_128x{256,192,128}" (fp32 C) and "tc_f16_of16_128x..." (fp16 C), with the layout infix _nt / _tn
  * / _tt as for bf16; operands that TMA cannot read take "generic_f16_64x64" (CUDA cores, sequential k). */
 int b200_gemm_bf16_ex(int op_a, int op_b, int m, int n, int k, float alpha,
@@ -171,6 +172,44 @@ int b200_gemm_bf16_ex(int op_a, int op_b, int m, int n, int k, float alpha,
 int b200_gemm_f16_ex(int op_a, int op_b, int m, int n, int k, float alpha,
                      const uint16_t* dA, int lda, const uint16_t* dB, int ldb, float beta,
                      void* dC, int ldc, int out_type, void* stream);
+
+/* 16-bit operands with a bias vector and an activation fused into the epilogue (cuBLASLt's CUBLASLT_EPILOGUE_BIAS,
+ * _RELU_BIAS, _GELU_BIAS): C = round_out(act(alpha * op(A)*op(B) + beta * C + bias)), what a PyTorch
+ * act(F.linear(x, W, b)) computes, in one launch.  Arguments as b200_gemm_bf16_ex / b200_gemm_f16_ex, plus:
+ *   dBias: n contiguous elements of the operand type (bf16 bits for _bf16_epi, fp16 bits for _f16_epi), one per column
+ *          of C, at any 2-byte-aligned device address; NULL = no bias.
+ *   act:   one of the B200_ACT_* codes below; any other value is B200_ERR_BAD_ARG.
+ * Per element, in fp32, with x the fp32 accumulator:
+ *   1. t = fma(beta, float(C), alpha * x), the _ex rule (beta == 0 never reads C);
+ *   2. t = t + float(bias[j]), one round-to-nearest add, skipped when dBias is NULL;
+ *   3. y = act(t);
+ *   4. C = round_out(y): the identity for fp32 C, one round-to-nearest-even to bf16 / fp16 otherwise (fp16 overflows
+ *      to +-inf).
+ * B200_ACT_RELU is t < 0 ? +0 : t (NaN stays NaN, -0 stays -0, as torch.relu).  The two GELUs are evaluated in fp32
+ * with CUDA's erfcf / tanhf (GELU as 0.5 t erfc(-t / sqrt 2), which keeps relative accuracy for negative t); at the
+ * ends of the range they give the limits of the function: +inf -> +inf, -inf -> -0, NaN -> NaN (torch on the CPU
+ * returns NaN for gelu(+-inf)).  The tensor-core and the generic kernel share one activation function, so both routes
+ * give the same bits for the same t.
+ * dBias == NULL with B200_ACT_NONE is the _ex call exactly: same kernel, kernel name, launches and bits.  The other
+ * argument rules of _ex apply (out_type pairing, ops, minimum ld, null pointers); m == 0 or n == 0 is a no-op, a NULL
+ * bias included.  alpha == 0 or k == 0 never reads A or B: one element-wise pass stores round_out(act(beta * float(C) +
+ * bias[j])), where beta == 0 contributes +0 and does not read C (so the result is act(+0 + bias[j]) down every row).
+ * A call with a bias or an activation never takes the K-split tail, fp32 C included: the activation is not linear and
+ * must see the complete sum.  Every layout is one launch on the tensor cores, tile widths 256 / 192 / 128 as for _ex;
+ * kernels are named with "_epi" after the C-type part ("tc_bf16_epi_128x256", "tc_bf16_obf16_epi_nt_128x192",
+ * "tc_f16_epi_tn_128x128", "tc_f16_of16_epi_tt_128x256").  Operands that TMA cannot read take the generic kernel
+ * ("generic_bf16_64x64" / "generic_f16_64x64", one launch).  No workspace. */
+#define B200_ACT_NONE      0   /* bias only (or nothing: then this is the _ex call)                                 */
+#define B200_ACT_RELU      1
+#define B200_ACT_GELU      2   /* x * Phi(x), the erf form (torch's default nn.GELU)                                */
+#define B200_ACT_GELU_TANH 3   /* 0.5 x (1 + tanh(sqrt(2/pi) (x + 0.044715 x^3))): cuBLASLt's GELU, torch's
+                                  approximate='tanh'                                                                 */
+int b200_gemm_bf16_epi(int op_a, int op_b, int m, int n, int k, float alpha,
+                       const uint16_t* dA, int lda, const uint16_t* dB, int ldb, float beta,
+                       void* dC, int ldc, int out_type, const uint16_t* dBias, int act, void* stream);
+int b200_gemm_f16_epi(int op_a, int op_b, int m, int n, int k, float alpha,
+                      const uint16_t* dA, int lda, const uint16_t* dB, int ldb, float beta,
+                      void* dC, int ldc, int out_type, const uint16_t* dBias, int act, void* stream);
 
 /* fp32 with HOST pointers and the CPU harness contract C += A*B
  * (aarch64/MMult0.cpp:11-19; harness zeroes C first, aarch64/test_MMult.cpp:107).
