@@ -222,7 +222,7 @@ def gemm(A, B, out=None, *, alpha=1.0, beta=0.0, bias=None, activation=None, mod
          stream=None):
     """C = alpha * A @ B + beta * C for fp32 (any precision mode), bf16 (fp32 or bf16 C), fp16 (fp32 or fp16 C) and
     int8 (int32 C) CUDA tensors.  Each operand may be row-major or the transpose of a row-major matrix (x @ W.t()
-    passes W as stored): it is read in place (b200_gemm_f32_op / _bf16_op / _bf16_ex / _f16_ex / _s8s32_op), never
+    passes W as stored): it is read in place (b200_gemm_f32_op / _bf16_epi / _f16_epi / _s8s32_op), never
     copied.  out must be row-major; it is read only when beta != 0.  int8 takes alpha = 1, beta = 0 only.
 
     bf16 and fp16 also take a bias (1-D, contiguous, n elements of the operands' dtype) and an activation (None,
@@ -259,20 +259,13 @@ def gemm(A, B, out=None, *, alpha=1.0, beta=0.0, bias=None, activation=None, mod
     if n > 1:
         assert out.stride(1) == 1, "out must be row-major"
     st = _stream_ptr(stream)
-    if epi:
+    if A.dtype == torch.float32:
+        _check(lib.b200_gemm_f32_op(op_a, op_b, m, n, k, alpha, A.data_ptr(), lda, B.data_ptr(), ldb, beta, out.data_ptr(),
+                                    _ld(out), mode, st))
+    elif A.dtype in (torch.bfloat16, torch.float16):
         fn, ot = (lib.b200_gemm_bf16_epi, OUT_BF16) if A.dtype == torch.bfloat16 else (lib.b200_gemm_f16_epi, OUT_F16)
         _check(fn(op_a, op_b, m, n, k, alpha, A.data_ptr(), lda, B.data_ptr(), ldb, beta, out.data_ptr(), _ld(out),
                   OUT_F32 if cdt == torch.float32 else ot, bias.data_ptr() if bias is not None else None, act, st))
-    elif A.dtype == torch.float32:
-        _check(lib.b200_gemm_f32_op(op_a, op_b, m, n, k, alpha, A.data_ptr(), lda, B.data_ptr(), ldb, beta, out.data_ptr(),
-                                    _ld(out), mode, st))
-    elif A.dtype == torch.bfloat16 and alpha == 1.0 and beta == 0.0:
-        _check(lib.b200_gemm_bf16_op(op_a, op_b, m, n, k, A.data_ptr(), lda, B.data_ptr(), ldb, out.data_ptr(), _ld(out),
-                                     OUT_F32 if cdt == torch.float32 else OUT_BF16, st))
-    elif A.dtype in (torch.bfloat16, torch.float16):
-        fn, ot = (lib.b200_gemm_bf16_ex, OUT_BF16) if A.dtype == torch.bfloat16 else (lib.b200_gemm_f16_ex, OUT_F16)
-        _check(fn(op_a, op_b, m, n, k, alpha, A.data_ptr(), lda, B.data_ptr(), ldb, beta, out.data_ptr(), _ld(out),
-                  OUT_F32 if cdt == torch.float32 else ot, st))
     else:
         _check(lib.b200_gemm_s8s32_op(op_a, op_b, m, n, k, A.data_ptr(), lda, B.data_ptr(), ldb, out.data_ptr(), _ld(out), st))
     return out

@@ -92,7 +92,7 @@ void rowpanel_free(b200_rowpanel* rp) {
   if (rp->hA) cudaFree(rp->hA);
   if (rp->hB) cudaFree(rp->hB);
   if (rp->hC) cudaFree(rp->hC);
-  if (rp->hpb) { pack_release(rp->hpb); delete rp->hpb; }
+  pack_destroy(rp->hpb);
   for (int j = 0; j < kMaxSlices; j++) { if (rp->ev_b[j]) cudaEventDestroy(rp->ev_b[j]); if (rp->ev_hb[j]) cudaEventDestroy(rp->ev_hb[j]); }
   for (auto& e : rp->tr) if (e) cudaEventDestroy(e);
   for (int j = 0; j < 8; j++) { if (rp->ev_in[j]) cudaEventDestroy(rp->ev_in[j]); if (rp->ev_out[j]) cudaEventDestroy(rp->ev_out[j]); }
@@ -209,13 +209,13 @@ int b200_rowpanel_create(b200_rowpanel** out, void* nccl_comm, int m_local_max, 
   RP_TRY(cudaEventCreateWithFlags(&rp->ev_done, cudaEventDisableTiming));
   for (int j = 0; j < rp->nslices; j++) RP_TRY(cudaEventCreateWithFlags(&rp->ev_b[j], cudaEventDisableTiming));
   if (rp->mode == B200_F32_F16X2) {
-    rp->a_pitch = f16_pitch(k);
-    rp->b_pitch = f16_pitch(n);
+    rp->a_pitch = plane_pitch(k);
+    rp->b_pitch = plane_pitch(n);
     RP_TRY(cudaMalloc(&rp->a_planes, (size_t)2 * m_local_max * rp->a_pitch * 2));
     RP_TRY(cudaMalloc(&rp->a_max, (size_t)m_local_max * 4));
     RP_TRY(cudaMalloc(&rp->b_max, (size_t)rp->nslices * n * 4));
     for (int j = 0; j < rp->nslices; j++) {
-      rp->b_rows[j] = f16_b_rows(rp->k0[j + 1] - rp->k0[j]);
+      rp->b_rows[j] = b_plane_rows(rp->k0[j + 1] - rp->k0[j]);
       RP_TRY(cudaMalloc(&rp->b_planes[j], (size_t)2 * rp->b_rows[j] * rp->b_pitch * 2));
     }
   }
@@ -286,11 +286,10 @@ int b200_gemm_f32_rowpanel(b200_rowpanel* rp, int m_local, int n, int k, const f
       rp_mark(rp, 8 + 6 * j + 3, st);
       const F16Operand oa{rp->a_planes + kk0, rp->a_pitch, m_local, rp->a_max};
       const F16Operand ob{rp->b_planes[j], rp->b_pitch, rp->b_rows[j], cmax};
-      const bool corun = rp->world > 1 && j + 1 < rp->nslices;      // a later slice is still being broadcast
-      t_sm_reserve = corun ? rp->reserve_sms : 0;
-      rc = gemm_f16x2_core(m_local, n, kr, oa, ob, dC, ldc, j > 0 ? 1 : 0, st);
-      t_sm_reserve = 0;
-      if (rc) return rc;
+      Call c{st};
+      c.acc = j > 0;
+      c.sm_reserve = rp->world > 1 && j + 1 < rp->nslices ? rp->reserve_sms : 0;   // a later slice is still being broadcast
+      if ((rc = gemm_f16x2_core(B200_OP_N, B200_OP_N, m_local, n, kr, oa, ob, dC, ldc, c))) return rc;
       rp_mark(rp, 8 + 6 * j + 4, st);
     }
     return 0;
@@ -298,11 +297,9 @@ int b200_gemm_f32_rowpanel(b200_rowpanel* rp, int m_local, int n, int k, const f
   for (int j = 0; j < rp->nslices; j++) {
     const int kk0 = rp->k0[j], kr = rp->k0[j + 1] - kk0;
     RP_CK(cudaStreamWaitEvent(st, rp->ev_b[j], 0));
-    const bool corun = rp->world > 1 && j + 1 < rp->nslices;
-    t_sm_reserve = corun ? rp->reserve_sms : 0;
-    rc = gemm_f32_impl(m_local, n, kr, dA + kk0, lda, dB + (size_t)kk0 * ldb, ldb, dC, ldc, rp->mode, j > 0 ? 1 : 0, st);
-    t_sm_reserve = 0;
-    if (rc) return rc;
+    const int reserve = rp->world > 1 && j + 1 < rp->nslices ? rp->reserve_sms : 0;
+    if ((rc = gemm_f32(B200_OP_N, B200_OP_N, m_local, n, kr, 1.f, dA + kk0, lda, dB + (size_t)kk0 * ldb, ldb, j > 0 ? 1.f : 0.f,
+                       dC, ldc, rp->mode, st, reserve))) return rc;
   }
   return 0;
 }
@@ -354,7 +351,7 @@ int b200_gemm_f32_rowpanel_host(b200_rowpanel* rp, int m_local, int n, int k, co
     RP_CK(cudaMemcpy2DAsync(dCi, (size_t)n * 4, C + (size_t)r0 * ldc, (size_t)ldc * 4, (size_t)n * 4, rows, cudaMemcpyHostToDevice, rp->h2d));
     RP_CK(cudaEventRecord(rp->ev_in[nb], rp->h2d));
     RP_CK(cudaStreamWaitEvent(rp->comp, rp->ev_in[nb], 0));
-    if ((rc = gemm_f32_impl(rows, n, k, dAi, k, rp->hB, n, dCi, n, rp->mode, /*accumulate=*/1, rp->comp))) return rc;
+    if ((rc = gemm_f32(B200_OP_N, B200_OP_N, rows, n, k, 1.f, dAi, k, rp->hB, n, 1.f, dCi, n, rp->mode, rp->comp))) return rc;
     RP_CK(cudaEventRecord(rp->ev_out[nb], rp->comp));
     RP_CK(cudaStreamWaitEvent(rp->d2h, rp->ev_out[nb], 0));
     RP_CK(cudaMemcpy2DAsync(C + (size_t)r0 * ldc, (size_t)ldc * 4, dCi, (size_t)n * 4, (size_t)n * 4, rows, cudaMemcpyDeviceToHost, rp->d2h));

@@ -116,7 +116,10 @@ void b200_gemm_set_default_f32_mode(int mode);
 /* The split-precision fp32 modes keep the planes of A and B in a per-device, grow-only workspace.  Its first
  * use and every growth allocate (and synchronise the device); steady-state calls never do.  Reserve it up front
  * — b200_gemm_reserve_workspace(b200_gemm_workspace_bytes(m, n, k, mode)) on the device that will run the
- * calls — to keep even the first call allocation-free (e.g. ahead of CUDA-graph capture).  State is per device:
+ * calls — to keep even the first call allocation-free (e.g. ahead of CUDA-graph capture).
+ * b200_gemm_workspace_bytes(m, n, k, mode) is b200_gemm_workspace_bytes_op(B200_OP_N, B200_OP_N, m, n, k, mode):
+ * for an explicit mode exactly what its route reserves, for AUTO the largest of the routes AUTO may take at this
+ * size (plain or with a general alpha / beta).  State is per device:
  * one process may drive several GPUs (make the device current on the calling thread); calls on different
  * streams of one device are serialised on the workspace by an event, not by the host.
  * The same workspace holds B^T for B200_F32_TF32 (counted by b200_gemm_workspace_bytes) and for the int8 entry
@@ -361,8 +364,9 @@ int  b200_rowpanel_create(b200_rowpanel** out, void* nccl_comm, int m_local_max,
                           int precision_mode, const int* slice_rows, int n_slices);
 void b200_rowpanel_destroy(b200_rowpanel* plan);
 /* Tuning.  While a later K-slice is still being broadcast, the GEMM of the current slice shares the GPU with NCCL's
- * copy kernels; those GEMMs therefore draw their tiles from an atomic counter (dynamic schedule: a CTA that gets its
- * SM late draws fewer tiles) and may leave `sms` SMs unused (default 0).  sms = -1 switches the dynamic schedule off. */
+ * copy kernels.  Their tensor-core kernels then launch `sms` fewer CTAs than the device has SMs (default 0; ignored
+ * unless more than 2 SMs stay in use), and the tiles are handed out round robin over the smaller grid.  sms = -1 is accepted and
+ * changes nothing. */
 int  b200_rowpanel_set_reserve_sms(b200_rowpanel* plan, int sms);
 /* Diagnostics: with tracing on, timing events bracket every stage of a call; the dump synchronises the device and
  * writes, in ms after the call began: A split done, then per K-slice {broadcast begin, broadcast end, slice visible

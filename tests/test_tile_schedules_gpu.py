@@ -39,8 +39,8 @@ TOL_STRICT = 2e-6            # strict / generic fp32 under a general alpha, beta
 #                                                     split = min(4, sms // rem, num_kb // 8), 1 when
 #                                                     rem * 8 epilogue warps exceed a 1024-int flag slot;
 #                                                     group_m = group rows / 128, default 2048 rows)
-#   launch_ffma(_fat)  -> ffma_halves()              (half tiles when the last round is at most half full)
-#   gemm_f32_impl      -> ffma_fat()                 (the fat kernel from 96 of its 128x256 tiles)
+#   launch_ffma        -> ffma_halves()              (half tiles when the last round is at most half full)
+#   strict_tma         -> ffma_fat()                 (the fat kernel from 96 of its 128x256 tiles)
 # BK is one 128-byte swizzled row of K per stage (64-byte rows for the split fp32 modes), TcConfig in
 # csrc/gemm_tc.cuh.  If a heuristic there changes, update it here: the generators below then still aim
 # at every path, and the model assertions of each GPU case fail instead of quietly losing coverage.

@@ -88,6 +88,23 @@ def test_workspace_bytes_op_counts_transposes_and_planes(gemm):
     assert ws(OP_N, OP_T, m, n, k, F32_MODES["f16x2"]) == r1k(r1k(r1k(a) + b) + 4 * m) + 4 * n
 
 
+def test_workspace_bytes_nn_is_what_the_route_reserves(gemm):
+    """NN: an explicit mode gives exactly what its route reserves, AUTO the largest of the routes it may take."""
+    ws = gemm.lib.b200_gemm_workspace_bytes
+    r1k = lambda b: -(-b // 1024) * 1024
+    p8, r32 = (lambda c: -(-c // 8) * 8), (lambda r: -(-r // 32) * 32)
+    m, n, k = 200, 136, 264
+    assert ws(m, n, k, F32_MODES["strict"]) == 0
+    assert ws(m, n, k, F32_MODES["tf32"]) == n * -(-k // 4) * 4 * 4                     # B^T, 16-byte pitch
+    for mode, np_ in (("bf16x3", 3), ("bf16x2", 2)):
+        assert ws(m, n, k, F32_MODES[mode]) == r1k(np_ * m * p8(k) * 2) + np_ * r32(k) * p8(n) * 2
+    # F16X2: planes of A and B, then A's row maxima
+    assert ws(m, n, k, F32_MODES["f16x2"]) == r1k(r1k(2 * m * p8(k) * 2) + 2 * r32(k) * p8(n) * 2) + 4 * m
+    # AUTO at m*n*k = 1.28e9 with the default F16X2 (or BF16X3) takes BF16X3, whose planes hold 960,000,000 bytes
+    if gemm.lib.b200_gemm_default_f32_mode() in (F32_MODES["f16x2"], F32_MODES["bf16x3"]):
+        assert ws(16, 16, 5_000_000, F32_MODES["auto"]) >= 960_000_000
+
+
 # ==== the Python layout resolver (no GPU) =====================================================================
 def test_operand_layout_resolver(gemm):
     lay = gemm.operand_layout
