@@ -29,14 +29,14 @@ EXPORTS = [
     "b200_mxf4_quantize_a", "b200_mxf4_quantize_b", "b200_gemm_mxf4", "b200_gemm_f32_host", "b200_gemm_bf16", "b200_gemm_f16", "b200_gemm_s8s32",
     "b200_gemm_s8s32_host", "b200_gemm_s8s8_requant", "b200_gemm_f32_pack_b", "b200_gemm_f32_packed",
     "b200_gemm_f32_pack_free", "b200_gemm_f32_op", "b200_gemm_bf16_op", "b200_gemm_bf16_ex", "b200_gemm_f16_ex",
-    "b200_gemm_bf16_epi", "b200_gemm_f16_epi",
+    "b200_gemm_bf16_epi", "b200_gemm_f16_epi", "b200_gemm_bf16_batched", "b200_gemm_f16_batched",
     "b200_gemm_s8s32_op", "b200_gemm_workspace_bytes_op",
     "b200_nccl_load", "b200_nccl_last_error", "b200_comm_unique_id", "b200_comm_init_rank",
     "b200_comm_destroy", "b200_rowpanel_create", "b200_rowpanel_destroy", "b200_rowpanel_slices", "b200_rowpanel_set_reserve_sms", "b200_rowpanel_trace", "b200_rowpanel_trace_dump", "b200_gemm_f32_rowpanel",
     "b200_gemm_f32_rowpanel_host", "b200_gemm_f32_pack_a", "b200_gemm_f32_packed_ab", "b200_gemm_f32_pack_free_a",
     "b200_convert_f32_to_bf16", "b200_gemm_debug_set_b_desc", "b200_gemm_debug_set_bn",
     "b200_gemm_debug_set_split_chunk", "b200_gemm_debug_kernel_timing", "b200_gemm_debug_kernel_time_ms",
-    "b200_gemm_debug_set_cta_group", "b200_gemm_debug_set_split_tail", "b200_gemm_debug_set_group_rows",
+    "b200_gemm_debug_set_cta_group", "b200_gemm_debug_set_split_tail", "b200_gemm_debug_last_schedule", "b200_gemm_debug_set_group_rows",
     "b200_gemm_debug_set_ffma_variant", "b200_gemm_debug_set_epilogue", "b200_gemm_debug_set_pdl", "b200_gemm_debug_set_dynamic_sched",
 ]
 
@@ -83,6 +83,11 @@ lib.b200_gemm_bf16_ex.argtypes = [_i, _i, _i, _i, _i, C.c_float, _vp, _i, _vp, _
 lib.b200_gemm_f16_ex.argtypes = [_i, _i, _i, _i, _i, C.c_float, _vp, _i, _vp, _i, C.c_float, _vp, _i, _i, _vp]
 lib.b200_gemm_bf16_epi.argtypes = [_i, _i, _i, _i, _i, C.c_float, _vp, _i, _vp, _i, C.c_float, _vp, _i, _i, _vp, _i, _vp]
 lib.b200_gemm_f16_epi.argtypes = [_i, _i, _i, _i, _i, C.c_float, _vp, _i, _vp, _i, C.c_float, _vp, _i, _i, _vp, _i, _vp]
+_ll = C.c_longlong
+lib.b200_gemm_bf16_batched.argtypes = [_i, _i, _i, _i, _i, C.c_float, _vp, _i, _ll, _vp, _i, _ll, C.c_float, _vp, _i, _ll,
+                                       _i, _i, _vp]
+lib.b200_gemm_f16_batched.argtypes = [_i, _i, _i, _i, _i, C.c_float, _vp, _i, _ll, _vp, _i, _ll, C.c_float, _vp, _i, _ll,
+                                      _i, _i, _vp]
 lib.b200_gemm_s8s32_op.argtypes = [_i, _i, _i, _i, _i, _vp, _i, _vp, _i, _vp, _i, _vp]
 lib.b200_gemm_workspace_bytes_op.argtypes = [_i, _i, _i, _i, _i, _i]
 lib.b200_gemm_workspace_bytes_op.restype = C.c_size_t
@@ -118,6 +123,8 @@ lib.b200_gemm_debug_set_split_chunk.argtypes = [_i, _i]
 lib.b200_gemm_debug_kernel_timing.argtypes = [_i]
 lib.b200_gemm_debug_set_cta_group.argtypes = [_i]
 lib.b200_gemm_debug_set_split_tail.argtypes = [_i]
+lib.b200_gemm_debug_last_schedule.argtypes = [C.POINTER(_i)] * 4
+lib.b200_gemm_debug_last_schedule.restype = None
 lib.b200_gemm_debug_set_pdl.argtypes = [_i]
 lib.b200_gemm_debug_set_dynamic_sched.argtypes = [_i]
 lib.b200_gemm_debug_kernel_time_ms.argtypes = [C.POINTER(C.c_double)]
@@ -201,6 +208,54 @@ def operand_layout(shape, strides):
                      "transpose of a row-major matrix")
 
 
+def batched_operand_layout(shape, strides):
+    """(op, ld, batch stride) under which the C ABI's batched entry points read a 3-D operand (batch, rows, cols) in
+    place: the last two dimensions resolve as operand_layout does, the batch stride is stride(0) (0 for an expand()ed
+    operand, which is broadcast over the batch; 0 as well for a batch of one, whose stride is never used)."""
+    op, ld = operand_layout(tuple(shape[1:]), tuple(strides[1:]))
+    return op, ld, (strides[0] if shape[0] > 1 else 0)
+
+
+def _gemm_batched(A, B, out, alpha, beta, bias, activation, out_dtype, stream):
+    """gemm() on 3-D operands: C[b] = alpha * A[b] @ B[b] + beta * C[b] in one call (b200_gemm_*_batched)."""
+    import torch
+    if A.dtype != B.dtype:
+        raise TypeError(f"operands of different dtypes: {A.dtype} and {B.dtype}")
+    if A.dtype not in (torch.bfloat16, torch.float16):
+        raise TypeError(f"batched (3-D) operands must be bf16 or fp16, not {A.dtype}")
+    if bias is not None or activation is not None:
+        raise ValueError("the batched GEMM has no bias / activation epilogue")
+    if A.dim() != 3 or B.dim() != 3:
+        raise ValueError(f"batched operands must both be 3-D (pass an expand()ed view to broadcast one), not "
+                         f"{A.dim()}-D and {B.dim()}-D")
+    batch, m, k = A.shape
+    batch_b, k2, n = B.shape
+    if batch_b != batch:
+        raise ValueError(f"batch sizes differ: {batch} and {batch_b}")
+    assert k == k2, (A.shape, B.shape)
+    op_a, lda, sa = batched_operand_layout(tuple(A.shape), A.stride())
+    op_b, ldb, sb = batched_operand_layout(tuple(B.shape), B.stride())
+    cdt = out_dtype or (out.dtype if out is not None else torch.float32)
+    assert cdt in (torch.float32, A.dtype), f"{A.dtype} operands write float32 or {A.dtype} C, not {cdt}"
+    if out is None:
+        assert beta == 0.0, "beta != 0 reads C: pass out"
+        out = torch.empty((batch, m, n), dtype=cdt, device=A.device)
+    assert out.dtype == cdt
+    if out.dim() != 3 or tuple(out.shape) != (batch, m, n):
+        raise ValueError(f"out must have shape {(batch, m, n)}, not {tuple(out.shape)}")
+    if batch == 0:
+        return out
+    if (n > 1 and out.stride(2) != 1) or (m > 1 and out.stride(1) < n):
+        raise ValueError("out must be row-major in its last two dimensions")
+    ldc = _ld(out[0])
+    sc = out.stride(0) if batch > 1 else 0
+    assert A.is_cuda and B.is_cuda and out.is_cuda
+    fn, ot = (lib.b200_gemm_bf16_batched, OUT_BF16) if A.dtype == torch.bfloat16 else (lib.b200_gemm_f16_batched, OUT_F16)
+    _check(fn(op_a, op_b, m, n, k, alpha, A.data_ptr(), lda, sa, B.data_ptr(), ldb, sb, beta, out.data_ptr(), ldc, sc,
+              batch, OUT_F32 if cdt == torch.float32 else ot, _stream_ptr(stream)))
+    return out
+
+
 def _epilogue_args(A, B, bias, activation):
     """Checks a bias / activation request of gemm() (before anything touches the device); returns the ACT_* code."""
     import torch
@@ -229,8 +284,17 @@ def gemm(A, B, out=None, *, alpha=1.0, beta=0.0, bias=None, activation=None, mod
     "relu", "gelu" or "gelu_tanh") fused into the epilogue (b200_gemm_bf16_epi / _f16_epi):
     C = act(alpha * A @ B + beta * C + bias), so gemm(x, W.t(), bias=b, activation="gelu") is
     F.gelu(F.linear(x, W, b)) in one launch.  Other operand dtypes refuse them with TypeError; a bias of another dtype
-    or length is a ValueError."""
+    or length is a ValueError.
+
+    3-D bf16 or fp16 operands (batch, rows, cols) with equal batch sizes are a strided batch, torch.bmm / baddbmm:
+    out[b] = alpha * A[b] @ B[b] + beta * out[b] in one launch (b200_gemm_bf16_batched / _f16_batched).  The last two
+    dimensions of each operand resolve as for 2-D operands and its batch stride is stride(0), so k.transpose(1, 2) and
+    expand()ed operands (stride 0, broadcast) are read in place.  out is 3-D and row-major in its last two dimensions.
+    3-D fp32 or int8 operands are a TypeError; a bias, an activation, unequal batch sizes or another out is a
+    ValueError."""
     import torch
+    if A.dim() == 3 or B.dim() == 3:
+        return _gemm_batched(A, B, out, alpha, beta, bias, activation, out_dtype, stream)
     epi = bias is not None or activation is not None
     act = _epilogue_args(A, B, bias, activation) if epi else ACT_NONE
     assert A.dim() == 2 and B.dim() == 2 and A.is_cuda and B.is_cuda

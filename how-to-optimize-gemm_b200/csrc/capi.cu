@@ -48,6 +48,8 @@ struct KernelTimer {
 } g_ktimer;
 std::atomic<int> g_default_f32_mode{-1};
 thread_local const char* t_last_kernel = "none";
+struct Schedule { int tiles = 0, split = 0, full_tiles = 0, ctas = 0; };
+thread_local Schedule t_last_schedule;     // of the last tensor-core launch (b200_gemm_debug_last_schedule)
 int g_dbg_b_lbo = 0, g_dbg_b_sbo = 0;
 
 // What one call asks of every launch it makes, built once by its entry point and passed down by reference.
@@ -186,9 +188,10 @@ int ensure_smem_attr(Kern kern, int bytes) {
 // back to back on the same operands (cuda/test_MMult.cpp:100-103).
 struct MapKey {
   const void* ptr; int dtype; unsigned long long d0, d1, ld_bytes; unsigned b0, b1; int swz; int dev;
+  unsigned long long d2, d2_bytes;     // 3-D maps (strided batch): entries and their stride; 0, 0 for a 2-D map
   bool operator==(const MapKey& o) const {
     return ptr == o.ptr && dtype == o.dtype && d0 == o.d0 && d1 == o.d1 && ld_bytes == o.ld_bytes &&
-           b0 == o.b0 && b1 == o.b1 && swz == o.swz && dev == o.dev;
+           b0 == o.b0 && b1 == o.b1 && swz == o.swz && dev == o.dev && d2 == o.d2 && d2_bytes == o.d2_bytes;
   }
 };
 struct MapEntry { MapKey key; CUtensorMap map; };
@@ -196,20 +199,23 @@ std::vector<MapEntry> g_maps;
 size_t g_map_next = 0;
 constexpr size_t kMapCache = 64;
 
-// 2-D row-major tensor: dim0 (inner, contiguous) x dim1 rows with pitch ld_bytes.
+// 2-D row-major tensor: dim0 (inner, contiguous) x dim1 rows with pitch ld_bytes.  entries > 0: a 3-D tensor of that
+// many such matrices, entry_bytes apart, read one entry per box (box extent 1), so that the zero fill past the rows and
+// the inner extent stays inside each entry.
 int get_map(CUtensorMap* out, const void* ptr, CUtensorMapDataType dt, int elem_bytes,
             unsigned long long inner, unsigned long long rows, unsigned long long ld_bytes,
-            unsigned box_inner, unsigned box_rows, int swizzle /*0 none, 1 = 128B, 2 = 128B atom 32B, 3 = 64B*/) {
-  MapKey key{ptr, (int)dt, inner, rows, ld_bytes, box_inner, box_rows, swizzle, t_ctx->dev};
+            unsigned box_inner, unsigned box_rows, int swizzle /*0 none, 1 = 128B, 2 = 128B atom 32B, 3 = 64B*/,
+            unsigned long long entries = 0, unsigned long long entry_bytes = 0) {
+  MapKey key{ptr, (int)dt, inner, rows, ld_bytes, box_inner, box_rows, swizzle, t_ctx->dev, entries, entry_bytes};
   std::lock_guard<std::mutex> lk(g_mu);
   for (auto& e : g_maps)
     if (e.key == key) { *out = e.map; return 0; }
-  cuuint64_t dims[2] = {inner, rows};
-  cuuint64_t strides[1] = {ld_bytes};
-  cuuint32_t box[2] = {box_inner, box_rows};
-  cuuint32_t estr[2] = {1, 1};
+  cuuint64_t dims[3] = {inner, rows, entries};
+  cuuint64_t strides[2] = {ld_bytes, entry_bytes};
+  cuuint32_t box[3] = {box_inner, box_rows, 1};
+  cuuint32_t estr[3] = {1, 1, 1};
   CUtensorMap m;
-  CUresult r = g_encode(&m, dt, 2, const_cast<void*>(ptr), dims, strides, box, estr,
+  CUresult r = g_encode(&m, dt, entries ? 3 : 2, const_cast<void*>(ptr), dims, strides, box, estr,
                         CU_TENSOR_MAP_INTERLEAVE_NONE,
                         swizzle == 1 ? CU_TENSOR_MAP_SWIZZLE_128B
                         : swizzle == 2 ? CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B
@@ -314,12 +320,15 @@ int g_ffma_halves = 1;        // strict kernel: split the tail round into half t
 // Stacked planes (split modes) lie along the rows, plane p at row p * a_plane_rows / p * b_plane_rows.  tf32 and
 // int8 take K-major A and B only (launch_tc_kmajor builds them).
 // EPI: the bias / activation kernel (c.bias / c.act), which never takes the K-split tail.
+// BATCHED: the strided-batched kernel over *bat (16-bit kinds, single plane): A and B as 3-D tensor maps, the work of
+// every entry in one launch, and the K-split tail (fp32 C) on the last partial round of the whole batch.
+struct Batch { int count; long long sa, sb, sc; };    // entries; strides in elements (0 broadcasts A or B)
 template <int KIND, int BN, int STAGES, typename OutT, class Prod = ProdSingle, int A_ROW_BYTES = 128, int AL = LAYOUT_K,
-          int BL = KindTraits<KIND>::B_LAYOUT, bool EPI = false>
+          int BL = KindTraits<KIND>::B_LAYOUT, bool EPI = false, bool BATCHED = false>
 int launch_tc(int m, int n, int k, const void* A, long long lda, int a_rows_total, int a_plane_rows,
               const void* B, long long ldb, int b_rows_total, int b_plane_rows, void* C, int ldc,
               const char* name, const Call& c, int chunk_k = 0, const float* row_max = nullptr,
-              const float* col_max = nullptr) {
+              const float* col_max = nullptr, const Batch* bat = nullptr) {
   using Cfg = TcConfig<KIND, BN, STAGES, Prod, A_ROW_BYTES, AL, BL>;
   using T = KindTraits<KIND>;
   constexpr CUtensorMapDataType dt = KIND == KIND_F16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
@@ -328,16 +337,26 @@ int launch_tc(int m, int n, int k, const void* A, long long lda, int a_rows_tota
                                                        : CU_TENSOR_MAP_DATA_TYPE_UINT8;
   CUtensorMap tmA, tmB;
   constexpr int kswz = A_ROW_BYTES == 128 ? 1 : 3;          // K-major rows: SWIZZLE_128B or _64B
+  // 3-D maps: a broadcast operand is one entry (its entry stride is then any legal value: the matrix's own extent)
+  unsigned long long ea = 0, eab = 0, eb = 0, ebb = 0;
+  if constexpr (BATCHED) {
+    const unsigned long long abytes = (unsigned long long)lda * T::ELEM, bbytes = (unsigned long long)ldb * T::ELEM;
+    ea = bat->sa ? bat->count : 1; eab = bat->sa ? (unsigned long long)bat->sa * T::ELEM : a_rows_total * abytes;
+    eb = bat->sb ? bat->count : 1; ebb = bat->sb ? (unsigned long long)bat->sb * T::ELEM : b_rows_total * bbytes;
+  }
   int rc;
   if constexpr (Cfg::A_MN)
-    rc = get_map(&tmA, A, dt, T::ELEM, m, a_rows_total, (unsigned long long)lda * T::ELEM, Cfg::MN_BOX_COLS, Cfg::BK, 1);
+    rc = get_map(&tmA, A, dt, T::ELEM, m, a_rows_total, (unsigned long long)lda * T::ELEM, Cfg::MN_BOX_COLS, Cfg::BK, 1, ea,
+                 eab);
   else
-    rc = get_map(&tmA, A, dt, T::ELEM, k, a_rows_total, (unsigned long long)lda * T::ELEM, Cfg::BK, Cfg::BM, kswz);
+    rc = get_map(&tmA, A, dt, T::ELEM, k, a_rows_total, (unsigned long long)lda * T::ELEM, Cfg::BK, Cfg::BM, kswz, ea, eab);
   if (rc) return rc;
   if constexpr (!Cfg::B_MN)
-    rc = get_map(&tmB, B, dt, T::ELEM, k, b_rows_total, (unsigned long long)ldb * T::ELEM, Cfg::BK, Cfg::B_BOX_ROWS, kswz);
+    rc = get_map(&tmB, B, dt, T::ELEM, k, b_rows_total, (unsigned long long)ldb * T::ELEM, Cfg::BK, Cfg::B_BOX_ROWS, kswz,
+                 eb, ebb);
   else
-    rc = get_map(&tmB, B, dt, T::ELEM, n, b_rows_total, (unsigned long long)ldb * T::ELEM, Cfg::B_BOX_COLS, Cfg::BK, 1);
+    rc = get_map(&tmB, B, dt, T::ELEM, n, b_rows_total, (unsigned long long)ldb * T::ELEM, Cfg::B_BOX_COLS, Cfg::BK, 1,
+                 eb, ebb);
   if (rc) return rc;
   TcParams p;
   p.C = C; p.ldc = ldc; p.M = m; p.N = n; p.K = k;
@@ -347,6 +366,7 @@ int launch_tc(int m, int n, int k, const void* A, long long lda, int a_rows_tota
   if (p.group_m < 1) p.group_m = 1;
   constexpr int OB = OutBytes<OutT>::V;
   p.vec_ok = aligned16(C) && ((long long)ldc * OB) % 16 == 0;
+  if constexpr (BATCHED) p.vec_ok = p.vec_ok && bat->sc % (16 / OB) == 0;    // every entry's C base as aligned
   p.a_plane_rows = a_plane_rows; p.b_plane_rows = b_plane_rows;
   p.chunk_kb = chunk_k > 0 ? (chunk_k + Cfg::BK - 1) / Cfg::BK : (k + Cfg::BK - 1) / Cfg::BK;
   if (p.chunk_kb < 1) p.chunk_kb = 1;
@@ -357,9 +377,15 @@ int launch_tc(int m, int n, int k, const void* A, long long lda, int a_rows_tota
   p.act = c.act;
   if constexpr (EPI) p.bias = c.bias;            // shares col_max's slot: EPI kernels are never scaled
   p.stream_c = g_stream_c < 0 ? (g_stream_c = (getenv("B200GEMM_STREAM_C") ? atoi(getenv("B200GEMM_STREAM_C")) : kStreamCDefault)) : g_stream_c;
-  auto kern = gemm_tc_kernel<KIND, BN, STAGES, OutT, Prod, A_ROW_BYTES, AL, BL, EPI>;
+  auto kern = [] {
+    if constexpr (BATCHED) return gemm_tc_batched_kernel<KIND, BN, STAGES, OutT, AL, BL>;
+    else return gemm_tc_kernel<KIND, BN, STAGES, OutT, Prod, A_ROW_BYTES, AL, BL, EPI>;
+  }();
   if (int arc = ensure_smem_attr(kern, Cfg::SMEM_BYTES)) return arc;
-  int tiles = p.tiles_m * p.tiles_n;
+  TcBatch bt{1, 0, 0, 0};
+  if constexpr (BATCHED) bt = TcBatch{bat->count, bat->sa ? 1 : 0, bat->sb ? 1 : 0, bat->sc};
+  // the whole batch's tiles (the entry point checked that they and their split parts fit the kernel's int index)
+  int tiles = p.tiles_m * p.tiles_n * bt.count;
   const int units_max = t_ctx->sms - c.sm_reserve > 2 ? t_ctx->sms - c.sm_reserve : t_ctx->sms;   // one CTA per SM
   // Wave quantisation: the last, partial round of tiles (or the only round of a small problem) is
   // cut along K so that every CTA has work: rem tiles x split parts <= units.
@@ -382,9 +408,12 @@ int launch_tc(int m, int n, int k, const void* A, long long lda, int a_rows_tota
   }
   const int items = p.full_tiles + (tiles - p.full_tiles) * split;
   const int units = items < units_max ? items : units_max;
+  t_last_schedule = Schedule{tiles, split, p.full_tiles, units};
   g_ktimer.begin(c.st);
   {
-    cudaError_t e = launch_pdl(kern, dim3(units), dim3(Cfg::THREADS), Cfg::SMEM_BYTES, c.st, 1, tmA, tmB, p);
+    cudaError_t e;
+    if constexpr (BATCHED) e = launch_pdl(kern, dim3(units), dim3(Cfg::THREADS), Cfg::SMEM_BYTES, c.st, 1, tmA, tmB, p, bt);
+    else e = launch_pdl(kern, dim3(units), dim3(Cfg::THREADS), Cfg::SMEM_BYTES, c.st, 1, tmA, tmB, p);
     if (e != cudaSuccess) { cudaGetLastError(); return (int)e; }
   }
   g_ktimer.end(c.st);
@@ -394,8 +423,9 @@ int launch_tc(int m, int n, int k, const void* A, long long lda, int a_rows_tota
 }
 
 // Tile width: fewest "wave x tile-time" units over the persistent grid (tile time ~ BN plus a
-// fixed per-tile cost); 128 x 256 has the best operand reuse, narrower tiles quantise better.
-int pick_bn(int m, int n, bool allow256, bool allow192 = true) {
+// fixed per-tile cost); 128 x 256 has the best operand reuse, narrower tiles quantise better.  A strided batch counts
+// the tiles of all its entries (one persistent grid walks them all).
+int pick_bn(int m, int n, bool allow256, bool allow192 = true, int batch = 1) {
   if (g_force_bn == 128 || (g_force_bn == 192 && allow192) || (g_force_bn == 256 && allow256)) return g_force_bn;
   const int cands[3] = {256, 192, 128};
   // relative per-tile efficiency assumed for the three widths: narrower tiles re-read A from shared memory
@@ -407,7 +437,7 @@ int pick_bn(int m, int n, bool allow256, bool allow192 = true) {
   for (int i = 0; i < 3; i++) {
     if (cands[i] == 256 && !allow256) continue;
     if (cands[i] == 192 && !allow192) continue;
-    const long long tiles = (long long)tm * ((n + cands[i] - 1) / cands[i]);
+    const long long tiles = (long long)tm * ((n + cands[i] - 1) / cands[i]) * batch;
     const long long waves = (tiles + t_ctx->sms - 1) / t_ctx->sms;
     const double cost = (double)waves * (cands[i] / eff[i] + 8.0);
     if (cost < best_cost) { best_cost = cost; best = cands[i]; }
@@ -420,8 +450,8 @@ template <int W> struct Width {
   static constexpr int BN = W, STAGES = W == 256 ? 4 : W == 192 ? 5 : 6, idx = W == 256 ? 0 : W == 192 ? 1 : 2;
 };
 template <bool ALLOW192 = true, class F>
-int with_width(int m, int n, F&& f) {
-  const int bn = pick_bn(m, n, true, ALLOW192);
+int with_width(int m, int n, F&& f, int batch = 1) {
+  const int bn = pick_bn(m, n, true, ALLOW192, batch);
   if (bn == 256) return f(Width<256>());
   if constexpr (ALLOW192) if (bn == 192) return f(Width<192>());
   return f(Width<128>());
@@ -443,39 +473,46 @@ typedef const char* const KernelNames[4][3];
    {P "_tn_128x256", P "_tn_128x192", P "_tn_128x128"}, {P "_tt_128x256", P "_tt_128x192", P "_tt_128x128"}}
 
 // 16-bit operands: KIND_F16 (bf16, C fp32 or bf16) and KIND_FP16 (fp16, C fp32 or fp16).  E is the generic kernel's
-// element type of the kind (uint16_t holds bf16 bits).  names[16-bit C][EPI].
+// element type of the kind (uint16_t holds bf16 bits).  names[16-bit C][EPI]; bat_names[16-bit C]: the strided-batched
+// kernels.
 template <int KIND> struct Kind16;
 template <> struct Kind16<KIND_F16> {
   using E = uint16_t;
   using Out16 = bf16_out;
   static constexpr int OUT16 = B200_OUT_BF16;
   static constexpr const char* kGeneric = "generic_bf16_64x64";
+  static constexpr const char* kGenericBat = "generic_bf16_bat_64x64";
   static constexpr KernelNames names[2][2] = {{TC_NAMES("tc_bf16"), TC_NAMES("tc_bf16_epi")},
                                               {TC_NAMES("tc_bf16_obf16"), TC_NAMES("tc_bf16_obf16_epi")}};
+  static constexpr KernelNames bat_names[2] = {TC_NAMES("tc_bf16_bat"), TC_NAMES("tc_bf16_obf16_bat")};
 };
 template <> struct Kind16<KIND_FP16> {
   using E = __half;
   using Out16 = f16_out;
   static constexpr int OUT16 = B200_OUT_F16;
   static constexpr const char* kGeneric = "generic_f16_64x64";
+  static constexpr const char* kGenericBat = "generic_f16_bat_64x64";
   static constexpr KernelNames names[2][2] = {{TC_NAMES("tc_f16"), TC_NAMES("tc_f16_epi")},
                                               {TC_NAMES("tc_f16_of16"), TC_NAMES("tc_f16_of16_epi")}};
+  static constexpr KernelNames bat_names[2] = {TC_NAMES("tc_f16_bat"), TC_NAMES("tc_f16_of16_bat")};
 };
 
 // The 16-bit GEMM on the tensor cores (OutT float, bf16_out or f16_out): every layout is read in place by one launch.
-// EPI: the bias / activation kernels.
-template <int KIND, typename OutT, bool EPI>
+// EPI: the bias / activation kernels.  BATCHED: the strided batch *bat in one launch (not with EPI).
+template <int KIND, typename OutT, bool EPI, bool BATCHED = false>
 int tc16(int op_a, int op_b, int m, int n, int k, const void* A, int lda, const void* B, int ldb, void* C, int ldc,
-         const Call& c) {
-  const KernelNames& names = Kind16<KIND>::names[!std::is_same<OutT, float>::value][EPI];
+         const Call& c, const Batch* bat = nullptr) {
+  static_assert(!(EPI && BATCHED), "the batched kernels have no bias / activation epilogue");
+  const KernelNames& names = BATCHED ? Kind16<KIND>::bat_names[!std::is_same<OutT, float>::value]
+                                     : Kind16<KIND>::names[!std::is_same<OutT, float>::value][EPI];
   return with_layout(op_a, op_b, [&](auto L) {
     using Lay = decltype(L);
     const int ar = Lay::AL == LAYOUT_MN ? k : m, br = Lay::BL == LAYOUT_MN ? k : n;      // rows of the operands as stored
     return with_width(m, n, [&](auto W) {
       using Wd = decltype(W);
-      return launch_tc<KIND, Wd::BN, Wd::STAGES, OutT, ProdSingle, 128, Lay::AL, Lay::BL, EPI>(
-          m, n, k, A, lda, ar, 0, B, ldb, br, 0, C, ldc, names[Lay::idx][Wd::idx], c);
-    });
+      return launch_tc<KIND, Wd::BN, Wd::STAGES, OutT, ProdSingle, 128, Lay::AL, Lay::BL, EPI, BATCHED>(
+          m, n, k, A, lda, ar, 0, B, ldb, br, 0, C, ldc, names[Lay::idx][Wd::idx], c, 0, nullptr, nullptr, bat);
+    }, bat ? bat->count : 1);
   });
 }
 
@@ -1025,6 +1062,95 @@ int gemm16(int op_a, int op_b, int m, int n, int k, float alpha, const uint16_t*
              : tc16<KIND, O16, false>(op_a, op_b, m, n, k, A, lda, B, ldb, C, ldc, c);
 }
 
+// ---- strided-batched 16-bit GEMM ----------------------------------------------------------------------------------
+// Grid z of the batched generic and element-wise kernels: the entries run over blockIdx.z, this many at a time.
+constexpr int kMaxGridZ = 65535;
+
+// k == 0 or alpha == 0 over every entry of a batch, one launch: C = beta * C (C unread when beta == 0).
+template <typename T>
+int degenerate_batched(int m, int n, void* C, int ldc, const Batch& bt, const Call& c) {
+  const int gz = bt.count < kMaxGridZ ? bt.count : kMaxGridZ;
+  int gy = 4096 / gz;
+  if (gy > m) gy = m;
+  if (gy < 1) gy = 1;
+  const dim3 grid((n + 255) / 256, gy, gz);
+  if (c.beta == 0.f) {          // 16-bit C is cleared as raw bits
+    using Z = typename std::conditional<sizeof(T) == 2, uint16_t, T>::type;
+    fill_zero_batched_kernel<Z><<<grid, 256, 0, c.st>>>(bt.count, m, n, static_cast<Z*>(C), ldc, bt.sc);
+    t_last_kernel = "fill_zero_bat";
+  } else {
+    scale_inplace_batched_kernel<T><<<grid, 256, 0, c.st>>>(bt.count, m, n, static_cast<T*>(C), ldc, bt.sc, c.beta);
+    t_last_kernel = "scale_inplace_bat";
+  }
+  g_launches++;
+  return last_launch_status();
+}
+
+// Operands TMA cannot describe, and overlapping input entries: the CUDA-core kernel, each entry as launch_generic
+// computes one matrix.
+template <typename InT, typename OutT>
+int launch_generic_batched(int op_a, int op_b, int m, int n, int k, const void* A, int lda, const void* B, int ldb,
+                           void* C, int ldc, const Batch& bt, const char* name, const Call& c) {
+  dim3 grid((n + 63) / 64, (m + 63) / 64, bt.count < kMaxGridZ ? bt.count : kMaxGridZ);
+  const long long a_rs = op_a ? 1 : lda, a_cs = op_a ? lda : 1, b_rs = op_b ? 1 : ldb, b_cs = op_b ? ldb : 1;
+  gemm_generic_batched_kernel<InT, OutT><<<grid, 256, 0, c.st>>>(
+      bt.count, m, n, k, static_cast<const InT*>(A), a_rs, a_cs, bt.sa, static_cast<const InT*>(B), b_rs, b_cs, bt.sb,
+      static_cast<OutT*>(C), ldc, bt.sc, c.axpby, c.alpha, c.beta);
+  g_launches++;
+  t_last_kernel = name;
+  return last_launch_status();
+}
+
+// One operand of a batch as a 3-D tensor map: its entry stride (elements) a 16-byte multiple that TMA can encode, and
+// either 0 (broadcast) or at least the entry's rows x ld, since the encoder documents each stride as covering the
+// dimension before it.  Overlapping entries (0 < stride < rows x ld, which cuBLAS allows for inputs) go to the
+// generic kernel.
+bool batch_tma_ok(long long stride, long long rows, long long ld, int elem) {
+  return stride == 0 || (stride < (1LL << 40) / elem && (stride * elem) % 16 == 0 && stride >= rows * ld);
+}
+
+// C_b = round_out(fma(beta, float(C_b), alpha * op(A_b) op(B_b))) for b < batch, X_b = X + b * stride_x (elements).
+// Argument rules (all before the device is touched): those of gemm16 per entry; batch < 0 or a negative stride is
+// B200_ERR_BAD_ARG; batch == 0, m == 0 or n == 0 is a no-op; batch > 1 with entries of C that overlap is
+// B200_ERR_BAD_ARG, as is a batch whose tiles the kernel's int work index cannot count.  batch == 1 is the _ex call.
+template <int KIND>
+int gemm16_batched(int op_a, int op_b, int m, int n, int k, float alpha, const uint16_t* A, int lda, long long stride_a,
+                   const uint16_t* B, int ldb, long long stride_b, float beta, void* C, int ldc, long long stride_c,
+                   int batch, int out_type, cudaStream_t st) {
+  using K16 = Kind16<KIND>;
+  using E = typename K16::E;
+  if (batch < 0 || stride_a < 0 || stride_b < 0 || stride_c < 0) return B200_ERR_BAD_ARG;
+  if (out_type != B200_OUT_F32 && out_type != K16::OUT16) return B200_ERR_BAD_ARG;
+  if ((op_a != B200_OP_N && op_a != B200_OP_T) || (op_b != B200_OP_N && op_b != B200_OP_T)) return B200_ERR_BAD_ARG;
+  if (m < 0 || n < 0 || k < 0) return B200_ERR_BAD_ARG;
+  if (batch == 0) return 0;
+  if (batch == 1)
+    return gemm16<KIND>(op_a, op_b, m, n, k, alpha, A, lda, B, ldb, beta, C, ldc, out_type, nullptr, B200_ACT_NONE, st);
+  int rc = check_args(m, n, k, A, lda, B, ldb, C, ldc, op_a, op_b);
+  if (rc == 1) return 0;
+  if (rc) return rc;
+  if (stride_c < (long long)(m - 1) * ldc + n) return B200_ERR_BAD_ARG;                 // entries of C would overlap
+  // Offsets: the last entry of each operand within 2^60 elements, so no byte offset wraps.  Tiles: the batch's tiles
+  // at the narrowest width, times up to 4 K-split parts, must fit the kernel's int work index.  Both by division.
+  const long long max_stride = (1LL << 60) / (batch - 1);
+  if (stride_a > max_stride || stride_b > max_stride || stride_c > max_stride) return B200_ERR_BAD_ARG;
+  const long long tiles1 = ((m + 127LL) / 128) * ((n + 127LL) / 128);                  // < 2^48
+  if (tiles1 > 0x7FFFFFFFLL / 4 / batch) return B200_ERR_BAD_ARG;
+  if ((rc = ensure_device())) return rc;
+  Call c{st};
+  if (alpha != 1.f || beta != 0.f) { c.axpby = 1; c.alpha = alpha; c.beta = beta; }
+  const bool c32 = out_type == B200_OUT_F32;
+  const Batch bt{batch, stride_a, stride_b, stride_c};
+  if (k == 0 || alpha == 0.f) return c32 ? degenerate_batched<float>(m, n, C, ldc, bt, c) : degenerate_batched<E>(m, n, C, ldc, bt, c);
+  const int ar = op_a ? k : m, br = op_b ? n : k;                                       // rows of the operands as stored
+  if (!tma_ok(A, lda, B, ldb, 2) || !batch_tma_ok(stride_a, ar, lda, 2) || !batch_tma_ok(stride_b, br, ldb, 2)) {
+    if (c32) return launch_generic_batched<E, float>(op_a, op_b, m, n, k, A, lda, B, ldb, C, ldc, bt, K16::kGenericBat, c);
+    return launch_generic_batched<E, E>(op_a, op_b, m, n, k, A, lda, B, ldb, C, ldc, bt, K16::kGenericBat, c);
+  }
+  if (c32) return tc16<KIND, float, false, true>(op_a, op_b, m, n, k, A, lda, B, ldb, C, ldc, c, &bt);
+  return tc16<KIND, typename K16::Out16, false, true>(op_a, op_b, m, n, k, A, lda, B, ldb, C, ldc, c, &bt);
+}
+
 static_assert(ACT_NONE == B200_ACT_NONE && ACT_RELU == B200_ACT_RELU && ACT_GELU == B200_ACT_GELU &&
               ACT_GELU_TANH == B200_ACT_GELU_TANH, "EpiAct follows the header's codes");
 
@@ -1076,6 +1202,13 @@ void b200_gemm_debug_set_pdl(int v) { g_pdl = (v & 1) != 0; g_prepass_fork = (v 
 void b200_gemm_debug_set_dynamic_sched(int) {}
 void b200_gemm_debug_set_cta_group(int) {}
 void b200_gemm_debug_set_split_tail(int on) { g_split_tail = on; }
+void b200_gemm_debug_last_schedule(int* tiles, int* split, int* full_tiles, int* ctas) {
+  const Schedule& s = t_last_schedule;
+  if (tiles) *tiles = s.tiles;
+  if (split) *split = s.split;
+  if (full_tiles) *full_tiles = s.full_tiles;
+  if (ctas) *ctas = s.ctas;
+}
 void b200_gemm_debug_set_epilogue(int) {}
 void b200_gemm_debug_set_group_rows(int rows) { g_group_rows = rows; }
 void b200_gemm_debug_set_ffma_variant(int v) { g_ffma_halves = v & 1; g_ffma_fat = v < 0 ? -1 : (v >> 1) & 1; }
@@ -1186,6 +1319,20 @@ int b200_gemm_f16_epi(int op_a, int op_b, int m, int n, int k, float alpha, cons
                       int act, void* stream) {
   return gemm16<KIND_FP16>(op_a, op_b, m, n, k, alpha, dA, lda, dB, ldb, beta, dC, ldc, out_type, dBias, act,
                            (cudaStream_t)stream);
+}
+
+int b200_gemm_bf16_batched(int op_a, int op_b, int m, int n, int k, float alpha, const uint16_t* dA, int lda,
+                           long long stride_a, const uint16_t* dB, int ldb, long long stride_b, float beta, void* dC,
+                           int ldc, long long stride_c, int batch, int out_type, void* stream) {
+  return gemm16_batched<KIND_F16>(op_a, op_b, m, n, k, alpha, dA, lda, stride_a, dB, ldb, stride_b, beta, dC, ldc,
+                                  stride_c, batch, out_type, (cudaStream_t)stream);
+}
+
+int b200_gemm_f16_batched(int op_a, int op_b, int m, int n, int k, float alpha, const uint16_t* dA, int lda,
+                          long long stride_a, const uint16_t* dB, int ldb, long long stride_b, float beta, void* dC,
+                          int ldc, long long stride_c, int batch, int out_type, void* stream) {
+  return gemm16_batched<KIND_FP16>(op_a, op_b, m, n, k, alpha, dA, lda, stride_a, dB, ldb, stride_b, beta, dC, ldc,
+                                   stride_c, batch, out_type, (cudaStream_t)stream);
 }
 
 int b200_gemm_s8s32(int m, int n, int k, const int8_t* dA, int lda, const int8_t* dB, int ldb,

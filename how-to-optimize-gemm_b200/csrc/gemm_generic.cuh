@@ -180,4 +180,95 @@ __global__ void fill_zero_kernel(int M, int N, T* __restrict__ C, long long ldc)
   for (int i = blockIdx.y; i < M; i += gridDim.y) C[(long long)i * ldc + j] = (T)0;
 }
 
+// ---- strided-batched 16-bit forms ----------------------------------------------------------------------------------
+// Entry z of each operand at X + z * x_bs (elements; 0 broadcasts A or B), the entries over blockIdx.z, gridDim.z at a
+// time.  Kernels of their own, so that the single-matrix kernels above keep their code exactly.
+
+// gemm_generic_kernel's tile for 16-bit operands with the alpha / beta epilogue (no accumulate, requant, bias or
+// activation): the same loads, the same fmaf chain in k order and the same store, so every entry equals the 2-D
+// generic call on that entry bit for bit.
+template <typename InT, typename OutT>
+__global__ void __launch_bounds__(256)
+gemm_generic_batched_kernel(int batch, int M, int N, int K, const InT* __restrict__ A, long long a_rs, long long a_cs,
+                            long long a_bs, const InT* __restrict__ B, long long b_rs, long long b_cs, long long b_bs,
+                            OutT* __restrict__ C, long long ldc, long long c_bs, int axpby, float alpha, float beta) {
+  static_assert(sizeof(InT) == 2, "strided-batched generic kernel: 16-bit operands");
+  __shared__ float As[16][64 + 4];
+  __shared__ float Bs[16][64 + 4];
+  const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
+  const int m0 = blockIdx.y * 64, n0 = blockIdx.x * 64;
+  for (int z = blockIdx.z; z < batch; z += gridDim.z) {
+    const InT* Az = A + z * a_bs;
+    const InT* Bz = B + z * b_bs;
+    OutT* Cz = C + z * c_bs;
+    float acc[4][4];
+#pragma unroll
+    for (int i = 0; i < 4; i++)
+#pragma unroll
+      for (int j = 0; j < 4; j++) acc[i][j] = 0.f;
+    for (int k0 = 0; k0 < K; k0 += 16) {
+#pragma unroll
+      for (int r = 0; r < 4; r++) {
+        const int idx = threadIdx.x + r * 256;
+        const int am = idx >> 4, ak = idx & 15;
+        const int gm = m0 + am, gk = k0 + ak;
+        As[ak][am] = (gm < M && gk < K) ? LoadAs<InT>::ld(Az + (long long)gm * a_rs + (long long)gk * a_cs) : 0.f;
+        const int bk = idx >> 6, bn = idx & 63;
+        const int gk2 = k0 + bk, gn = n0 + bn;
+        Bs[bk][bn] = (gk2 < K && gn < N) ? LoadAs<InT>::ld(Bz + (long long)gk2 * b_rs + (long long)gn * b_cs) : 0.f;
+      }
+      __syncthreads();
+#pragma unroll
+      for (int kk = 0; kk < 16; kk++) {
+        float a[4], b[4];
+#pragma unroll
+        for (int i = 0; i < 4; i++) a[i] = As[kk][ty + 16 * i];
+#pragma unroll
+        for (int j = 0; j < 4; j++) b[j] = Bs[kk][tx + 16 * j];
+#pragma unroll
+        for (int i = 0; i < 4; i++)
+#pragma unroll
+          for (int j = 0; j < 4; j++) acc[i][j] = fmaf(a[i], b[j], acc[i][j]);
+      }
+      __syncthreads();                                 // also orders this entry's last reads before the next's loads
+    }
+#pragma unroll
+    for (int i = 0; i < 4; i++) {
+      const int gm = m0 + ty + 16 * i;
+      if (gm >= M) continue;
+#pragma unroll
+      for (int j = 0; j < 4; j++) {
+        const int gn = n0 + tx + 16 * j;
+        if (gn < N) {
+          float v = acc[i][j];
+          if (axpby) {
+            v *= alpha;
+            if (beta != 0.f) v = fmaf(beta, LoadAs<OutT>::ld(Cz + (long long)gm * ldc + gn), v);
+          }
+          store_out<float, OutT>(Cz + (long long)gm * ldc + gn, v);
+        }
+      }
+    }
+  }
+}
+
+// scale_inplace_kernel (s != 0) and fill_zero_kernel (s == 0) over every entry: the k == 0 / alpha == 0 pass.
+template <typename T>
+__global__ void scale_inplace_batched_kernel(int batch, int M, int N, T* __restrict__ C, long long ldc, long long c_bs,
+                                             float s) {
+  for (int z = blockIdx.z; z < batch; z += gridDim.z)
+    for (int r = blockIdx.y; r < M; r += gridDim.y)
+      for (int c = blockIdx.x * blockDim.x + threadIdx.x; c < N; c += gridDim.x * blockDim.x) {
+        T* e = C + z * c_bs + (long long)r * ldc + c;
+        store_out<float, T>(e, s * LoadAs<T>::ld(e));
+      }
+}
+template <typename T>
+__global__ void fill_zero_batched_kernel(int batch, int M, int N, T* __restrict__ C, long long ldc, long long c_bs) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= N) return;
+  for (int z = blockIdx.z; z < batch; z += gridDim.z)
+    for (int i = blockIdx.y; i < M; i += gridDim.y) C[z * c_bs + (long long)i * ldc + j] = (T)0;
+}
+
 }  // namespace b200

@@ -103,6 +103,15 @@ struct TcParams {
   int act;                 // EPI kernels: y = act(t + bias[col]) after the alpha / beta step; an EpiAct (ptx.cuh)
 };
 
+// Strided-batched kernels (gemm_tc_batched_kernel) only: a second kernel argument, so that TcParams, and with it the
+// code of every single-matrix kernel, is unchanged.  The operands are 3-D tensor maps (inner, rows, entry); a broadcast
+// operand (stride 0) has one entry and is read at entry coordinate 0.
+struct TcBatch {
+  int count;               // entries; the work index runs over count x tiles_m x tiles_n, entry outermost
+  int a_step, b_step;      // entry coordinate of A / B per entry: 1, or 0 for a broadcast operand
+  long long stride_c;      // elements between consecutive entries of C
+};
+
 // REGACC (split-precision fp32 modes): the tensor core adds into its fp32 accumulator with truncation,
 // so a long K chain drifts (error grows ~K).  K is cut into chunks of chunk_kb k-blocks; each chunk starts a
 // fresh wgmma accumulator that is added, with a rounded fp32 add, to the tile's running sum in registers.
@@ -559,6 +568,172 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           }
         }
       }
+      if (w >= p.full_tiles && p.split > 1) {          // publish this part (the last one re-arms the flag)
+        __threadfence();
+        __syncwarp();
+        if (lane == 0) {
+          const int nv = it.part + 1 == p.split ? 0 : it.part + 1;
+          asm volatile("st.release.gpu.global.s32 [%0], %1;" ::"l"(flag), "r"(nv) : "memory");
+        }
+      }
+    }
+  }
+}
+
+// ---- strided-batched 16-bit GEMM ----------------------------------------------------------------------
+// gemm_tc_kernel's persistent schedule over a stack of matrices, cut down to what the strided-batched calls need:
+// 16-bit operands, one plane, 128-byte rows, fp32 or 16-bit C, no bias / activation, no scaling.  It is a kernel of
+// its own rather than a flag of gemm_tc_kernel so that the single-matrix kernels keep their code exactly.  Its MMA
+// chain (k-blocks in order, one accumulator) and its epilogue (store_pair, the same fold / alpha / beta rules) are
+// gemm_tc_kernel's, so every entry equals the single-matrix call on that entry bit for bit at the same tile width.
+// Work item w covers bt.count x tiles_m x tiles_n with the entry outermost: one entry's tiles are adjacent and share
+// its B in L2; inside an entry tile_coords walks its raster groups as for one matrix.  The K-split tail (fp32 C)
+// cuts the last partial round of the whole batch.  A and B are 3-D tensor maps (inner, rows, entry) read one entry
+// per box, so TMA's zero fill past the rows and the inner extent stays inside the entry; entry e of C is at
+// C + e * stride_c (64-bit).
+template <int KIND, int BN, int STAGES, typename OutT, int AL, int BL>
+__global__ void __launch_bounds__((TcConfig<KIND, BN, STAGES, ProdSingle, 128, AL, BL>::THREADS), 1)
+gemm_tc_batched_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                       const TcParams p, const TcBatch bt) {
+  using Cfg = TcConfig<KIND, BN, STAGES, ProdSingle, 128, AL, BL>;
+  using MMA = typename Cfg::MMA;
+  using Acc = typename MMA::Acc;
+  static_assert(KindTraits<KIND>::ELEM == 2 && (std::is_same<OutT, float>::value || OutBytes<OutT>::V == 2),
+                "strided-batched: 16-bit kinds with fp32 or 16-bit C");
+
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;   // swizzle atoms need 1 KB
+  const uint32_t sA = smem_base;
+  const uint32_t sB = sA + STAGES * Cfg::A_STAGE;
+  const uint32_t bar_full = sB + STAGES * Cfg::B_STAGE;
+  const uint32_t bar_empty = bar_full + 8 * STAGES;
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmA);
+    tma_prefetch_desc(&tmB);
+    for (int i = 0; i < STAGES; i++) {
+      mbar_init(bar_full + 8 * i, 1);
+      mbar_init(bar_empty + 8 * i, Cfg::CONSUMERS);
+    }
+    fence_barrier_init();
+  }
+  __syncthreads();
+  griddep_launch();
+  griddep_wait();
+
+  const int per_entry = p.tiles_m * p.tiles_n;
+  const int num_tiles = per_entry * bt.count;
+  const int num_items = p.full_tiles + (num_tiles - p.full_tiles) * p.split;
+  const int num_kb = (p.K + Cfg::BK - 1) / Cfg::BK;
+
+  if (warp < 4) {
+    // ===================== TMA producer (warpgroup 0) =====================
+    setmaxnreg_dec<40>();
+    if (warp == 0 && lane == 0) {
+      int s = 0;
+      uint32_t ph = 0;
+      for (int w = blockIdx.x; w < num_items; w += gridDim.x) {
+        const WorkItem it = work_item(w, p, num_kb);
+        const int e = it.tile / per_entry;
+        int mb, nb;
+        tile_coords(it.tile - e * per_entry, p.tiles_m, p.tiles_n, p.group_m, mb, nb);
+        const int m0 = mb * Cfg::BM, n0 = nb * BN, ea = e * bt.a_step, eb = e * bt.b_step;
+        for (int kb = it.kb0; kb < it.kb1; kb++) {
+          mbar_wait(bar_empty + 8 * s, ph ^ 1);
+          const uint32_t full = bar_full + 8 * s;
+          mbar_arrive_expect_tx(full, Cfg::STAGE_BYTES);
+          if constexpr (Cfg::A_MN) {                  // A^T (k x m): one 64-column box per consumer
+#pragma unroll
+            for (int j = 0; j < Cfg::A_BOXES; j++)
+              tma_load_3d(sA + s * Cfg::A_STAGE + j * Cfg::MN_BOX_BYTES, &tmA, full, m0 + j * Cfg::MN_BOX_COLS,
+                          kb * Cfg::BK, ea);
+          } else {
+            tma_load_3d(sA + s * Cfg::A_STAGE, &tmA, full, kb * Cfg::BK, m0, ea);
+          }
+          if constexpr (!Cfg::B_MN) {                 // B^T (n x k): one box of BN rows
+            tma_load_3d(sB + s * Cfg::B_STAGE, &tmB, full, kb * Cfg::BK, n0, eb);
+          } else {
+#pragma unroll
+            for (int j = 0; j < Cfg::B_BOXES; j++)
+              tma_load_3d(sB + s * Cfg::B_STAGE + j * Cfg::B_BOX_BYTES, &tmB, full, n0 + j * Cfg::B_BOX_COLS,
+                          kb * Cfg::BK, eb);
+          }
+          if (++s == STAGES) { s = 0; ph ^= 1; }
+        }
+      }
+    }
+  } else {
+    // ===================== consumers (warpgroups 1 and 2): MMA chain + epilogue =====================
+    setmaxnreg_inc<232>();
+    const int cw = warp / 4 - 1;                    // consumer warpgroup: rows [64 cw, 64 cw + 64) of the tile
+    const int ew = warp - 4;                        // consumer warp 0..7: 16 rows each
+    const bool wg_leader = (threadIdx.x & 127) == 0;
+    const uint32_t b_lbo = p.dbg_b_lbo ? (uint32_t)p.dbg_b_lbo : (uint32_t)Cfg::B_BOX_BYTES;
+    const uint32_t b_sbo = p.dbg_b_sbo ? (uint32_t)p.dbg_b_sbo : 1024u;
+    int s = 0;
+    uint32_t ph = 0;
+    Acc acc[Cfg::ACC];
+    for (int w = blockIdx.x; w < num_items; w += gridDim.x) {
+      const WorkItem it = work_item(w, p, num_kb);
+      const int e = it.tile / per_entry;
+      int mb, nb;
+      tile_coords(it.tile - e * per_entry, p.tiles_m, p.tiles_n, p.group_m, mb, nb);
+      const int m0 = mb * Cfg::BM, n0 = nb * BN;
+      int prev = -1;
+      for (int kb = it.kb0; kb < it.kb1; kb++) {
+        mbar_wait(bar_full + 8 * s, ph);
+        const uint32_t a0 = sA + s * Cfg::A_STAGE + cw * Cfg::A_WG;
+        const uint32_t b0 = sB + s * Cfg::B_STAGE;
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < Cfg::MMAS_PER_STAGE; k++) {
+          uint64_t ad, bd;
+          if constexpr (Cfg::A_MN) ad = make_sdesc(a0 + k * Cfg::A_KADV, Cfg::MN_BOX_BYTES, 1024, SWZ_128B);
+          else ad = make_sdesc(a0 + k * Cfg::A_KADV, 16, Cfg::A_SBO, Cfg::A_SWZ);
+          if constexpr (Cfg::B_MN) bd = make_sdesc(b0 + k * Cfg::B_KADV, b_lbo, b_sbo, SWZ_128B);
+          else bd = make_sdesc(b0 + k * Cfg::B_KADV, 16, Cfg::A_SBO, Cfg::A_SWZ);
+          MMA::mma(acc, ad, bd, ((kb - it.kb0) | k) != 0 ? 1u : 0u);
+        }
+        wgmma_commit();
+        wgmma_wait<1>();                              // the previous k-block's products retired: its stage is free
+        if (prev >= 0 && wg_leader) mbar_arrive(bar_empty + 8 * prev);
+        prev = s;
+        if (++s == STAGES) { s = 0; ph ^= 1; }
+      }
+      wgmma_wait<0>();
+      wgmma_fence_regs(acc);
+      if (prev >= 0 && wg_leader) mbar_arrive(bar_empty + 8 * prev);
+
+      // ---- this warp's 16 rows of the tile into entry e of C ----
+      int* flag = p.flags + (it.tile - p.full_tiles) * Cfg::EPI_WARPS + ew;
+      if (it.part > 0) {                               // K-split tail: wait until parts < it.part are in C
+        if (lane == 0) {
+          const long long t0 = clock64();
+          while (true) {
+            int v;
+            asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(flag) : "memory");
+            if (v == it.part) break;
+            if (clock64() - t0 > 4000000000LL) { asm volatile("trap;"); }
+          }
+        }
+        __syncwarp();
+      }
+      const bool fold = p.accumulate != 0 || it.part > 0 || (p.axpby && p.beta != 0.f);
+      const float al = p.axpby ? p.alpha : 1.f;
+      const float be = (p.axpby && it.part == 0) ? p.beta : 1.f;
+      const int row0 = m0 + ew * 16 + (lane >> 2);
+      const int col0 = n0 + 2 * (lane & 3);
+      TcParams pc = p;
+      pc.C = static_cast<uint8_t*>(p.C) + (long long)e * bt.stride_c * OutBytes<OutT>::V;
+      const int ce[2] = {0, 0};
+#pragma unroll
+      for (int j = 0; j < BN / 8; j++)
+#pragma unroll
+        for (int h = 0; h < 2; h++)
+          store_pair<OutT>(pc, row0 + 8 * h, col0 + 8 * j, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], fold, it.part > 0,
+                           al, be, 0, ce, 0.f, 0.f);
       if (w >= p.full_tiles && p.split > 1) {          // publish this part (the last one re-arms the flag)
         __threadfence();
         __syncwarp();

@@ -64,6 +64,15 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst_smem, const CUtensorMap
       ::"r"(dst_smem), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar), "r"(c0), "r"(c1)
       : "memory");
 }
+// 3D tiled load (inner, rows, batch): the strided-batched kernels read entry c2 of a stack of matrices.
+__device__ __forceinline__ void tma_load_3d(uint32_t dst_smem, const CUtensorMap* m, uint32_t bar,
+                                            int c0, int c1, int c2) {
+  asm volatile(
+      "cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes "
+      "[%0], [%1, {%3, %4, %5}], [%2];"
+      ::"r"(dst_smem), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar), "r"(c0), "r"(c1), "r"(c2)
+      : "memory");
+}
 __device__ __forceinline__ void tma_load_2d_hint(uint32_t dst_smem, const CUtensorMap* m,
                                                  uint32_t bar, int c0, int c1, uint64_t policy) {
   asm volatile(

@@ -176,6 +176,38 @@ int b200_gemm_f16_ex(int op_a, int op_b, int m, int n, int k, float alpha,
                      const uint16_t* dA, int lda, const uint16_t* dB, int ldb, float beta,
                      void* dC, int ldc, int out_type, void* stream);
 
+/* Strided-batched 16-bit GEMM (cublasGemmStridedBatchedEx; torch.bmm / torch.baddbmm): for b = 0 .. batch - 1,
+ *   C_b = round_out(fma(beta, float(C_b), alpha * op(A_b) * op(B_b))),   X_b = X + b * stride_x  (strides in elements).
+ * Each entry follows the rules of b200_gemm_bf16_ex / b200_gemm_f16_ex exactly: ops, minimum ld, out_type pairing,
+ * beta == 0 never reads C, alpha == 0 or k == 0 never reads A or B.  Further rules, each checked before the device is
+ * touched:
+ *   - batch < 0 or a negative stride is B200_ERR_BAD_ARG; batch == 0, m == 0 or n == 0 is a no-op, NULL pointers
+ *     included; a NULL pointer with work to do is B200_ERR_BAD_ARG.
+ *   - stride_a and stride_b may be 0: one operand broadcast over the batch.  They may also be smaller than an entry of
+ *     the operand (overlapping input entries); such a call runs on the generic kernel.
+ *   - batch > 1 with stride_c < (m - 1) * ldc + n is B200_ERR_BAD_ARG: two entries of C would overlap.
+ *   - batch * ceil(m / 128) * ceil(n / 128) * 4 above 2^31 - 1 is B200_ERR_BAD_ARG: the kernel counts the batch's
+ *     tiles (and their K-split parts) in an int.  So is (batch - 1) * stride above 2^60 elements for any operand.
+ *   - batch == 1 is the _ex call exactly: same kernel, kernel name, launches and bits.
+ * Every other call is one launch for the whole batch (see the launch table below):
+ *   - 16-byte-aligned bases with lda, ldb, stride_a and stride_b multiples of 16 bytes, each input stride 0 or at least
+ *     its entry's rows x ld as stored: the persistent tensor-core kernel walks the tiles of every entry, entry outermost,
+ *     tile width chosen for the whole batch's tile count.  fp32 C may take the K-split tail on the last partial round
+ *     of the whole batch; 16-bit C never does.  Kernels "tc_bf16_bat_128x256", "tc_bf16_obf16_bat_nt_128x192",
+ *     "tc_f16_bat_tn_128x128", "tc_f16_of16_bat_tt_128x256", ...
+ *   - any other operands: the generic kernel, "generic_bf16_bat_64x64" / "generic_f16_bat_64x64", every entry bit for
+ *     bit as the 2-D generic kernel computes it.
+ *   - alpha == 0 or k == 0: one element-wise pass over every entry, "fill_zero_bat" (beta == 0) or "scale_inplace_bat".
+ * No workspace.  Operand types and out_type as for _bf16_ex / _f16_ex. */
+int b200_gemm_bf16_batched(int op_a, int op_b, int m, int n, int k, float alpha,
+                           const uint16_t* dA, int lda, long long stride_a,
+                           const uint16_t* dB, int ldb, long long stride_b, float beta,
+                           void* dC, int ldc, long long stride_c, int batch, int out_type, void* stream);
+int b200_gemm_f16_batched(int op_a, int op_b, int m, int n, int k, float alpha,
+                          const uint16_t* dA, int lda, long long stride_a,
+                          const uint16_t* dB, int ldb, long long stride_b, float beta,
+                          void* dC, int ldc, long long stride_c, int batch, int out_type, void* stream);
+
 /* 16-bit operands with a bias vector and an activation fused into the epilogue (cuBLASLt's CUBLASLT_EPILOGUE_BIAS,
  * _RELU_BIAS, _GELU_BIAS): C = round_out(act(alpha * op(A)*op(B) + beta * C + bias)), what a PyTorch
  * act(F.linear(x, W, b)) computes, in one launch.  Arguments as b200_gemm_bf16_ex / b200_gemm_f16_ex, plus:
@@ -264,6 +296,8 @@ int b200_gemm_s8s32_host(int m, int n, int k,
  *   path                    NN   NT (B^T given)   TN (A^T given)   TT
  *   bf16 -> fp32 / bf16      1   1                1                1     operands read in place
  *   fp16 -> fp32 / fp16      1   1                1                1     operands read in place (b200_gemm_f16_ex)
+ *   bf16 / fp16 batched      1   1                1                1     every entry in one launch (_batched; also
+ *                                                                        generic and alpha == 0 / k == 0: 1)
  *   TF32, int8               2   1                3                2     transposes into the workspace
  *   BF16X3, BF16X2           2   2                2                2     one split launch for both operands
  *   F16X2                    4   3                5                4     B^T's column maxima are its row maxima (the
@@ -427,6 +461,10 @@ void b200_gemm_debug_set_cta_group(int cg);
 /* Tuning hook: 1 (default) = the last partial round of tiles is split along K across the idle
  * CTAs and folded into C in order; 0 = whole tiles only. */
 void b200_gemm_debug_set_split_tail(int on);
+/* Test hook: the work schedule of the last tensor-core GEMM launch issued by the calling thread.  tiles: output
+ * tiles of the launch (of every entry for a batched call); split: K parts of each tile of the last partial round
+ * (1 = whole tiles only); full_tiles: tiles computed whole; ctas: the persistent grid.  Any pointer may be NULL. */
+void b200_gemm_debug_last_schedule(int* tiles, int* split, int* full_tiles, int* ctas);
 /* Tuning hook: K extent the tensor core accumulates before the epilogue folds the partial sum
  * into C with a rounded fp32 add (two-level accumulation of the split modes); 0 = whole K.
  * bf16x2_k sets both BF16X2 and F16X2.  A negative value restores the built-in default of its
