@@ -30,6 +30,7 @@ EXPORTS = [
     "b200_gemm_s8s32_host", "b200_gemm_s8s8_requant", "b200_gemm_f32_pack_b", "b200_gemm_f32_packed",
     "b200_gemm_f32_pack_free", "b200_gemm_f32_op", "b200_gemm_bf16_op", "b200_gemm_bf16_ex", "b200_gemm_f16_ex",
     "b200_gemm_bf16_epi", "b200_gemm_f16_epi", "b200_gemm_bf16_batched", "b200_gemm_f16_batched",
+    "b200_gemm_bf16_grouped", "b200_gemm_f16_grouped",
     "b200_gemm_s8s32_op", "b200_gemm_workspace_bytes_op",
     "b200_nccl_load", "b200_nccl_last_error", "b200_comm_unique_id", "b200_comm_init_rank",
     "b200_comm_destroy", "b200_rowpanel_create", "b200_rowpanel_destroy", "b200_rowpanel_slices", "b200_rowpanel_set_reserve_sms", "b200_rowpanel_trace", "b200_rowpanel_trace_dump", "b200_gemm_f32_rowpanel",
@@ -88,6 +89,10 @@ lib.b200_gemm_bf16_batched.argtypes = [_i, _i, _i, _i, _i, C.c_float, _vp, _i, _
                                        _i, _i, _vp]
 lib.b200_gemm_f16_batched.argtypes = [_i, _i, _i, _i, _i, C.c_float, _vp, _i, _ll, _vp, _i, _ll, C.c_float, _vp, _i, _ll,
                                       _i, _i, _vp]
+lib.b200_gemm_bf16_grouped.argtypes = [_i, _i, _i, _i, C.c_float, _vp, _i, _vp, _i, _ll, _vp, _i, C.c_float, _vp, _i, _i,
+                                       _vp]
+lib.b200_gemm_f16_grouped.argtypes = [_i, _i, _i, _i, C.c_float, _vp, _i, _vp, _i, _ll, _vp, _i, C.c_float, _vp, _i, _i,
+                                      _vp]
 lib.b200_gemm_s8s32_op.argtypes = [_i, _i, _i, _i, _i, _vp, _i, _vp, _i, _vp, _i, _vp]
 lib.b200_gemm_workspace_bytes_op.argtypes = [_i, _i, _i, _i, _i, _i]
 lib.b200_gemm_workspace_bytes_op.restype = C.c_size_t
@@ -256,6 +261,66 @@ def _gemm_batched(A, B, out, alpha, beta, bias, activation, out_dtype, stream):
     return out
 
 
+def grouped_layout(A, B, offs):
+    """(total_m, n, k, op_b, ldb, stride_b, groups) under which b200_gemm_*_grouped reads gemm(A, B, offs=offs) in place:
+    A (total_m x k) row-major, B (groups x k x n) whose last two dimensions resolve as batched_operand_layout does (so
+    W.transpose(-2, -1) of a (groups, n, k) weight is op_b = OP_T), offs a contiguous 1-D int32 tensor of groups
+    cumulative end rows.  Raises ValueError for anything else, a broadcast or overlapping B included; the device of the
+    tensors is not checked here."""
+    import torch
+    if A.dim() != 2 or B.dim() != 3:
+        raise ValueError(f"a grouped GEMM takes a 2-D A and a 3-D B, not {A.dim()}-D and {B.dim()}-D")
+    if not isinstance(offs, torch.Tensor) or offs.dtype != torch.int32 or offs.dim() != 1:
+        raise ValueError("offs must be a 1-D int32 tensor")
+    if not offs.is_contiguous():
+        raise ValueError("offs must be contiguous")
+    groups, k2, n = B.shape
+    total_m, k = A.shape
+    if offs.numel() != groups:
+        raise ValueError(f"offs has {offs.numel()} elements for {groups} groups of B")
+    if k2 != k:
+        raise ValueError(f"inner dimensions differ: A is {tuple(A.shape)}, B is {tuple(B.shape)}")
+    op_a, _ = operand_layout(tuple(A.shape), A.stride())
+    if op_a != OP_N:
+        raise ValueError("A of a grouped GEMM must be row-major")
+    op_b, ldb, sb = batched_operand_layout(tuple(B.shape), B.stride())
+    if groups > 1 and sb < (n if op_b == OP_T else k) * ldb:
+        raise ValueError(f"the groups of B must not overlap or be broadcast (stride(0) = {B.stride(0)})")
+    return total_m, n, k, op_b, ldb, sb, groups
+
+
+def _gemm_grouped(A, B, out, offs, alpha, beta, bias, activation, out_dtype, stream):
+    """gemm(A, B, offs=offs): rows [offs[g-1], offs[g]) of out = alpha * A[rows] @ B[g] + beta * out[rows], one launch
+    (b200_gemm_*_grouped)."""
+    import torch
+    if A.dtype != B.dtype:
+        raise TypeError(f"operands of different dtypes: {A.dtype} and {B.dtype}")
+    if A.dtype not in (torch.bfloat16, torch.float16):
+        raise TypeError(f"grouped operands must be bf16 or fp16, not {A.dtype}")
+    if bias is not None or activation is not None:
+        raise ValueError("the grouped GEMM has no bias / activation epilogue")
+    total_m, n, k, op_b, ldb, sb, groups = grouped_layout(A, B, offs)
+    cdt = out_dtype or (out.dtype if out is not None else torch.float32)
+    if cdt not in (torch.float32, A.dtype):
+        raise ValueError(f"{A.dtype} operands write float32 or {A.dtype} C, not {cdt}")
+    if out is not None:
+        if out.dtype != cdt:
+            raise ValueError(f"out is {out.dtype}, not {cdt}")
+        if out.dim() != 2 or tuple(out.shape) != (total_m, n):
+            raise ValueError(f"out must have shape {(total_m, n)}, not {tuple(out.shape)}")
+        if (n > 1 and out.stride(1) != 1) or (total_m > 1 and out.stride(0) < n):
+            raise ValueError("out must be row-major")
+    if not (A.is_cuda and B.is_cuda and offs.is_cuda and (out is None or out.is_cuda)):
+        raise ValueError("A, B, offs and out must be CUDA tensors")
+    if out is None:
+        assert beta == 0.0, "beta != 0 reads C: pass out"
+        out = torch.empty((total_m, n), dtype=cdt, device=A.device)
+    fn, ot = (lib.b200_gemm_bf16_grouped, OUT_BF16) if A.dtype == torch.bfloat16 else (lib.b200_gemm_f16_grouped, OUT_F16)
+    _check(fn(op_b, total_m, n, k, alpha, A.data_ptr(), _ld(A), B.data_ptr(), ldb, sb, offs.data_ptr(), groups, beta,
+              out.data_ptr(), _ld(out), OUT_F32 if cdt == torch.float32 else ot, _stream_ptr(stream)))
+    return out
+
+
 def _epilogue_args(A, B, bias, activation):
     """Checks a bias / activation request of gemm() (before anything touches the device); returns the ACT_* code."""
     import torch
@@ -273,8 +338,8 @@ def _epilogue_args(A, B, bias, activation):
     return ACTIVATIONS[activation]
 
 
-def gemm(A, B, out=None, *, alpha=1.0, beta=0.0, bias=None, activation=None, mode=F32_AUTO, out_dtype=None,
-         stream=None):
+def gemm(A, B, out=None, *, offs=None, alpha=1.0, beta=0.0, bias=None, activation=None, mode=F32_AUTO,
+         out_dtype=None, stream=None):
     """C = alpha * A @ B + beta * C for fp32 (any precision mode), bf16 (fp32 or bf16 C), fp16 (fp32 or fp16 C) and
     int8 (int32 C) CUDA tensors.  Each operand may be row-major or the transpose of a row-major matrix (x @ W.t()
     passes W as stored): it is read in place (b200_gemm_f32_op / _bf16_epi / _f16_epi / _s8s32_op), never
@@ -291,8 +356,19 @@ def gemm(A, B, out=None, *, alpha=1.0, beta=0.0, bias=None, activation=None, mod
     dimensions of each operand resolve as for 2-D operands and its batch stride is stride(0), so k.transpose(1, 2) and
     expand()ed operands (stride 0, broadcast) are read in place.  out is 3-D and row-major in its last two dimensions.
     3-D fp32 or int8 operands are a TypeError; a bias, an activation, unequal batch sizes or another out is a
-    ValueError."""
+    ValueError.
+
+    offs (a contiguous 1-D int32 CUDA tensor, one cumulative end row per group) makes it a grouped GEMM,
+    torch._grouped_mm(A, B, offs=offs): A is 2-D row-major (total_m x k), B is 3-D bf16 or fp16 (groups x k x n,
+    W.transpose(-2, -1) of a (groups, n, k) weight read in place), and rows [offs[g-1], offs[g]) of out are
+    alpha * A[rows] @ B[g] + beta * out[rows], every group in one launch (b200_gemm_bf16_grouped / _f16_grouped).  The
+    offsets stay on the device (the call never synchronises).  out is row-major (total_m x n); a new one is
+    torch.empty, so its rows from offs[-1] on are unspecified, as in torch.  out_dtype defaults to float32 as for every
+    16-bit gemm() (torch._grouped_mm's default is the operands' dtype).  fp32 or int8 operands are a TypeError; a bias,
+    an activation, another offs, A or out, or a broadcast or overlapping B is a ValueError."""
     import torch
+    if offs is not None:
+        return _gemm_grouped(A, B, out, offs, alpha, beta, bias, activation, out_dtype, stream)
     if A.dim() == 3 or B.dim() == 3:
         return _gemm_batched(A, B, out, alpha, beta, bias, activation, out_dtype, stream)
     epi = bias is not None or activation is not None

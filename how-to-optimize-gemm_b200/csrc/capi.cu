@@ -474,7 +474,7 @@ typedef const char* const KernelNames[4][3];
 
 // 16-bit operands: KIND_F16 (bf16, C fp32 or bf16) and KIND_FP16 (fp16, C fp32 or fp16).  E is the generic kernel's
 // element type of the kind (uint16_t holds bf16 bits).  names[16-bit C][EPI]; bat_names[16-bit C]: the strided-batched
-// kernels.
+// kernels; grp_names[16-bit C]: the grouped kernels (rows NN and NT only: A is row-major).
 template <int KIND> struct Kind16;
 template <> struct Kind16<KIND_F16> {
   using E = uint16_t;
@@ -485,6 +485,8 @@ template <> struct Kind16<KIND_F16> {
   static constexpr KernelNames names[2][2] = {{TC_NAMES("tc_bf16"), TC_NAMES("tc_bf16_epi")},
                                               {TC_NAMES("tc_bf16_obf16"), TC_NAMES("tc_bf16_obf16_epi")}};
   static constexpr KernelNames bat_names[2] = {TC_NAMES("tc_bf16_bat"), TC_NAMES("tc_bf16_obf16_bat")};
+  static constexpr const char* kGenericGrp = "generic_bf16_grp_64x64";
+  static constexpr KernelNames grp_names[2] = {TC_NAMES("tc_bf16_grp"), TC_NAMES("tc_bf16_obf16_grp")};
 };
 template <> struct Kind16<KIND_FP16> {
   using E = __half;
@@ -495,6 +497,8 @@ template <> struct Kind16<KIND_FP16> {
   static constexpr KernelNames names[2][2] = {{TC_NAMES("tc_f16"), TC_NAMES("tc_f16_epi")},
                                               {TC_NAMES("tc_f16_of16"), TC_NAMES("tc_f16_of16_epi")}};
   static constexpr KernelNames bat_names[2] = {TC_NAMES("tc_f16_bat"), TC_NAMES("tc_f16_of16_bat")};
+  static constexpr const char* kGenericGrp = "generic_f16_grp_64x64";
+  static constexpr KernelNames grp_names[2] = {TC_NAMES("tc_f16_grp"), TC_NAMES("tc_f16_of16_grp")};
 };
 
 // The 16-bit GEMM on the tensor cores (OutT float, bf16_out or f16_out): every layout is read in place by one launch.
@@ -1151,6 +1155,155 @@ int gemm16_batched(int op_a, int op_b, int m, int n, int k, float alpha, const u
   return tc16<KIND, typename K16::Out16, false, true>(op_a, op_b, m, n, k, A, lda, B, ldb, C, ldc, c, &bt);
 }
 
+// ---- grouped 16-bit GEMM (torch._grouped_mm) -----------------------------------------------------------------------
+// The offsets stay on the device: every launch below reads them there, and the host never waits for them.
+struct Group { const int32_t* offs; int count; int total_m; long long sb; };   // sb: elements between B_g and B_g+1
+
+// Upper bound of the 128-row tiles of a grouped call whatever its offsets: each group adds at most one partial tile.
+long long grouped_tile_rows(int total_m, int groups) { return (total_m + 127LL) / 128 + groups; }
+
+// k == 0 or alpha == 0: C = beta * C (C unread when beta == 0) on rows [0, end of the last group), one launch.
+template <typename T>
+int degenerate_grouped(int n, void* C, int ldc, const Group& gr, const Call& c) {
+  const dim3 grid((n + 255) / 256, gr.total_m < 4096 ? gr.total_m : 4096);
+  if (c.beta == 0.f) {          // 16-bit C is cleared as raw bits
+    using Z = typename std::conditional<sizeof(T) == 2, uint16_t, T>::type;
+    fill_zero_grouped_kernel<Z><<<grid, 256, 0, c.st>>>(gr.offs, gr.count, gr.total_m, n, static_cast<Z*>(C), ldc);
+    t_last_kernel = "fill_zero_grp";
+  } else {
+    scale_inplace_grouped_kernel<T><<<grid, 256, 0, c.st>>>(gr.offs, gr.count, gr.total_m, n, static_cast<T*>(C), ldc,
+                                                            c.beta);
+    t_last_kernel = "scale_inplace_grp";
+  }
+  g_launches++;
+  return last_launch_status();
+}
+
+// Operands TMA cannot describe: the CUDA-core kernel, each group as launch_generic computes its rows.  The grid counts
+// the 64-row blocks of every group at their upper bound; the column blocks run gridDim.y at a time.
+template <typename InT, typename OutT>
+int launch_generic_grouped(int op_b, int n, int k, const void* A, int lda, const void* B, int ldb, void* C, int ldc,
+                           const Group& gr, const char* name, const Call& c) {
+  const int tn = (n + 63) / 64;
+  dim3 grid((int)((gr.total_m + 63LL) / 64 + gr.count), tn < 65535 ? tn : 65535);
+  const long long b_rs = op_b ? 1 : ldb, b_cs = op_b ? ldb : 1;
+  gemm_generic_grouped_kernel<InT, OutT><<<grid, 256, 0, c.st>>>(
+      gr.offs, gr.count, gr.total_m, n, k, static_cast<const InT*>(A), lda, static_cast<const InT*>(B), b_rs, b_cs,
+      gr.sb, static_cast<OutT*>(C), ldc, c.axpby, c.alpha, c.beta);
+  g_launches++;
+  t_last_kernel = name;
+  return last_launch_status();
+}
+
+// The grouped tensor-core kernel: A (total_m x k, row-major) as one 2-D tensor map, B as a 3-D map with one entry per
+// group (BL = LAYOUT_MN: each B_g is k x n; LAYOUT_K: stored n x k).  The grid covers the tile bound; CTAs beyond the
+// tiles the offsets give find no work.  Whole tiles only.
+template <int KIND, int BN, int STAGES, typename OutT, int BL>
+int launch_tc_grouped(int n, int k, const void* A, int lda, const void* B, int ldb, void* C, int ldc, const Group& gr,
+                      const char* name, const Call& c) {
+  using Cfg = TcConfig<KIND, BN, STAGES, ProdSingle, 128, LAYOUT_K, BL>;
+  constexpr CUtensorMapDataType dt = KIND == KIND_F16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+  constexpr int OB = OutBytes<OutT>::V;
+  const unsigned long long bbytes = (unsigned long long)ldb * 2, b_rows = Cfg::B_MN ? k : n;
+  const unsigned long long eb = gr.count > 1 ? (unsigned long long)gr.sb * 2 : b_rows * bbytes;   // one group: any
+  CUtensorMap tmA, tmB;
+  int rc = get_map(&tmA, A, dt, 2, k, gr.total_m, (unsigned long long)lda * 2, Cfg::BK, Cfg::BM, 1);
+  if (rc) return rc;
+  if constexpr (!Cfg::B_MN)
+    rc = get_map(&tmB, B, dt, 2, k, b_rows, bbytes, Cfg::BK, Cfg::B_BOX_ROWS, 1, gr.count, eb);
+  else
+    rc = get_map(&tmB, B, dt, 2, n, b_rows, bbytes, Cfg::B_BOX_COLS, Cfg::BK, 1, gr.count, eb);
+  if (rc) return rc;
+  TcParams p;
+  memset(&p, 0, sizeof p);
+  p.C = C; p.ldc = ldc; p.M = gr.total_m; p.N = n; p.K = k;
+  const long long tile_rows = grouped_tile_rows(gr.total_m, gr.count);
+  p.tiles_m = (int)tile_rows;             // a bound: the kernel takes each group's own count from its table
+  p.tiles_n = (n + BN - 1) / BN;
+  p.group_m = (g_group_rows > 0 ? g_group_rows : 2048) / Cfg::TILE_M;
+  if (p.group_m < 1) p.group_m = 1;
+  p.vec_ok = aligned16(C) && ((long long)ldc * OB) % 16 == 0;     // every group's first row is then as aligned
+  p.chunk_kb = (k + Cfg::BK - 1) / Cfg::BK;
+  p.dbg_b_lbo = g_dbg_b_lbo; p.dbg_b_sbo = g_dbg_b_sbo;
+  p.axpby = c.axpby; p.alpha = c.alpha; p.beta = c.beta;
+  p.act = c.act;
+  p.split = 1;
+  const int tiles = (int)(tile_rows * p.tiles_n);                 // the entry point checked that it fits an int
+  p.full_tiles = tiles;
+  auto kern = gemm_tc_grouped_kernel<KIND, BN, STAGES, OutT, BL>;
+  if (int arc = ensure_smem_attr(kern, Cfg::SMEM_BYTES)) return arc;
+  const int units_max = t_ctx->sms - c.sm_reserve > 2 ? t_ctx->sms - c.sm_reserve : t_ctx->sms;
+  const int units = tiles < units_max ? tiles : units_max;
+  t_last_schedule = Schedule{tiles, 1, tiles, units};
+  const TcGroup tg{gr.offs, gr.count, gr.total_m};
+  g_ktimer.begin(c.st);
+  {
+    cudaError_t e = launch_pdl(kern, dim3(units), dim3(Cfg::THREADS), Cfg::SMEM_BYTES, c.st, 1, tmA, tmB, p, tg);
+    if (e != cudaSuccess) { cudaGetLastError(); return (int)e; }
+  }
+  g_ktimer.end(c.st);
+  g_launches++;
+  t_last_kernel = name;
+  return last_launch_status();
+}
+
+// Tile width from the tile bound (pick_bn over that many 128-row tile rows), then the layout of B.
+template <int KIND, typename OutT>
+int tc16_grouped(int op_b, int n, int k, const void* A, int lda, const void* B, int ldb, void* C, int ldc,
+                 const Group& gr, const Call& c) {
+  const KernelNames& names = Kind16<KIND>::grp_names[!std::is_same<OutT, float>::value];
+  return with_width(128, n, [&](auto W) {
+    using Wd = decltype(W);
+    if (op_b) return launch_tc_grouped<KIND, Wd::BN, Wd::STAGES, OutT, LAYOUT_K>(n, k, A, lda, B, ldb, C, ldc, gr,
+                                                                                  names[1][Wd::idx], c);
+    return launch_tc_grouped<KIND, Wd::BN, Wd::STAGES, OutT, LAYOUT_MN>(n, k, A, lda, B, ldb, C, ldc, gr,
+                                                                       names[0][Wd::idx], c);
+  }, (int)grouped_tile_rows(gr.total_m, gr.count));
+}
+
+// Rows [end_{g-1}, end_g) of C = round_out(fma(beta, float(C), alpha * A_rows op(B_g))), B_g = B + g * stride_b, with
+// end_{-1} = 0 and end_g = min(max(offs[g], end_{g-1}), total_m) on the device.  Argument rules (all before the device
+// is touched, all by division): those of gemm16 for an m = total_m call with op_a = N; negative sizes or stride;
+// groups > kMaxGroups; groups > 1 with B_g overlapping (stride_b < rows x ldb); (groups - 1) * stride_b above 2^60;
+// a tile bound the kernel's int work index cannot count; a null offs with work to do.  groups == 0, total_m == 0 or
+// n == 0 is a no-op.
+template <int KIND>
+int gemm16_grouped(int op_b, int total_m, int n, int k, float alpha, const uint16_t* A, int lda, const uint16_t* B,
+                   int ldb, long long stride_b, const int32_t* offs, int groups, float beta, void* C, int ldc,
+                   int out_type, cudaStream_t st) {
+  using K16 = Kind16<KIND>;
+  using E = typename K16::E;
+  if (groups < 0 || stride_b < 0 || groups > kMaxGroups) return B200_ERR_BAD_ARG;
+  if (out_type != B200_OUT_F32 && out_type != K16::OUT16) return B200_ERR_BAD_ARG;
+  if (op_b != B200_OP_N && op_b != B200_OP_T) return B200_ERR_BAD_ARG;
+  if (total_m < 0 || n < 0 || k < 0) return B200_ERR_BAD_ARG;
+  if (groups == 0) return 0;
+  int rc = check_args(total_m, n, k, A, lda, B, ldb, C, ldc, B200_OP_N, op_b);
+  if (rc == 1) return 0;
+  if (rc) return rc;
+  if (!offs) return B200_ERR_BAD_ARG;
+  const long long b_rows = op_b ? n : k;                                               // rows of one B_g as stored
+  if (groups > 1) {
+    if (stride_b < b_rows * ldb) return B200_ERR_BAD_ARG;                            // B_g would overlap
+    if (stride_b > (1LL << 60) / (groups - 1)) return B200_ERR_BAD_ARG;
+  }
+  // the tile bound at the narrowest width, with room for w + gridDim.x, in the kernel's int work index
+  const long long tiles_n = (n + 127LL) / 128;
+  if (tiles_n > 0x3FFFFFFFLL / grouped_tile_rows(total_m, groups)) return B200_ERR_BAD_ARG;
+  if ((rc = ensure_device())) return rc;
+  Call c{st};
+  if (alpha != 1.f || beta != 0.f) { c.axpby = 1; c.alpha = alpha; c.beta = beta; }
+  const bool c32 = out_type == B200_OUT_F32;
+  const Group gr{offs, groups, total_m, groups > 1 ? stride_b : 0};
+  if (k == 0 || alpha == 0.f) return c32 ? degenerate_grouped<float>(n, C, ldc, gr, c) : degenerate_grouped<E>(n, C, ldc, gr, c);
+  if (!tma_ok(A, lda, B, ldb, 2) || (groups > 1 && !batch_tma_ok(stride_b, b_rows, ldb, 2))) {
+    if (c32) return launch_generic_grouped<E, float>(op_b, n, k, A, lda, B, ldb, C, ldc, gr, K16::kGenericGrp, c);
+    return launch_generic_grouped<E, E>(op_b, n, k, A, lda, B, ldb, C, ldc, gr, K16::kGenericGrp, c);
+  }
+  if (c32) return tc16_grouped<KIND, float>(op_b, n, k, A, lda, B, ldb, C, ldc, gr, c);
+  return tc16_grouped<KIND, typename K16::Out16>(op_b, n, k, A, lda, B, ldb, C, ldc, gr, c);
+}
+
 static_assert(ACT_NONE == B200_ACT_NONE && ACT_RELU == B200_ACT_RELU && ACT_GELU == B200_ACT_GELU &&
               ACT_GELU_TANH == B200_ACT_GELU_TANH, "EpiAct follows the header's codes");
 
@@ -1333,6 +1486,20 @@ int b200_gemm_f16_batched(int op_a, int op_b, int m, int n, int k, float alpha, 
                           int ldc, long long stride_c, int batch, int out_type, void* stream) {
   return gemm16_batched<KIND_FP16>(op_a, op_b, m, n, k, alpha, dA, lda, stride_a, dB, ldb, stride_b, beta, dC, ldc,
                                    stride_c, batch, out_type, (cudaStream_t)stream);
+}
+
+int b200_gemm_bf16_grouped(int op_b, int total_m, int n, int k, float alpha, const uint16_t* dA, int lda,
+                           const uint16_t* dB, int ldb, long long stride_b, const int32_t* dOffs, int groups, float beta,
+                           void* dC, int ldc, int out_type, void* stream) {
+  return gemm16_grouped<KIND_F16>(op_b, total_m, n, k, alpha, dA, lda, dB, ldb, stride_b, dOffs, groups, beta, dC, ldc,
+                                  out_type, (cudaStream_t)stream);
+}
+
+int b200_gemm_f16_grouped(int op_b, int total_m, int n, int k, float alpha, const uint16_t* dA, int lda,
+                          const uint16_t* dB, int ldb, long long stride_b, const int32_t* dOffs, int groups, float beta,
+                          void* dC, int ldc, int out_type, void* stream) {
+  return gemm16_grouped<KIND_FP16>(op_b, total_m, n, k, alpha, dA, lda, dB, ldb, stride_b, dOffs, groups, beta, dC, ldc,
+                                   out_type, (cudaStream_t)stream);
 }
 
 int b200_gemm_s8s32(int m, int n, int k, const int8_t* dA, int lda, const int8_t* dB, int ldb,

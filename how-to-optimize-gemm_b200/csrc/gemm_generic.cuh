@@ -271,4 +271,120 @@ __global__ void fill_zero_batched_kernel(int batch, int M, int N, T* __restrict_
     for (int i = blockIdx.y; i < M; i += gridDim.y) C[z * c_bs + (long long)i * ldc + j] = (T)0;
 }
 
+// ---- grouped 16-bit forms ------------------------------------------------------------------------------------------
+// Group g is rows [end[g], end[g + 1]) of one stacked row-major A (total_m x k, pitch lda) and C, times B_g at
+// B + g * b_gs (group_table, ptx.cuh, clamps the offsets).  Kernels of their own beside the 2-D and batched ones.
+
+// gemm_generic_kernel's tile for 16-bit operands with the alpha / beta epilogue, on 64-row blocks that each lie inside
+// one group: blockIdx.x counts the blocks of every group in order (surplus blocks exit), blockIdx.y the column blocks,
+// gridDim.y at a time.  The same loads, the same fmaf chain in k order and the same store as the 2-D kernel, so every
+// group equals the 2-D generic call on its rows bit for bit.
+template <typename InT, typename OutT>
+__global__ void __launch_bounds__(256)
+gemm_generic_grouped_kernel(const int* __restrict__ offs, int groups, int total_m, int N, int K,
+                            const InT* __restrict__ A, long long lda, const InT* __restrict__ B, long long b_rs,
+                            long long b_cs, long long b_gs, OutT* __restrict__ C, long long ldc, int axpby, float alpha,
+                            float beta) {
+  static_assert(sizeof(InT) == 2, "grouped generic kernel: 16-bit operands");
+  __shared__ int grp_end[kMaxGroups + 1];
+  __shared__ int grp_blk[kMaxGroups + 1];
+  __shared__ float As[16][64 + 4];
+  __shared__ float Bs[16][64 + 4];
+  group_table(offs, groups, total_m, 64, grp_end, grp_blk);
+  const int q = blockIdx.x;
+  if (q >= grp_blk[groups]) return;                  // the grid counts every group's blocks at their upper bound
+  const int g = group_of(grp_blk, groups, q);
+  const int M = grp_end[g + 1] - grp_end[g];
+  const InT* Ag = A + (long long)grp_end[g] * lda;
+  const InT* Bg = B + g * b_gs;
+  OutT* Cg = C + (long long)grp_end[g] * ldc;
+  const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
+  const int m0 = (q - grp_blk[g]) * 64;
+  for (int n0 = blockIdx.y * 64; n0 < N; n0 += gridDim.y * 64) {
+    float acc[4][4];
+#pragma unroll
+    for (int i = 0; i < 4; i++)
+#pragma unroll
+      for (int j = 0; j < 4; j++) acc[i][j] = 0.f;
+    for (int k0 = 0; k0 < K; k0 += 16) {
+#pragma unroll
+      for (int r = 0; r < 4; r++) {
+        const int idx = threadIdx.x + r * 256;
+        const int am = idx >> 4, ak = idx & 15;
+        const int gm = m0 + am, gk = k0 + ak;
+        As[ak][am] = (gm < M && gk < K) ? LoadAs<InT>::ld(Ag + (long long)gm * lda + gk) : 0.f;
+        const int bk = idx >> 6, bn = idx & 63;
+        const int gk2 = k0 + bk, gn = n0 + bn;
+        Bs[bk][bn] = (gk2 < K && gn < N) ? LoadAs<InT>::ld(Bg + (long long)gk2 * b_rs + (long long)gn * b_cs) : 0.f;
+      }
+      __syncthreads();
+#pragma unroll
+      for (int kk = 0; kk < 16; kk++) {
+        float a[4], b[4];
+#pragma unroll
+        for (int i = 0; i < 4; i++) a[i] = As[kk][ty + 16 * i];
+#pragma unroll
+        for (int j = 0; j < 4; j++) b[j] = Bs[kk][tx + 16 * j];
+#pragma unroll
+        for (int i = 0; i < 4; i++)
+#pragma unroll
+          for (int j = 0; j < 4; j++) acc[i][j] = fmaf(a[i], b[j], acc[i][j]);
+      }
+      __syncthreads();                                 // also orders this column block's last reads before the next's
+    }
+#pragma unroll
+    for (int i = 0; i < 4; i++) {
+      const int gm = m0 + ty + 16 * i;
+      if (gm >= M) continue;
+#pragma unroll
+      for (int j = 0; j < 4; j++) {
+        const int gn = n0 + tx + 16 * j;
+        if (gn < N) {
+          float v = acc[i][j];
+          if (axpby) {
+            v *= alpha;
+            if (beta != 0.f) v = fmaf(beta, LoadAs<OutT>::ld(Cg + (long long)gm * ldc + gn), v);
+          }
+          store_out<float, OutT>(Cg + (long long)gm * ldc + gn, v);
+        }
+      }
+    }
+  }
+}
+
+// The rows a grouped call writes, min(max(0, offs[0..groups)), total_m) = end[groups] of group_table, computed by
+// every thread of the block.
+__device__ __forceinline__ int grouped_rows(const int* __restrict__ offs, int groups, int total_m, int* s_max) {
+  if (threadIdx.x == 0) *s_max = 0;
+  __syncthreads();
+  int v = 0;
+  for (int i = threadIdx.x; i < groups; i += blockDim.x) v = max(v, offs[i]);
+  atomicMax(s_max, v);
+  __syncthreads();
+  return min(*s_max, total_m);
+}
+
+// scale_inplace_kernel (s != 0) and fill_zero_kernel (s == 0) over rows [0, end[groups]): the k == 0 / alpha == 0
+// pass of a grouped call.
+template <typename T>
+__global__ void scale_inplace_grouped_kernel(const int* __restrict__ offs, int groups, int total_m, int N,
+                                             T* __restrict__ C, long long ldc, float s) {
+  __shared__ int s_max;
+  const int M = grouped_rows(offs, groups, total_m, &s_max);
+  for (int r = blockIdx.y; r < M; r += gridDim.y)
+    for (int c = blockIdx.x * blockDim.x + threadIdx.x; c < N; c += gridDim.x * blockDim.x) {
+      T* e = C + (long long)r * ldc + c;
+      store_out<float, T>(e, s * LoadAs<T>::ld(e));
+    }
+}
+template <typename T>
+__global__ void fill_zero_grouped_kernel(const int* __restrict__ offs, int groups, int total_m, int N,
+                                         T* __restrict__ C, long long ldc) {
+  __shared__ int s_max;
+  const int M = grouped_rows(offs, groups, total_m, &s_max);
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= N) return;
+  for (int i = blockIdx.y; i < M; i += gridDim.y) C[(long long)i * ldc + j] = (T)0;
+}
+
 }  // namespace b200

@@ -112,6 +112,13 @@ struct TcBatch {
   long long stride_c;      // elements between consecutive entries of C
 };
 
+// Grouped kernels (gemm_tc_grouped_kernel) only: the second kernel argument, as TcBatch is for the batched kernels.
+struct TcGroup {
+  const int* offs;         // [count] cumulative end rows of the groups, on the device (read after griddep_wait)
+  int count;               // groups, 1 .. kMaxGroups
+  int total_m;             // rows of the stacked A and C
+};
+
 // REGACC (split-precision fp32 modes): the tensor core adds into its fp32 accumulator with truncation,
 // so a long K chain drifts (error grows ~K).  K is cut into chunks of chunk_kb k-blocks; each chunk starts a
 // fresh wgmma accumulator that is added, with a rounded fp32 add, to the tile's running sum in registers.
@@ -742,6 +749,145 @@ gemm_tc_batched_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
           asm volatile("st.release.gpu.global.s32 [%0], %1;" ::"l"(flag), "r"(nv) : "memory");
         }
       }
+    }
+  }
+}
+
+// ---- grouped 16-bit GEMM (torch._grouped_mm) -----------------------------------------------------------------------
+// Group g is rows [end_g-1, end_g) of one stacked row-major A (total_m x k) and C, times its own B_g, entry g of a 3-D
+// tensor map (inner, rows, group) as the batched kernel reads it.  The group sizes exist only on the device, so the
+// schedule is built here: after griddep_wait every CTA reads the offsets, clamps them and scans the 128-row tiles of
+// each group into shared memory (group_table).  Work item w covers tiles x tiles_n, group outermost; producer and
+// consumers find w's group by binary search, and tile_coords walks the raster groups of that group's tiles_m.  A is
+// one 2-D map: a tile at row end_g-1 + 128 mb may load rows of the next group (or TMA's zeros past total_m), but each
+// row of C depends only on its own row of A and store_pair, on a TcParams whose C starts at row end_g-1 and whose M is
+// the group's rows, never stores those rows.  The MMA chain and the epilogue are the batched kernel's, so each group
+// equals the _ex call on its rows bit for bit.  No K-split tail: the host does not know the tile count.  A kernel of
+// its own, so that the other kernels keep their code exactly.
+template <int KIND, int BN, int STAGES, typename OutT, int BL>
+__global__ void __launch_bounds__((TcConfig<KIND, BN, STAGES, ProdSingle, 128, LAYOUT_K, BL>::THREADS), 1)
+gemm_tc_grouped_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                       const TcParams p, const TcGroup gp) {
+  using Cfg = TcConfig<KIND, BN, STAGES, ProdSingle, 128, LAYOUT_K, BL>;
+  using MMA = typename Cfg::MMA;
+  using Acc = typename MMA::Acc;
+  static_assert(KindTraits<KIND>::ELEM == 2 && (std::is_same<OutT, float>::value || OutBytes<OutT>::V == 2),
+                "grouped: 16-bit kinds with fp32 or 16-bit C");
+  static_assert(Cfg::SMEM_BYTES + 2 * (kMaxGroups + 1) * (int)sizeof(int) <= 232448,
+                "the pipeline and the group tables exceed the 227 KB of shared memory of sm_90");
+  __shared__ int grp_end[kMaxGroups + 1];     // group g: rows [grp_end[g], grp_end[g + 1])
+  __shared__ int grp_tile[kMaxGroups + 1];    // group g: tiles [grp_tile[g], grp_tile[g + 1]) of the tile order
+
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;   // swizzle atoms need 1 KB
+  const uint32_t sA = smem_base;
+  const uint32_t sB = sA + STAGES * Cfg::A_STAGE;
+  const uint32_t bar_full = sB + STAGES * Cfg::B_STAGE;
+  const uint32_t bar_empty = bar_full + 8 * STAGES;
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmA);
+    tma_prefetch_desc(&tmB);
+    for (int i = 0; i < STAGES; i++) {
+      mbar_init(bar_full + 8 * i, 1);
+      mbar_init(bar_empty + 8 * i, Cfg::CONSUMERS);
+    }
+    fence_barrier_init();
+  }
+  __syncthreads();
+  griddep_launch();
+  griddep_wait();
+  group_table(gp.offs, gp.count, gp.total_m, Cfg::BM, grp_end, grp_tile);     // ends in __syncthreads
+
+  const int num_items = grp_tile[gp.count] * p.tiles_n;       // CTAs past it have no work
+  const int num_kb = (p.K + Cfg::BK - 1) / Cfg::BK;
+
+  if (warp < 4) {
+    // ===================== TMA producer (warpgroup 0) =====================
+    setmaxnreg_dec<40>();
+    if (warp == 0 && lane == 0) {
+      int s = 0;
+      uint32_t ph = 0;
+      for (int w = blockIdx.x; w < num_items; w += gridDim.x) {
+        const int g = group_of(grp_tile, gp.count, w / p.tiles_n);
+        int mb, nb;
+        tile_coords(w - grp_tile[g] * p.tiles_n, grp_tile[g + 1] - grp_tile[g], p.tiles_n, p.group_m, mb, nb);
+        const int m0 = grp_end[g] + mb * Cfg::BM, n0 = nb * BN;
+        for (int kb = 0; kb < num_kb; kb++) {
+          mbar_wait(bar_empty + 8 * s, ph ^ 1);
+          const uint32_t full = bar_full + 8 * s;
+          mbar_arrive_expect_tx(full, Cfg::STAGE_BYTES);
+          tma_load_2d(sA + s * Cfg::A_STAGE, &tmA, full, kb * Cfg::BK, m0);
+          if constexpr (!Cfg::B_MN) {                 // B_g^T (n x k): one box of BN rows
+            tma_load_3d(sB + s * Cfg::B_STAGE, &tmB, full, kb * Cfg::BK, n0, g);
+          } else {
+#pragma unroll
+            for (int j = 0; j < Cfg::B_BOXES; j++)
+              tma_load_3d(sB + s * Cfg::B_STAGE + j * Cfg::B_BOX_BYTES, &tmB, full, n0 + j * Cfg::B_BOX_COLS,
+                          kb * Cfg::BK, g);
+          }
+          if (++s == STAGES) { s = 0; ph ^= 1; }
+        }
+      }
+    }
+  } else {
+    // ===================== consumers (warpgroups 1 and 2): MMA chain + epilogue =====================
+    setmaxnreg_inc<232>();
+    const int cw = warp / 4 - 1;                    // consumer warpgroup: rows [64 cw, 64 cw + 64) of the tile
+    const int ew = warp - 4;                        // consumer warp 0..7: 16 rows each
+    const bool wg_leader = (threadIdx.x & 127) == 0;
+    const uint32_t b_lbo = p.dbg_b_lbo ? (uint32_t)p.dbg_b_lbo : (uint32_t)Cfg::B_BOX_BYTES;
+    const uint32_t b_sbo = p.dbg_b_sbo ? (uint32_t)p.dbg_b_sbo : 1024u;
+    int s = 0;
+    uint32_t ph = 0;
+    Acc acc[Cfg::ACC];
+    for (int w = blockIdx.x; w < num_items; w += gridDim.x) {
+      const int g = group_of(grp_tile, gp.count, w / p.tiles_n);
+      int mb, nb;
+      tile_coords(w - grp_tile[g] * p.tiles_n, grp_tile[g + 1] - grp_tile[g], p.tiles_n, p.group_m, mb, nb);
+      const int m0 = mb * Cfg::BM, n0 = nb * BN;      // m0: row inside the group
+      int prev = -1;
+      for (int kb = 0; kb < num_kb; kb++) {
+        mbar_wait(bar_full + 8 * s, ph);
+        const uint32_t a0 = sA + s * Cfg::A_STAGE + cw * Cfg::A_WG;
+        const uint32_t b0 = sB + s * Cfg::B_STAGE;
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < Cfg::MMAS_PER_STAGE; k++) {
+          const uint64_t ad = make_sdesc(a0 + k * Cfg::A_KADV, 16, Cfg::A_SBO, Cfg::A_SWZ);
+          uint64_t bd;
+          if constexpr (Cfg::B_MN) bd = make_sdesc(b0 + k * Cfg::B_KADV, b_lbo, b_sbo, SWZ_128B);
+          else bd = make_sdesc(b0 + k * Cfg::B_KADV, 16, Cfg::A_SBO, Cfg::A_SWZ);
+          MMA::mma(acc, ad, bd, (kb | k) != 0 ? 1u : 0u);
+        }
+        wgmma_commit();
+        wgmma_wait<1>();                              // the previous k-block's products retired: its stage is free
+        if (prev >= 0 && wg_leader) mbar_arrive(bar_empty + 8 * prev);
+        prev = s;
+        if (++s == STAGES) { s = 0; ph ^= 1; }
+      }
+      wgmma_wait<0>();
+      wgmma_fence_regs(acc);
+      if (prev >= 0 && wg_leader) mbar_arrive(bar_empty + 8 * prev);
+
+      // ---- this warp's 16 rows of the tile into group g's rows of C ----
+      const bool fold = p.axpby && p.beta != 0.f;
+      const float al = p.axpby ? p.alpha : 1.f;
+      const float be = p.axpby ? p.beta : 1.f;
+      const int row0 = m0 + ew * 16 + (lane >> 2);
+      const int col0 = n0 + 2 * (lane & 3);
+      TcParams pc = p;
+      pc.C = static_cast<uint8_t*>(p.C) + (long long)grp_end[g] * p.ldc * OutBytes<OutT>::V;
+      pc.M = grp_end[g + 1] - grp_end[g];
+      const int ce[2] = {0, 0};
+#pragma unroll
+      for (int j = 0; j < BN / 8; j++)
+#pragma unroll
+        for (int h = 0; h < 2; h++)
+          store_pair<OutT>(pc, row0 + 8 * h, col0 + 8 * j, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], fold, false, al,
+                           be, 0, ce, 0.f, 0.f);
     }
   }
 }

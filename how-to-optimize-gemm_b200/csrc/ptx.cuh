@@ -160,4 +160,57 @@ __device__ __forceinline__ bool elect_one() {
   return pred != 0;
 }
 
+// ---- grouped GEMMs: the row blocks of each group, built on the device from its offsets ----------------------------
+// Groups of one grouped call (b200_gemm_bf16_grouped): the shared-memory tables below hold kMaxGroups + 1 entries.
+constexpr int kMaxGroups = 1024;
+
+// Every thread of the block calls this (after griddep_wait where the kernel has one).  Group g covers rows
+// [end[g], end[g + 1]) of the stacked A and C, with end[0] = 0 and end[g + 1] = min(max(offs[g], end[g]), total_m), so
+// any offsets give ordered, in-range groups; block[g] counts the `rows`-row blocks of the groups before g
+// (block[groups] = all of them).  Raw offsets are staged in end[], then warp 0 scans 32 groups per step: a running max
+// (the clamp), the blocks of each group, and their prefix sum, each carried from one step to the next.
+__device__ __forceinline__ void group_table(const int* __restrict__ offs, int groups, int total_m, int rows, int* end,
+                                            int* block) {
+  for (int i = threadIdx.x; i < groups; i += blockDim.x) end[i + 1] = offs[i];
+  __syncthreads();
+  if (threadIdx.x < 32) {
+    const int lane = threadIdx.x;
+    int run_end = 0, run_blocks = 0;
+    for (int base = 0; base < groups; base += 32) {
+      const int g = base + lane;
+      int e = max(g < groups ? end[g + 1] : 0, run_end);
+#pragma unroll
+      for (int d = 1; d < 32; d <<= 1) {
+        const int o = __shfl_up_sync(0xffffffffu, e, d);
+        if (lane >= d) e = max(e, o);
+      }
+      e = min(e, total_m);
+      int prev = __shfl_up_sync(0xffffffffu, e, 1);
+      if (lane == 0) prev = run_end;
+      int b = (e - prev) / rows + ((e - prev) % rows != 0);           // no int overflow near total_m = 2^31 - 1
+#pragma unroll
+      for (int d = 1; d < 32; d <<= 1) {
+        const int o = __shfl_up_sync(0xffffffffu, b, d);
+        if (lane >= d) b += o;
+      }
+      if (g < groups) { end[g + 1] = e; block[g + 1] = run_blocks + b; }
+      run_end = __shfl_sync(0xffffffffu, e, 31);
+      run_blocks += __shfl_sync(0xffffffffu, b, 31);
+    }
+    if (lane == 0) { end[0] = 0; block[0] = 0; }
+  }
+  __syncthreads();
+}
+
+// The group of row block q < block[groups]: the last g with block[g] <= q, which is never an empty group.
+__device__ __forceinline__ int group_of(const int* block, int groups, int q) {
+  int lo = 0, hi = groups - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (block[mid] <= q) lo = mid;
+    else hi = mid - 1;
+  }
+  return lo;
+}
+
 }  // namespace b200

@@ -208,6 +208,52 @@ int b200_gemm_f16_batched(int op_a, int op_b, int m, int n, int k, float alpha,
                           const uint16_t* dB, int ldb, long long stride_b, float beta,
                           void* dC, int ldc, long long stride_c, int batch, int out_type, void* stream);
 
+/* Grouped 16-bit GEMM (torch._grouped_mm(x, W, offs=offs); a mixture-of-experts layer): the rows routed to each group
+ * are stacked in one row-major A (total_m x k, lda >= k), the groups' B_g lie at dB + g * stride_b (elements), and
+ * dOffs holds `groups` int32 cumulative end rows on the DEVICE.  With end_{-1} = 0 and
+ *   end_g = min(max(dOffs[g], end_{g-1}), total_m),
+ * rows [end_{g-1}, end_g) of C (total_m x n, row-major, ldc >= n) become
+ *   round_out(fma(beta, float(C), alpha * A_rows * op(B_g))).
+ * op_b follows _ex: B200_OP_N, each B_g is k x n (ldb >= n); B200_OP_T, each B_g is stored n x k (ldb >= k), which is
+ * how a (groups, n, k) weight W is passed for x @ W_g^T.  A is always N.
+ * dOffs is read only on the device, after the work the stream already holds (a routing kernel may write it): the host
+ * never reads it and never synchronises, so the call can be captured in a CUDA graph and replayed with new offsets.
+ * The clamp makes every offset legal: non-monotone, negative or too-large offsets give the groups above (an empty
+ * group where an offset goes back), and no row outside [0, total_m) is ever read or written.  Rows at or after
+ * end_{groups-1} are never written.  Each group is bit for bit the _ex call on a contiguous copy of its rows of A and
+ * on B_g, at the same tile width (the tensor-core kernel never takes the K-split tail, so the _ex call with it off).
+ * Argument rules, each checked before the device is touched:
+ *   - the _ex rules for an m = total_m call with op_a = N: op_b, minimum ld, out_type pairing; beta == 0 never reads C;
+ *     alpha == 0 or k == 0 never reads A or B.
+ *   - negative sizes, groups or stride_b, and groups > 1024, are B200_ERR_BAD_ARG.
+ *   - groups > 1 with stride_b < (rows of B_g as stored) * ldb is B200_ERR_BAD_ARG: the B_g may not overlap or be
+ *     broadcast.  (groups == 1 ignores stride_b.)  So is (groups - 1) * stride_b above 2^60 elements.
+ *   - (ceil(total_m / 128) + groups) * ceil(n / 128) above 2^30 - 1 is B200_ERR_BAD_ARG: the kernel counts its tile
+ *     bound in an int.
+ *   - groups == 0, total_m == 0 or n == 0 is a no-op, NULL pointers included; a NULL pointer with work to do, dOffs
+ *     included, is B200_ERR_BAD_ARG.
+ * Routes, each one launch, no workspace:
+ *   - 16-byte-aligned A and B with lda, ldb and stride_b multiples of 16 bytes: the persistent tensor-core kernel.  It
+ *     builds its tile schedule from dOffs on the device; the host sizes its grid and tile width for the bound
+ *     ceil(total_m / 128) + groups tile rows (each group adds at most one partial tile), which
+ *     b200_gemm_debug_last_schedule reports as tiles (a bound, not the tiles the offsets give), with split 1.  Kernels
+ *     "tc_bf16_grp_128x256", "tc_bf16_obf16_grp_nt_128x192", "tc_f16_grp_128x128", "tc_f16_of16_grp_nt_128x256", ...
+ *   - any other operands: the generic kernel, "generic_bf16_grp_64x64" / "generic_f16_grp_64x64", every group bit for
+ *     bit as the 2-D generic kernel computes its rows.
+ *   - alpha == 0 or k == 0: one element-wise pass over rows [0, end_{groups-1}), "fill_zero_grp" (beta == 0) or
+ *     "scale_inplace_grp".
+ * No bias or activation epilogue. */
+int b200_gemm_bf16_grouped(int op_b, int total_m, int n, int k, float alpha,
+                           const uint16_t* dA, int lda,
+                           const uint16_t* dB, int ldb, long long stride_b,
+                           const int32_t* dOffs, int groups, float beta,
+                           void* dC, int ldc, int out_type, void* stream);
+int b200_gemm_f16_grouped(int op_b, int total_m, int n, int k, float alpha,
+                          const uint16_t* dA, int lda,
+                          const uint16_t* dB, int ldb, long long stride_b,
+                          const int32_t* dOffs, int groups, float beta,
+                          void* dC, int ldc, int out_type, void* stream);
+
 /* 16-bit operands with a bias vector and an activation fused into the epilogue (cuBLASLt's CUBLASLT_EPILOGUE_BIAS,
  * _RELU_BIAS, _GELU_BIAS): C = round_out(act(alpha * op(A)*op(B) + beta * C + bias)), what a PyTorch
  * act(F.linear(x, W, b)) computes, in one launch.  Arguments as b200_gemm_bf16_ex / b200_gemm_f16_ex, plus:
@@ -297,6 +343,8 @@ int b200_gemm_s8s32_host(int m, int n, int k,
  *   bf16 -> fp32 / bf16      1   1                1                1     operands read in place
  *   fp16 -> fp32 / fp16      1   1                1                1     operands read in place (b200_gemm_f16_ex)
  *   bf16 / fp16 batched      1   1                1                1     every entry in one launch (_batched; also
+ *                                                                        generic and alpha == 0 / k == 0: 1)
+ *   bf16 / fp16 grouped      1   1                -                -     every group in one launch (_grouped; also
  *                                                                        generic and alpha == 0 / k == 0: 1)
  *   TF32, int8               2   1                3                2     transposes into the workspace
  *   BF16X3, BF16X2           2   2                2                2     one split launch for both operands
