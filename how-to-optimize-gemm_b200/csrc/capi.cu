@@ -70,9 +70,13 @@ struct Call {
 // ---- per-device state ------------------------------------------------------------------------------
 // Everything the library caches on a GPU lives in the context of THAT device (flags, split workspace,
 // host-path staging buffers and streams, which kernels already had their dynamic shared memory limit
-// raised), so one process may drive several GPUs (one host thread or one stream per GPU).  The split
-// workspace is shared by all streams of a device: users are serialised by ws_mu on the host and by an
-// event recorded after the consuming GEMM on the device (a call on another stream waits for it).
+// raised), so one process may drive several GPUs (one host thread or one stream per GPU).  Two things are
+// shared by all streams of a device, and each is ordered between streams by events:
+//   - the split workspace and the F16X2 maxima: users are serialised by ws_mu on the host and by an event
+//     recorded after the consuming GEMM on the device (a call on another stream waits for it);
+//   - the K-split flag slots: a slot taken on another stream than its last user's waits for the event
+//     recorded after that user's launch (take_flag_slot).
+constexpr int kFlagSlots = 16;
 struct Scratch { void* p = nullptr; size_t bytes = 0; };
 struct HostPipe {
   bool ready = false;
@@ -96,8 +100,14 @@ struct DevCtx {
   int ok = 0;          // 1 usable, -1 not usable, 0 unknown
   int sms = 0;
   int dev = -1;
-  int* flags = nullptr;      // tail-split ordering flags (zero between launches), 16 rotating slots of 1024 ints
-  unsigned flag_slot = 0;
+  int* flags = nullptr;      // tail-split ordering flags (zero between launches), kFlagSlots rotating slots of 1024 ints
+  std::mutex flag_mu;        // held from taking a slot until its launch is queued and flag_user[slot] updated
+  unsigned flag_slot = 0;    // counts split launches only
+  struct FlagUser {
+    cudaStream_t st = nullptr;       // stream of the slot's last launch
+    cudaEvent_t ev = nullptr;        // recorded on st right after that launch
+    bool used = false;
+  } flag_user[kFlagSlots];
   // split-precision workspace (planes of A and B, row / column maxima): cached, grow-only
   std::mutex ws_mu;
   Scratch ws;
@@ -131,11 +141,19 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t,
 EncodeTiledFn g_encode = nullptr;
 
 thread_local DevCtx* t_ctx = nullptr;   // context of the device current on this thread (set by ensure_device)
+thread_local int t_bound_dev = -1;      // device whose primary CUDA context this thread has made current
 
 // Binds t_ctx to the CUDA device current on the calling thread, initialising its context on first use.
 int ensure_device() {
   int dev = -1;
   if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= kMaxDevices) { cudaGetLastError(); t_ctx = nullptr; return B200_ERR_NO_DEVICE; }
+  // cudaGetDevice does not make a context current, and a host thread that has made no other runtime call has none:
+  // the first driver call of a compute call (cuTensorMapEncodeTiled) would then fail with an invalid context.
+  // cudaSetDevice makes the device's primary context current, once per thread and device.
+  if (t_bound_dev != dev) {
+    if (cudaSetDevice(dev) != cudaSuccess) { cudaGetLastError(); t_ctx = nullptr; return B200_ERR_NO_DEVICE; }
+    t_bound_dev = dev;
+  }
   DevCtx* c = &g_ctx[dev];
   t_ctx = c;
   if (c->ok == 1) return 0;
@@ -156,13 +174,18 @@ int ensure_device() {
     g_encode = reinterpret_cast<EncodeTiledFn>(fn);
   }
   if (!c->flags) {
-    if (cudaMalloc(&c->flags, 16 * 1024 * sizeof(int)) != cudaSuccess || cudaMemset(c->flags, 0, 16 * 1024 * sizeof(int)) != cudaSuccess) {
+    if (cudaMalloc(&c->flags, kFlagSlots * 1024 * sizeof(int)) != cudaSuccess ||
+        cudaMemset(c->flags, 0, kFlagSlots * 1024 * sizeof(int)) != cudaSuccess) {
       cudaGetLastError(); c->flags = nullptr; c->ok = -1; return B200_ERR_NO_DEVICE;
     }
   }
   if (!c->ws_event && cudaEventCreateWithFlags(&c->ws_event, cudaEventDisableTiming) != cudaSuccess) {
     cudaGetLastError(); c->ok = -1; return B200_ERR_NO_DEVICE;
   }
+  for (auto& u : c->flag_user)
+    if (!u.ev && cudaEventCreateWithFlags(&u.ev, cudaEventDisableTiming) != cudaSuccess) {
+      cudaGetLastError(); u.ev = nullptr; c->ok = -1; return B200_ERR_NO_DEVICE;
+    }
   c->dev = dev;
   c->sms = prop.multiProcessorCount;
   c->ok = 1;
@@ -306,6 +329,46 @@ int launch_generic_requant(int m, int n, int k, const int8_t* A, int lda, const 
   return last_launch_status();
 }
 
+// ---- K-split flag slots --------------------------------------------------------------------
+// Every launch with split > 1 takes the next of the device's kFlagSlots slots, whatever its stream, and clears it
+// on its stream before the kernel runs.  Parts > 0 of a split tile spin until its flag reaches their part number.
+// So a slot that comes back while its previous launch still runs on another stream must not be cleared or
+// published into before that launch is done: the clear would strand a waiting part, and a publish would let it fold
+// into C before the parts ahead of it had stored.  The caller holds t_ctx->flag_mu from here until
+// release_flag_slot, so that two host threads never take one slot and the next taker sees this launch's event.
+// On the slot's stream of last use nothing is waited for: stream order already serialises the two launches.
+// Under stream capture nothing is waited for or recorded (an event recorded outside the capture cannot be waited
+// on inside it), and *user stays null: a replayed graph is not ordered against split launches on other streams.
+int take_flag_slot(cudaStream_t st, int** flags, DevCtx::FlagUser** user) {
+  DevCtx* c = t_ctx;
+  const unsigned slot = c->flag_slot++ % kFlagSlots;
+  *flags = c->flags + slot * 1024;
+  *user = nullptr;
+  cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+  if (cudaStreamIsCapturing(st, &cs) != cudaSuccess) { cudaGetLastError(); cs = cudaStreamCaptureStatusActive; }
+  DevCtx::FlagUser* u = &c->flag_user[slot];
+  cudaError_t e;
+  if (cs == cudaStreamCaptureStatusNone) {
+    // the per-thread default stream is one handle for a different stream on every host thread
+    if (u->used && (u->st != st || st == cudaStreamPerThread) && (e = cudaStreamWaitEvent(st, u->ev, 0)) != cudaSuccess) {
+      cudaGetLastError();
+      return (int)e;
+    }
+    *user = u;
+  }
+  // the ordering flags start from zero whatever an aborted earlier launch left behind
+  if ((e = cudaMemsetAsync(*flags, 0, 1024 * sizeof(int), st)) != cudaSuccess) { cudaGetLastError(); return (int)e; }
+  return 0;
+}
+// Records the event the slot's next taker on another stream waits for: right after the launch (whether or not it
+// was accepted: the clear before it was queued).
+void release_flag_slot(DevCtx::FlagUser* u, cudaStream_t st) {
+  if (!u) return;
+  if (cudaEventRecord(u->ev, st) != cudaSuccess) { cudaGetLastError(); return; }
+  u->st = st;
+  u->used = true;
+}
+
 // ---- tensor-core launch -------------------------------------------------------------------
 int g_force_bn = 0;          // test/tuning hook (b200_gemm_debug_set_bn): 0 = heuristic
 int g_group_rows = 0;         // tuning hook: rows per raster group of the tensor-core kernels (0 = 2048)
@@ -401,10 +464,12 @@ int launch_tc(int m, int n, int k, const void* A, long long lda, int a_rows_tota
   }
   p.split = split;
   p.full_tiles = split > 1 ? tiles - rem : tiles;
-  p.flags = t_ctx->flags + (t_ctx->flag_slot++ % 16) * 1024;
-  if (split > 1) {          // the ordering flags start from zero whatever an aborted earlier launch left behind
-    cudaError_t e = cudaMemsetAsync(p.flags, 0, 1024 * sizeof(int), c.st);
-    if (e != cudaSuccess) { cudaGetLastError(); return (int)e; }
+  p.flags = t_ctx->flags;                   // read by split tiles only
+  std::unique_lock<std::mutex> flag_lk;     // a split launch's slot: held until its event is recorded
+  DevCtx::FlagUser* flag_user = nullptr;
+  if (split > 1) {
+    flag_lk = std::unique_lock<std::mutex>(t_ctx->flag_mu);
+    if (int rc = take_flag_slot(c.st, &p.flags, &flag_user)) return rc;
   }
   const int items = p.full_tiles + (tiles - p.full_tiles) * split;
   const int units = items < units_max ? items : units_max;
@@ -414,6 +479,7 @@ int launch_tc(int m, int n, int k, const void* A, long long lda, int a_rows_tota
     cudaError_t e;
     if constexpr (BATCHED) e = launch_pdl(kern, dim3(units), dim3(Cfg::THREADS), Cfg::SMEM_BYTES, c.st, 1, tmA, tmB, p, bt);
     else e = launch_pdl(kern, dim3(units), dim3(Cfg::THREADS), Cfg::SMEM_BYTES, c.st, 1, tmA, tmB, p);
+    release_flag_slot(flag_user, c.st);
     if (e != cudaSuccess) { cudaGetLastError(); return (int)e; }
   }
   g_ktimer.end(c.st);

@@ -28,7 +28,8 @@
  * as void*; NULL = the legacy default stream the reference harness uses,
  * cuda/test_MMult.cpp:98-110), never synchronise or allocate in steady state (see
  * b200_gemm_reserve_workspace for the first call) and may be called on any stream of any
- * sm_90 device (per-device state; make the device current on the calling thread).  They return 0 on success or a cudaError_t /
+ * sm_90 device (per-device state; make the device current on the calling thread; a thread needs no CUDA call of
+ * its own before the first: that call makes the device's primary context current).  They return 0 on success or a cudaError_t /
  * negative B200_ERR_* code.  There is NO CPU fallback: without a CUDA device of
  * compute capability 9.x every compute entry point returns
  * B200_ERR_NO_DEVICE.
@@ -120,8 +121,10 @@ void b200_gemm_set_default_f32_mode(int mode);
  * b200_gemm_workspace_bytes(m, n, k, mode) is b200_gemm_workspace_bytes_op(B200_OP_N, B200_OP_N, m, n, k, mode):
  * for an explicit mode exactly what its route reserves, for AUTO the largest of the routes AUTO may take at this
  * size (plain or with a general alpha / beta).  State is per device:
- * one process may drive several GPUs (make the device current on the calling thread); calls on different
- * streams of one device are serialised on the workspace by an event, not by the host.
+ * one process may drive several GPUs (make the device current on the calling thread).  Calls on different
+ * streams (or host threads) of one device are ordered by events, not by the host, on what they share: the
+ * workspace, the F16X2 column maxima and the K-split flag slots.  Under stream capture the flag slots are not
+ * ordered: a replayed graph must not run beside split-tail calls on other streams of the device.
  * The same workspace holds B^T for B200_F32_TF32 (counted by b200_gemm_workspace_bytes) and for the int8 entry
  * points (n * k16 bytes, k16 = k rounded up to 16), and the bf16 expansions of both operands for b200_gemm_mxf4
  * (round1024(2 * m * kpad) + 2 * kpad * n8 bytes, kpad = k rounded up to 128, n8 = n rounded up to 8): reserve
