@@ -383,15 +383,28 @@ int g_ffma_halves = 1;        // strict kernel: split the tail round into half t
 // Stacked planes (split modes) lie along the rows, plane p at row p * a_plane_rows / p * b_plane_rows.  tf32 and
 // int8 take K-major A and B only (launch_tc_kmajor builds them).
 // EPI: the bias / activation kernel (c.bias / c.act), which never takes the K-split tail.
-// BATCHED: the strided-batched kernel over *bat (16-bit kinds, single plane): A and B as 3-D tensor maps, the work of
-// every entry in one launch, and the K-split tail (fp32 C) on the last partial round of the whole batch.
-struct Batch { int count; long long sa, sb, sc; };    // entries; strides in elements (0 broadcasts A or B)
+// STACK: the stacked kernel (gemm_tc_stacked_kernel; 16-bit kinds, single plane) over *stk, the work of every entry in
+// one launch, with A and B as 3-D tensor maps.
+//   STACK_BATCH: entry b of each operand at X + b * stride (elements; 0 broadcasts A or B), and the K-split tail (fp32
+//   C) on the last partial round of the whole batch.
+//   STACK_GROUP: groups of rows [end_g-1, end_g) of one row-major A and C (m = total_m rows; sa = sc = 0: A and C are
+//   broadcast) times B_g = B + g * sb, with the ends read on the device.  The tile rows are a bound,
+//   grouped_tile_rows, and there is no K split: the host does not know the tile count.
+enum Stacking { STACK_NONE, STACK_BATCH, STACK_GROUP };
+struct Stack {
+  int count;               // entries of a batch, or groups
+  long long sa, sb, sc;    // elements between consecutive entries of A, B and C
+  const int32_t* offs;     // STACK_GROUP: [count] cumulative end rows of the groups, on the device
+};
+// Upper bound of the 128-row tiles of a grouped call whatever its offsets: each group adds at most one partial tile.
+long long grouped_tile_rows(int total_m, int groups) { return (total_m + 127LL) / 128 + groups; }
+
 template <int KIND, int BN, int STAGES, typename OutT, class Prod = ProdSingle, int A_ROW_BYTES = 128, int AL = LAYOUT_K,
-          int BL = KindTraits<KIND>::B_LAYOUT, bool EPI = false, bool BATCHED = false>
+          int BL = KindTraits<KIND>::B_LAYOUT, bool EPI = false, int STACK = STACK_NONE>
 int launch_tc(int m, int n, int k, const void* A, long long lda, int a_rows_total, int a_plane_rows,
               const void* B, long long ldb, int b_rows_total, int b_plane_rows, void* C, int ldc,
               const char* name, const Call& c, int chunk_k = 0, const float* row_max = nullptr,
-              const float* col_max = nullptr, const Batch* bat = nullptr) {
+              const float* col_max = nullptr, const Stack* stk = nullptr) {
   using Cfg = TcConfig<KIND, BN, STAGES, Prod, A_ROW_BYTES, AL, BL>;
   using T = KindTraits<KIND>;
   constexpr CUtensorMapDataType dt = KIND == KIND_F16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
@@ -402,10 +415,10 @@ int launch_tc(int m, int n, int k, const void* A, long long lda, int a_rows_tota
   constexpr int kswz = A_ROW_BYTES == 128 ? 1 : 3;          // K-major rows: SWIZZLE_128B or _64B
   // 3-D maps: a broadcast operand is one entry (its entry stride is then any legal value: the matrix's own extent)
   unsigned long long ea = 0, eab = 0, eb = 0, ebb = 0;
-  if constexpr (BATCHED) {
+  if constexpr (STACK != STACK_NONE) {
     const unsigned long long abytes = (unsigned long long)lda * T::ELEM, bbytes = (unsigned long long)ldb * T::ELEM;
-    ea = bat->sa ? bat->count : 1; eab = bat->sa ? (unsigned long long)bat->sa * T::ELEM : a_rows_total * abytes;
-    eb = bat->sb ? bat->count : 1; ebb = bat->sb ? (unsigned long long)bat->sb * T::ELEM : b_rows_total * bbytes;
+    ea = stk->sa ? stk->count : 1; eab = stk->sa ? (unsigned long long)stk->sa * T::ELEM : a_rows_total * abytes;
+    eb = stk->sb ? stk->count : 1; ebb = stk->sb ? (unsigned long long)stk->sb * T::ELEM : b_rows_total * bbytes;
   }
   int rc;
   if constexpr (Cfg::A_MN)
@@ -423,13 +436,14 @@ int launch_tc(int m, int n, int k, const void* A, long long lda, int a_rows_tota
   if (rc) return rc;
   TcParams p;
   p.C = C; p.ldc = ldc; p.M = m; p.N = n; p.K = k;
-  p.tiles_m = (m + Cfg::TILE_M - 1) / Cfg::TILE_M;
+  // grouped: a bound, the kernel takes each group's own count from its table
+  p.tiles_m = STACK == STACK_GROUP ? (int)grouped_tile_rows(m, stk->count) : (m + Cfg::TILE_M - 1) / Cfg::TILE_M;
   p.tiles_n = (n + BN - 1) / BN;
   p.group_m = (g_group_rows > 0 ? g_group_rows : 2048) / Cfg::TILE_M;     // rows of A per raster group
   if (p.group_m < 1) p.group_m = 1;
   constexpr int OB = OutBytes<OutT>::V;
   p.vec_ok = aligned16(C) && ((long long)ldc * OB) % 16 == 0;
-  if constexpr (BATCHED) p.vec_ok = p.vec_ok && bat->sc % (16 / OB) == 0;    // every entry's C base as aligned
+  if constexpr (STACK != STACK_NONE) p.vec_ok = p.vec_ok && stk->sc % (16 / OB) == 0;    // every entry's C base as aligned
   p.a_plane_rows = a_plane_rows; p.b_plane_rows = b_plane_rows;
   p.chunk_kb = chunk_k > 0 ? (chunk_k + Cfg::BK - 1) / Cfg::BK : (k + Cfg::BK - 1) / Cfg::BK;
   if (p.chunk_kb < 1) p.chunk_kb = 1;
@@ -441,21 +455,23 @@ int launch_tc(int m, int n, int k, const void* A, long long lda, int a_rows_tota
   if constexpr (EPI) p.bias = c.bias;            // shares col_max's slot: EPI kernels are never scaled
   p.stream_c = g_stream_c < 0 ? (g_stream_c = (getenv("B200GEMM_STREAM_C") ? atoi(getenv("B200GEMM_STREAM_C")) : kStreamCDefault)) : g_stream_c;
   auto kern = [] {
-    if constexpr (BATCHED) return gemm_tc_batched_kernel<KIND, BN, STAGES, OutT, AL, BL>;
+    if constexpr (STACK != STACK_NONE) return gemm_tc_stacked_kernel<KIND, BN, STAGES, OutT, AL, BL, STACK == STACK_GROUP>;
     else return gemm_tc_kernel<KIND, BN, STAGES, OutT, Prod, A_ROW_BYTES, AL, BL, EPI>;
   }();
   if (int arc = ensure_smem_attr(kern, Cfg::SMEM_BYTES)) return arc;
-  TcBatch bt{1, 0, 0, 0};
-  if constexpr (BATCHED) bt = TcBatch{bat->count, bat->sa ? 1 : 0, bat->sb ? 1 : 0, bat->sc};
-  // the whole batch's tiles (the entry point checked that they and their split parts fit the kernel's int index)
-  int tiles = p.tiles_m * p.tiles_n * bt.count;
+  TcStack ts{1, 0, 0, 0, nullptr};
+  if constexpr (STACK != STACK_NONE) ts = TcStack{stk->count, stk->sa ? 1 : 0, stk->sb ? 1 : 0, stk->sc, stk->offs};
+  // the whole batch's tiles, or the grouped call's bound on them (the entry point checked that they and their split
+  // parts fit the kernel's int index)
+  int tiles = p.tiles_m * p.tiles_n * (STACK == STACK_GROUP ? 1 : ts.count);
   const int units_max = t_ctx->sms - c.sm_reserve > 2 ? t_ctx->sms - c.sm_reserve : t_ctx->sms;   // one CTA per SM
   // Wave quantisation: the last, partial round of tiles (or the only round of a small problem) is
   // cut along K so that every CTA has work: rem tiles x split parts <= units.
   const int num_kb = (k + Cfg::BK - 1) / Cfg::BK;
   const int rem = tiles % units_max;
   int split = 1;
-  if (!EPI && g_split_tail && OB == 4 && rem > 0) {    // an activation must see the complete sum: no split
+  // an activation must see the complete sum, and a grouped call's tile count is not known here: no split
+  if (!EPI && STACK != STACK_GROUP && g_split_tail && OB == 4 && rem > 0) {
     split = units_max / rem;
     if (split > 4) split = 4;
     if (split > num_kb / 8) split = num_kb / 8;       // keep >= 8 k-blocks per part
@@ -477,7 +493,7 @@ int launch_tc(int m, int n, int k, const void* A, long long lda, int a_rows_tota
   g_ktimer.begin(c.st);
   {
     cudaError_t e;
-    if constexpr (BATCHED) e = launch_pdl(kern, dim3(units), dim3(Cfg::THREADS), Cfg::SMEM_BYTES, c.st, 1, tmA, tmB, p, bt);
+    if constexpr (STACK != STACK_NONE) e = launch_pdl(kern, dim3(units), dim3(Cfg::THREADS), Cfg::SMEM_BYTES, c.st, 1, tmA, tmB, p, ts);
     else e = launch_pdl(kern, dim3(units), dim3(Cfg::THREADS), Cfg::SMEM_BYTES, c.st, 1, tmA, tmB, p);
     release_flag_slot(flag_user, c.st);
     if (e != cudaSuccess) { cudaGetLastError(); return (int)e; }
@@ -490,7 +506,7 @@ int launch_tc(int m, int n, int k, const void* A, long long lda, int a_rows_tota
 
 // Tile width: fewest "wave x tile-time" units over the persistent grid (tile time ~ BN plus a
 // fixed per-tile cost); 128 x 256 has the best operand reuse, narrower tiles quantise better.  A strided batch counts
-// the tiles of all its entries (one persistent grid walks them all).
+// the tiles of all its entries (one persistent grid walks them all), a grouped call its tile bound.
 int pick_bn(int m, int n, bool allow256, bool allow192 = true, int batch = 1) {
   if (g_force_bn == 128 || (g_force_bn == 192 && allow192) || (g_force_bn == 256 && allow256)) return g_force_bn;
   const int cands[3] = {256, 192, 128};
@@ -524,12 +540,13 @@ int with_width(int m, int n, F&& f, int batch = 1) {
 }
 
 // Calls f with the kernel layouts (AL, BL) of (op_a, op_b) and their index: 0 = NN, 1 = NT (B given as B^T), 2 = TN
-// (A given as A^T), 3 = TT.  A^T is the MN-major A, B^T the K-major B.
+// (A given as A^T), 3 = TT.  A^T is the MN-major A, B^T the K-major B.  !ALLOW_AT: row-major A only.
 template <int A_L, int B_L, int I> struct Layout { static constexpr int AL = A_L, BL = B_L, idx = I; };
-template <class F>
+template <bool ALLOW_AT = true, class F>
 int with_layout(int op_a, int op_b, F&& f) {
   if (!op_a) return op_b ? f(Layout<LAYOUT_K, LAYOUT_K, 1>()) : f(Layout<LAYOUT_K, LAYOUT_MN, 0>());
-  return op_b ? f(Layout<LAYOUT_MN, LAYOUT_K, 3>()) : f(Layout<LAYOUT_MN, LAYOUT_MN, 2>());
+  if constexpr (!ALLOW_AT) return B200_ERR_BAD_ARG;
+  else return op_b ? f(Layout<LAYOUT_MN, LAYOUT_K, 3>()) : f(Layout<LAYOUT_MN, LAYOUT_MN, 2>());
 }
 
 // Kernel names by [layout index][width index].
@@ -568,21 +585,25 @@ template <> struct Kind16<KIND_FP16> {
 };
 
 // The 16-bit GEMM on the tensor cores (OutT float, bf16_out or f16_out): every layout is read in place by one launch.
-// EPI: the bias / activation kernels.  BATCHED: the strided batch *bat in one launch (not with EPI).
-template <int KIND, typename OutT, bool EPI, bool BATCHED = false>
+// EPI: the bias / activation kernels.  STACK: the stacked call *stk in one launch (not with EPI; see launch_tc).
+template <int KIND, typename OutT, bool EPI, int STACK = STACK_NONE>
 int tc16(int op_a, int op_b, int m, int n, int k, const void* A, int lda, const void* B, int ldb, void* C, int ldc,
-         const Call& c, const Batch* bat = nullptr) {
-  static_assert(!(EPI && BATCHED), "the batched kernels have no bias / activation epilogue");
-  const KernelNames& names = BATCHED ? Kind16<KIND>::bat_names[!std::is_same<OutT, float>::value]
-                                     : Kind16<KIND>::names[!std::is_same<OutT, float>::value][EPI];
-  return with_layout(op_a, op_b, [&](auto L) {
+         const Call& c, const Stack* stk = nullptr) {
+  static_assert(!(EPI && STACK != STACK_NONE), "the stacked kernels have no bias / activation epilogue");
+  constexpr bool c16 = !std::is_same<OutT, float>::value;
+  const KernelNames& names = STACK == STACK_BATCH ? Kind16<KIND>::bat_names[c16]
+                           : STACK == STACK_GROUP ? Kind16<KIND>::grp_names[c16] : Kind16<KIND>::names[c16][EPI];
+  // pick_bn: a batch's tiles are those of all its entries; a grouped call's, its bound of tile rows, one row each
+  const int bn_m = STACK == STACK_GROUP ? 128 : m;
+  const int bn_batch = STACK == STACK_GROUP ? (int)grouped_tile_rows(m, stk->count) : stk ? stk->count : 1;
+  return with_layout<STACK != STACK_GROUP>(op_a, op_b, [&](auto L) {
     using Lay = decltype(L);
     const int ar = Lay::AL == LAYOUT_MN ? k : m, br = Lay::BL == LAYOUT_MN ? k : n;      // rows of the operands as stored
-    return with_width(m, n, [&](auto W) {
+    return with_width(bn_m, n, [&](auto W) {
       using Wd = decltype(W);
-      return launch_tc<KIND, Wd::BN, Wd::STAGES, OutT, ProdSingle, 128, Lay::AL, Lay::BL, EPI, BATCHED>(
-          m, n, k, A, lda, ar, 0, B, ldb, br, 0, C, ldc, names[Lay::idx][Wd::idx], c, 0, nullptr, nullptr, bat);
-    }, bat ? bat->count : 1);
+      return launch_tc<KIND, Wd::BN, Wd::STAGES, OutT, ProdSingle, 128, Lay::AL, Lay::BL, EPI, STACK>(
+          m, n, k, A, lda, ar, 0, B, ldb, br, 0, C, ldc, names[Lay::idx][Wd::idx], c, 0, nullptr, nullptr, stk);
+    }, bn_batch);
   });
 }
 
@@ -1138,7 +1159,7 @@ constexpr int kMaxGridZ = 65535;
 
 // k == 0 or alpha == 0 over every entry of a batch, one launch: C = beta * C (C unread when beta == 0).
 template <typename T>
-int degenerate_batched(int m, int n, void* C, int ldc, const Batch& bt, const Call& c) {
+int degenerate_batched(int m, int n, void* C, int ldc, const Stack& bt, const Call& c) {
   const int gz = bt.count < kMaxGridZ ? bt.count : kMaxGridZ;
   int gy = 4096 / gz;
   if (gy > m) gy = m;
@@ -1160,7 +1181,7 @@ int degenerate_batched(int m, int n, void* C, int ldc, const Batch& bt, const Ca
 // computes one matrix.
 template <typename InT, typename OutT>
 int launch_generic_batched(int op_a, int op_b, int m, int n, int k, const void* A, int lda, const void* B, int ldb,
-                           void* C, int ldc, const Batch& bt, const char* name, const Call& c) {
+                           void* C, int ldc, const Stack& bt, const char* name, const Call& c) {
   dim3 grid((n + 63) / 64, (m + 63) / 64, bt.count < kMaxGridZ ? bt.count : kMaxGridZ);
   const long long a_rs = op_a ? 1 : lda, a_cs = op_a ? lda : 1, b_rs = op_b ? 1 : ldb, b_cs = op_b ? ldb : 1;
   gemm_generic_batched_kernel<InT, OutT><<<grid, 256, 0, c.st>>>(
@@ -1210,34 +1231,31 @@ int gemm16_batched(int op_a, int op_b, int m, int n, int k, float alpha, const u
   Call c{st};
   if (alpha != 1.f || beta != 0.f) { c.axpby = 1; c.alpha = alpha; c.beta = beta; }
   const bool c32 = out_type == B200_OUT_F32;
-  const Batch bt{batch, stride_a, stride_b, stride_c};
+  const Stack bt{batch, stride_a, stride_b, stride_c, nullptr};
   if (k == 0 || alpha == 0.f) return c32 ? degenerate_batched<float>(m, n, C, ldc, bt, c) : degenerate_batched<E>(m, n, C, ldc, bt, c);
   const int ar = op_a ? k : m, br = op_b ? n : k;                                       // rows of the operands as stored
   if (!tma_ok(A, lda, B, ldb, 2) || !batch_tma_ok(stride_a, ar, lda, 2) || !batch_tma_ok(stride_b, br, ldb, 2)) {
     if (c32) return launch_generic_batched<E, float>(op_a, op_b, m, n, k, A, lda, B, ldb, C, ldc, bt, K16::kGenericBat, c);
     return launch_generic_batched<E, E>(op_a, op_b, m, n, k, A, lda, B, ldb, C, ldc, bt, K16::kGenericBat, c);
   }
-  if (c32) return tc16<KIND, float, false, true>(op_a, op_b, m, n, k, A, lda, B, ldb, C, ldc, c, &bt);
-  return tc16<KIND, typename K16::Out16, false, true>(op_a, op_b, m, n, k, A, lda, B, ldb, C, ldc, c, &bt);
+  if (c32) return tc16<KIND, float, false, STACK_BATCH>(op_a, op_b, m, n, k, A, lda, B, ldb, C, ldc, c, &bt);
+  return tc16<KIND, typename K16::Out16, false, STACK_BATCH>(op_a, op_b, m, n, k, A, lda, B, ldb, C, ldc, c, &bt);
 }
 
 // ---- grouped 16-bit GEMM (torch._grouped_mm) -----------------------------------------------------------------------
-// The offsets stay on the device: every launch below reads them there, and the host never waits for them.
-struct Group { const int32_t* offs; int count; int total_m; long long sb; };   // sb: elements between B_g and B_g+1
-
-// Upper bound of the 128-row tiles of a grouped call whatever its offsets: each group adds at most one partial tile.
-long long grouped_tile_rows(int total_m, int groups) { return (total_m + 127LL) / 128 + groups; }
+// The offsets stay on the device: every launch below reads them there, and the host never waits for them.  A grouped
+// call is a Stack with offs set (launch_tc); total_m is its m.
 
 // k == 0 or alpha == 0: C = beta * C (C unread when beta == 0) on rows [0, end of the last group), one launch.
 template <typename T>
-int degenerate_grouped(int n, void* C, int ldc, const Group& gr, const Call& c) {
-  const dim3 grid((n + 255) / 256, gr.total_m < 4096 ? gr.total_m : 4096);
+int degenerate_grouped(int total_m, int n, void* C, int ldc, const Stack& gr, const Call& c) {
+  const dim3 grid((n + 255) / 256, total_m < 4096 ? total_m : 4096);
   if (c.beta == 0.f) {          // 16-bit C is cleared as raw bits
     using Z = typename std::conditional<sizeof(T) == 2, uint16_t, T>::type;
-    fill_zero_grouped_kernel<Z><<<grid, 256, 0, c.st>>>(gr.offs, gr.count, gr.total_m, n, static_cast<Z*>(C), ldc);
+    fill_zero_grouped_kernel<Z><<<grid, 256, 0, c.st>>>(gr.offs, gr.count, total_m, n, static_cast<Z*>(C), ldc);
     t_last_kernel = "fill_zero_grp";
   } else {
-    scale_inplace_grouped_kernel<T><<<grid, 256, 0, c.st>>>(gr.offs, gr.count, gr.total_m, n, static_cast<T*>(C), ldc,
+    scale_inplace_grouped_kernel<T><<<grid, 256, 0, c.st>>>(gr.offs, gr.count, total_m, n, static_cast<T*>(C), ldc,
                                                             c.beta);
     t_last_kernel = "scale_inplace_grp";
   }
@@ -1248,83 +1266,17 @@ int degenerate_grouped(int n, void* C, int ldc, const Group& gr, const Call& c) 
 // Operands TMA cannot describe: the CUDA-core kernel, each group as launch_generic computes its rows.  The grid counts
 // the 64-row blocks of every group at their upper bound; the column blocks run gridDim.y at a time.
 template <typename InT, typename OutT>
-int launch_generic_grouped(int op_b, int n, int k, const void* A, int lda, const void* B, int ldb, void* C, int ldc,
-                           const Group& gr, const char* name, const Call& c) {
+int launch_generic_grouped(int op_b, int total_m, int n, int k, const void* A, int lda, const void* B, int ldb, void* C,
+                           int ldc, const Stack& gr, const char* name, const Call& c) {
   const int tn = (n + 63) / 64;
-  dim3 grid((int)((gr.total_m + 63LL) / 64 + gr.count), tn < 65535 ? tn : 65535);
+  dim3 grid((int)((total_m + 63LL) / 64 + gr.count), tn < 65535 ? tn : 65535);
   const long long b_rs = op_b ? 1 : ldb, b_cs = op_b ? ldb : 1;
   gemm_generic_grouped_kernel<InT, OutT><<<grid, 256, 0, c.st>>>(
-      gr.offs, gr.count, gr.total_m, n, k, static_cast<const InT*>(A), lda, static_cast<const InT*>(B), b_rs, b_cs,
+      gr.offs, gr.count, total_m, n, k, static_cast<const InT*>(A), lda, static_cast<const InT*>(B), b_rs, b_cs,
       gr.sb, static_cast<OutT*>(C), ldc, c.axpby, c.alpha, c.beta);
   g_launches++;
   t_last_kernel = name;
   return last_launch_status();
-}
-
-// The grouped tensor-core kernel: A (total_m x k, row-major) as one 2-D tensor map, B as a 3-D map with one entry per
-// group (BL = LAYOUT_MN: each B_g is k x n; LAYOUT_K: stored n x k).  The grid covers the tile bound; CTAs beyond the
-// tiles the offsets give find no work.  Whole tiles only.
-template <int KIND, int BN, int STAGES, typename OutT, int BL>
-int launch_tc_grouped(int n, int k, const void* A, int lda, const void* B, int ldb, void* C, int ldc, const Group& gr,
-                      const char* name, const Call& c) {
-  using Cfg = TcConfig<KIND, BN, STAGES, ProdSingle, 128, LAYOUT_K, BL>;
-  constexpr CUtensorMapDataType dt = KIND == KIND_F16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
-  constexpr int OB = OutBytes<OutT>::V;
-  const unsigned long long bbytes = (unsigned long long)ldb * 2, b_rows = Cfg::B_MN ? k : n;
-  const unsigned long long eb = gr.count > 1 ? (unsigned long long)gr.sb * 2 : b_rows * bbytes;   // one group: any
-  CUtensorMap tmA, tmB;
-  int rc = get_map(&tmA, A, dt, 2, k, gr.total_m, (unsigned long long)lda * 2, Cfg::BK, Cfg::BM, 1);
-  if (rc) return rc;
-  if constexpr (!Cfg::B_MN)
-    rc = get_map(&tmB, B, dt, 2, k, b_rows, bbytes, Cfg::BK, Cfg::B_BOX_ROWS, 1, gr.count, eb);
-  else
-    rc = get_map(&tmB, B, dt, 2, n, b_rows, bbytes, Cfg::B_BOX_COLS, Cfg::BK, 1, gr.count, eb);
-  if (rc) return rc;
-  TcParams p;
-  memset(&p, 0, sizeof p);
-  p.C = C; p.ldc = ldc; p.M = gr.total_m; p.N = n; p.K = k;
-  const long long tile_rows = grouped_tile_rows(gr.total_m, gr.count);
-  p.tiles_m = (int)tile_rows;             // a bound: the kernel takes each group's own count from its table
-  p.tiles_n = (n + BN - 1) / BN;
-  p.group_m = (g_group_rows > 0 ? g_group_rows : 2048) / Cfg::TILE_M;
-  if (p.group_m < 1) p.group_m = 1;
-  p.vec_ok = aligned16(C) && ((long long)ldc * OB) % 16 == 0;     // every group's first row is then as aligned
-  p.chunk_kb = (k + Cfg::BK - 1) / Cfg::BK;
-  p.dbg_b_lbo = g_dbg_b_lbo; p.dbg_b_sbo = g_dbg_b_sbo;
-  p.axpby = c.axpby; p.alpha = c.alpha; p.beta = c.beta;
-  p.act = c.act;
-  p.split = 1;
-  const int tiles = (int)(tile_rows * p.tiles_n);                 // the entry point checked that it fits an int
-  p.full_tiles = tiles;
-  auto kern = gemm_tc_grouped_kernel<KIND, BN, STAGES, OutT, BL>;
-  if (int arc = ensure_smem_attr(kern, Cfg::SMEM_BYTES)) return arc;
-  const int units_max = t_ctx->sms - c.sm_reserve > 2 ? t_ctx->sms - c.sm_reserve : t_ctx->sms;
-  const int units = tiles < units_max ? tiles : units_max;
-  t_last_schedule = Schedule{tiles, 1, tiles, units};
-  const TcGroup tg{gr.offs, gr.count, gr.total_m};
-  g_ktimer.begin(c.st);
-  {
-    cudaError_t e = launch_pdl(kern, dim3(units), dim3(Cfg::THREADS), Cfg::SMEM_BYTES, c.st, 1, tmA, tmB, p, tg);
-    if (e != cudaSuccess) { cudaGetLastError(); return (int)e; }
-  }
-  g_ktimer.end(c.st);
-  g_launches++;
-  t_last_kernel = name;
-  return last_launch_status();
-}
-
-// Tile width from the tile bound (pick_bn over that many 128-row tile rows), then the layout of B.
-template <int KIND, typename OutT>
-int tc16_grouped(int op_b, int n, int k, const void* A, int lda, const void* B, int ldb, void* C, int ldc,
-                 const Group& gr, const Call& c) {
-  const KernelNames& names = Kind16<KIND>::grp_names[!std::is_same<OutT, float>::value];
-  return with_width(128, n, [&](auto W) {
-    using Wd = decltype(W);
-    if (op_b) return launch_tc_grouped<KIND, Wd::BN, Wd::STAGES, OutT, LAYOUT_K>(n, k, A, lda, B, ldb, C, ldc, gr,
-                                                                                  names[1][Wd::idx], c);
-    return launch_tc_grouped<KIND, Wd::BN, Wd::STAGES, OutT, LAYOUT_MN>(n, k, A, lda, B, ldb, C, ldc, gr,
-                                                                       names[0][Wd::idx], c);
-  }, (int)grouped_tile_rows(gr.total_m, gr.count));
 }
 
 // Rows [end_{g-1}, end_g) of C = round_out(fma(beta, float(C), alpha * A_rows op(B_g))), B_g = B + g * stride_b, with
@@ -1360,14 +1312,16 @@ int gemm16_grouped(int op_b, int total_m, int n, int k, float alpha, const uint1
   Call c{st};
   if (alpha != 1.f || beta != 0.f) { c.axpby = 1; c.alpha = alpha; c.beta = beta; }
   const bool c32 = out_type == B200_OUT_F32;
-  const Group gr{offs, groups, total_m, groups > 1 ? stride_b : 0};
-  if (k == 0 || alpha == 0.f) return c32 ? degenerate_grouped<float>(n, C, ldc, gr, c) : degenerate_grouped<E>(n, C, ldc, gr, c);
+  const Stack gr{groups, 0, groups > 1 ? stride_b : 0, 0, offs};
+  if (k == 0 || alpha == 0.f)
+    return c32 ? degenerate_grouped<float>(total_m, n, C, ldc, gr, c) : degenerate_grouped<E>(total_m, n, C, ldc, gr, c);
   if (!tma_ok(A, lda, B, ldb, 2) || (groups > 1 && !batch_tma_ok(stride_b, b_rows, ldb, 2))) {
-    if (c32) return launch_generic_grouped<E, float>(op_b, n, k, A, lda, B, ldb, C, ldc, gr, K16::kGenericGrp, c);
-    return launch_generic_grouped<E, E>(op_b, n, k, A, lda, B, ldb, C, ldc, gr, K16::kGenericGrp, c);
+    if (c32) return launch_generic_grouped<E, float>(op_b, total_m, n, k, A, lda, B, ldb, C, ldc, gr, K16::kGenericGrp, c);
+    return launch_generic_grouped<E, E>(op_b, total_m, n, k, A, lda, B, ldb, C, ldc, gr, K16::kGenericGrp, c);
   }
-  if (c32) return tc16_grouped<KIND, float>(op_b, n, k, A, lda, B, ldb, C, ldc, gr, c);
-  return tc16_grouped<KIND, typename K16::Out16>(op_b, n, k, A, lda, B, ldb, C, ldc, gr, c);
+  if (c32) return tc16<KIND, float, false, STACK_GROUP>(B200_OP_N, op_b, total_m, n, k, A, lda, B, ldb, C, ldc, c, &gr);
+  return tc16<KIND, typename K16::Out16, false, STACK_GROUP>(B200_OP_N, op_b, total_m, n, k, A, lda, B, ldb, C, ldc, c,
+                                                              &gr);
 }
 
 static_assert(ACT_NONE == B200_ACT_NONE && ACT_RELU == B200_ACT_RELU && ACT_GELU == B200_ACT_GELU &&

@@ -180,76 +180,84 @@ __global__ void fill_zero_kernel(int M, int N, T* __restrict__ C, long long ldc)
   for (int i = blockIdx.y; i < M; i += gridDim.y) C[(long long)i * ldc + j] = (T)0;
 }
 
-// ---- strided-batched 16-bit forms ----------------------------------------------------------------------------------
-// Entry z of each operand at X + z * x_bs (elements; 0 broadcasts A or B), the entries over blockIdx.z, gridDim.z at a
-// time.  Kernels of their own, so that the single-matrix kernels above keep their code exactly.
+// ---- stacked 16-bit forms: strided batch and grouped -----------------------------------------------------------
+// Kernels of their own, so that the single-matrix kernels above keep their code exactly.
 
 // gemm_generic_kernel's tile for 16-bit operands with the alpha / beta epilogue (no accumulate, requant, bias or
-// activation): the same loads, the same fmaf chain in k order and the same store, so every entry equals the 2-D
-// generic call on that entry bit for bit.
+// activation) at (m0, n0) of one M x N matrix: the same loads, the same fmaf chain in k order and the same store, so
+// every matrix of a stacked call equals the 2-D generic call on that matrix bit for bit.  Every thread of the block
+// calls it; it ends in __syncthreads (K > 0), so the block may call it again for another tile.  As / Bs are the
+// calling kernel's own shared arrays: static __shared__ arrays here would be module-scope symbols shared by several
+// kernels, and that alone changes the code ptxas emits for the unrelated 2-D generic kernels.
+typedef float GenericTile[16][64 + 4];
+template <typename InT, typename OutT>
+__device__ __forceinline__ void generic_tile16(GenericTile& As, GenericTile& Bs, int m0, int n0, int M, int N, int K,
+                                               const InT* __restrict__ A, long long a_rs, long long a_cs,
+                                               const InT* __restrict__ B, long long b_rs, long long b_cs,
+                                               OutT* __restrict__ C, long long ldc, int axpby, float alpha, float beta) {
+  static_assert(sizeof(InT) == 2, "stacked generic kernels: 16-bit operands");
+  const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
+  float acc[4][4];
+#pragma unroll
+  for (int i = 0; i < 4; i++)
+#pragma unroll
+    for (int j = 0; j < 4; j++) acc[i][j] = 0.f;
+  for (int k0 = 0; k0 < K; k0 += 16) {
+#pragma unroll
+    for (int r = 0; r < 4; r++) {
+      const int idx = threadIdx.x + r * 256;
+      const int am = idx >> 4, ak = idx & 15;
+      const int gm = m0 + am, gk = k0 + ak;
+      As[ak][am] = (gm < M && gk < K) ? LoadAs<InT>::ld(A + (long long)gm * a_rs + (long long)gk * a_cs) : 0.f;
+      const int bk = idx >> 6, bn = idx & 63;
+      const int gk2 = k0 + bk, gn = n0 + bn;
+      Bs[bk][bn] = (gk2 < K && gn < N) ? LoadAs<InT>::ld(B + (long long)gk2 * b_rs + (long long)gn * b_cs) : 0.f;
+    }
+    __syncthreads();
+#pragma unroll
+    for (int kk = 0; kk < 16; kk++) {
+      float a[4], b[4];
+#pragma unroll
+      for (int i = 0; i < 4; i++) a[i] = As[kk][ty + 16 * i];
+#pragma unroll
+      for (int j = 0; j < 4; j++) b[j] = Bs[kk][tx + 16 * j];
+#pragma unroll
+      for (int i = 0; i < 4; i++)
+#pragma unroll
+        for (int j = 0; j < 4; j++) acc[i][j] = fmaf(a[i], b[j], acc[i][j]);
+    }
+    __syncthreads();                                   // also orders this tile's last reads before the next tile's loads
+  }
+#pragma unroll
+  for (int i = 0; i < 4; i++) {
+    const int gm = m0 + ty + 16 * i;
+    if (gm >= M) continue;
+#pragma unroll
+    for (int j = 0; j < 4; j++) {
+      const int gn = n0 + tx + 16 * j;
+      if (gn < N) {
+        float v = acc[i][j];
+        if (axpby) {
+          v *= alpha;
+          if (beta != 0.f) v = fmaf(beta, LoadAs<OutT>::ld(C + (long long)gm * ldc + gn), v);
+        }
+        store_out<float, OutT>(C + (long long)gm * ldc + gn, v);
+      }
+    }
+  }
+}
+
+// Strided batch: entry z of each operand at X + z * x_bs (elements; 0 broadcasts A or B), the entries over
+// blockIdx.z, gridDim.z at a time.
 template <typename InT, typename OutT>
 __global__ void __launch_bounds__(256)
 gemm_generic_batched_kernel(int batch, int M, int N, int K, const InT* __restrict__ A, long long a_rs, long long a_cs,
                             long long a_bs, const InT* __restrict__ B, long long b_rs, long long b_cs, long long b_bs,
                             OutT* __restrict__ C, long long ldc, long long c_bs, int axpby, float alpha, float beta) {
-  static_assert(sizeof(InT) == 2, "strided-batched generic kernel: 16-bit operands");
-  __shared__ float As[16][64 + 4];
-  __shared__ float Bs[16][64 + 4];
-  const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
-  const int m0 = blockIdx.y * 64, n0 = blockIdx.x * 64;
-  for (int z = blockIdx.z; z < batch; z += gridDim.z) {
-    const InT* Az = A + z * a_bs;
-    const InT* Bz = B + z * b_bs;
-    OutT* Cz = C + z * c_bs;
-    float acc[4][4];
-#pragma unroll
-    for (int i = 0; i < 4; i++)
-#pragma unroll
-      for (int j = 0; j < 4; j++) acc[i][j] = 0.f;
-    for (int k0 = 0; k0 < K; k0 += 16) {
-#pragma unroll
-      for (int r = 0; r < 4; r++) {
-        const int idx = threadIdx.x + r * 256;
-        const int am = idx >> 4, ak = idx & 15;
-        const int gm = m0 + am, gk = k0 + ak;
-        As[ak][am] = (gm < M && gk < K) ? LoadAs<InT>::ld(Az + (long long)gm * a_rs + (long long)gk * a_cs) : 0.f;
-        const int bk = idx >> 6, bn = idx & 63;
-        const int gk2 = k0 + bk, gn = n0 + bn;
-        Bs[bk][bn] = (gk2 < K && gn < N) ? LoadAs<InT>::ld(Bz + (long long)gk2 * b_rs + (long long)gn * b_cs) : 0.f;
-      }
-      __syncthreads();
-#pragma unroll
-      for (int kk = 0; kk < 16; kk++) {
-        float a[4], b[4];
-#pragma unroll
-        for (int i = 0; i < 4; i++) a[i] = As[kk][ty + 16 * i];
-#pragma unroll
-        for (int j = 0; j < 4; j++) b[j] = Bs[kk][tx + 16 * j];
-#pragma unroll
-        for (int i = 0; i < 4; i++)
-#pragma unroll
-          for (int j = 0; j < 4; j++) acc[i][j] = fmaf(a[i], b[j], acc[i][j]);
-      }
-      __syncthreads();                                 // also orders this entry's last reads before the next's loads
-    }
-#pragma unroll
-    for (int i = 0; i < 4; i++) {
-      const int gm = m0 + ty + 16 * i;
-      if (gm >= M) continue;
-#pragma unroll
-      for (int j = 0; j < 4; j++) {
-        const int gn = n0 + tx + 16 * j;
-        if (gn < N) {
-          float v = acc[i][j];
-          if (axpby) {
-            v *= alpha;
-            if (beta != 0.f) v = fmaf(beta, LoadAs<OutT>::ld(Cz + (long long)gm * ldc + gn), v);
-          }
-          store_out<float, OutT>(Cz + (long long)gm * ldc + gn, v);
-        }
-      }
-    }
-  }
+  __shared__ GenericTile As, Bs;
+  for (int z = blockIdx.z; z < batch; z += gridDim.z)
+    generic_tile16(As, Bs, blockIdx.y * 64, blockIdx.x * 64, M, N, K, A + z * a_bs, a_rs, a_cs, B + z * b_bs, b_rs,
+                   b_cs, C + z * c_bs, ldc, axpby, alpha, beta);
 }
 
 // scale_inplace_kernel (s != 0) and fill_zero_kernel (s == 0) over every entry: the k == 0 / alpha == 0 pass.
@@ -271,85 +279,27 @@ __global__ void fill_zero_batched_kernel(int batch, int M, int N, T* __restrict_
     for (int i = blockIdx.y; i < M; i += gridDim.y) C[z * c_bs + (long long)i * ldc + j] = (T)0;
 }
 
-// ---- grouped 16-bit forms ------------------------------------------------------------------------------------------
-// Group g is rows [end[g], end[g + 1]) of one stacked row-major A (total_m x k, pitch lda) and C, times B_g at
-// B + g * b_gs (group_table, ptx.cuh, clamps the offsets).  Kernels of their own beside the 2-D and batched ones.
-
-// gemm_generic_kernel's tile for 16-bit operands with the alpha / beta epilogue, on 64-row blocks that each lie inside
-// one group: blockIdx.x counts the blocks of every group in order (surplus blocks exit), blockIdx.y the column blocks,
-// gridDim.y at a time.  The same loads, the same fmaf chain in k order and the same store as the 2-D kernel, so every
-// group equals the 2-D generic call on its rows bit for bit.
+// Grouped: group g is rows [end[g], end[g + 1]) of one stacked row-major A (total_m x k, pitch lda) and C, times B_g
+// at B + g * b_gs (group_table, ptx.cuh, clamps the offsets).  The tiles are 64-row blocks that each lie inside one
+// group: blockIdx.x counts the blocks of every group in order (surplus blocks exit), blockIdx.y the column blocks,
+// gridDim.y at a time.
 template <typename InT, typename OutT>
 __global__ void __launch_bounds__(256)
 gemm_generic_grouped_kernel(const int* __restrict__ offs, int groups, int total_m, int N, int K,
                             const InT* __restrict__ A, long long lda, const InT* __restrict__ B, long long b_rs,
                             long long b_cs, long long b_gs, OutT* __restrict__ C, long long ldc, int axpby, float alpha,
                             float beta) {
-  static_assert(sizeof(InT) == 2, "grouped generic kernel: 16-bit operands");
   __shared__ int grp_end[kMaxGroups + 1];
   __shared__ int grp_blk[kMaxGroups + 1];
-  __shared__ float As[16][64 + 4];
-  __shared__ float Bs[16][64 + 4];
+  __shared__ GenericTile As, Bs;
   group_table(offs, groups, total_m, 64, grp_end, grp_blk);
   const int q = blockIdx.x;
   if (q >= grp_blk[groups]) return;                  // the grid counts every group's blocks at their upper bound
   const int g = group_of(grp_blk, groups, q);
-  const int M = grp_end[g + 1] - grp_end[g];
-  const InT* Ag = A + (long long)grp_end[g] * lda;
-  const InT* Bg = B + g * b_gs;
-  OutT* Cg = C + (long long)grp_end[g] * ldc;
-  const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
   const int m0 = (q - grp_blk[g]) * 64;
-  for (int n0 = blockIdx.y * 64; n0 < N; n0 += gridDim.y * 64) {
-    float acc[4][4];
-#pragma unroll
-    for (int i = 0; i < 4; i++)
-#pragma unroll
-      for (int j = 0; j < 4; j++) acc[i][j] = 0.f;
-    for (int k0 = 0; k0 < K; k0 += 16) {
-#pragma unroll
-      for (int r = 0; r < 4; r++) {
-        const int idx = threadIdx.x + r * 256;
-        const int am = idx >> 4, ak = idx & 15;
-        const int gm = m0 + am, gk = k0 + ak;
-        As[ak][am] = (gm < M && gk < K) ? LoadAs<InT>::ld(Ag + (long long)gm * lda + gk) : 0.f;
-        const int bk = idx >> 6, bn = idx & 63;
-        const int gk2 = k0 + bk, gn = n0 + bn;
-        Bs[bk][bn] = (gk2 < K && gn < N) ? LoadAs<InT>::ld(Bg + (long long)gk2 * b_rs + (long long)gn * b_cs) : 0.f;
-      }
-      __syncthreads();
-#pragma unroll
-      for (int kk = 0; kk < 16; kk++) {
-        float a[4], b[4];
-#pragma unroll
-        for (int i = 0; i < 4; i++) a[i] = As[kk][ty + 16 * i];
-#pragma unroll
-        for (int j = 0; j < 4; j++) b[j] = Bs[kk][tx + 16 * j];
-#pragma unroll
-        for (int i = 0; i < 4; i++)
-#pragma unroll
-          for (int j = 0; j < 4; j++) acc[i][j] = fmaf(a[i], b[j], acc[i][j]);
-      }
-      __syncthreads();                                 // also orders this column block's last reads before the next's
-    }
-#pragma unroll
-    for (int i = 0; i < 4; i++) {
-      const int gm = m0 + ty + 16 * i;
-      if (gm >= M) continue;
-#pragma unroll
-      for (int j = 0; j < 4; j++) {
-        const int gn = n0 + tx + 16 * j;
-        if (gn < N) {
-          float v = acc[i][j];
-          if (axpby) {
-            v *= alpha;
-            if (beta != 0.f) v = fmaf(beta, LoadAs<OutT>::ld(Cg + (long long)gm * ldc + gn), v);
-          }
-          store_out<float, OutT>(Cg + (long long)gm * ldc + gn, v);
-        }
-      }
-    }
-  }
+  for (int n0 = blockIdx.y * 64; n0 < N; n0 += gridDim.y * 64)
+    generic_tile16(As, Bs, m0, n0, grp_end[g + 1] - grp_end[g], N, K, A + (long long)grp_end[g] * lda, lda, 1,
+                   B + g * b_gs, b_rs, b_cs, C + (long long)grp_end[g] * ldc, ldc, axpby, alpha, beta);
 }
 
 // The rows a grouped call writes, min(max(0, offs[0..groups)), total_m) = end[groups] of group_table, computed by

@@ -103,20 +103,15 @@ struct TcParams {
   int act;                 // EPI kernels: y = act(t + bias[col]) after the alpha / beta step; an EpiAct (ptx.cuh)
 };
 
-// Strided-batched kernels (gemm_tc_batched_kernel) only: a second kernel argument, so that TcParams, and with it the
-// code of every single-matrix kernel, is unchanged.  The operands are 3-D tensor maps (inner, rows, entry); a broadcast
-// operand (stride 0) has one entry and is read at entry coordinate 0.
-struct TcBatch {
-  int count;               // entries; the work index runs over count x tiles_m x tiles_n, entry outermost
+// Stacked kernels (gemm_tc_stacked_kernel) only: a second kernel argument, so that TcParams, and with it the code of
+// every single-matrix kernel, is unchanged.  The operands are 3-D tensor maps (inner, rows, entry); a broadcast
+// operand (stride 0) has one entry and is read at entry coordinate 0.  A grouped call is a stack whose A and C are
+// broadcast: its groups are row ranges of both, and its entries are the B_g.
+struct TcStack {
+  int count;               // entries of a batch, or groups (1 .. kMaxGroups)
   int a_step, b_step;      // entry coordinate of A / B per entry: 1, or 0 for a broadcast operand
-  long long stride_c;      // elements between consecutive entries of C
-};
-
-// Grouped kernels (gemm_tc_grouped_kernel) only: the second kernel argument, as TcBatch is for the batched kernels.
-struct TcGroup {
-  const int* offs;         // [count] cumulative end rows of the groups, on the device (read after griddep_wait)
-  int count;               // groups, 1 .. kMaxGroups
-  int total_m;             // rows of the stacked A and C
+  long long stride_c;      // batch: elements between consecutive entries of C
+  const int* offs;         // grouped: [count] cumulative end rows of the groups, on the device (read after griddep_wait)
 };
 
 // REGACC (split-precision fp32 modes): the tensor core adds into its fp32 accumulator with truncation,
@@ -587,26 +582,69 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   }
 }
 
-// ---- strided-batched 16-bit GEMM ----------------------------------------------------------------------
-// gemm_tc_kernel's persistent schedule over a stack of matrices, cut down to what the strided-batched calls need:
-// 16-bit operands, one plane, 128-byte rows, fp32 or 16-bit C, no bias / activation, no scaling.  It is a kernel of
-// its own rather than a flag of gemm_tc_kernel so that the single-matrix kernels keep their code exactly.  Its MMA
-// chain (k-blocks in order, one accumulator) and its epilogue (store_pair, the same fold / alpha / beta rules) are
+// ---- stacked 16-bit GEMMs: strided batch and grouped (torch._grouped_mm) --------------------------------------------
+// gemm_tc_kernel's persistent schedule over a stack of matrices, cut down to what the stacked calls need: 16-bit
+// operands, one plane, 128-byte rows, fp32 or 16-bit C, no bias / activation, no scaling.  It is a kernel of its own
+// rather than a flag of gemm_tc_kernel so that the single-matrix kernels keep their code exactly.  Its MMA chain
+// (k-blocks in order, one accumulator) and its epilogue (store_pair, the same fold / alpha / beta rules) are
 // gemm_tc_kernel's, so every entry equals the single-matrix call on that entry bit for bit at the same tile width.
-// Work item w covers bt.count x tiles_m x tiles_n with the entry outermost: one entry's tiles are adjacent and share
-// its B in L2; inside an entry tile_coords walks its raster groups as for one matrix.  The K-split tail (fp32 C)
-// cuts the last partial round of the whole batch.  A and B are 3-D tensor maps (inner, rows, entry) read one entry
-// per box, so TMA's zero fill past the rows and the inner extent stays inside the entry; entry e of C is at
-// C + e * stride_c (64-bit).
-template <int KIND, int BN, int STAGES, typename OutT, int AL, int BL>
+// Work item w covers the tiles of every entry, entry outermost: one entry's tiles are adjacent and share its B in L2;
+// inside an entry tile_coords walks its raster groups as for one matrix.  A and B are 3-D tensor maps (inner, rows,
+// entry) read one entry per box, so TMA's zero fill past the rows and the inner extent stays inside the entry.
+//   Strided batch: entry e is A_e, B_e and C + e * stride_c (64-bit), tiles_m x tiles_n tiles each.  The K-split tail
+//   (fp32 C) cuts the last partial round of the whole batch.
+//   GROUPED: group g is rows [end_g-1, end_g) of one stacked row-major A (total_m = p.M rows) and C, times B_g, entry g
+//   of B.  The group sizes exist only on the device, so the schedule is built here: after griddep_wait every CTA reads
+//   the offsets, clamps them and scans the 128-row tiles of each group into shared memory (group_table); producer and
+//   consumers find a tile's group by binary search.  A is one entry: a tile at row end_g-1 + 128 mb may load rows of
+//   the next group (or TMA's zeros past total_m), but each row of C depends only on its own row of A, and store_pair,
+//   on a TcParams whose C starts at row end_g-1 and whose M is the group's rows, never stores those rows.  The host
+//   sizes the grid for a bound on the tiles (p.tiles_m tile rows) and takes no K split (split = 1, full_tiles = that
+//   bound): it does not know the tile count.
+struct StackEntry {
+  int tile0, tiles_m;      // the entry's first work tile and its tile rows (tile_coords)
+  int a_row, a_entry;      // A: row of the entry's first row, entry coordinate
+  int b_entry;             // B: entry coordinate
+  int M;                   // rows of the entry's C
+  long long c_off;         // elements from C to the entry's first row
+};
+// The entry of work tile `tile`.  grp_end / grp_tile: the GROUPED kernels' tables (group_table), else unused.
+template <bool GROUPED>
+__device__ __forceinline__ StackEntry stack_entry(int tile, const TcParams& p, const TcStack& st, const int* grp_end,
+                                                  const int* grp_tile) {
+  StackEntry se;
+  int e;
+  if constexpr (GROUPED) {
+    e = group_of(grp_tile, st.count, tile / p.tiles_n);
+    se.tile0 = grp_tile[e] * p.tiles_n;
+    se.tiles_m = grp_tile[e + 1] - grp_tile[e];
+    se.a_row = grp_end[e];
+    se.M = grp_end[e + 1] - grp_end[e];
+    se.c_off = (long long)grp_end[e] * p.ldc;
+  } else {
+    const int per_entry = p.tiles_m * p.tiles_n;
+    e = tile / per_entry;
+    se.tile0 = e * per_entry;
+    se.tiles_m = p.tiles_m;
+    se.a_row = 0;
+    se.M = p.M;
+    se.c_off = (long long)e * st.stride_c;
+  }
+  se.a_entry = e * st.a_step;
+  se.b_entry = e * st.b_step;
+  return se;
+}
+
+template <int KIND, int BN, int STAGES, typename OutT, int AL, int BL, bool GROUPED>
 __global__ void __launch_bounds__((TcConfig<KIND, BN, STAGES, ProdSingle, 128, AL, BL>::THREADS), 1)
-gemm_tc_batched_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                       const TcParams p, const TcBatch bt) {
+gemm_tc_stacked_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                       const TcParams p, const TcStack st) {
   using Cfg = TcConfig<KIND, BN, STAGES, ProdSingle, 128, AL, BL>;
   using MMA = typename Cfg::MMA;
   using Acc = typename MMA::Acc;
   static_assert(KindTraits<KIND>::ELEM == 2 && (std::is_same<OutT, float>::value || OutBytes<OutT>::V == 2),
-                "strided-batched: 16-bit kinds with fp32 or 16-bit C");
+                "stacked: 16-bit kinds with fp32 or 16-bit C");
+  static_assert(!GROUPED || AL == LAYOUT_K, "grouped: A is row-major");
 
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;   // swizzle atoms need 1 KB
@@ -630,10 +668,25 @@ gemm_tc_batched_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
   griddep_launch();
   griddep_wait();
 
-  const int per_entry = p.tiles_m * p.tiles_n;
-  const int num_tiles = per_entry * bt.count;
+  const int* grp_end = nullptr;               // GROUPED: group g is rows [grp_end[g], grp_end[g + 1])
+  const int* grp_tile = nullptr;              //          and tiles [grp_tile[g], grp_tile[g + 1]) of the tile order
+  int num_tiles;
+  if constexpr (GROUPED) {                    // the batched kernels declare no tables
+    static_assert(Cfg::SMEM_BYTES + 2 * (kMaxGroups + 1) * (int)sizeof(int) <= 232448,
+                  "the pipeline and the group tables exceed the 227 KB of shared memory of sm_90");
+    __shared__ int s_end[kMaxGroups + 1];
+    __shared__ int s_tile[kMaxGroups + 1];
+    group_table(st.offs, st.count, p.M, Cfg::BM, s_end, s_tile);     // ends in __syncthreads
+    grp_end = s_end;
+    grp_tile = s_tile;
+    num_tiles = grp_tile[st.count] * p.tiles_n;                      // CTAs past it have no work
+  } else {
+    num_tiles = p.tiles_m * p.tiles_n * st.count;
+  }
   const int num_items = p.full_tiles + (num_tiles - p.full_tiles) * p.split;
   const int num_kb = (p.K + Cfg::BK - 1) / Cfg::BK;
+  // GROUPED work items are whole tiles (split = 1), known at compile time: with a run-time part the split tail's
+  // branches stay in the epilogue, and ptxas specialises its store loop less (DESIGN §9: 1-2.5 % slower on an H100)
 
   if (warp < 4) {
     // ===================== TMA producer (warpgroup 0) =====================
@@ -642,11 +695,11 @@ gemm_tc_batched_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
       int s = 0;
       uint32_t ph = 0;
       for (int w = blockIdx.x; w < num_items; w += gridDim.x) {
-        const WorkItem it = work_item(w, p, num_kb);
-        const int e = it.tile / per_entry;
+        const WorkItem it = GROUPED ? WorkItem{w, 0, 0, num_kb} : work_item(w, p, num_kb);
+        const StackEntry se = stack_entry<GROUPED>(it.tile, p, st, grp_end, grp_tile);
         int mb, nb;
-        tile_coords(it.tile - e * per_entry, p.tiles_m, p.tiles_n, p.group_m, mb, nb);
-        const int m0 = mb * Cfg::BM, n0 = nb * BN, ea = e * bt.a_step, eb = e * bt.b_step;
+        tile_coords(it.tile - se.tile0, se.tiles_m, p.tiles_n, p.group_m, mb, nb);
+        const int m0 = se.a_row + mb * Cfg::BM, n0 = nb * BN;
         for (int kb = it.kb0; kb < it.kb1; kb++) {
           mbar_wait(bar_empty + 8 * s, ph ^ 1);
           const uint32_t full = bar_full + 8 * s;
@@ -655,17 +708,17 @@ gemm_tc_batched_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
 #pragma unroll
             for (int j = 0; j < Cfg::A_BOXES; j++)
               tma_load_3d(sA + s * Cfg::A_STAGE + j * Cfg::MN_BOX_BYTES, &tmA, full, m0 + j * Cfg::MN_BOX_COLS,
-                          kb * Cfg::BK, ea);
+                          kb * Cfg::BK, se.a_entry);
           } else {
-            tma_load_3d(sA + s * Cfg::A_STAGE, &tmA, full, kb * Cfg::BK, m0, ea);
+            tma_load_3d(sA + s * Cfg::A_STAGE, &tmA, full, kb * Cfg::BK, m0, se.a_entry);
           }
           if constexpr (!Cfg::B_MN) {                 // B^T (n x k): one box of BN rows
-            tma_load_3d(sB + s * Cfg::B_STAGE, &tmB, full, kb * Cfg::BK, n0, eb);
+            tma_load_3d(sB + s * Cfg::B_STAGE, &tmB, full, kb * Cfg::BK, n0, se.b_entry);
           } else {
 #pragma unroll
             for (int j = 0; j < Cfg::B_BOXES; j++)
               tma_load_3d(sB + s * Cfg::B_STAGE + j * Cfg::B_BOX_BYTES, &tmB, full, n0 + j * Cfg::B_BOX_COLS,
-                          kb * Cfg::BK, eb);
+                          kb * Cfg::BK, se.b_entry);
           }
           if (++s == STAGES) { s = 0; ph ^= 1; }
         }
@@ -683,11 +736,11 @@ gemm_tc_batched_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
     uint32_t ph = 0;
     Acc acc[Cfg::ACC];
     for (int w = blockIdx.x; w < num_items; w += gridDim.x) {
-      const WorkItem it = work_item(w, p, num_kb);
-      const int e = it.tile / per_entry;
+      const WorkItem it = GROUPED ? WorkItem{w, 0, 0, num_kb} : work_item(w, p, num_kb);
+      const StackEntry se = stack_entry<GROUPED>(it.tile, p, st, grp_end, grp_tile);
       int mb, nb;
-      tile_coords(it.tile - e * per_entry, p.tiles_m, p.tiles_n, p.group_m, mb, nb);
-      const int m0 = mb * Cfg::BM, n0 = nb * BN;
+      tile_coords(it.tile - se.tile0, se.tiles_m, p.tiles_n, p.group_m, mb, nb);
+      const int m0 = mb * Cfg::BM, n0 = nb * BN;      // m0: row inside the entry
       int prev = -1;
       for (int kb = it.kb0; kb < it.kb1; kb++) {
         mbar_wait(bar_full + 8 * s, ph);
@@ -713,7 +766,7 @@ gemm_tc_batched_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
       wgmma_fence_regs(acc);
       if (prev >= 0 && wg_leader) mbar_arrive(bar_empty + 8 * prev);
 
-      // ---- this warp's 16 rows of the tile into entry e of C ----
+      // ---- this warp's 16 rows of the tile into the entry's C ----
       int* flag = p.flags + (it.tile - p.full_tiles) * Cfg::EPI_WARPS + ew;
       if (it.part > 0) {                               // K-split tail: wait until parts < it.part are in C
         if (lane == 0) {
@@ -733,7 +786,8 @@ gemm_tc_batched_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
       const int row0 = m0 + ew * 16 + (lane >> 2);
       const int col0 = n0 + 2 * (lane & 3);
       TcParams pc = p;
-      pc.C = static_cast<uint8_t*>(p.C) + (long long)e * bt.stride_c * OutBytes<OutT>::V;
+      pc.C = static_cast<uint8_t*>(p.C) + se.c_off * OutBytes<OutT>::V;
+      pc.M = se.M;
       const int ce[2] = {0, 0};
 #pragma unroll
       for (int j = 0; j < BN / 8; j++)
@@ -749,145 +803,6 @@ gemm_tc_batched_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
           asm volatile("st.release.gpu.global.s32 [%0], %1;" ::"l"(flag), "r"(nv) : "memory");
         }
       }
-    }
-  }
-}
-
-// ---- grouped 16-bit GEMM (torch._grouped_mm) -----------------------------------------------------------------------
-// Group g is rows [end_g-1, end_g) of one stacked row-major A (total_m x k) and C, times its own B_g, entry g of a 3-D
-// tensor map (inner, rows, group) as the batched kernel reads it.  The group sizes exist only on the device, so the
-// schedule is built here: after griddep_wait every CTA reads the offsets, clamps them and scans the 128-row tiles of
-// each group into shared memory (group_table).  Work item w covers tiles x tiles_n, group outermost; producer and
-// consumers find w's group by binary search, and tile_coords walks the raster groups of that group's tiles_m.  A is
-// one 2-D map: a tile at row end_g-1 + 128 mb may load rows of the next group (or TMA's zeros past total_m), but each
-// row of C depends only on its own row of A and store_pair, on a TcParams whose C starts at row end_g-1 and whose M is
-// the group's rows, never stores those rows.  The MMA chain and the epilogue are the batched kernel's, so each group
-// equals the _ex call on its rows bit for bit.  No K-split tail: the host does not know the tile count.  A kernel of
-// its own, so that the other kernels keep their code exactly.
-template <int KIND, int BN, int STAGES, typename OutT, int BL>
-__global__ void __launch_bounds__((TcConfig<KIND, BN, STAGES, ProdSingle, 128, LAYOUT_K, BL>::THREADS), 1)
-gemm_tc_grouped_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                       const TcParams p, const TcGroup gp) {
-  using Cfg = TcConfig<KIND, BN, STAGES, ProdSingle, 128, LAYOUT_K, BL>;
-  using MMA = typename Cfg::MMA;
-  using Acc = typename MMA::Acc;
-  static_assert(KindTraits<KIND>::ELEM == 2 && (std::is_same<OutT, float>::value || OutBytes<OutT>::V == 2),
-                "grouped: 16-bit kinds with fp32 or 16-bit C");
-  static_assert(Cfg::SMEM_BYTES + 2 * (kMaxGroups + 1) * (int)sizeof(int) <= 232448,
-                "the pipeline and the group tables exceed the 227 KB of shared memory of sm_90");
-  __shared__ int grp_end[kMaxGroups + 1];     // group g: rows [grp_end[g], grp_end[g + 1])
-  __shared__ int grp_tile[kMaxGroups + 1];    // group g: tiles [grp_tile[g], grp_tile[g + 1]) of the tile order
-
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;   // swizzle atoms need 1 KB
-  const uint32_t sA = smem_base;
-  const uint32_t sB = sA + STAGES * Cfg::A_STAGE;
-  const uint32_t bar_full = sB + STAGES * Cfg::B_STAGE;
-  const uint32_t bar_empty = bar_full + 8 * STAGES;
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  if (threadIdx.x == 0) {
-    tma_prefetch_desc(&tmA);
-    tma_prefetch_desc(&tmB);
-    for (int i = 0; i < STAGES; i++) {
-      mbar_init(bar_full + 8 * i, 1);
-      mbar_init(bar_empty + 8 * i, Cfg::CONSUMERS);
-    }
-    fence_barrier_init();
-  }
-  __syncthreads();
-  griddep_launch();
-  griddep_wait();
-  group_table(gp.offs, gp.count, gp.total_m, Cfg::BM, grp_end, grp_tile);     // ends in __syncthreads
-
-  const int num_items = grp_tile[gp.count] * p.tiles_n;       // CTAs past it have no work
-  const int num_kb = (p.K + Cfg::BK - 1) / Cfg::BK;
-
-  if (warp < 4) {
-    // ===================== TMA producer (warpgroup 0) =====================
-    setmaxnreg_dec<40>();
-    if (warp == 0 && lane == 0) {
-      int s = 0;
-      uint32_t ph = 0;
-      for (int w = blockIdx.x; w < num_items; w += gridDim.x) {
-        const int g = group_of(grp_tile, gp.count, w / p.tiles_n);
-        int mb, nb;
-        tile_coords(w - grp_tile[g] * p.tiles_n, grp_tile[g + 1] - grp_tile[g], p.tiles_n, p.group_m, mb, nb);
-        const int m0 = grp_end[g] + mb * Cfg::BM, n0 = nb * BN;
-        for (int kb = 0; kb < num_kb; kb++) {
-          mbar_wait(bar_empty + 8 * s, ph ^ 1);
-          const uint32_t full = bar_full + 8 * s;
-          mbar_arrive_expect_tx(full, Cfg::STAGE_BYTES);
-          tma_load_2d(sA + s * Cfg::A_STAGE, &tmA, full, kb * Cfg::BK, m0);
-          if constexpr (!Cfg::B_MN) {                 // B_g^T (n x k): one box of BN rows
-            tma_load_3d(sB + s * Cfg::B_STAGE, &tmB, full, kb * Cfg::BK, n0, g);
-          } else {
-#pragma unroll
-            for (int j = 0; j < Cfg::B_BOXES; j++)
-              tma_load_3d(sB + s * Cfg::B_STAGE + j * Cfg::B_BOX_BYTES, &tmB, full, n0 + j * Cfg::B_BOX_COLS,
-                          kb * Cfg::BK, g);
-          }
-          if (++s == STAGES) { s = 0; ph ^= 1; }
-        }
-      }
-    }
-  } else {
-    // ===================== consumers (warpgroups 1 and 2): MMA chain + epilogue =====================
-    setmaxnreg_inc<232>();
-    const int cw = warp / 4 - 1;                    // consumer warpgroup: rows [64 cw, 64 cw + 64) of the tile
-    const int ew = warp - 4;                        // consumer warp 0..7: 16 rows each
-    const bool wg_leader = (threadIdx.x & 127) == 0;
-    const uint32_t b_lbo = p.dbg_b_lbo ? (uint32_t)p.dbg_b_lbo : (uint32_t)Cfg::B_BOX_BYTES;
-    const uint32_t b_sbo = p.dbg_b_sbo ? (uint32_t)p.dbg_b_sbo : 1024u;
-    int s = 0;
-    uint32_t ph = 0;
-    Acc acc[Cfg::ACC];
-    for (int w = blockIdx.x; w < num_items; w += gridDim.x) {
-      const int g = group_of(grp_tile, gp.count, w / p.tiles_n);
-      int mb, nb;
-      tile_coords(w - grp_tile[g] * p.tiles_n, grp_tile[g + 1] - grp_tile[g], p.tiles_n, p.group_m, mb, nb);
-      const int m0 = mb * Cfg::BM, n0 = nb * BN;      // m0: row inside the group
-      int prev = -1;
-      for (int kb = 0; kb < num_kb; kb++) {
-        mbar_wait(bar_full + 8 * s, ph);
-        const uint32_t a0 = sA + s * Cfg::A_STAGE + cw * Cfg::A_WG;
-        const uint32_t b0 = sB + s * Cfg::B_STAGE;
-        wgmma_fence();
-#pragma unroll
-        for (int k = 0; k < Cfg::MMAS_PER_STAGE; k++) {
-          const uint64_t ad = make_sdesc(a0 + k * Cfg::A_KADV, 16, Cfg::A_SBO, Cfg::A_SWZ);
-          uint64_t bd;
-          if constexpr (Cfg::B_MN) bd = make_sdesc(b0 + k * Cfg::B_KADV, b_lbo, b_sbo, SWZ_128B);
-          else bd = make_sdesc(b0 + k * Cfg::B_KADV, 16, Cfg::A_SBO, Cfg::A_SWZ);
-          MMA::mma(acc, ad, bd, (kb | k) != 0 ? 1u : 0u);
-        }
-        wgmma_commit();
-        wgmma_wait<1>();                              // the previous k-block's products retired: its stage is free
-        if (prev >= 0 && wg_leader) mbar_arrive(bar_empty + 8 * prev);
-        prev = s;
-        if (++s == STAGES) { s = 0; ph ^= 1; }
-      }
-      wgmma_wait<0>();
-      wgmma_fence_regs(acc);
-      if (prev >= 0 && wg_leader) mbar_arrive(bar_empty + 8 * prev);
-
-      // ---- this warp's 16 rows of the tile into group g's rows of C ----
-      const bool fold = p.axpby && p.beta != 0.f;
-      const float al = p.axpby ? p.alpha : 1.f;
-      const float be = p.axpby ? p.beta : 1.f;
-      const int row0 = m0 + ew * 16 + (lane >> 2);
-      const int col0 = n0 + 2 * (lane & 3);
-      TcParams pc = p;
-      pc.C = static_cast<uint8_t*>(p.C) + (long long)grp_end[g] * p.ldc * OutBytes<OutT>::V;
-      pc.M = grp_end[g + 1] - grp_end[g];
-      const int ce[2] = {0, 0};
-#pragma unroll
-      for (int j = 0; j < BN / 8; j++)
-#pragma unroll
-        for (int h = 0; h < 2; h++)
-          store_pair<OutT>(pc, row0 + 8 * h, col0 + 8 * j, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], fold, false, al,
-                           be, 0, ce, 0.f, 0.f);
     }
   }
 }
