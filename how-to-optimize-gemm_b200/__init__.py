@@ -30,7 +30,7 @@ EXPORTS = [
     "b200_gemm_s8s32_host", "b200_gemm_s8s8_requant", "b200_gemm_f32_pack_b", "b200_gemm_f32_packed",
     "b200_gemm_f32_pack_free", "b200_gemm_f32_op", "b200_gemm_bf16_op", "b200_gemm_bf16_ex", "b200_gemm_f16_ex",
     "b200_gemm_bf16_epi", "b200_gemm_f16_epi", "b200_gemm_bf16_batched", "b200_gemm_f16_batched",
-    "b200_gemm_bf16_grouped", "b200_gemm_f16_grouped",
+    "b200_gemm_bf16_grouped", "b200_gemm_f16_grouped", "b200_gemm_bf16_grouped_k", "b200_gemm_f16_grouped_k",
     "b200_gemm_s8s32_op", "b200_gemm_workspace_bytes_op",
     "b200_nccl_load", "b200_nccl_last_error", "b200_comm_unique_id", "b200_comm_init_rank",
     "b200_comm_destroy", "b200_rowpanel_create", "b200_rowpanel_destroy", "b200_rowpanel_slices", "b200_rowpanel_set_reserve_sms", "b200_rowpanel_trace", "b200_rowpanel_trace_dump", "b200_gemm_f32_rowpanel",
@@ -93,6 +93,10 @@ lib.b200_gemm_bf16_grouped.argtypes = [_i, _i, _i, _i, C.c_float, _vp, _i, _vp, 
                                        _vp]
 lib.b200_gemm_f16_grouped.argtypes = [_i, _i, _i, _i, C.c_float, _vp, _i, _vp, _i, _ll, _vp, _i, C.c_float, _vp, _i, _i,
                                       _vp]
+lib.b200_gemm_bf16_grouped_k.argtypes = [_i, _i, _i, _i, _i, C.c_float, _vp, _i, _vp, _i, _vp, _i, C.c_float, _vp, _i, _ll,
+                                         _i, _vp]
+lib.b200_gemm_f16_grouped_k.argtypes = [_i, _i, _i, _i, _i, C.c_float, _vp, _i, _vp, _i, _vp, _i, C.c_float, _vp, _i, _ll,
+                                        _i, _vp]
 lib.b200_gemm_s8s32_op.argtypes = [_i, _i, _i, _i, _i, _vp, _i, _vp, _i, _vp, _i, _vp]
 lib.b200_gemm_workspace_bytes_op.argtypes = [_i, _i, _i, _i, _i, _i]
 lib.b200_gemm_workspace_bytes_op.restype = C.c_size_t
@@ -261,19 +265,23 @@ def _gemm_batched(A, B, out, alpha, beta, bias, activation, out_dtype, stream):
     return out
 
 
+def _check_offs(offs):
+    import torch
+    if not isinstance(offs, torch.Tensor) or offs.dtype != torch.int32 or offs.dim() != 1:
+        raise ValueError("offs must be a 1-D int32 tensor")
+    if not offs.is_contiguous():
+        raise ValueError("offs must be contiguous")
+
+
 def grouped_layout(A, B, offs):
     """(total_m, n, k, op_b, ldb, stride_b, groups) under which b200_gemm_*_grouped reads gemm(A, B, offs=offs) in place:
     A (total_m x k) row-major, B (groups x k x n) whose last two dimensions resolve as batched_operand_layout does (so
     W.transpose(-2, -1) of a (groups, n, k) weight is op_b = OP_T), offs a contiguous 1-D int32 tensor of groups
     cumulative end rows.  Raises ValueError for anything else, a broadcast or overlapping B included; the device of the
     tensors is not checked here."""
-    import torch
     if A.dim() != 2 or B.dim() != 3:
         raise ValueError(f"a grouped GEMM takes a 2-D A and a 3-D B, not {A.dim()}-D and {B.dim()}-D")
-    if not isinstance(offs, torch.Tensor) or offs.dtype != torch.int32 or offs.dim() != 1:
-        raise ValueError("offs must be a 1-D int32 tensor")
-    if not offs.is_contiguous():
-        raise ValueError("offs must be contiguous")
+    _check_offs(offs)
     groups, k2, n = B.shape
     total_m, k = A.shape
     if offs.numel() != groups:
@@ -321,6 +329,57 @@ def _gemm_grouped(A, B, out, offs, alpha, beta, bias, activation, out_dtype, str
     return out
 
 
+def grouped_k_layout(A, B, offs):
+    """(m, n, total_k, op_a, lda, op_b, ldb, groups) under which b200_gemm_*_grouped_k reads gemm(A, B, offs=offs) for a
+    2-D A (m x total_k) and a 2-D B (total_k x n) in place: each resolves as operand_layout does (so dy.t() of a
+    row-major dy is op_a = OP_T and a row-major x is op_b = OP_N), offs a contiguous 1-D int32 tensor of groups
+    cumulative ends along K.  Raises ValueError for anything else; the device of the tensors is not checked here."""
+    _check_offs(offs)
+    m, total_k = A.shape
+    k2, n = B.shape
+    if k2 != total_k:
+        raise ValueError(f"inner dimensions differ: A is {tuple(A.shape)}, B is {tuple(B.shape)}")
+    op_a, lda = operand_layout(tuple(A.shape), A.stride())
+    op_b, ldb = operand_layout(tuple(B.shape), B.stride())
+    return m, n, total_k, op_a, lda, op_b, ldb, offs.numel()
+
+
+def _gemm_grouped_k(A, B, out, offs, alpha, beta, bias, activation, out_dtype, stream):
+    """gemm(A, B, offs=offs) with a 2-D B: out[g] = alpha * A[:, K_g] @ B[K_g, :] + beta * out[g] for the K ranges
+    K_g = [offs[g-1], offs[g]), one launch (b200_gemm_*_grouped_k)."""
+    import torch
+    if A.dtype != B.dtype:
+        raise TypeError(f"operands of different dtypes: {A.dtype} and {B.dtype}")
+    if A.dtype not in (torch.bfloat16, torch.float16):
+        raise TypeError(f"grouped operands must be bf16 or fp16, not {A.dtype}")
+    if bias is not None or activation is not None:
+        raise ValueError("the grouped GEMM has no bias / activation epilogue")
+    m, n, total_k, op_a, lda, op_b, ldb, groups = grouped_k_layout(A, B, offs)
+    cdt = out_dtype or (out.dtype if out is not None else torch.float32)
+    if cdt not in (torch.float32, A.dtype):
+        raise ValueError(f"{A.dtype} operands write float32 or {A.dtype} C, not {cdt}")
+    if out is not None:
+        if out.dtype != cdt:
+            raise ValueError(f"out is {out.dtype}, not {cdt}")
+        if out.dim() != 3 or tuple(out.shape) != (groups, m, n):
+            raise ValueError(f"out must have shape {(groups, m, n)}, not {tuple(out.shape)}")
+        if (n > 1 and out.stride(2) != 1) or (m > 1 and out.stride(1) < n):
+            raise ValueError("out must be row-major in its last two dimensions")
+        if groups > 1 and m * n > 0 and out.stride(0) < (m - 1) * out.stride(1) + n:
+            raise ValueError(f"the groups of out must not overlap (stride(0) = {out.stride(0)})")
+    if not (A.is_cuda and B.is_cuda and offs.is_cuda and (out is None or out.is_cuda)):
+        raise ValueError("A, B, offs and out must be CUDA tensors")
+    if out is None:
+        assert beta == 0.0, "beta != 0 reads C: pass out"
+        out = torch.empty((groups, m, n), dtype=cdt, device=A.device)
+    if groups == 0:
+        return out
+    fn, ot = (lib.b200_gemm_bf16_grouped_k, OUT_BF16) if A.dtype == torch.bfloat16 else (lib.b200_gemm_f16_grouped_k, OUT_F16)
+    _check(fn(op_a, op_b, m, n, total_k, alpha, A.data_ptr(), lda, B.data_ptr(), ldb, offs.data_ptr(), groups, beta,
+              out.data_ptr(), _ld(out[0]), out.stride(0), OUT_F32 if cdt == torch.float32 else ot, _stream_ptr(stream)))
+    return out
+
+
 def _epilogue_args(A, B, bias, activation):
     """Checks a bias / activation request of gemm() (before anything touches the device); returns the ACT_* code."""
     import torch
@@ -365,9 +424,19 @@ def gemm(A, B, out=None, *, offs=None, alpha=1.0, beta=0.0, bias=None, activatio
     offsets stay on the device (the call never synchronises).  out is row-major (total_m x n); a new one is
     torch.empty, so its rows from offs[-1] on are unspecified, as in torch.  out_dtype defaults to float32 as for every
     16-bit gemm() (torch._grouped_mm's default is the operands' dtype).  fp32 or int8 operands are a TypeError; a bias,
-    an activation, another offs, A or out, or a broadcast or overlapping B is a ValueError."""
+    an activation, another offs, A or out, or a broadcast or overlapping B is a ValueError.
+
+    offs with a 2-D A and a 2-D B is torch._grouped_mm's 2-D x 2-D form, where the offsets split K: the weight gradient
+    dW_g = dy_g^T x_g of such a layer is gemm(dy.t(), x, offs=offs).  A is m x total_k and B is total_k x n, each
+    row-major or transposed and read in place; out[g] = alpha * A[:, K_g] @ B[K_g, :] + beta * out[g] for the K range
+    K_g = [offs[g-1], offs[g]) (clamped as above, to total_k), every group in one launch (b200_gemm_bf16_grouped_k /
+    _f16_grouped_k).  out is (groups, m, n), row-major in its last two dimensions, with out.stride(0) between groups;
+    every group is written, an empty one with zeros (beta * out[g] when beta != 0).  out_dtype defaults to float32.
+    The refusals are those of the grouped form, and an overlapping out is a ValueError."""
     import torch
     if offs is not None:
+        if A.dim() == 2 and B.dim() == 2:
+            return _gemm_grouped_k(A, B, out, offs, alpha, beta, bias, activation, out_dtype, stream)
         return _gemm_grouped(A, B, out, offs, alpha, beta, bias, activation, out_dtype, stream)
     if A.dim() == 3 or B.dim() == 3:
         return _gemm_batched(A, B, out, alpha, beta, bias, activation, out_dtype, stream)

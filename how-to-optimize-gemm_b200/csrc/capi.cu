@@ -390,11 +390,13 @@ int g_ffma_halves = 1;        // strict kernel: split the tail round into half t
 //   STACK_GROUP: groups of rows [end_g-1, end_g) of one row-major A and C (m = total_m rows; sa = sc = 0: A and C are
 //   broadcast) times B_g = B + g * sb, with the ends read on the device.  The tile rows are a bound,
 //   grouped_tile_rows, and there is no K split: the host does not know the tile count.
-enum Stacking { STACK_NONE, STACK_BATCH, STACK_GROUP };
+//   STACK_KGROUP: groups of K rows [end_g-1, end_g) of one A^T and one B (k = total_k; sa = sb = 0: A and B are
+//   broadcast), C_g = C + g * sc, with the ends read on the device.  The tiles are a batch's, with no K split.
+// (Stacking, gemm_tc.cuh, names the forms.)
 struct Stack {
   int count;               // entries of a batch, or groups
   long long sa, sb, sc;    // elements between consecutive entries of A, B and C
-  const int32_t* offs;     // STACK_GROUP: [count] cumulative end rows of the groups, on the device
+  const int32_t* offs;     // STACK_GROUP / STACK_KGROUP: [count] cumulative ends of the groups, on the device
 };
 // Upper bound of the 128-row tiles of a grouped call whatever its offsets: each group adds at most one partial tile.
 long long grouped_tile_rows(int total_m, int groups) { return (total_m + 127LL) / 128 + groups; }
@@ -455,7 +457,7 @@ int launch_tc(int m, int n, int k, const void* A, long long lda, int a_rows_tota
   if constexpr (EPI) p.bias = c.bias;            // shares col_max's slot: EPI kernels are never scaled
   p.stream_c = g_stream_c < 0 ? (g_stream_c = (getenv("B200GEMM_STREAM_C") ? atoi(getenv("B200GEMM_STREAM_C")) : kStreamCDefault)) : g_stream_c;
   auto kern = [] {
-    if constexpr (STACK != STACK_NONE) return gemm_tc_stacked_kernel<KIND, BN, STAGES, OutT, AL, BL, STACK == STACK_GROUP>;
+    if constexpr (STACK != STACK_NONE) return gemm_tc_stacked_kernel<KIND, BN, STAGES, OutT, AL, BL, STACK>;
     else return gemm_tc_kernel<KIND, BN, STAGES, OutT, Prod, A_ROW_BYTES, AL, BL, EPI>;
   }();
   if (int arc = ensure_smem_attr(kern, Cfg::SMEM_BYTES)) return arc;
@@ -470,8 +472,9 @@ int launch_tc(int m, int n, int k, const void* A, long long lda, int a_rows_tota
   const int num_kb = (k + Cfg::BK - 1) / Cfg::BK;
   const int rem = tiles % units_max;
   int split = 1;
-  // an activation must see the complete sum, and a grouped call's tile count is not known here: no split
-  if (!EPI && STACK != STACK_GROUP && g_split_tail && OB == 4 && rem > 0) {
+  // an activation must see the complete sum, and a grouped call's tile count is not known here: no split.  Nor for a
+  // K-grouped call, whose tiles have their groups' k-blocks.
+  if (!EPI && STACK != STACK_GROUP && STACK != STACK_KGROUP && g_split_tail && OB == 4 && rem > 0) {
     split = units_max / rem;
     if (split > 4) split = 4;
     if (split > num_kb / 8) split = num_kb / 8;       // keep >= 8 k-blocks per part
@@ -557,7 +560,8 @@ typedef const char* const KernelNames[4][3];
 
 // 16-bit operands: KIND_F16 (bf16, C fp32 or bf16) and KIND_FP16 (fp16, C fp32 or fp16).  E is the generic kernel's
 // element type of the kind (uint16_t holds bf16 bits).  names[16-bit C][EPI]; bat_names[16-bit C]: the strided-batched
-// kernels; grp_names[16-bit C]: the grouped kernels (rows NN and NT only: A is row-major).
+// kernels; grp_names[16-bit C]: the grouped kernels (rows NN and NT only: A is row-major); kgrp_names[16-bit C]: the
+// K-grouped kernels (row TN only).
 template <int KIND> struct Kind16;
 template <> struct Kind16<KIND_F16> {
   using E = uint16_t;
@@ -570,6 +574,8 @@ template <> struct Kind16<KIND_F16> {
   static constexpr KernelNames bat_names[2] = {TC_NAMES("tc_bf16_bat"), TC_NAMES("tc_bf16_obf16_bat")};
   static constexpr const char* kGenericGrp = "generic_bf16_grp_64x64";
   static constexpr KernelNames grp_names[2] = {TC_NAMES("tc_bf16_grp"), TC_NAMES("tc_bf16_obf16_grp")};
+  static constexpr const char* kGenericKgrp = "generic_bf16_kgrp_64x64";
+  static constexpr KernelNames kgrp_names[2] = {TC_NAMES("tc_bf16_kgrp"), TC_NAMES("tc_bf16_obf16_kgrp")};
 };
 template <> struct Kind16<KIND_FP16> {
   using E = __half;
@@ -582,6 +588,8 @@ template <> struct Kind16<KIND_FP16> {
   static constexpr KernelNames bat_names[2] = {TC_NAMES("tc_f16_bat"), TC_NAMES("tc_f16_of16_bat")};
   static constexpr const char* kGenericGrp = "generic_f16_grp_64x64";
   static constexpr KernelNames grp_names[2] = {TC_NAMES("tc_f16_grp"), TC_NAMES("tc_f16_of16_grp")};
+  static constexpr const char* kGenericKgrp = "generic_f16_kgrp_64x64";
+  static constexpr KernelNames kgrp_names[2] = {TC_NAMES("tc_f16_kgrp"), TC_NAMES("tc_f16_of16_kgrp")};
 };
 
 // The 16-bit GEMM on the tensor cores (OutT float, bf16_out or f16_out): every layout is read in place by one launch.
@@ -591,20 +599,30 @@ int tc16(int op_a, int op_b, int m, int n, int k, const void* A, int lda, const 
          const Call& c, const Stack* stk = nullptr) {
   static_assert(!(EPI && STACK != STACK_NONE), "the stacked kernels have no bias / activation epilogue");
   constexpr bool c16 = !std::is_same<OutT, float>::value;
-  const KernelNames& names = STACK == STACK_BATCH ? Kind16<KIND>::bat_names[c16]
-                           : STACK == STACK_GROUP ? Kind16<KIND>::grp_names[c16] : Kind16<KIND>::names[c16][EPI];
-  // pick_bn: a batch's tiles are those of all its entries; a grouped call's, its bound of tile rows, one row each
-  const int bn_m = STACK == STACK_GROUP ? 128 : m;
-  const int bn_batch = STACK == STACK_GROUP ? (int)grouped_tile_rows(m, stk->count) : stk ? stk->count : 1;
-  return with_layout<STACK != STACK_GROUP>(op_a, op_b, [&](auto L) {
-    using Lay = decltype(L);
-    const int ar = Lay::AL == LAYOUT_MN ? k : m, br = Lay::BL == LAYOUT_MN ? k : n;      // rows of the operands as stored
-    return with_width(bn_m, n, [&](auto W) {
+  if constexpr (STACK == STACK_KGROUP) {        // (T, N) only: both operands MN-major, K rows of total_k each
+    (void)op_a; (void)op_b;
+    return with_width(m, n, [&](auto W) {
       using Wd = decltype(W);
-      return launch_tc<KIND, Wd::BN, Wd::STAGES, OutT, ProdSingle, 128, Lay::AL, Lay::BL, EPI, STACK>(
-          m, n, k, A, lda, ar, 0, B, ldb, br, 0, C, ldc, names[Lay::idx][Wd::idx], c, 0, nullptr, nullptr, stk);
-    }, bn_batch);
-  });
+      return launch_tc<KIND, Wd::BN, Wd::STAGES, OutT, ProdSingle, 128, LAYOUT_MN, LAYOUT_MN, false, STACK>(
+          m, n, k, A, lda, k, 0, B, ldb, k, 0, C, ldc, Kind16<KIND>::kgrp_names[c16][2][Wd::idx], c, 0, nullptr,
+          nullptr, stk);
+    }, stk->count);
+  } else {
+    const KernelNames& names = STACK == STACK_BATCH ? Kind16<KIND>::bat_names[c16]
+                             : STACK == STACK_GROUP ? Kind16<KIND>::grp_names[c16] : Kind16<KIND>::names[c16][EPI];
+    // pick_bn: a batch's tiles are those of all its entries; a grouped call's, its bound of tile rows, one row each
+    const int bn_m = STACK == STACK_GROUP ? 128 : m;
+    const int bn_batch = STACK == STACK_GROUP ? (int)grouped_tile_rows(m, stk->count) : stk ? stk->count : 1;
+    return with_layout<STACK != STACK_GROUP>(op_a, op_b, [&](auto L) {
+      using Lay = decltype(L);
+      const int ar = Lay::AL == LAYOUT_MN ? k : m, br = Lay::BL == LAYOUT_MN ? k : n;    // rows of the operands as stored
+      return with_width(bn_m, n, [&](auto W) {
+        using Wd = decltype(W);
+        return launch_tc<KIND, Wd::BN, Wd::STAGES, OutT, ProdSingle, 128, Lay::AL, Lay::BL, EPI, STACK>(
+            m, n, k, A, lda, ar, 0, B, ldb, br, 0, C, ldc, names[Lay::idx][Wd::idx], c, 0, nullptr, nullptr, stk);
+      }, bn_batch);
+    });
+  }
 }
 
 // ---- split-precision fp32 on the tensor cores ---------------------------------------------------
@@ -1324,6 +1342,71 @@ int gemm16_grouped(int op_b, int total_m, int n, int k, float alpha, const uint1
                                                               &gr);
 }
 
+// ---- K-grouped 16-bit GEMM (torch._grouped_mm 2-D x 2-D: the weight gradient of a grouped layer) -------------------
+// total_k: the largest K extent; every K row coordinate the kernels form, end + 64 included, stays below 2^31.
+constexpr int kMaxTotalK = 0x7FFFFFFF - 64;
+
+// Layouts other than (T, N) and operands TMA cannot describe: the CUDA-core kernel, each group as launch_generic
+// computes C_g from copies of its K range.
+template <typename InT, typename OutT>
+int launch_generic_kgrouped(int op_a, int op_b, int m, int n, int total_k, const void* A, int lda, const void* B,
+                            int ldb, void* C, int ldc, const Stack& kg, const char* name, const Call& c) {
+  const int tm = (m + 63) / 64;
+  dim3 grid((n + 63) / 64, tm < 65535 ? tm : 65535, kg.count);
+  const long long a_rs = op_a ? 1 : lda, a_cs = op_a ? lda : 1, b_rs = op_b ? 1 : ldb, b_cs = op_b ? ldb : 1;
+  gemm_generic_kgrouped_kernel<InT, OutT><<<grid, 256, 0, c.st>>>(
+      kg.offs, kg.count, m, n, total_k, static_cast<const InT*>(A), a_rs, a_cs, static_cast<const InT*>(B), b_rs, b_cs,
+      static_cast<OutT*>(C), ldc, kg.sc, c.axpby, c.alpha, c.beta);
+  g_launches++;
+  t_last_kernel = name;
+  return last_launch_status();
+}
+
+// C_g = round_out(fma(beta, float(C_g), alpha * op(A)[:, K_g] op(B)[K_g, :])) for g < groups, C_g = C + g * stride_c,
+// K_g = [end_{g-1}, end_g) with end_{-1} = 0 and end_g = min(max(offs[g], end_{g-1}), total_k) on the device; an empty
+// group stores the k == 0 result of _ex.  Argument rules (all before the device is touched, all by division): those
+// of gemm16 for an (m, n, total_k) call; negative sizes, groups or stride_c; groups > kMaxGroups; total_k above
+// kMaxTotalK; groups > 1 with C_g overlapping (stride_c < (m - 1) * ldc + n); (groups - 1) * stride_c above 2^60;
+// tiles the kernel's int work index cannot count; a null offs with work to do.  groups == 0, m == 0 or n == 0 is a
+// no-op.
+template <int KIND>
+int gemm16_grouped_k(int op_a, int op_b, int m, int n, int total_k, float alpha, const uint16_t* A, int lda,
+                     const uint16_t* B, int ldb, const int32_t* offs, int groups, float beta, void* C, int ldc,
+                     long long stride_c, int out_type, cudaStream_t st) {
+  using K16 = Kind16<KIND>;
+  using E = typename K16::E;
+  if (groups < 0 || stride_c < 0 || groups > kMaxGroups) return B200_ERR_BAD_ARG;
+  if (out_type != B200_OUT_F32 && out_type != K16::OUT16) return B200_ERR_BAD_ARG;
+  if ((op_a != B200_OP_N && op_a != B200_OP_T) || (op_b != B200_OP_N && op_b != B200_OP_T)) return B200_ERR_BAD_ARG;
+  if (m < 0 || n < 0 || total_k < 0 || total_k > kMaxTotalK) return B200_ERR_BAD_ARG;
+  if (groups == 0) return 0;
+  int rc = check_args(m, n, total_k, A, lda, B, ldb, C, ldc, op_a, op_b);
+  if (rc == 1) return 0;
+  if (rc) return rc;
+  if (!offs) return B200_ERR_BAD_ARG;
+  if (groups > 1) {
+    if (stride_c < (long long)(m - 1) * ldc + n) return B200_ERR_BAD_ARG;               // C_g would overlap
+    if (stride_c > (1LL << 60) / (groups - 1)) return B200_ERR_BAD_ARG;
+  }
+  // every group's tiles at the narrowest width, with room for w + gridDim.x, in the kernel's int work index
+  const long long tiles1 = ((m + 127LL) / 128) * ((n + 127LL) / 128);                   // < 2^48
+  if (tiles1 > 0x3FFFFFFFLL / groups) return B200_ERR_BAD_ARG;
+  if ((rc = ensure_device())) return rc;
+  Call c{st};
+  if (alpha != 1.f || beta != 0.f) { c.axpby = 1; c.alpha = alpha; c.beta = beta; }
+  const bool c32 = out_type == B200_OUT_F32;
+  const Stack kg{groups, 0, 0, groups > 1 ? stride_c : 0, offs};
+  if (total_k == 0 || alpha == 0.f)
+    return c32 ? degenerate_batched<float>(m, n, C, ldc, kg, c) : degenerate_batched<E>(m, n, C, ldc, kg, c);
+  if (op_a != B200_OP_T || op_b != B200_OP_N || !tma_ok(A, lda, B, ldb, 2)) {
+    if (c32)
+      return launch_generic_kgrouped<E, float>(op_a, op_b, m, n, total_k, A, lda, B, ldb, C, ldc, kg, K16::kGenericKgrp, c);
+    return launch_generic_kgrouped<E, E>(op_a, op_b, m, n, total_k, A, lda, B, ldb, C, ldc, kg, K16::kGenericKgrp, c);
+  }
+  if (c32) return tc16<KIND, float, false, STACK_KGROUP>(op_a, op_b, m, n, total_k, A, lda, B, ldb, C, ldc, c, &kg);
+  return tc16<KIND, typename K16::Out16, false, STACK_KGROUP>(op_a, op_b, m, n, total_k, A, lda, B, ldb, C, ldc, c, &kg);
+}
+
 static_assert(ACT_NONE == B200_ACT_NONE && ACT_RELU == B200_ACT_RELU && ACT_GELU == B200_ACT_GELU &&
               ACT_GELU_TANH == B200_ACT_GELU_TANH, "EpiAct follows the header's codes");
 
@@ -1520,6 +1603,20 @@ int b200_gemm_f16_grouped(int op_b, int total_m, int n, int k, float alpha, cons
                           void* dC, int ldc, int out_type, void* stream) {
   return gemm16_grouped<KIND_FP16>(op_b, total_m, n, k, alpha, dA, lda, dB, ldb, stride_b, dOffs, groups, beta, dC, ldc,
                                    out_type, (cudaStream_t)stream);
+}
+
+int b200_gemm_bf16_grouped_k(int op_a, int op_b, int m, int n, int total_k, float alpha, const uint16_t* dA, int lda,
+                             const uint16_t* dB, int ldb, const int32_t* dOffs, int groups, float beta, void* dC,
+                             int ldc, long long stride_c, int out_type, void* stream) {
+  return gemm16_grouped_k<KIND_F16>(op_a, op_b, m, n, total_k, alpha, dA, lda, dB, ldb, dOffs, groups, beta, dC, ldc,
+                                    stride_c, out_type, (cudaStream_t)stream);
+}
+
+int b200_gemm_f16_grouped_k(int op_a, int op_b, int m, int n, int total_k, float alpha, const uint16_t* dA, int lda,
+                            const uint16_t* dB, int ldb, const int32_t* dOffs, int groups, float beta, void* dC,
+                            int ldc, long long stride_c, int out_type, void* stream) {
+  return gemm16_grouped_k<KIND_FP16>(op_a, op_b, m, n, total_k, alpha, dA, lda, dB, ldb, dOffs, groups, beta, dC, ldc,
+                                     stride_c, out_type, (cudaStream_t)stream);
 }
 
 int b200_gemm_s8s32(int m, int n, int k, const int8_t* dA, int lda, const int8_t* dB, int ldb,

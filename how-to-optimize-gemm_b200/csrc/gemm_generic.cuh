@@ -302,6 +302,42 @@ gemm_generic_grouped_kernel(const int* __restrict__ offs, int groups, int total_
                    B + g * b_gs, b_rs, b_cs, C + (long long)grp_end[g] * ldc, ldc, axpby, alpha, beta);
 }
 
+// K-grouped (the weight gradient of a grouped layer): group g is K rows [end[g], end[g + 1]) of op(A) (M x total_k) and
+// op(B) (total_k x N), element strides as gemm_generic_kernel's, and C_g = C + g * c_gs is a whole M x N matrix.  The
+// groups run over blockIdx.z, gridDim.z at a time, and the row blocks over blockIdx.y, gridDim.y at a time.  An empty
+// group stores what the 2-D call with k == 0 stores: round_out(beta * float(C)), or +0 without reading C when beta == 0.
+template <typename InT, typename OutT>
+__global__ void __launch_bounds__(256)
+gemm_generic_kgrouped_kernel(const int* __restrict__ offs, int groups, int M, int N, int total_k,
+                             const InT* __restrict__ A, long long a_rs, long long a_cs, const InT* __restrict__ B,
+                             long long b_rs, long long b_cs, OutT* __restrict__ C, long long ldc, long long c_gs,
+                             int axpby, float alpha, float beta) {
+  __shared__ int grp_end[kMaxGroups + 1];
+  __shared__ int grp_blk[kMaxGroups + 1];
+  __shared__ GenericTile As, Bs;
+  group_table(offs, groups, total_k, 64, grp_end, grp_blk);         // only the K ends are used
+  const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
+  const int n0 = blockIdx.x * 64;
+  for (int g = blockIdx.z; g < groups; g += gridDim.z) {
+    const int k0 = grp_end[g], kg = grp_end[g + 1] - k0;
+    OutT* Cg = C + g * c_gs;
+    for (int m0 = blockIdx.y * 64; m0 < M; m0 += gridDim.y * 64) {
+      if (kg > 0) {
+        generic_tile16(As, Bs, m0, n0, M, N, kg, A + k0 * a_cs, a_rs, a_cs, B + k0 * b_rs, b_rs, b_cs, Cg, ldc, axpby,
+                       alpha, beta);
+        continue;
+      }
+      for (int i = 0; i < 4; i++)
+        for (int j = 0; j < 4; j++) {
+          const int gm = m0 + ty + 16 * i, gn = n0 + tx + 16 * j;
+          if (gm >= M || gn >= N) continue;
+          OutT* e = Cg + (long long)gm * ldc + gn;
+          store_out<float, OutT>(e, axpby && beta != 0.f ? beta * LoadAs<OutT>::ld(e) : 0.f);
+        }
+    }
+  }
+}
+
 // The rows a grouped call writes, min(max(0, offs[0..groups)), total_m) = end[groups] of group_table, computed by
 // every thread of the block.
 __device__ __forceinline__ int grouped_rows(const int* __restrict__ offs, int groups, int total_m, int* s_max) {

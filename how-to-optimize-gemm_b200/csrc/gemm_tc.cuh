@@ -106,12 +106,14 @@ struct TcParams {
 // Stacked kernels (gemm_tc_stacked_kernel) only: a second kernel argument, so that TcParams, and with it the code of
 // every single-matrix kernel, is unchanged.  The operands are 3-D tensor maps (inner, rows, entry); a broadcast
 // operand (stride 0) has one entry and is read at entry coordinate 0.  A grouped call is a stack whose A and C are
-// broadcast: its groups are row ranges of both, and its entries are the B_g.
+// broadcast: its groups are row ranges of both, and its entries are the B_g.  A K-grouped call is a stack whose A and B
+// are broadcast: its groups are K ranges of both, and its entries are the C_g.
+enum Stacking { STACK_NONE, STACK_BATCH, STACK_GROUP, STACK_KGROUP };
 struct TcStack {
   int count;               // entries of a batch, or groups (1 .. kMaxGroups)
   int a_step, b_step;      // entry coordinate of A / B per entry: 1, or 0 for a broadcast operand
-  long long stride_c;      // batch: elements between consecutive entries of C
-  const int* offs;         // grouped: [count] cumulative end rows of the groups, on the device (read after griddep_wait)
+  long long stride_c;      // batch, K-grouped: elements between consecutive entries of C
+  const int* offs;         // (K-)grouped: [count] cumulative ends of the groups, on the device (read after griddep_wait)
 };
 
 // REGACC (split-precision fp32 modes): the tensor core adds into its fp32 accumulator with truncation,
@@ -601,20 +603,31 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 //   on a TcParams whose C starts at row end_g-1 and whose M is the group's rows, never stores those rows.  The host
 //   sizes the grid for a bound on the tiles (p.tiles_m tile rows) and takes no K split (split = 1, full_tiles = that
 //   bound): it does not know the tile count.
+//   KGROUP (the weight gradient of a grouped layer, torch._grouped_mm 2-D x 2-D): group g is K rows
+//   [end_g-1, end_g) of one A^T (total_k x m, p.K = total_k) and one B (total_k x n), both MN-major and read as one
+//   entry; C_g = C + g * stride_c is a whole m x n matrix.  The tiles are a batch's (entry outermost, p.tiles_m x
+//   p.tiles_n per group, known to the host), whole tiles only.  Every CTA builds the clamped K ends (group_table) after
+//   griddep_wait.  k-block kb of group g is loaded at K row end_g-1 + 64 kb; the last one of a group whose k_g is not a
+//   multiple of 64 also holds rows of the next group (real data: 0 * inf would be NaN) or TMA's zeros past total_k, so
+//   the consumers zero its rows >= k_g - 64 kb in shared memory before its MMAs (zero_k_tail).  The MMA count is
+//   unchanged, so every C_g is bit for bit the _ex call with k = k_g, whose TMA zero-fills those rows.  A group with
+//   k_g = 0 issues no loads or MMAs and stores the _ex k == 0 result (store_beta_c).
 struct StackEntry {
   int tile0, tiles_m;      // the entry's first work tile and its tile rows (tile_coords)
   int a_row, a_entry;      // A: row of the entry's first row, entry coordinate
   int b_entry;             // B: entry coordinate
   int M;                   // rows of the entry's C
   long long c_off;         // elements from C to the entry's first row
+  int k0, k_len;           // KGROUP: the group's first K row and its k_g
 };
-// The entry of work tile `tile`.  grp_end / grp_tile: the GROUPED kernels' tables (group_table), else unused.
-template <bool GROUPED>
+// The entry of work tile `tile`.  grp_end / grp_tile: the GROUP kernels' tables (group_table), grp_end the KGROUP
+// kernels' K ends, else unused.
+template <int STACK>
 __device__ __forceinline__ StackEntry stack_entry(int tile, const TcParams& p, const TcStack& st, const int* grp_end,
                                                   const int* grp_tile) {
   StackEntry se;
   int e;
-  if constexpr (GROUPED) {
+  if constexpr (STACK == STACK_GROUP) {
     e = group_of(grp_tile, st.count, tile / p.tiles_n);
     se.tile0 = grp_tile[e] * p.tiles_n;
     se.tiles_m = grp_tile[e + 1] - grp_tile[e];
@@ -630,21 +643,72 @@ __device__ __forceinline__ StackEntry stack_entry(int tile, const TcParams& p, c
     se.M = p.M;
     se.c_off = (long long)e * st.stride_c;
   }
+  if constexpr (STACK == STACK_KGROUP) {
+    se.k0 = grp_end[e];
+    se.k_len = grp_end[e + 1] - grp_end[e];
+  } else {
+    se.k0 = 0;
+    se.k_len = p.K;
+  }
   se.a_entry = e * st.a_step;
   se.b_entry = e * st.b_step;
   return se;
 }
 
-template <int KIND, int BN, int STAGES, typename OutT, int AL, int BL, bool GROUPED>
+// KGROUP: zeroes K rows [r0, BK) of one stage's MN-major boxes (A's, then B's; contiguous in shared memory), where one
+// K row of a SWIZZLE_128B box is one whole 128-byte line, so no swizzle arithmetic is needed.  The 256 consumer threads
+// share the lines; each then makes its stores visible to the tensor cores' async proxy, and both consumer warpgroups
+// meet at named barrier 1 before either issues the stage's MMAs.
+template <class Cfg>
+__device__ __forceinline__ void zero_k_tail(uint32_t sA_stage, uint32_t sB_stage, int r0, int tid) {
+  static_assert(Cfg::A_MN && Cfg::B_MN, "K-grouped: MN-major A and B");
+  constexpr int BOXES = Cfg::A_BOXES + Cfg::B_BOXES;
+  static_assert(Cfg::A_STAGE == Cfg::A_BOXES * Cfg::MN_BOX_BYTES && Cfg::B_BOX_BYTES == Cfg::MN_BOX_BYTES,
+                "K-grouped: the stage is A's boxes then B's, each BK lines of 128 bytes");
+  const int rows = Cfg::BK - r0;
+  const int chunks = BOXES * rows * 8;                              // 16-byte chunks to clear
+  for (int i = tid; i < chunks; i += 256) {
+    const int box = i / (rows * 8), rest = i - box * (rows * 8);
+    const int line = r0 + (rest >> 3);
+    const uint32_t base = box < Cfg::A_BOXES ? sA_stage + box * Cfg::MN_BOX_BYTES
+                                             : sB_stage + (box - Cfg::A_BOXES) * Cfg::MN_BOX_BYTES;
+    const uint32_t addr = base + line * 128 + (rest & 7) * 16;
+    asm volatile("st.shared.v4.u32 [%0], {%1, %1, %1, %1};" ::"r"(addr), "r"(0u) : "memory");
+  }
+  fence_proxy_async();
+  asm volatile("bar.sync 1, 256;" ::: "memory");
+}
+
+// KGROUP, a group with k_g = 0: the element of the _ex call with k == 0, round_out(beta * float(C)), or raw +0 without
+// reading C when beta == 0 (not fma(beta, C, alpha * 0), whose zero signs differ).
+template <typename OutT>
+__device__ __forceinline__ void store_beta_c(const TcParams& p, int row, int col, float be) {
+  if (row >= p.M || col >= p.N) return;
+  if constexpr (std::is_same<OutT, float>::value) {
+    float* dst = reinterpret_cast<float*>(p.C) + (long long)row * p.ldc + col;
+    *dst = be != 0.f ? be * *dst : 0.f;
+  } else {
+    uint16_t* dst = reinterpret_cast<uint16_t*>(p.C) + (long long)row * p.ldc + col;
+    if (be == 0.f) { *dst = 0; return; }
+    const float x = be * c16_to_f32<OutT>(*dst);
+    const uint32_t w = std::is_same<OutT, f16_out>::value ? cvt_f16x2(x, 0.f) : cvt_bf16x2(x, 0.f);
+    *dst = (uint16_t)w;
+  }
+}
+
+template <int KIND, int BN, int STAGES, typename OutT, int AL, int BL, int STACK>
 __global__ void __launch_bounds__((TcConfig<KIND, BN, STAGES, ProdSingle, 128, AL, BL>::THREADS), 1)
 gemm_tc_stacked_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                        const TcParams p, const TcStack st) {
   using Cfg = TcConfig<KIND, BN, STAGES, ProdSingle, 128, AL, BL>;
   using MMA = typename Cfg::MMA;
   using Acc = typename MMA::Acc;
+  constexpr bool GROUPED = STACK == STACK_GROUP, KGROUP = STACK == STACK_KGROUP;
   static_assert(KindTraits<KIND>::ELEM == 2 && (std::is_same<OutT, float>::value || OutBytes<OutT>::V == 2),
                 "stacked: 16-bit kinds with fp32 or 16-bit C");
+  static_assert(STACK == STACK_BATCH || GROUPED || KGROUP, "stacked: a batch, a grouped or a K-grouped call");
   static_assert(!GROUPED || AL == LAYOUT_K, "grouped: A is row-major");
+  static_assert(!KGROUP || (AL == LAYOUT_MN && BL == LAYOUT_MN), "K-grouped: A^T and B, both MN-major");
 
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;   // swizzle atoms need 1 KB
@@ -670,23 +734,30 @@ gemm_tc_stacked_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
 
   const int* grp_end = nullptr;               // GROUPED: group g is rows [grp_end[g], grp_end[g + 1])
   const int* grp_tile = nullptr;              //          and tiles [grp_tile[g], grp_tile[g + 1]) of the tile order
-  int num_tiles;
-  if constexpr (GROUPED) {                    // the batched kernels declare no tables
+  int num_tiles;                              // KGROUP: group g is K rows [grp_end[g], grp_end[g + 1])
+  if constexpr (GROUPED || KGROUP) {          // the batched kernels declare no tables
     static_assert(Cfg::SMEM_BYTES + 2 * (kMaxGroups + 1) * (int)sizeof(int) <= 232448,
                   "the pipeline and the group tables exceed the 227 KB of shared memory of sm_90");
     __shared__ int s_end[kMaxGroups + 1];
     __shared__ int s_tile[kMaxGroups + 1];
-    group_table(st.offs, st.count, p.M, Cfg::BM, s_end, s_tile);     // ends in __syncthreads
-    grp_end = s_end;
-    grp_tile = s_tile;
-    num_tiles = grp_tile[st.count] * p.tiles_n;                      // CTAs past it have no work
+    if constexpr (GROUPED) {
+      group_table(st.offs, st.count, p.M, Cfg::BM, s_end, s_tile);   // ends in __syncthreads
+      grp_end = s_end;
+      grp_tile = s_tile;
+      num_tiles = grp_tile[st.count] * p.tiles_n;                    // CTAs past it have no work
+    } else {
+      group_table(st.offs, st.count, p.K, Cfg::BK, s_end, s_tile);   // only the K ends are used
+      grp_end = s_end;
+      num_tiles = p.tiles_m * p.tiles_n * st.count;
+    }
   } else {
     num_tiles = p.tiles_m * p.tiles_n * st.count;
   }
   const int num_items = p.full_tiles + (num_tiles - p.full_tiles) * p.split;
   const int num_kb = (p.K + Cfg::BK - 1) / Cfg::BK;
-  // GROUPED work items are whole tiles (split = 1), known at compile time: with a run-time part the split tail's
-  // branches stay in the epilogue, and ptxas specialises its store loop less (DESIGN §9: 1-2.5 % slower on an H100)
+  // GROUPED and KGROUP work items are whole tiles (split = 1), known at compile time: with a run-time part the split
+  // tail's branches stay in the epilogue, and ptxas specialises its store loop less (DESIGN §9: 1-2.5 % slower on an
+  // H100).  A KGROUP tile's k-blocks are its group's.
 
   if (warp < 4) {
     // ===================== TMA producer (warpgroup 0) =====================
@@ -695,8 +766,9 @@ gemm_tc_stacked_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
       int s = 0;
       uint32_t ph = 0;
       for (int w = blockIdx.x; w < num_items; w += gridDim.x) {
-        const WorkItem it = GROUPED ? WorkItem{w, 0, 0, num_kb} : work_item(w, p, num_kb);
-        const StackEntry se = stack_entry<GROUPED>(it.tile, p, st, grp_end, grp_tile);
+        WorkItem it = STACK == STACK_BATCH ? work_item(w, p, num_kb) : WorkItem{w, 0, 0, num_kb};
+        const StackEntry se = stack_entry<STACK>(it.tile, p, st, grp_end, grp_tile);
+        if constexpr (KGROUP) it.kb1 = (se.k_len + Cfg::BK - 1) / Cfg::BK;
         int mb, nb;
         tile_coords(it.tile - se.tile0, se.tiles_m, p.tiles_n, p.group_m, mb, nb);
         const int m0 = se.a_row + mb * Cfg::BM, n0 = nb * BN;
@@ -704,21 +776,22 @@ gemm_tc_stacked_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
           mbar_wait(bar_empty + 8 * s, ph ^ 1);
           const uint32_t full = bar_full + 8 * s;
           mbar_arrive_expect_tx(full, Cfg::STAGE_BYTES);
+          const int kr = se.k0 + kb * Cfg::BK;        // K row of the box (se.k0 = 0 but for KGROUP)
           if constexpr (Cfg::A_MN) {                  // A^T (k x m): one 64-column box per consumer
 #pragma unroll
             for (int j = 0; j < Cfg::A_BOXES; j++)
               tma_load_3d(sA + s * Cfg::A_STAGE + j * Cfg::MN_BOX_BYTES, &tmA, full, m0 + j * Cfg::MN_BOX_COLS,
-                          kb * Cfg::BK, se.a_entry);
+                          kr, se.a_entry);
           } else {
-            tma_load_3d(sA + s * Cfg::A_STAGE, &tmA, full, kb * Cfg::BK, m0, se.a_entry);
+            tma_load_3d(sA + s * Cfg::A_STAGE, &tmA, full, kr, m0, se.a_entry);
           }
           if constexpr (!Cfg::B_MN) {                 // B^T (n x k): one box of BN rows
-            tma_load_3d(sB + s * Cfg::B_STAGE, &tmB, full, kb * Cfg::BK, n0, se.b_entry);
+            tma_load_3d(sB + s * Cfg::B_STAGE, &tmB, full, kr, n0, se.b_entry);
           } else {
 #pragma unroll
             for (int j = 0; j < Cfg::B_BOXES; j++)
               tma_load_3d(sB + s * Cfg::B_STAGE + j * Cfg::B_BOX_BYTES, &tmB, full, n0 + j * Cfg::B_BOX_COLS,
-                          kb * Cfg::BK, se.b_entry);
+                          kr, se.b_entry);
           }
           if (++s == STAGES) { s = 0; ph ^= 1; }
         }
@@ -736,8 +809,9 @@ gemm_tc_stacked_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
     uint32_t ph = 0;
     Acc acc[Cfg::ACC];
     for (int w = blockIdx.x; w < num_items; w += gridDim.x) {
-      const WorkItem it = GROUPED ? WorkItem{w, 0, 0, num_kb} : work_item(w, p, num_kb);
-      const StackEntry se = stack_entry<GROUPED>(it.tile, p, st, grp_end, grp_tile);
+      WorkItem it = STACK == STACK_BATCH ? work_item(w, p, num_kb) : WorkItem{w, 0, 0, num_kb};
+      const StackEntry se = stack_entry<STACK>(it.tile, p, st, grp_end, grp_tile);
+      if constexpr (KGROUP) it.kb1 = (se.k_len + Cfg::BK - 1) / Cfg::BK;
       int mb, nb;
       tile_coords(it.tile - se.tile0, se.tiles_m, p.tiles_n, p.group_m, mb, nb);
       const int m0 = mb * Cfg::BM, n0 = nb * BN;      // m0: row inside the entry
@@ -746,6 +820,10 @@ gemm_tc_stacked_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
         mbar_wait(bar_full + 8 * s, ph);
         const uint32_t a0 = sA + s * Cfg::A_STAGE + cw * Cfg::A_WG;
         const uint32_t b0 = sB + s * Cfg::B_STAGE;
+        if constexpr (KGROUP) {                        // the group's last box: rows past k_g are not its own
+          const int r0 = se.k_len - kb * Cfg::BK;
+          if (r0 < Cfg::BK) zero_k_tail<Cfg>(sA + s * Cfg::A_STAGE, b0, r0, threadIdx.x - 128);
+        }
         wgmma_fence();
 #pragma unroll
         for (int k = 0; k < Cfg::MMAS_PER_STAGE; k++) {
@@ -788,6 +866,15 @@ gemm_tc_stacked_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
       TcParams pc = p;
       pc.C = static_cast<uint8_t*>(p.C) + se.c_off * OutBytes<OutT>::V;
       pc.M = se.M;
+      if constexpr (KGROUP) {
+        if (it.kb1 == 0) {                             // an empty group: the _ex k == 0 result
+          const float beta0 = p.axpby ? p.beta : 0.f;
+          for (int j = 0; j < BN / 8; j++)
+            for (int h = 0; h < 2; h++)
+              for (int e = 0; e < 2; e++) store_beta_c<OutT>(pc, row0 + 8 * h, col0 + 8 * j + e, beta0);
+          continue;
+        }
+      }
       const int ce[2] = {0, 0};
 #pragma unroll
       for (int j = 0; j < BN / 8; j++)

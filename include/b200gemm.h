@@ -257,6 +257,48 @@ int b200_gemm_f16_grouped(int op_b, int total_m, int n, int k, float alpha,
                           const int32_t* dOffs, int groups, float beta,
                           void* dC, int ldc, int out_type, void* stream);
 
+/* K-grouped 16-bit GEMM (torch._grouped_mm(dy.t(), x, offs=offs), 2-D x 2-D; the weight gradient dW_g = dy_g^T x_g of
+ * a mixture-of-experts layer): the offsets split the contraction dimension, and every group writes a whole C_g.
+ * op(A) is m x total_k and op(B) is total_k x n, each stored as for _ex: op_a = B200_OP_T, A stored total_k x m
+ * (lda >= m, the dy.t() of a row-major dy); op_b = B200_OP_N, B is total_k x n (ldb >= n, a row-major x); N and T
+ * otherwise as in b200_gemm_f32_op.  dOffs holds `groups` int32 cumulative ends on the DEVICE; with end_{-1} = 0,
+ *   end_g = min(max(dOffs[g], end_{g-1}), total_k),   k_g = end_g - end_{g-1},
+ *   C_g = round_out(fma(beta, float(C_g), alpha * op(A)[:, end_{g-1}:end_g] * op(B)[end_{g-1}:end_g, :]))
+ * for every g < groups, with C_g (m x n, row-major, ldc >= n) at dC + g * stride_c (elements).  Every group is
+ * written: an empty one (k_g = 0) stores exactly what _ex with k == 0 stores, raw +0 when beta == 0 (C unread) and
+ * round_out(beta * float(C)) otherwise.  Each C_g is bit for bit the _ex call with k = k_g on contiguous copies of its
+ * K range of A and B, at the same tile width (the _ex call with the K-split tail off).  The host never reads dOffs and
+ * never synchronises, so the call can be captured in a CUDA graph and replayed with new offsets.
+ * Argument rules, each checked before the device is touched:
+ *   - the _ex rules for an (m, n, total_k) call: ops, minimum ld, out_type pairing; beta == 0 never reads C; alpha == 0
+ *     or total_k == 0 never reads A or B.
+ *   - negative sizes, groups or stride_c, groups > 1024, and total_k > 2^31 - 65 (K row coordinates up to end + 64
+ *     stay within int32) are B200_ERR_BAD_ARG.
+ *   - groups > 1 with stride_c < (m - 1) * ldc + n is B200_ERR_BAD_ARG: two C_g would overlap.  So is
+ *     (groups - 1) * stride_c above 2^60 elements.
+ *   - groups * ceil(m / 128) * ceil(n / 128) above 2^30 - 1 is B200_ERR_BAD_ARG: the kernel counts its tiles in an int.
+ *   - groups == 0, m == 0 or n == 0 is a no-op, NULL pointers included; a NULL pointer with work to do, dOffs
+ *     included, is B200_ERR_BAD_ARG.  total_k == 0 is not a no-op: every C_g becomes beta * C_g, or zeros.
+ * Routes, each one launch, no workspace, no K-split tail:
+ *   - (op_a, op_b) = (T, N) with 16-byte-aligned A and B and lda, ldb multiples of 16 bytes: the persistent tensor-core
+ *     kernel over every group's tiles, group outermost, tile width chosen for groups x m x n as for a batch;
+ *     b200_gemm_debug_last_schedule reports tiles = groups * ceil(m / 128) * ceil(n / BN), split 1.  Kernels
+ *     "tc_bf16_kgrp_tn_128x256", "tc_bf16_obf16_kgrp_tn_128x192", "tc_f16_kgrp_tn_128x128",
+ *     "tc_f16_of16_kgrp_tn_128x256", ...
+ *   - every other layout, and operands TMA cannot read: the generic kernel, "generic_bf16_kgrp_64x64" /
+ *     "generic_f16_kgrp_64x64", every group bit for bit as the 2-D generic kernel computes it.
+ *   - alpha == 0 or total_k == 0: one element-wise pass over every C_g, "fill_zero_bat" (beta == 0) or
+ *     "scale_inplace_bat".
+ * No bias or activation epilogue. */
+int b200_gemm_bf16_grouped_k(int op_a, int op_b, int m, int n, int total_k, float alpha,
+                             const uint16_t* dA, int lda, const uint16_t* dB, int ldb,
+                             const int32_t* dOffs, int groups, float beta,
+                             void* dC, int ldc, long long stride_c, int out_type, void* stream);
+int b200_gemm_f16_grouped_k(int op_a, int op_b, int m, int n, int total_k, float alpha,
+                            const uint16_t* dA, int lda, const uint16_t* dB, int ldb,
+                            const int32_t* dOffs, int groups, float beta,
+                            void* dC, int ldc, long long stride_c, int out_type, void* stream);
+
 /* 16-bit operands with a bias vector and an activation fused into the epilogue (cuBLASLt's CUBLASLT_EPILOGUE_BIAS,
  * _RELU_BIAS, _GELU_BIAS): C = round_out(act(alpha * op(A)*op(B) + beta * C + bias)), what a PyTorch
  * act(F.linear(x, W, b)) computes, in one launch.  Arguments as b200_gemm_bf16_ex / b200_gemm_f16_ex, plus:
@@ -349,6 +391,9 @@ int b200_gemm_s8s32_host(int m, int n, int k,
  *                                                                        generic and alpha == 0 / k == 0: 1)
  *   bf16 / fp16 grouped      1   1                -                -     every group in one launch (_grouped; also
  *                                                                        generic and alpha == 0 / k == 0: 1)
+ *   bf16 / fp16 grouped (K)  1   1                1                1     every group in one launch (_grouped_k; TN on
+ *                                                                        the tensor cores, NN / NT / TT generic;
+ *                                                                        alpha == 0 / total_k == 0: 1)
  *   TF32, int8               2   1                3                2     transposes into the workspace
  *   BF16X3, BF16X2           2   2                2                2     one split launch for both operands
  *   F16X2                    4   3                5                4     B^T's column maxima are its row maxima (the
