@@ -21,6 +21,7 @@ OUT_F32, OUT_BF16, OUT_F16 = 0, 1, 2
 OP_N, OP_T = 0, 1
 ACT_NONE, ACT_RELU, ACT_GELU, ACT_GELU_TANH = 0, 1, 2, 3
 ACTIVATIONS = {None: ACT_NONE, "relu": ACT_RELU, "gelu": ACT_GELU, "gelu_tanh": ACT_GELU_TANH}
+FP8_E4M3, FP8_E5M2 = 0, 1
 
 EXPORTS = [
     "b200_gemm_version", "b200_gemm_device_ok", "b200_gemm_strerror", "b200_gemm_last_kernel",
@@ -31,7 +32,7 @@ EXPORTS = [
     "b200_gemm_f32_pack_free", "b200_gemm_f32_op", "b200_gemm_bf16_op", "b200_gemm_bf16_ex", "b200_gemm_f16_ex",
     "b200_gemm_bf16_epi", "b200_gemm_f16_epi", "b200_gemm_bf16_batched", "b200_gemm_f16_batched",
     "b200_gemm_bf16_grouped", "b200_gemm_f16_grouped", "b200_gemm_bf16_grouped_k", "b200_gemm_f16_grouped_k",
-    "b200_gemm_s8s32_op", "b200_gemm_workspace_bytes_op",
+    "b200_gemm_s8s32_op", "b200_gemm_workspace_bytes_op", "b200_gemm_fp8",
     "b200_nccl_load", "b200_nccl_last_error", "b200_comm_unique_id", "b200_comm_init_rank",
     "b200_comm_destroy", "b200_rowpanel_create", "b200_rowpanel_destroy", "b200_rowpanel_slices", "b200_rowpanel_set_reserve_sms", "b200_rowpanel_trace", "b200_rowpanel_trace_dump", "b200_gemm_f32_rowpanel",
     "b200_gemm_f32_rowpanel_host", "b200_gemm_f32_pack_a", "b200_gemm_f32_packed_ab", "b200_gemm_f32_pack_free_a",
@@ -99,6 +100,7 @@ lib.b200_gemm_f16_grouped_k.argtypes = [_i, _i, _i, _i, _i, C.c_float, _vp, _i, 
                                         _i, _vp]
 lib.b200_gemm_s8s32_op.argtypes = [_i, _i, _i, _i, _i, _vp, _i, _vp, _i, _vp, _i, _vp]
 lib.b200_gemm_workspace_bytes_op.argtypes = [_i, _i, _i, _i, _i, _i]
+lib.b200_gemm_fp8.argtypes = [_i, _i, _i, _i, _i, _i, _i, _vp, _i, _vp, _i, _vp, _i, _vp, _i, _vp, _vp, _i, _i, _i, _vp]
 lib.b200_gemm_workspace_bytes_op.restype = C.c_size_t
 lib.b200_gemm_f32_pack_b.argtypes = [_i, _i, _vp, _i, _i, C.POINTER(_vp), _vp]
 lib.b200_gemm_f32_packed.argtypes = [_i, _i, _i, _vp, _i, _vp, _vp, _i, _i, _vp]
@@ -477,6 +479,72 @@ def gemm(A, B, out=None, *, offs=None, alpha=1.0, beta=0.0, bias=None, activatio
                   OUT_F32 if cdt == torch.float32 else ot, bias.data_ptr() if bias is not None else None, act, st))
     else:
         _check(lib.b200_gemm_s8s32_op(op_a, op_b, m, n, k, A.data_ptr(), lda, B.data_ptr(), ldb, out.data_ptr(), _ld(out), st))
+    return out
+
+
+def _fp8_type(t):
+    import torch
+    return {torch.float8_e4m3fn: FP8_E4M3, torch.float8_e5m2: FP8_E5M2}.get(t.dtype)
+
+
+def scaled_mm(A, B, scale_a, scale_b, bias=None, out_dtype=None, use_fast_accum=False, out=None, stream=None):
+    """torch._scaled_mm for FP8 CUDA tensors: out = ((A @ B) * scale_a) * scale_b + bias, each step rounded in fp32 and
+    the result rounded once to out_dtype (b200_gemm_fp8).
+
+    A (m x k) and B (k x n) are float8_e4m3fn or float8_e5m2 (not both e5m2), each row-major or the transpose of a
+    row-major matrix and read in place; torch's layout is a row-major A and a column-major B (x @ W.t()).  scale_a and
+    scale_b are float32 CUDA tensors: one element each (tensorwise), or scale_a (m, 1) and scale_b (1, n) (rowwise).
+    They stay on the device: the call never synchronises.  bias: None or n contiguous elements of out_dtype.  out_dtype
+    is torch.bfloat16 (the default), torch.float16 or torch.float32.  use_fast_accum = False promotes the tensor core's
+    FP8 sums to fp32 every 128 elements of K; True keeps one tensor-core accumulator over K (faster, less precise).
+    Operands of other dtypes, or two e5m2 operands, are a TypeError; a scale of another shape or dtype, a CPU tensor,
+    another bias, out_dtype or out (shape, dtype, or rows that overlap) is a ValueError."""
+    import torch
+    out_dtype = out_dtype or (out.dtype if out is not None else torch.bfloat16)
+    ta, tb = _fp8_type(A), _fp8_type(B)
+    if ta is None or tb is None:
+        raise TypeError(f"operands must be float8_e4m3fn or float8_e5m2, not {A.dtype} and {B.dtype}")
+    if ta == FP8_E5M2 and tb == FP8_E5M2:
+        raise TypeError("float8_e5m2 x float8_e5m2 is not supported (as in torch._scaled_mm)")
+    if A.dim() != 2 or B.dim() != 2 or A.shape[1] != B.shape[0]:
+        raise ValueError(f"A and B must be 2-D with matching inner dimensions, not {tuple(A.shape)} and {tuple(B.shape)}")
+    m, k = A.shape
+    n = B.shape[1]
+    if out_dtype not in (torch.bfloat16, torch.float16, torch.float32):
+        raise ValueError(f"out_dtype must be bfloat16, float16 or float32, not {out_dtype}")
+    rows = []
+    for name, s, length, shape in (("scale_a", scale_a, m, (m, 1)), ("scale_b", scale_b, n, (1, n))):
+        if s.dtype != torch.float32:
+            raise ValueError(f"{name} must be float32, not {s.dtype}")
+        if s.numel() == 1:
+            rows.append(0)
+        elif s.numel() == length and tuple(s.shape) == shape and s.is_contiguous():
+            rows.append(1)
+        else:
+            raise ValueError(f"{name} must have one element or shape {shape}, not {tuple(s.shape)}")
+    if bias is not None:
+        if bias.dtype != out_dtype:
+            raise ValueError(f"the bias must have dtype {out_dtype}, not {bias.dtype}")
+        if bias.dim() != 1 or bias.shape[0] != n or not bias.is_contiguous():
+            raise ValueError(f"the bias must be contiguous and 1-D with n = {n} elements, not of shape {tuple(bias.shape)}")
+    if out is not None:
+        if out.dtype != out_dtype or tuple(out.shape) != (m, n):
+            raise ValueError(f"out must be {out_dtype} of shape {(m, n)}, not {out.dtype} of shape {tuple(out.shape)}")
+        if (n > 1 and out.stride(1) != 1) or (m > 1 and out.stride(0) < n):
+            raise ValueError(f"out must be row-major with rows that do not overlap, not of strides {tuple(out.stride())}")
+    op_a, lda = operand_layout(tuple(A.shape), A.stride())
+    op_b, ldb = operand_layout(tuple(B.shape), B.stride())
+    tensors = [A, B, scale_a, scale_b] + [t for t in (bias, out) if t is not None]
+    if not all(t.is_cuda for t in tensors):
+        raise ValueError("A, B, the scales, the bias and out must be CUDA tensors")
+    if out is None:
+        out = torch.empty((m, n), dtype=out_dtype, device=A.device)
+    if m == 0 or n == 0:
+        return out
+    ot = {torch.float32: OUT_F32, torch.bfloat16: OUT_BF16, torch.float16: OUT_F16}[out_dtype]
+    _check(lib.b200_gemm_fp8(op_a, op_b, ta, tb, m, n, k, A.data_ptr(), lda, B.data_ptr(), ldb, scale_a.data_ptr(),
+                             rows[0], scale_b.data_ptr(), rows[1], bias.data_ptr() if bias is not None else None,
+                             out.data_ptr(), _ld(out), ot, int(bool(use_fast_accum)), _stream_ptr(stream)))
     return out
 
 

@@ -393,6 +393,7 @@ int g_ffma_halves = 1;        // strict kernel: split the tail round into half t
 //   STACK_KGROUP: groups of K rows [end_g-1, end_g) of one A^T and one B (k = total_k; sa = sb = 0: A and B are
 //   broadcast), C_g = C + g * sc, with the ends read on the device.  The tiles are a batch's, with no K split.
 // (Stacking, gemm_tc.cuh, names the forms.)
+// FP8 kinds (KIND_E4M3, ...): gemm_tc_fp8_kernel with the scales and bias *scl; K-major A and B, no K split.
 struct Stack {
   int count;               // entries of a batch, or groups
   long long sa, sb, sc;    // elements between consecutive entries of A, B and C
@@ -406,9 +407,10 @@ template <int KIND, int BN, int STAGES, typename OutT, class Prod = ProdSingle, 
 int launch_tc(int m, int n, int k, const void* A, long long lda, int a_rows_total, int a_plane_rows,
               const void* B, long long ldb, int b_rows_total, int b_plane_rows, void* C, int ldc,
               const char* name, const Call& c, int chunk_k = 0, const float* row_max = nullptr,
-              const float* col_max = nullptr, const Stack* stk = nullptr) {
+              const float* col_max = nullptr, const Stack* stk = nullptr, const TcScale* scl = nullptr) {
   using Cfg = TcConfig<KIND, BN, STAGES, Prod, A_ROW_BYTES, AL, BL>;
   using T = KindTraits<KIND>;
+  constexpr bool FP8 = KIND == KIND_E4M3 || KIND == KIND_E4M3E5M2 || KIND == KIND_E5M2E4M3;
   constexpr CUtensorMapDataType dt = KIND == KIND_F16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
                                    : KIND == KIND_FP16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16
                                    : KIND == KIND_TF32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32
@@ -458,6 +460,7 @@ int launch_tc(int m, int n, int k, const void* A, long long lda, int a_rows_tota
   p.stream_c = g_stream_c < 0 ? (g_stream_c = (getenv("B200GEMM_STREAM_C") ? atoi(getenv("B200GEMM_STREAM_C")) : kStreamCDefault)) : g_stream_c;
   auto kern = [] {
     if constexpr (STACK != STACK_NONE) return gemm_tc_stacked_kernel<KIND, BN, STAGES, OutT, AL, BL, STACK>;
+    else if constexpr (FP8) return gemm_tc_fp8_kernel<KIND, BN, STAGES, OutT, Prod>;
     else return gemm_tc_kernel<KIND, BN, STAGES, OutT, Prod, A_ROW_BYTES, AL, BL, EPI>;
   }();
   if (int arc = ensure_smem_attr(kern, Cfg::SMEM_BYTES)) return arc;
@@ -473,8 +476,8 @@ int launch_tc(int m, int n, int k, const void* A, long long lda, int a_rows_tota
   const int rem = tiles % units_max;
   int split = 1;
   // an activation must see the complete sum, and a grouped call's tile count is not known here: no split.  Nor for a
-  // K-grouped call, whose tiles have their groups' k-blocks.
-  if (!EPI && STACK != STACK_GROUP && STACK != STACK_KGROUP && g_split_tail && OB == 4 && rem > 0) {
+  // K-grouped call, whose tiles have their groups' k-blocks, or for FP8, whose scaled epilogue must see the whole sum.
+  if (!EPI && !FP8 && STACK != STACK_GROUP && STACK != STACK_KGROUP && g_split_tail && OB == 4 && rem > 0) {
     split = units_max / rem;
     if (split > 4) split = 4;
     if (split > num_kb / 8) split = num_kb / 8;       // keep >= 8 k-blocks per part
@@ -497,6 +500,7 @@ int launch_tc(int m, int n, int k, const void* A, long long lda, int a_rows_tota
   {
     cudaError_t e;
     if constexpr (STACK != STACK_NONE) e = launch_pdl(kern, dim3(units), dim3(Cfg::THREADS), Cfg::SMEM_BYTES, c.st, 1, tmA, tmB, p, ts);
+    else if constexpr (FP8) e = launch_pdl(kern, dim3(units), dim3(Cfg::THREADS), Cfg::SMEM_BYTES, c.st, 1, tmA, tmB, p, *scl);
     else e = launch_pdl(kern, dim3(units), dim3(Cfg::THREADS), Cfg::SMEM_BYTES, c.st, 1, tmA, tmB, p);
     release_flag_slot(flag_user, c.st);
     if (e != cudaSuccess) { cudaGetLastError(); return (int)e; }
@@ -688,6 +692,40 @@ size_t kmajor_ws_bytes(int op_a, int op_b, int m, int n, int k, int elem) {
   return a ? round1024(b) + a : b;
 }
 
+// The K-major A (m x k) and B^T (n x k) that wgmma reads for tf32, int8 and FP8, staged in the workspace `ws` laid out
+// as kmajor_ws_bytes(op_a, op_b) says: a row-major B and an A given as A^T are transposed there.  So is, copied at a
+// 16-byte pitch in one pass, an operand given K-major that TMA cannot describe (base or pitch not a 16-byte multiple):
+// the caller passes it as op_a = T / op_b = N with `copy_a` / `copy_b` set (FP8 only; tf32 and int8 take such
+// operands to the generic kernel).
+template <typename E>
+int stage_kmajor(int op_a, int op_b, int m, int n, int k, const void*& A, long long& lda, const void*& B, long long& ldb,
+                 uint8_t* ws, cudaStream_t st, bool copy_a = false, bool copy_b = false) {
+  const long long kp = pitch16(k, sizeof(E));
+  if (!op_b) {
+    E* d = reinterpret_cast<E*>(ws);
+    if (copy_b) {                                                                                  // B^T -> B^T
+      const cudaError_t e = cudaMemcpy2DAsync(d, kp * sizeof(E), B, ldb * sizeof(E), (size_t)k * sizeof(E), n,
+                                              cudaMemcpyDeviceToDevice, st);
+      if (e != cudaSuccess) { cudaGetLastError(); return (int)e; }
+    } else if (int rc = launch_transpose<E>(static_cast<const E*>(B), ldb, k, n, d, kp, st)) {    // B -> B^T
+      return rc;
+    }
+    B = d; ldb = kp;
+  }
+  if (op_a) {
+    E* d = reinterpret_cast<E*>(ws + (op_b ? 0 : round1024((size_t)n * kp * sizeof(E))));
+    if (copy_a) {                                                                                  // A -> A
+      const cudaError_t e = cudaMemcpy2DAsync(d, kp * sizeof(E), A, lda * sizeof(E), (size_t)k * sizeof(E), m,
+                                              cudaMemcpyDeviceToDevice, st);
+      if (e != cudaSuccess) { cudaGetLastError(); return (int)e; }
+    } else if (int rc = launch_transpose<E>(static_cast<const E*>(A), lda, k, m, d, kp, st)) {    // A^T -> A
+      return rc;
+    }
+    A = d; lda = kp;
+  }
+  return 0;
+}
+
 // tf32 / int8 with any layout: wgmma reads these operand types only K-major.  B given as B^T is read in place (NT
 // needs no transpose and no workspace); a row-major B, and an A given as A^T, are transposed into the workspace first.
 template <int KIND, int BN, int STAGES, typename OutT>
@@ -696,19 +734,9 @@ int launch_tc_kmajor(int op_a, int op_b, int m, int n, int k, const void* A, lon
                      const float* col_max = nullptr) {
   if (!op_a && op_b) return launch_tc<KIND, BN, STAGES, OutT>(m, n, k, A, lda, m, 0, B, ldb, n, 0, C, ldc, name, c, 0, row_max, col_max);
   using E = typename std::conditional<KIND == KIND_TF32, float, uint8_t>::type;
-  const long long kp = pitch16(k, sizeof(E));
   WsLease ws(kmajor_ws_bytes(op_a, op_b, m, n, k, sizeof(E)), c.st);
   if (ws.rc) return ws.rc;
-  if (!op_b) {
-    E* d = reinterpret_cast<E*>(ws.base());
-    if (int rc = launch_transpose<E>(static_cast<const E*>(B), ldb, k, n, d, kp, c.st)) return rc;   // B -> B^T
-    B = d; ldb = kp;
-  }
-  if (op_a) {
-    E* d = reinterpret_cast<E*>(ws.base() + (op_b ? 0 : round1024((size_t)n * kp * sizeof(E))));
-    if (int rc = launch_transpose<E>(static_cast<const E*>(A), lda, k, m, d, kp, c.st)) return rc;   // A^T -> A
-    A = d; lda = kp;
-  }
+  if (int rc = stage_kmajor<E>(op_a, op_b, m, n, k, A, lda, B, ldb, ws.base(), c.st)) return rc;
   return launch_tc<KIND, BN, STAGES, OutT>(m, n, k, A, lda, m, 0, B, ldb, n, 0, C, ldc, name, c, 0, row_max, col_max);
 }
 
@@ -1424,6 +1452,80 @@ int gemm_s8(int op_a, int op_b, int m, int n, int k, const int8_t* A, int lda, c
   return tc_s8(op_a, op_b, m, n, k, A, lda, B, ldb, C, ldc, c);
 }
 
+// ---- FP8 (torch._scaled_mm) ------------------------------------------------------------------------------------------
+// Kernel names by [kind][C type][width index, 3 = promoted].
+#define FP8_NAMES(P)                                                                                      \
+  {{P "_of32_128x256", P "_of32_128x192", P "_of32_128x128", P "_of32_acc_128x128"},                      \
+   {P "_obf16_128x256", P "_obf16_128x192", P "_obf16_128x128", P "_obf16_acc_128x128"},                  \
+   {P "_of16_128x256", P "_of16_128x192", P "_of16_128x128", P "_of16_acc_128x128"}}
+const char* const kFp8Names[3][3][4] = {FP8_NAMES("tc_e4m3"), FP8_NAMES("tc_e4m3e5m2"), FP8_NAMES("tc_e5m2e4m3")};
+
+// Every layout and pitch runs on the tensor cores: (N, T) with TMA-able operands is read in place; otherwise the
+// operands are made K-major and TMA-able in the workspace (stage_kmajor), which holds the same bytes, so every route is
+// bit-identical to the aligned (N, T) call.  fast: one accumulator over K at pick_bn's width; else promoted per
+// 128-element k-block (two 64 x BN fp32 tiles in registers: BN = 128).
+template <int KIND, typename OutT>
+int tc_fp8(int op_a, int op_b, int m, int n, int k, const void* A, long long lda, const void* B, long long ldb, void* C,
+           int ldc, const TcScale& sc, bool fast, const char* const (&names)[4], const Call& c) {
+  const bool copy_a = !op_a && !(aligned16(A) && lda % 16 == 0);
+  const bool copy_b = op_b && !(aligned16(B) && ldb % 16 == 0);
+  const int sa = op_a || copy_a, sb = op_b && !copy_b;          // kmajor_ws_bytes / stage_kmajor's view of the layout
+  auto run = [&](const void* a, long long la, const void* b, long long lb) {
+    if (fast)
+      return with_width(m, n, [&](auto W) {
+        using Wd = decltype(W);
+        return launch_tc<KIND, Wd::BN, Wd::STAGES, OutT>(m, n, k, a, la, m, 0, b, lb, n, 0, C, ldc, names[Wd::idx], c,
+                                                         0, nullptr, nullptr, nullptr, &sc);
+      });
+    return launch_tc<KIND, 128, Width<128>::STAGES, OutT, ProdPromoted>(m, n, k, a, la, m, 0, b, lb, n, 0, C, ldc,
+                                                                          names[3], c, 128, nullptr, nullptr, nullptr,
+                                                                          &sc);
+  };
+  if (!sa && sb) return run(A, lda, B, ldb);
+  WsLease ws(kmajor_ws_bytes(sa, sb, m, n, k, 1), c.st);
+  if (ws.rc) return ws.rc;
+  if (int rc = stage_kmajor<uint8_t>(sa, sb, m, n, k, A, lda, B, ldb, ws.base(), c.st, copy_a, copy_b)) return rc;
+  return run(A, lda, B, ldb);
+}
+
+template <int KIND>
+int gemm_fp8_kind(int op_a, int op_b, int m, int n, int k, const void* A, int lda, const void* B, int ldb, void* C, int ldc,
+                  int out_type, const TcScale& sc, bool fast, const Call& c) {
+  const auto& names = kFp8Names[KIND - KIND_E4M3][out_type];
+  if (out_type == B200_OUT_F32) return tc_fp8<KIND, float>(op_a, op_b, m, n, k, A, lda, B, ldb, C, ldc, sc, fast, names, c);
+  if (out_type == B200_OUT_BF16) return tc_fp8<KIND, bf16_out>(op_a, op_b, m, n, k, A, lda, B, ldb, C, ldc, sc, fast, names, c);
+  return tc_fp8<KIND, f16_out>(op_a, op_b, m, n, k, A, lda, B, ldb, C, ldc, sc, fast, names, c);
+}
+
+// C = round_out((op(A) op(B) * sa_i) * sb_j + bias_j); every argument is checked before the device is touched.
+int gemm_fp8(int op_a, int op_b, int a_type, int b_type, int m, int n, int k, const uint8_t* A, int lda, const uint8_t* B,
+             int ldb, const float* scale_a, int scale_a_rowwise, const float* scale_b, int scale_b_colwise,
+             const void* bias, void* C, int ldc, int out_type, int fast_accum, cudaStream_t st) {
+  auto fp8 = [](int t) { return t == B200_FP8_E4M3 || t == B200_FP8_E5M2; };
+  if (!fp8(a_type) || !fp8(b_type)) return B200_ERR_BAD_ARG;
+  if (out_type != B200_OUT_F32 && out_type != B200_OUT_BF16 && out_type != B200_OUT_F16) return B200_ERR_BAD_ARG;
+  if ((scale_a_rowwise != 0 && scale_a_rowwise != 1) || (scale_b_colwise != 0 && scale_b_colwise != 1)) return B200_ERR_BAD_ARG;
+  if (fast_accum != 0 && fast_accum != 1) return B200_ERR_BAD_ARG;
+  int rc = check_args(m, n, k, A, lda, B, ldb, C, ldc, op_a, op_b);
+  if (rc < 0) return rc;
+  if (a_type == B200_FP8_E5M2 && b_type == B200_FP8_E5M2) return B200_ERR_UNSUPPORTED;
+  if (rc == 1) return 0;
+  if (!scale_a || !scale_b) return B200_ERR_BAD_ARG;
+  if ((rc = ensure_device())) return rc;
+  Call c{st};
+  if (k == 0) {                 // round_out(+0 + bias_j), or +0: the bias pass with beta = 0, or the zero fill
+    if (bias) { c.bias = bias; c.act = ACT_NONE; }
+    if (out_type == B200_OUT_F32) return degenerate<float, float>(m, n, C, ldc, c);
+    if (out_type == B200_OUT_BF16) return degenerate<uint16_t, uint16_t>(m, n, C, ldc, c);
+    return degenerate<__half, __half>(m, n, C, ldc, c);
+  }
+  const TcScale sc{scale_a, scale_b, scale_a_rowwise, scale_b_colwise, bias};
+  if (a_type == B200_FP8_E5M2) return gemm_fp8_kind<KIND_E5M2E4M3>(op_a, op_b, m, n, k, A, lda, B, ldb, C, ldc, out_type, sc, fast_accum, c);
+  if (b_type == B200_FP8_E5M2) return gemm_fp8_kind<KIND_E4M3E5M2>(op_a, op_b, m, n, k, A, lda, B, ldb, C, ldc, out_type, sc, fast_accum, c);
+  return gemm_fp8_kind<KIND_E4M3>(op_a, op_b, m, n, k, A, lda, B, ldb, C, ldc, out_type, sc, fast_accum, c);
+}
+static_assert(KIND_E4M3E5M2 == KIND_E4M3 + 1 && KIND_E5M2E4M3 == KIND_E4M3 + 2, "kFp8Names rows follow the kinds");
+
 }  // namespace
 
 extern "C" {
@@ -1622,6 +1724,13 @@ int b200_gemm_f16_grouped_k(int op_a, int op_b, int m, int n, int total_k, float
 int b200_gemm_s8s32(int m, int n, int k, const int8_t* dA, int lda, const int8_t* dB, int ldb,
                     int32_t* dC, int ldc, void* stream) {
   return gemm_s8(B200_OP_N, B200_OP_N, m, n, k, dA, lda, dB, ldb, dC, ldc, (cudaStream_t)stream);
+}
+
+int b200_gemm_fp8(int op_a, int op_b, int a_type, int b_type, int m, int n, int k, const uint8_t* dA, int lda,
+                  const uint8_t* dB, int ldb, const float* dScaleA, int scale_a_rowwise, const float* dScaleB,
+                  int scale_b_colwise, const void* dBias, void* dC, int ldc, int out_type, int fast_accum, void* stream) {
+  return gemm_fp8(op_a, op_b, a_type, b_type, m, n, k, dA, lda, dB, ldb, dScaleA, scale_a_rowwise, dScaleB,
+                  scale_b_colwise, dBias, dC, ldc, out_type, fast_accum, (cudaStream_t)stream);
 }
 
 int b200_gemm_s8s32_op(int op_a, int op_b, int m, int n, int k, const int8_t* dA, int lda, const int8_t* dB, int ldb,

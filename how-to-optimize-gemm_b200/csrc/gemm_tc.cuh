@@ -48,6 +48,9 @@ template <> struct KindTraits<KIND_F16>  { static constexpr int ELEM = 2; static
 template <> struct KindTraits<KIND_FP16> { static constexpr int ELEM = 2; static constexpr int B_LAYOUT = LAYOUT_MN; };
 template <> struct KindTraits<KIND_TF32> { static constexpr int ELEM = 4; static constexpr int B_LAYOUT = LAYOUT_K; };
 template <> struct KindTraits<KIND_I8>   { static constexpr int ELEM = 1; static constexpr int B_LAYOUT = LAYOUT_K; };
+template <> struct KindTraits<KIND_E4M3> { static constexpr int ELEM = 1; static constexpr int B_LAYOUT = LAYOUT_K; };
+template <> struct KindTraits<KIND_E4M3E5M2> { static constexpr int ELEM = 1; static constexpr int B_LAYOUT = LAYOUT_K; };
+template <> struct KindTraits<KIND_E5M2E4M3> { static constexpr int ELEM = 1; static constexpr int B_LAYOUT = LAYOUT_K; };
 
 // Plane products issued per k-step.  Single: plain GEMM.  X3: a=a1+a2+a3, b likewise, all terms down
 // to 2^-16 relative (a1b3, a3b1, a2b2, a1b2, a2b1, a1b1) — dropped terms are <= 2^-24.  X2: two planes,
@@ -67,6 +70,11 @@ struct ProdX2 {   // (0,1) (1,0) (0,0)
   __host__ __device__ static constexpr int ia(int i) { return i == 1 ? 1 : 0; }
   __host__ __device__ static constexpr int ib(int i) { return i == 0 ? 1 : 0; }
 };
+// One plane, promoted: every chunk of TcParams::chunk_kb k-blocks starts a fresh wgmma accumulator that is added to the
+// tile's fp32 running sum in registers (REGACC), as the split modes do.  The FP8 kernels use it with chunks of one k-block.
+struct ProdPromoted : ProdSingle {};
+template <class Prod> struct Promotes { static constexpr bool V = Prod::N > 1; };
+template <> struct Promotes<ProdPromoted> { static constexpr bool V = true; };
 
 struct TcParams {
   void* C;
@@ -126,7 +134,7 @@ template <int KIND, int BN, int STAGES, class Prod, int A_ROW_BYTES, int AL = LA
 struct TcConfig {
   using T = KindTraits<KIND>;
   static constexpr bool A_MN = AL == LAYOUT_MN, B_MN = BL == LAYOUT_MN;
-  static constexpr bool REGACC = Prod::N > 1;
+  static constexpr bool REGACC = Promotes<Prod>::V;       // Prod::N > 1, or ProdPromoted
   static constexpr int BM = 128;
   static constexpr int TILE_M = BM;                         // rows of C per work unit
   static constexpr int CONSUMERS = 2;                       // warpgroups, 64 rows each
@@ -578,6 +586,157 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         if (lane == 0) {
           const int nv = it.part + 1 == p.split ? 0 : it.part + 1;
           asm volatile("st.release.gpu.global.s32 [%0], %1;" ::"l"(flag), "r"(nv) : "memory");
+        }
+      }
+    }
+  }
+}
+
+// ---- FP8 GEMM (torch._scaled_mm) ---------------------------------------------------------------------------------------
+// C = round_out((acc * sa_i) * sb_j + bias_j), each step one fp32 round-to-nearest operation (explicit intrinsics: no
+// FMA contraction).  acc is op(A) op(B) of the FP8 operands: with ProdSingle one wgmma accumulator over all of K
+// (fast accumulation); with ProdPromoted every chunk of p.chunk_kb k-blocks (the host passes one k-block, 128 elements)
+// starts a fresh accumulator that is added, rounded, to the tile's fp32 running sum in registers.  The scales are fp32
+// on the device, read here and never by the host: row i of A takes a[i * a_step] and column j of B b[j * b_step], a step
+// of 0 for one tensorwise scale and 1 for a vector.  It is a kernel of its own (a second argument, no K split, no
+// alpha / beta) so that gemm_tc_kernel and TcParams keep their code; its producer and MMA chain are gemm_tc_kernel's for
+// K-major A and B, and its store is store_pair's bias path.
+struct TcScale {
+  const float* a;          // [m] or [1]
+  const float* b;          // [n] or [1]
+  int a_step, b_step;      // 0 = tensorwise, 1 = one scale per row of A / column of B
+  const void* bias;        // [n] of C's type (bf16 / fp16 bits, or fp32), null = none
+};
+
+template <int KIND, int BN, int STAGES, typename OutT, class Prod>
+__global__ void __launch_bounds__((TcConfig<KIND, BN, STAGES, Prod, 128>::THREADS), 1)
+gemm_tc_fp8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const TcParams p,
+                   const TcScale sc) {
+  using Cfg = TcConfig<KIND, BN, STAGES, Prod, 128>;
+  using MMA = typename Cfg::MMA;
+  static_assert(KIND == KIND_E4M3 || KIND == KIND_E4M3E5M2 || KIND == KIND_E5M2E4M3, "FP8 kinds");
+  static_assert(!Cfg::A_MN && !Cfg::B_MN && Prod::NPA == 1 && Prod::NPB == 1, "FP8: K-major A and B, one plane");
+  static_assert(std::is_same<OutT, float>::value || OutBytes<OutT>::V == 2, "FP8: fp32, bf16 or fp16 C");
+
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;   // swizzle atoms need 1 KB
+  const uint32_t sA = smem_base;
+  const uint32_t sB = sA + STAGES * Cfg::A_STAGE;
+  const uint32_t bar_full = sB + STAGES * Cfg::B_STAGE;
+  const uint32_t bar_empty = bar_full + 8 * STAGES;
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmA);
+    tma_prefetch_desc(&tmB);
+    for (int i = 0; i < STAGES; i++) {
+      mbar_init(bar_full + 8 * i, 1);
+      mbar_init(bar_empty + 8 * i, Cfg::CONSUMERS);
+    }
+    fence_barrier_init();
+  }
+  __syncthreads();
+  griddep_launch();
+  griddep_wait();
+
+  const int num_tiles = p.tiles_m * p.tiles_n;
+  const int num_kb = (p.K + Cfg::BK - 1) / Cfg::BK;
+
+  if (warp < 4) {
+    // ===================== TMA producer (warpgroup 0) =====================
+    setmaxnreg_dec<40>();
+    if (warp == 0 && lane == 0) {
+      int s = 0;
+      uint32_t ph = 0;
+      for (int w = blockIdx.x; w < num_tiles; w += gridDim.x) {
+        int mb, nb;
+        tile_coords(w, p.tiles_m, p.tiles_n, p.group_m, mb, nb);
+        const int m0 = mb * Cfg::BM, n0 = nb * BN;
+        for (int kb = 0; kb < num_kb; kb++) {
+          mbar_wait(bar_empty + 8 * s, ph ^ 1);
+          const uint32_t full = bar_full + 8 * s;
+          mbar_arrive_expect_tx(full, Cfg::STAGE_BYTES);
+          tma_load_2d(sA + s * Cfg::A_STAGE, &tmA, full, kb * Cfg::BK, m0);
+          tma_load_2d(sB + s * Cfg::B_STAGE, &tmB, full, kb * Cfg::BK, n0);
+          if (++s == STAGES) { s = 0; ph ^= 1; }
+        }
+      }
+    }
+  } else {
+    // ===================== consumers (warpgroups 1 and 2): MMA chain + scaled epilogue =====================
+    setmaxnreg_inc<232>();
+    const int cw = warp / 4 - 1;
+    const int ew = warp - 4;
+    const bool wg_leader = (threadIdx.x & 127) == 0;
+    int s = 0;
+    uint32_t ph = 0;
+    float acc[Cfg::ACC];
+    float sum[Cfg::REGACC ? Cfg::ACC : 1];
+    for (int w = blockIdx.x; w < num_tiles; w += gridDim.x) {
+      int mb, nb;
+      tile_coords(w, p.tiles_m, p.tiles_n, p.group_m, mb, nb);
+      const int m0 = mb * Cfg::BM, n0 = nb * BN;
+      const int chunk = Cfg::REGACC ? p.chunk_kb : num_kb;
+      for (int c0 = 0; c0 < num_kb; c0 += chunk) {
+        const int c1 = min(c0 + chunk, num_kb);
+        int prev = -1;
+        for (int kb = c0; kb < c1; kb++) {
+          mbar_wait(bar_full + 8 * s, ph);
+          const uint32_t a0 = sA + s * Cfg::A_STAGE + cw * Cfg::A_WG;
+          const uint32_t b0 = sB + s * Cfg::B_STAGE;
+          wgmma_fence();
+#pragma unroll
+          for (int k = 0; k < Cfg::MMAS_PER_STAGE; k++) {
+            const uint64_t ad = make_sdesc(a0 + k * Cfg::A_KADV, 16, Cfg::A_SBO, Cfg::A_SWZ);
+            const uint64_t bd = make_sdesc(b0 + k * Cfg::B_KADV, 16, Cfg::A_SBO, Cfg::A_SWZ);
+            MMA::mma(acc, ad, bd, ((kb - c0) | k) != 0 ? 1u : 0u);
+          }
+          wgmma_commit();
+          wgmma_wait<1>();
+          if (prev >= 0 && wg_leader) mbar_arrive(bar_empty + 8 * prev);
+          prev = s;
+          if (++s == STAGES) { s = 0; ph ^= 1; }
+        }
+        wgmma_wait<0>();
+        wgmma_fence_regs(acc);
+        if (prev >= 0 && wg_leader) mbar_arrive(bar_empty + 8 * prev);
+        if constexpr (Cfg::REGACC) {
+#pragma unroll
+          for (int i = 0; i < Cfg::ACC; i++) sum[i] = c0 == 0 ? acc[i] : __fadd_rn(sum[i], acc[i]);
+        }
+      }
+
+      // ---- this warp's 16 rows of the tile into C: (acc * sa) * sb, then + bias in store_pair ----
+      const int row0 = m0 + ew * 16 + (lane >> 2);
+      const int col0 = n0 + 2 * (lane & 3);
+      float sa[2] = {0.f, 0.f};
+#pragma unroll
+      for (int h = 0; h < 2; h++)
+        if (row0 + 8 * h < p.M) sa[h] = __ldg(sc.a + (long long)(row0 + 8 * h) * sc.a_step);
+      const int ce[2] = {0, 0};
+#pragma unroll
+      for (int j = 0; j < BN / 8; j++) {
+        const int col = col0 + 8 * j;
+        float sb[2] = {0.f, 0.f}, bi[2] = {-0.f, -0.f};
+#pragma unroll
+        for (int e = 0; e < 2; e++) {
+          if (col + e >= p.N) continue;
+          sb[e] = __ldg(sc.b + (long long)(col + e) * sc.b_step);
+          if (sc.bias != nullptr) {
+            if constexpr (std::is_same<OutT, float>::value)
+              bi[e] = __ldg(reinterpret_cast<const float*>(sc.bias) + col + e);
+            else
+              bi[e] = c16_to_f32<OutT>(__ldg(reinterpret_cast<const unsigned short*>(sc.bias) + col + e));
+          }
+        }
+#pragma unroll
+        for (int h = 0; h < 2; h++) {
+          const float v0 = Cfg::REGACC ? sum[4 * j + 2 * h] : acc[4 * j + 2 * h];
+          const float v1 = Cfg::REGACC ? sum[4 * j + 2 * h + 1] : acc[4 * j + 2 * h + 1];
+          store_pair<OutT, float, ACT_NONE>(p, row0 + 8 * h, col, __fmul_rn(__fmul_rn(v0, sa[h]), sb[0]),
+                                            __fmul_rn(__fmul_rn(v1, sa[h]), sb[1]), false, false, 1.f, 1.f, 0, ce, 0.f,
+                                            0.f, bi[0], bi[1]);
         }
       }
     }

@@ -87,7 +87,9 @@ __device__ __forceinline__ void tma_load_2d_hint(uint32_t dst_smem, const CUtens
 //   [0,14) start>>4  [16,30) LBO>>4  [32,46) SBO>>4  [49,52) base offset (0: atoms 1 KB aligned)  [62,64) swizzle
 // swizzle: 1 = 128B, 2 = 64B, 3 = 32B.  K-major operands: SBO = stride between 8-row groups, LBO unused.
 // MN-major operands: LBO = stride between 64-element (128-byte) column blocks, SBO = stride between 8-row k groups.
-enum MmaKind { KIND_F16 = 0 /*bf16 operands*/, KIND_TF32 = 1, KIND_I8 = 2, KIND_FP16 = 3 /*fp16 operands*/ };
+// FP8 kinds name (A type, B type): torch._scaled_mm accepts these three pairs (not e5m2 x e5m2).
+enum MmaKind { KIND_F16 = 0 /*bf16 operands*/, KIND_TF32 = 1, KIND_I8 = 2, KIND_FP16 = 3 /*fp16 operands*/,
+               KIND_E4M3 = 4 /*e4m3 x e4m3*/, KIND_E4M3E5M2 = 5 /*e4m3 x e5m2*/, KIND_E5M2E4M3 = 6 /*e5m2 x e4m3*/ };
 enum Swz { SWZ_128B = 1, SWZ_64B = 2 };
 
 __device__ __forceinline__ uint64_t make_sdesc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes, uint32_t swz) {

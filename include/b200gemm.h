@@ -424,6 +424,41 @@ int b200_gemm_s8s32_op(int op_a, int op_b, int m, int n, int k,
                        int32_t* dC, int ldc, void* stream);
 size_t b200_gemm_workspace_bytes_op(int op_a, int op_b, int m, int n, int k, int precision_mode);
 
+/* ---- FP8 tensor-core GEMM (torch._scaled_mm) ----------------------------------------------------------------------
+ *   C = round_out( (acc * sa_i) * sb_j + bias_j )
+ * acc is op(A) op(B) of the FP8 operands (raw bytes), op_a / op_b and lda / ldb as for the _op entry points; each step
+ * is one fp32 round-to-nearest operation (no FMA contraction) and round_out one rounding to out_type (B200_OUT_F32,
+ * _BF16 or _F16; fp16 overflows to +-inf).
+ *   a_type / b_type: B200_FP8_E4M3 or B200_FP8_E5M2.  (e4m3, e4m3), (e4m3, e5m2) and (e5m2, e4m3) are supported, as in
+ *     torch; (e5m2, e5m2) is B200_ERR_UNSUPPORTED.  e4m3 has NaN but no inf; e5m2 has both.  Non-finite operands and
+ *     scales propagate as IEEE arithmetic does (0 * inf is NaN).
+ *   dScaleA / dScaleB: fp32 on the device, never read by the host (no synchronisation; the call can be captured in a
+ *     CUDA graph and the scales rewritten between replays).  scale_a_rowwise = 0: one element; 1: m elements, one per row
+ *     of op(A).  scale_b_colwise = 0: one element; 1: n elements, one per column of op(B).  Any other flag is
+ *     B200_ERR_BAD_ARG, and so is a null scale when there is work to do.
+ *   dBias: null, or n elements of C's type (bf16 / fp16 bits, or fp32 for B200_OUT_F32), added after scaling.
+ *   fast_accum = 0 (torch's default): every k-block of 128 elements starts a fresh tensor-core accumulator, added with a
+ *     rounded fp32 add to the tile's running sum in registers; 128 x 128 tiles.  The tensor core keeps 14 significant
+ *     bits when it adds FP8 products into its accumulator (measured on an H100 80GB HBM3 with crafted sums, DESIGN
+ *     §4.7), so the error is bounded by that of 128-term chunks plus an fp32 running sum:
+ *     |acc - exact| <= (8 * 2^-13 + ceil(k / 128) * 2^-24) * sum_k |a_k b_k|; measured on random e4m3 operands up to
+ *     k = 16384: <= 4e-5 of sum |a b|, equal to torch._scaled_mm(use_fast_accum=False) on the same card.
+ *     fast_accum = 1: one tensor-core accumulator over all of K (torch's use_fast_accum), 128 x 256 / 192 / 128 tiles;
+ *     its error grows with K: measured 3.0e-4 to 3.9e-4 of sum |a b| for k = 1024 to 16384.
+ * Any m, n, k; m == 0 or n == 0 is a no-op; k == 0 stores round_out(+0 + bias_j), or +0.  No K-split tail.  Every call
+ * runs on the tensor cores: (N, T) with 16-byte aligned bases and pitches (torch's row-major A and column-major B) is
+ * read in place; B given row-major and A given transposed are transposed into the workspace, and an operand whose base
+ * or pitch is not a multiple of 16 bytes is copied there at a 16-byte pitch.  Every layout and pitch gives the bits of
+ * the aligned (N, T) call.  Workspace: n * k16 bytes for B unless it is read in place, then m * k16 for A (at a 1 KB
+ * aligned offset after B's) unless A is read in place, k16 = k rounded up to 16; reserve that much before the first
+ * such call to keep it allocation-free.  Kernels: "tc_e4m3_obf16_128x256", "tc_e4m3e5m2_of32_acc_128x128", ... */
+#define B200_FP8_E4M3 0
+#define B200_FP8_E5M2 1
+int b200_gemm_fp8(int op_a, int op_b, int a_type, int b_type, int m, int n, int k,
+                  const uint8_t* dA, int lda, const uint8_t* dB, int ldb,
+                  const float* dScaleA, int scale_a_rowwise, const float* dScaleB, int scale_b_colwise,
+                  const void* dBias, void* dC, int ldc, int out_type, int fast_accum, void* stream);
+
 /* Pre-split operands for the split-precision modes (AUTO = the library default): the reference
  * leaves its "packAB interface open" for callers that reuse one operand (README.md:85; PackMatrixA/B,
  * aarch64/MMult_4x4_13.cpp:259,361).  TMA needs no repacking of row-major operands, but the fp32 ->
