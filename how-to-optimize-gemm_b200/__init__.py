@@ -32,7 +32,7 @@ EXPORTS = [
     "b200_gemm_f32_pack_free", "b200_gemm_f32_op", "b200_gemm_bf16_op", "b200_gemm_bf16_ex", "b200_gemm_f16_ex",
     "b200_gemm_bf16_epi", "b200_gemm_f16_epi", "b200_gemm_bf16_batched", "b200_gemm_f16_batched",
     "b200_gemm_bf16_grouped", "b200_gemm_f16_grouped", "b200_gemm_bf16_grouped_k", "b200_gemm_f16_grouped_k",
-    "b200_gemm_s8s32_op", "b200_gemm_workspace_bytes_op", "b200_gemm_fp8",
+    "b200_gemm_s8s32_op", "b200_gemm_workspace_bytes_op", "b200_gemm_fp8", "b200_gemm_fp8_blockwise",
     "b200_nccl_load", "b200_nccl_last_error", "b200_comm_unique_id", "b200_comm_init_rank",
     "b200_comm_destroy", "b200_rowpanel_create", "b200_rowpanel_destroy", "b200_rowpanel_slices", "b200_rowpanel_set_reserve_sms", "b200_rowpanel_trace", "b200_rowpanel_trace_dump", "b200_gemm_f32_rowpanel",
     "b200_gemm_f32_rowpanel_host", "b200_gemm_f32_pack_a", "b200_gemm_f32_packed_ab", "b200_gemm_f32_pack_free_a",
@@ -101,6 +101,8 @@ lib.b200_gemm_f16_grouped_k.argtypes = [_i, _i, _i, _i, _i, C.c_float, _vp, _i, 
 lib.b200_gemm_s8s32_op.argtypes = [_i, _i, _i, _i, _i, _vp, _i, _vp, _i, _vp, _i, _vp]
 lib.b200_gemm_workspace_bytes_op.argtypes = [_i, _i, _i, _i, _i, _i]
 lib.b200_gemm_fp8.argtypes = [_i, _i, _i, _i, _i, _i, _i, _vp, _i, _vp, _i, _vp, _i, _vp, _i, _vp, _vp, _i, _i, _i, _vp]
+lib.b200_gemm_fp8_blockwise.argtypes = [_i, _i, _i, _i, _i, _i, _i, _vp, _i, _vp, _i, _vp, _i, _ll, _ll, _vp, _i, _ll, _ll,
+                                        _vp, _vp, _i, _i, _vp]
 lib.b200_gemm_workspace_bytes_op.restype = C.c_size_t
 lib.b200_gemm_f32_pack_b.argtypes = [_i, _i, _vp, _i, _i, C.POINTER(_vp), _vp]
 lib.b200_gemm_f32_packed.argtypes = [_i, _i, _i, _vp, _i, _vp, _vp, _i, _i, _vp]
@@ -487,16 +489,39 @@ def _fp8_type(t):
     return {torch.float8_e4m3fn: FP8_E4M3, torch.float8_e5m2: FP8_E5M2}.get(t.dtype)
 
 
+def _blockwise_recipe(scale_a, scale_b, m, n, k):
+    """(scale_a_block, scale_b_block) of torch._scaled_mm's blockwise recipes, resolved from the scales' shapes in the
+    order torch checks them, or None.  Both scales must be 2-D float32 tensors."""
+    import torch
+    if scale_a.dtype != torch.float32 or scale_b.dtype != torch.float32 or scale_a.dim() != 2 or scale_b.dim() != 2:
+        return None
+    q, mb, nb = -(-k // 128), -(-m // 128), -(-n // 128)
+    sa, sb = tuple(scale_a.shape), tuple(scale_b.shape)
+    for blocks, want_a, want_b in (((1, 128), (m, q), (q, nb)), ((1, 1), (m, q), (q, n)), ((128, 1), (mb, q), (q, n))):
+        if sa == want_a and sb == want_b:
+            return blocks
+    return None
+
+
 def scaled_mm(A, B, scale_a, scale_b, bias=None, out_dtype=None, use_fast_accum=False, out=None, stream=None):
     """torch._scaled_mm for FP8 CUDA tensors: out = ((A @ B) * scale_a) * scale_b + bias, each step rounded in fp32 and
-    the result rounded once to out_dtype (b200_gemm_fp8).
+    the result rounded once to out_dtype (b200_gemm_fp8), or with blockwise scales the sum over 128-element k-blocks
+    of each block's product times its scales (b200_gemm_fp8_blockwise).
 
     A (m x k) and B (k x n) are float8_e4m3fn or float8_e5m2 (not both e5m2), each row-major or the transpose of a
     row-major matrix and read in place; torch's layout is a row-major A and a column-major B (x @ W.t()).  scale_a and
     scale_b are float32 CUDA tensors: one element each (tensorwise), or scale_a (m, 1) and scale_b (1, n) (rowwise).
-    They stay on the device: the call never synchronises.  bias: None or n contiguous elements of out_dtype.  out_dtype
-    is torch.bfloat16 (the default), torch.float16 or torch.float32.  use_fast_accum = False promotes the tensor core's
-    FP8 sums to fp32 every 128 elements of K; True keeps one tensor-core accumulator over K (faster, less precise).
+    Or, with q = ceil(k / 128), blockwise, as 2-D tensors of any non-negative strides:
+      scale_a (m, q) with scale_b (q, ceil(n / 128))    1 x 128 activations, 128 x 128 weights (x @ W.t(), DeepSeek-V3)
+      scale_a (m, q) with scale_b (q, n)                1 x 128 both (the weight gradient, K = tokens)
+      scale_a (ceil(m / 128), q) with scale_b (q, n)    128 x 128 A, 1 x 128 B
+    Each k-block's product is then added to an fp32 running sum with one fused multiply-add by rn(sa * sb); see
+    b200_gemm_fp8_blockwise.  Where k <= 128 a blockwise shape can also be a tensorwise / rowwise one ((m, 1) with (1, 1)
+    or (1, n)); such scales keep their tensorwise / rowwise meaning, whose rounding rn(rn(acc * sa) * sb) differs from
+    the blockwise rn(acc * rn(sa * sb)).  The scales stay on the device: the call never synchronises.  bias: None or n
+    contiguous elements of out_dtype.  out_dtype is torch.bfloat16 (the default), torch.float16 or torch.float32.
+    use_fast_accum = False promotes the tensor core's FP8 sums to fp32 every 128 elements of K; True keeps one
+    tensor-core accumulator over K (faster, less precise) and is refused with blockwise scales.
     Operands of other dtypes, or two e5m2 operands, are a TypeError; a scale of another shape or dtype, a CPU tensor,
     another bias, out_dtype or out (shape, dtype, or rows that overlap) is a ValueError."""
     import torch
@@ -521,7 +546,16 @@ def scaled_mm(A, B, scale_a, scale_b, bias=None, out_dtype=None, use_fast_accum=
         elif s.numel() == length and tuple(s.shape) == shape and s.is_contiguous():
             rows.append(1)
         else:
-            raise ValueError(f"{name} must have one element or shape {shape}, not {tuple(s.shape)}")
+            rows = None
+            break
+    blocks = _blockwise_recipe(scale_a, scale_b, m, n, k) if rows is None else None
+    if rows is None and blocks is None:
+        q = -(-k // 128)
+        raise ValueError(f"scale_a and scale_b must have one element, shapes (m, 1) and (1, n), or blockwise shapes "
+                         f"(({m}, {q}), ({q}, {-(-n // 128)})), (({m}, {q}), ({q}, {n})) or "
+                         f"(({-(-m // 128)}, {q}), ({q}, {n})), not {tuple(scale_a.shape)} and {tuple(scale_b.shape)}")
+    if blocks is not None and use_fast_accum:
+        raise ValueError("use_fast_accum=True is not available with blockwise scales: their scales change every k-block")
     if bias is not None:
         if bias.dtype != out_dtype:
             raise ValueError(f"the bias must have dtype {out_dtype}, not {bias.dtype}")
@@ -542,6 +576,13 @@ def scaled_mm(A, B, scale_a, scale_b, bias=None, out_dtype=None, use_fast_accum=
     if m == 0 or n == 0:
         return out
     ot = {torch.float32: OUT_F32, torch.bfloat16: OUT_BF16, torch.float16: OUT_F16}[out_dtype]
+    if blocks is not None:
+        _check(lib.b200_gemm_fp8_blockwise(op_a, op_b, ta, tb, m, n, k, A.data_ptr(), lda, B.data_ptr(), ldb,
+                                           scale_a.data_ptr(), blocks[0], scale_a.stride(0), scale_a.stride(1),
+                                           scale_b.data_ptr(), blocks[1], scale_b.stride(0), scale_b.stride(1),
+                                           bias.data_ptr() if bias is not None else None, out.data_ptr(), _ld(out), ot,
+                                           _stream_ptr(stream)))
+        return out
     _check(lib.b200_gemm_fp8(op_a, op_b, ta, tb, m, n, k, A.data_ptr(), lda, B.data_ptr(), ldb, scale_a.data_ptr(),
                              rows[0], scale_b.data_ptr(), rows[1], bias.data_ptr() if bias is not None else None,
                              out.data_ptr(), _ld(out), ot, int(bool(use_fast_accum)), _stream_ptr(stream)))

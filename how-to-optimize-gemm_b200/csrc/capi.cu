@@ -393,7 +393,8 @@ int g_ffma_halves = 1;        // strict kernel: split the tail round into half t
 //   STACK_KGROUP: groups of K rows [end_g-1, end_g) of one A^T and one B (k = total_k; sa = sb = 0: A and B are
 //   broadcast), C_g = C + g * sc, with the ends read on the device.  The tiles are a batch's, with no K split.
 // (Stacking, gemm_tc.cuh, names the forms.)
-// FP8 kinds (KIND_E4M3, ...): gemm_tc_fp8_kernel with the scales and bias *scl; K-major A and B, no K split.
+// FP8 kinds (KIND_E4M3, ...): gemm_tc_fp8_kernel with the scales and bias *scl; K-major A and B, no K split.  A
+// TcBlockScale (ScaleT) selects its blockwise-scaled form, whose stages carry their scales in shared memory.
 struct Stack {
   int count;               // entries of a batch, or groups
   long long sa, sb, sc;    // elements between consecutive entries of A, B and C
@@ -403,14 +404,16 @@ struct Stack {
 long long grouped_tile_rows(int total_m, int groups) { return (total_m + 127LL) / 128 + groups; }
 
 template <int KIND, int BN, int STAGES, typename OutT, class Prod = ProdSingle, int A_ROW_BYTES = 128, int AL = LAYOUT_K,
-          int BL = KindTraits<KIND>::B_LAYOUT, bool EPI = false, int STACK = STACK_NONE>
+          int BL = KindTraits<KIND>::B_LAYOUT, bool EPI = false, int STACK = STACK_NONE, class ScaleT = TcScale>
 int launch_tc(int m, int n, int k, const void* A, long long lda, int a_rows_total, int a_plane_rows,
               const void* B, long long ldb, int b_rows_total, int b_plane_rows, void* C, int ldc,
               const char* name, const Call& c, int chunk_k = 0, const float* row_max = nullptr,
-              const float* col_max = nullptr, const Stack* stk = nullptr, const TcScale* scl = nullptr) {
+              const float* col_max = nullptr, const Stack* stk = nullptr, const ScaleT* scl = nullptr) {
   using Cfg = TcConfig<KIND, BN, STAGES, Prod, A_ROW_BYTES, AL, BL>;
   using T = KindTraits<KIND>;
   constexpr bool FP8 = KIND == KIND_E4M3 || KIND == KIND_E4M3E5M2 || KIND == KIND_E5M2E4M3;
+  constexpr bool BLK = std::is_same<ScaleT, TcBlockScale>::value;
+  constexpr int smem = Cfg::SMEM_BYTES + (BLK ? STAGES * kBlkScaleStageBytes : 0);
   constexpr CUtensorMapDataType dt = KIND == KIND_F16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
                                    : KIND == KIND_FP16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16
                                    : KIND == KIND_TF32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32
@@ -460,10 +463,10 @@ int launch_tc(int m, int n, int k, const void* A, long long lda, int a_rows_tota
   p.stream_c = g_stream_c < 0 ? (g_stream_c = (getenv("B200GEMM_STREAM_C") ? atoi(getenv("B200GEMM_STREAM_C")) : kStreamCDefault)) : g_stream_c;
   auto kern = [] {
     if constexpr (STACK != STACK_NONE) return gemm_tc_stacked_kernel<KIND, BN, STAGES, OutT, AL, BL, STACK>;
-    else if constexpr (FP8) return gemm_tc_fp8_kernel<KIND, BN, STAGES, OutT, Prod>;
+    else if constexpr (FP8) return gemm_tc_fp8_kernel<KIND, BN, STAGES, OutT, Prod, BLK>;
     else return gemm_tc_kernel<KIND, BN, STAGES, OutT, Prod, A_ROW_BYTES, AL, BL, EPI>;
   }();
-  if (int arc = ensure_smem_attr(kern, Cfg::SMEM_BYTES)) return arc;
+  if (int arc = ensure_smem_attr(kern, smem)) return arc;
   TcStack ts{1, 0, 0, 0, nullptr};
   if constexpr (STACK != STACK_NONE) ts = TcStack{stk->count, stk->sa ? 1 : 0, stk->sb ? 1 : 0, stk->sc, stk->offs};
   // the whole batch's tiles, or the grouped call's bound on them (the entry point checked that they and their split
@@ -499,9 +502,9 @@ int launch_tc(int m, int n, int k, const void* A, long long lda, int a_rows_tota
   g_ktimer.begin(c.st);
   {
     cudaError_t e;
-    if constexpr (STACK != STACK_NONE) e = launch_pdl(kern, dim3(units), dim3(Cfg::THREADS), Cfg::SMEM_BYTES, c.st, 1, tmA, tmB, p, ts);
-    else if constexpr (FP8) e = launch_pdl(kern, dim3(units), dim3(Cfg::THREADS), Cfg::SMEM_BYTES, c.st, 1, tmA, tmB, p, *scl);
-    else e = launch_pdl(kern, dim3(units), dim3(Cfg::THREADS), Cfg::SMEM_BYTES, c.st, 1, tmA, tmB, p);
+    if constexpr (STACK != STACK_NONE) e = launch_pdl(kern, dim3(units), dim3(Cfg::THREADS), smem, c.st, 1, tmA, tmB, p, ts);
+    else if constexpr (FP8) e = launch_pdl(kern, dim3(units), dim3(Cfg::THREADS), smem, c.st, 1, tmA, tmB, p, *scl);
+    else e = launch_pdl(kern, dim3(units), dim3(Cfg::THREADS), smem, c.st, 1, tmA, tmB, p);
     release_flag_slot(flag_user, c.st);
     if (e != cudaSuccess) { cudaGetLastError(); return (int)e; }
   }
@@ -1453,33 +1456,36 @@ int gemm_s8(int op_a, int op_b, int m, int n, int k, const int8_t* A, int lda, c
 }
 
 // ---- FP8 (torch._scaled_mm) ------------------------------------------------------------------------------------------
-// Kernel names by [kind][C type][width index, 3 = promoted].
-#define FP8_NAMES(P)                                                                                      \
-  {{P "_of32_128x256", P "_of32_128x192", P "_of32_128x128", P "_of32_acc_128x128"},                      \
-   {P "_obf16_128x256", P "_obf16_128x192", P "_obf16_128x128", P "_obf16_acc_128x128"},                  \
-   {P "_of16_128x256", P "_of16_128x192", P "_of16_128x128", P "_of16_acc_128x128"}}
-const char* const kFp8Names[3][3][4] = {FP8_NAMES("tc_e4m3"), FP8_NAMES("tc_e4m3e5m2"), FP8_NAMES("tc_e5m2e4m3")};
+// Kernel names by [kind][C type][width index, 3 = promoted, 4 = blockwise].
+#define FP8_NAMES(P)                                                                                                  \
+  {{P "_of32_128x256", P "_of32_128x192", P "_of32_128x128", P "_of32_acc_128x128", P "_of32_blk_128x128"},           \
+   {P "_obf16_128x256", P "_obf16_128x192", P "_obf16_128x128", P "_obf16_acc_128x128", P "_obf16_blk_128x128"},      \
+   {P "_of16_128x256", P "_of16_128x192", P "_of16_128x128", P "_of16_acc_128x128", P "_of16_blk_128x128"}}
+const char* const kFp8Names[3][3][5] = {FP8_NAMES("tc_e4m3"), FP8_NAMES("tc_e4m3e5m2"), FP8_NAMES("tc_e5m2e4m3")};
 
 // Every layout and pitch runs on the tensor cores: (N, T) with TMA-able operands is read in place; otherwise the
 // operands are made K-major and TMA-able in the workspace (stage_kmajor), which holds the same bytes, so every route is
 // bit-identical to the aligned (N, T) call.  fast: one accumulator over K at pick_bn's width; else promoted per
-// 128-element k-block (two 64 x BN fp32 tiles in registers: BN = 128).
-template <int KIND, typename OutT>
+// 128-element k-block (two 64 x BN fp32 tiles in registers: BN = 128).  Blockwise scales (Scale = TcBlockScale) are
+// always promoted; their indices are logical (row, k-block) / (k-block, column), so staging never touches them.
+template <int KIND, typename OutT, class Scale>
 int tc_fp8(int op_a, int op_b, int m, int n, int k, const void* A, long long lda, const void* B, long long ldb, void* C,
-           int ldc, const TcScale& sc, bool fast, const char* const (&names)[4], const Call& c) {
+           int ldc, const Scale& sc, bool fast, const char* const (&names)[5], const Call& c) {
   const bool copy_a = !op_a && !(aligned16(A) && lda % 16 == 0);
   const bool copy_b = op_b && !(aligned16(B) && ldb % 16 == 0);
   const int sa = op_a || copy_a, sb = op_b && !copy_b;          // kmajor_ws_bytes / stage_kmajor's view of the layout
   auto run = [&](const void* a, long long la, const void* b, long long lb) {
-    if (fast)
-      return with_width(m, n, [&](auto W) {
-        using Wd = decltype(W);
-        return launch_tc<KIND, Wd::BN, Wd::STAGES, OutT>(m, n, k, a, la, m, 0, b, lb, n, 0, C, ldc, names[Wd::idx], c,
-                                                         0, nullptr, nullptr, nullptr, &sc);
-      });
+    constexpr bool blk = std::is_same<Scale, TcBlockScale>::value;
+    if constexpr (!blk)
+      if (fast)
+        return with_width(m, n, [&](auto W) {
+          using Wd = decltype(W);
+          return launch_tc<KIND, Wd::BN, Wd::STAGES, OutT>(m, n, k, a, la, m, 0, b, lb, n, 0, C, ldc, names[Wd::idx], c,
+                                                           0, nullptr, nullptr, nullptr, &sc);
+        });
     return launch_tc<KIND, 128, Width<128>::STAGES, OutT, ProdPromoted>(m, n, k, a, la, m, 0, b, lb, n, 0, C, ldc,
-                                                                          names[3], c, 128, nullptr, nullptr, nullptr,
-                                                                          &sc);
+                                                                          names[blk ? 4 : 3], c, 128, nullptr, nullptr,
+                                                                          nullptr, &sc);
   };
   if (!sa && sb) return run(A, lda, B, ldb);
   WsLease ws(kmajor_ws_bytes(sa, sb, m, n, k, 1), c.st);
@@ -1488,13 +1494,31 @@ int tc_fp8(int op_a, int op_b, int m, int n, int k, const void* A, long long lda
   return run(A, lda, B, ldb);
 }
 
-template <int KIND>
+template <int KIND, class Scale>
 int gemm_fp8_kind(int op_a, int op_b, int m, int n, int k, const void* A, int lda, const void* B, int ldb, void* C, int ldc,
-                  int out_type, const TcScale& sc, bool fast, const Call& c) {
+                  int out_type, const Scale& sc, bool fast, const Call& c) {
   const auto& names = kFp8Names[KIND - KIND_E4M3][out_type];
   if (out_type == B200_OUT_F32) return tc_fp8<KIND, float>(op_a, op_b, m, n, k, A, lda, B, ldb, C, ldc, sc, fast, names, c);
   if (out_type == B200_OUT_BF16) return tc_fp8<KIND, bf16_out>(op_a, op_b, m, n, k, A, lda, B, ldb, C, ldc, sc, fast, names, c);
   return tc_fp8<KIND, f16_out>(op_a, op_b, m, n, k, A, lda, B, ldb, C, ldc, sc, fast, names, c);
+}
+
+// Every FP8 call after its argument checks: k == 0 stores round_out(+0 + bias_j) (or +0) through the bias pass with
+// beta = 0 or the zero fill, reading no scale; otherwise the kind and C type select the kernel.
+template <class Scale>
+int fp8_run(int op_a, int op_b, int a_type, int b_type, int m, int n, int k, const uint8_t* A, int lda, const uint8_t* B,
+            int ldb, void* C, int ldc, int out_type, const Scale& sc, int fast_accum, cudaStream_t st) {
+  if (int rc = ensure_device()) return rc;
+  Call c{st};
+  if (k == 0) {
+    if (sc.bias) { c.bias = sc.bias; c.act = ACT_NONE; }
+    if (out_type == B200_OUT_F32) return degenerate<float, float>(m, n, C, ldc, c);
+    if (out_type == B200_OUT_BF16) return degenerate<uint16_t, uint16_t>(m, n, C, ldc, c);
+    return degenerate<__half, __half>(m, n, C, ldc, c);
+  }
+  if (a_type == B200_FP8_E5M2) return gemm_fp8_kind<KIND_E5M2E4M3>(op_a, op_b, m, n, k, A, lda, B, ldb, C, ldc, out_type, sc, fast_accum, c);
+  if (b_type == B200_FP8_E5M2) return gemm_fp8_kind<KIND_E4M3E5M2>(op_a, op_b, m, n, k, A, lda, B, ldb, C, ldc, out_type, sc, fast_accum, c);
+  return gemm_fp8_kind<KIND_E4M3>(op_a, op_b, m, n, k, A, lda, B, ldb, C, ldc, out_type, sc, fast_accum, c);
 }
 
 // C = round_out((op(A) op(B) * sa_i) * sb_j + bias_j); every argument is checked before the device is touched.
@@ -1511,20 +1535,42 @@ int gemm_fp8(int op_a, int op_b, int a_type, int b_type, int m, int n, int k, co
   if (a_type == B200_FP8_E5M2 && b_type == B200_FP8_E5M2) return B200_ERR_UNSUPPORTED;
   if (rc == 1) return 0;
   if (!scale_a || !scale_b) return B200_ERR_BAD_ARG;
-  if ((rc = ensure_device())) return rc;
-  Call c{st};
-  if (k == 0) {                 // round_out(+0 + bias_j), or +0: the bias pass with beta = 0, or the zero fill
-    if (bias) { c.bias = bias; c.act = ACT_NONE; }
-    if (out_type == B200_OUT_F32) return degenerate<float, float>(m, n, C, ldc, c);
-    if (out_type == B200_OUT_BF16) return degenerate<uint16_t, uint16_t>(m, n, C, ldc, c);
-    return degenerate<__half, __half>(m, n, C, ldc, c);
-  }
-  const TcScale sc{scale_a, scale_b, scale_a_rowwise, scale_b_colwise, bias};
-  if (a_type == B200_FP8_E5M2) return gemm_fp8_kind<KIND_E5M2E4M3>(op_a, op_b, m, n, k, A, lda, B, ldb, C, ldc, out_type, sc, fast_accum, c);
-  if (b_type == B200_FP8_E5M2) return gemm_fp8_kind<KIND_E4M3E5M2>(op_a, op_b, m, n, k, A, lda, B, ldb, C, ldc, out_type, sc, fast_accum, c);
-  return gemm_fp8_kind<KIND_E4M3>(op_a, op_b, m, n, k, A, lda, B, ldb, C, ldc, out_type, sc, fast_accum, c);
+  return fp8_run(op_a, op_b, a_type, b_type, m, n, k, A, lda, B, ldb, C, ldc, out_type,
+                 TcScale{scale_a, scale_b, scale_a_rowwise, scale_b_colwise, bias}, fast_accum, st);
 }
 static_assert(KIND_E4M3E5M2 == KIND_E4M3 + 1 && KIND_E5M2E4M3 == KIND_E4M3 + 2, "kFp8Names rows follow the kinds");
+
+// Element index of the last scale a blockwise operand reads, (rows - 1) * row_stride + (q - 1) * kb_stride, in 128
+// bits: the C ABI refuses one whose byte offset does not fit a signed 64-bit integer.
+__int128 last_scale_index(long long rows, long long q, long long row_stride, long long kb_stride) {
+  return (__int128)(rows - 1) * row_stride + (__int128)(q > 0 ? q - 1 : 0) * kb_stride;
+}
+
+// C = round_out(sum + bias_j), sum = fma(acc_kb, rn(sa_kb(i) * sb_kb(j)), sum) over the k-blocks in order from +0;
+// every argument is checked before the device is touched.
+int gemm_fp8_blockwise(int op_a, int op_b, int a_type, int b_type, int m, int n, int k, const uint8_t* A, int lda,
+                       const uint8_t* B, int ldb, const float* scale_a, int a_blk, long long sa_row, long long sa_kb,
+                       const float* scale_b, int b_blk, long long sb_kb, long long sb_col, const void* bias, void* C,
+                       int ldc, int out_type, cudaStream_t st) {
+  auto fp8 = [](int t) { return t == B200_FP8_E4M3 || t == B200_FP8_E5M2; };
+  if (!fp8(a_type) || !fp8(b_type)) return B200_ERR_BAD_ARG;
+  if (out_type != B200_OUT_F32 && out_type != B200_OUT_BF16 && out_type != B200_OUT_F16) return B200_ERR_BAD_ARG;
+  if ((a_blk != 1 && a_blk != 128) || (b_blk != 1 && b_blk != 128)) return B200_ERR_BAD_ARG;
+  if (sa_row < 0 || sa_kb < 0 || sb_kb < 0 || sb_col < 0) return B200_ERR_BAD_ARG;
+  int rc = check_args(m, n, k, A, lda, B, ldb, C, ldc, op_a, op_b);
+  if (rc < 0) return rc;
+  if (a_type == B200_FP8_E5M2 && b_type == B200_FP8_E5M2) return B200_ERR_UNSUPPORTED;
+  if (a_blk == 128 && b_blk == 128) return B200_ERR_UNSUPPORTED;      // not a torch recipe
+  if (rc == 1) return 0;
+  if (!scale_a || !scale_b) return B200_ERR_BAD_ARG;
+  const long long q = (k + 127LL) / 128;
+  const __int128 max_index = INT64_MAX / 4;                           // the byte offset fits a signed 64-bit integer
+  if (last_scale_index(a_blk == 1 ? m : (m + 127LL) / 128, q, sa_row, sa_kb) > max_index ||
+      last_scale_index(b_blk == 1 ? n : (n + 127LL) / 128, q, sb_col, sb_kb) > max_index)
+    return B200_ERR_BAD_ARG;
+  return fp8_run(op_a, op_b, a_type, b_type, m, n, k, A, lda, B, ldb, C, ldc, out_type,
+                 TcBlockScale{scale_a, scale_b, sa_row, sa_kb, sb_kb, sb_col, a_blk, b_blk, bias}, 0, st);
+}
 
 }  // namespace
 
@@ -1731,6 +1777,15 @@ int b200_gemm_fp8(int op_a, int op_b, int a_type, int b_type, int m, int n, int 
                   int scale_b_colwise, const void* dBias, void* dC, int ldc, int out_type, int fast_accum, void* stream) {
   return gemm_fp8(op_a, op_b, a_type, b_type, m, n, k, dA, lda, dB, ldb, dScaleA, scale_a_rowwise, dScaleB,
                   scale_b_colwise, dBias, dC, ldc, out_type, fast_accum, (cudaStream_t)stream);
+}
+
+int b200_gemm_fp8_blockwise(int op_a, int op_b, int a_type, int b_type, int m, int n, int k, const uint8_t* dA, int lda,
+                            const uint8_t* dB, int ldb, const float* dScaleA, int scale_a_block, long long sa_row_stride,
+                            long long sa_kb_stride, const float* dScaleB, int scale_b_block, long long sb_kb_stride,
+                            long long sb_col_stride, const void* dBias, void* dC, int ldc, int out_type, void* stream) {
+  return gemm_fp8_blockwise(op_a, op_b, a_type, b_type, m, n, k, dA, lda, dB, ldb, dScaleA, scale_a_block, sa_row_stride,
+                            sa_kb_stride, dScaleB, scale_b_block, sb_kb_stride, sb_col_stride, dBias, dC, ldc, out_type,
+                            (cudaStream_t)stream);
 }
 
 int b200_gemm_s8s32_op(int op_a, int op_b, int m, int n, int k, const int8_t* dA, int lda, const int8_t* dB, int ldb,

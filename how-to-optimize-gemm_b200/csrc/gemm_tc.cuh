@@ -608,15 +608,82 @@ struct TcScale {
   const void* bias;        // [n] of C's type (bf16 / fp16 bits, or fp32), null = none
 };
 
-template <int KIND, int BN, int STAGES, typename OutT, class Prod>
+// Blockwise scales (BLOCKWISE kernels, torch._scaled_mm's 1 x 128 / 128 x 128 recipes): k-block kb (K elements
+// [128 kb, 128 kb + 128)) of row i takes sa = a[ia * a_row + kb * a_kb] and of column j sb = b[kb * b_kb + jb * b_col],
+// ia = i for a_blk = 1 and i / 128 for 128, jb likewise; strides in elements, any non-negative value (0 broadcasts).
+// The promotion of that k-block is sum = fma(acc_kb, rn(sa * sb), sum) from sum = +0, and the store is store_pair's
+// bias path with no further scaling.  Its own argument type, so that TcScale, and the existing FP8 kernels, keep
+// their layout and code.
+struct TcBlockScale {
+  const float* a;
+  const float* b;
+  long long a_row, a_kb;   // scale_a strides: per row (a_blk = 1) or 128-row block (128), per k-block
+  long long b_kb, b_col;   // scale_b strides: per k-block, per column (b_blk = 1) or 128-column block (128)
+  int a_blk, b_blk;        // 1 or 128, never both 128
+  const void* bias;        // as TcScale::bias
+};
+// Shared memory of one stage's block scales: 128 floats of A (one per tile row), then 128 of B (one per tile column).
+constexpr int kBlkScaleStageBytes = 2 * 128 * 4;
+
+// The producer warpgroup's scale loaders (BLOCKWISE): warp 1 fills the A half and warp 2 the B half of each stage's
+// slot, walking the same tiles and k-blocks as the TMA thread.  Each lane copies its four scales with cp.async and
+// has the copies arrive on the stage's full barrier when they land (cp.async.mbarrier.arrive.noinc: 64 arrivals per
+// stage), so a loader never waits for a load's latency, only for a free stage, and keeps up with the TMA thread.
+// Rows >= M and columns >= N are zero-filled without a read: no load leaves the scale tensors.
+constexpr int kBlkScaleArrivals = 2 * 32;
+template <class Cfg, int BN, int STAGES>
+__device__ __forceinline__ void fp8_block_scale_loader(const TcParams& p, const TcBlockScale& sc, uint32_t slots,
+                                                       uint32_t bar_full, uint32_t bar_empty, bool is_b, int lane) {
+  // The producer warpgroup runs on 40 registers (setmaxnreg): per tile, one source pointer per lane that advances by
+  // the k-block stride, and a step of 32 rows / columns between its four scales (0 for a per-block recipe).
+  const float* base = is_b ? sc.b : sc.a;
+  const long long blk_stride = is_b ? sc.b_col : sc.a_row, kb_stride = is_b ? sc.b_kb : sc.a_kb;
+  const bool per_block = (is_b ? sc.b_blk : sc.a_blk) == 128;
+  const int num_kb = (p.K + Cfg::BK - 1) / Cfg::BK;
+  const uint32_t half = slots + (is_b ? 512u : 0u) + 4u * lane;
+  int s = 0;
+  uint32_t ph = 0;
+  for (int w = blockIdx.x; w < p.tiles_m * p.tiles_n; w += gridDim.x) {
+    int mb, nb;
+    tile_coords(w, p.tiles_m, p.tiles_n, p.group_m, mb, nb);
+    const int t = is_b ? nb : mb;
+    const int i0 = t * (is_b ? BN : Cfg::BM) + lane;
+    const int valid = (is_b ? p.N : p.M) - i0;               // scale q of this lane exists iff 32 q < valid
+    const float* src = base + (long long)(per_block ? t : i0) * blk_stride;
+    const long long step = per_block ? 0 : 32 * blk_stride;
+    for (int kb = 0; kb < num_kb; kb++, src += kb_stride) {
+      mbar_wait(bar_empty + 8 * s, ph ^ 1);
+      const uint32_t dst = half + s * kBlkScaleStageBytes;
+#pragma unroll
+      for (int q = 0; q < 4; q++) {
+        const bool in = 32 * q < valid;
+        asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;" ::"r"(dst + 128u * q), "l"(in ? src + q * step : base),
+                     "r"(in ? 4 : 0) : "memory");
+      }
+      asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(bar_full + 8 * s) : "memory");
+      if (++s == STAGES) { s = 0; ph ^= 1; }
+    }
+  }
+  asm volatile("cp.async.wait_all;" ::: "memory");
+}
+
+// BLOCKWISE = true: the blockwise-scaled kernels (ProdPromoted, BN = 128, argument TcBlockScale, shared memory
+// Cfg::SMEM_BYTES + STAGES * kBlkScaleStageBytes).  The TMA thread and the MMA chain are unchanged; warps 1 and 2 load
+// the stage's scales (fp8_block_scale_loader), whose copies also arrive on the stage's full barrier, and each consumer
+// warp releases a stage itself (eight arrivals) once its own reads of the stage's scales are done.  false: the code of the
+// tensorwise / rowwise kernels, unchanged.
+template <int KIND, int BN, int STAGES, typename OutT, class Prod, bool BLOCKWISE = false>
 __global__ void __launch_bounds__((TcConfig<KIND, BN, STAGES, Prod, 128>::THREADS), 1)
 gemm_tc_fp8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const TcParams p,
-                   const TcScale sc) {
+                   const typename std::conditional<BLOCKWISE, TcBlockScale, TcScale>::type sc) {
   using Cfg = TcConfig<KIND, BN, STAGES, Prod, 128>;
   using MMA = typename Cfg::MMA;
   static_assert(KIND == KIND_E4M3 || KIND == KIND_E4M3E5M2 || KIND == KIND_E5M2E4M3, "FP8 kinds");
   static_assert(!Cfg::A_MN && !Cfg::B_MN && Prod::NPA == 1 && Prod::NPB == 1, "FP8: K-major A and B, one plane");
   static_assert(std::is_same<OutT, float>::value || OutBytes<OutT>::V == 2, "FP8: fp32, bf16 or fp16 C");
+  static_assert(!BLOCKWISE || (std::is_same<Prod, ProdPromoted>::value && BN == 128 && Cfg::BK == 128),
+                "blockwise scales: one 128-element k-block per promotion, tiles on the 128 x 128 scale blocks");
+  static_assert(!BLOCKWISE || Cfg::SMEM_BYTES + STAGES * kBlkScaleStageBytes <= 232448, "blockwise: shared memory");
 
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;   // swizzle atoms need 1 KB
@@ -624,6 +691,7 @@ gemm_tc_fp8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
   const uint32_t sB = sA + STAGES * Cfg::A_STAGE;
   const uint32_t bar_full = sB + STAGES * Cfg::B_STAGE;
   const uint32_t bar_empty = bar_full + 8 * STAGES;
+  [[maybe_unused]] const uint32_t s_scale = bar_empty + 8 * STAGES;   // BLOCKWISE: STAGES slots of kBlkScaleStageBytes
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -631,8 +699,8 @@ gemm_tc_fp8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
     for (int i = 0; i < STAGES; i++) {
-      mbar_init(bar_full + 8 * i, 1);
-      mbar_init(bar_empty + 8 * i, Cfg::CONSUMERS);
+      mbar_init(bar_full + 8 * i, BLOCKWISE ? 1 + kBlkScaleArrivals : 1);
+      mbar_init(bar_empty + 8 * i, BLOCKWISE ? Cfg::EPI_WARPS : Cfg::CONSUMERS);
     }
     fence_barrier_init();
   }
@@ -663,6 +731,9 @@ gemm_tc_fp8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
         }
       }
     }
+    if constexpr (BLOCKWISE)
+      if (warp == 1 || warp == 2)
+        fp8_block_scale_loader<Cfg, BN, STAGES>(p, sc, s_scale, bar_full, bar_empty, warp == 2, lane);
   } else {
     // ===================== consumers (warpgroups 1 and 2): MMA chain + scaled epilogue =====================
     setmaxnreg_inc<232>();
@@ -673,16 +744,27 @@ gemm_tc_fp8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
     uint32_t ph = 0;
     float acc[Cfg::ACC];
     float sum[Cfg::REGACC ? Cfg::ACC : 1];
+    // BLOCKWISE: this thread's rows and first column inside the tile, and its A scales of the current k-block (and B's,
+    // when b_blk = 128: one value for the tile), read from the stage's slot before the MMAs are issued.
+    [[maybe_unused]] const int r_loc = ew * 16 + (lane >> 2), c_loc = 2 * (lane & 3);
+    [[maybe_unused]] float ssa[2] = {0.f, 0.f}, ssb = 0.f;
     for (int w = blockIdx.x; w < num_tiles; w += gridDim.x) {
       int mb, nb;
       tile_coords(w, p.tiles_m, p.tiles_n, p.group_m, mb, nb);
       const int m0 = mb * Cfg::BM, n0 = nb * BN;
-      const int chunk = Cfg::REGACC ? p.chunk_kb : num_kb;
+      const int chunk = BLOCKWISE ? 1 : Cfg::REGACC ? p.chunk_kb : num_kb;
       for (int c0 = 0; c0 < num_kb; c0 += chunk) {
         const int c1 = min(c0 + chunk, num_kb);
         int prev = -1;
         for (int kb = c0; kb < c1; kb++) {
           mbar_wait(bar_full + 8 * s, ph);
+          if constexpr (BLOCKWISE) {
+            const float* slot = reinterpret_cast<const float*>(smem_raw + (s_scale - smem_u32(smem_raw))) +
+                                s * (kBlkScaleStageBytes / 4);
+            ssa[0] = slot[r_loc];
+            ssa[1] = slot[r_loc + 8];
+            if (sc.b_blk == 128) ssb = slot[128];
+          }
           const uint32_t a0 = sA + s * Cfg::A_STAGE + cw * Cfg::A_WG;
           const uint32_t b0 = sB + s * Cfg::B_STAGE;
           wgmma_fence();
@@ -694,26 +776,50 @@ gemm_tc_fp8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
           }
           wgmma_commit();
           wgmma_wait<1>();
-          if (prev >= 0 && wg_leader) mbar_arrive(bar_empty + 8 * prev);
+          if (!BLOCKWISE && prev >= 0 && wg_leader) mbar_arrive(bar_empty + 8 * prev);
           prev = s;
           if (++s == STAGES) { s = 0; ph ^= 1; }
         }
         wgmma_wait<0>();
         wgmma_fence_regs(acc);
-        if (prev >= 0 && wg_leader) mbar_arrive(bar_empty + 8 * prev);
-        if constexpr (Cfg::REGACC) {
+        if constexpr (BLOCKWISE) {
+          // sum = fma(acc, rn(sa * sb), sum), from sum = +0; then this warp's reads of the stage are done and it
+          // releases the stage (one arrival per consumer warp)
+          if (sc.b_blk == 128) {
+            const float s2[2] = {__fmul_rn(ssa[0], ssb), __fmul_rn(ssa[1], ssb)};
 #pragma unroll
-          for (int i = 0; i < Cfg::ACC; i++) sum[i] = c0 == 0 ? acc[i] : __fadd_rn(sum[i], acc[i]);
+            for (int i = 0; i < Cfg::ACC; i++) sum[i] = __fmaf_rn(acc[i], s2[(i >> 1) & 1], c0 == 0 ? 0.f : sum[i]);
+          } else {
+            const float* slot = reinterpret_cast<const float*>(smem_raw + (s_scale - smem_u32(smem_raw))) +
+                                prev * (kBlkScaleStageBytes / 4) + 128 + c_loc;
+#pragma unroll
+            for (int j = 0; j < BN / 8; j++) {
+              const float2 b2 = *reinterpret_cast<const float2*>(slot + 8 * j);
+#pragma unroll
+              for (int i = 4 * j; i < 4 * j + 4; i++)
+                sum[i] = __fmaf_rn(acc[i], __fmul_rn(ssa[(i >> 1) & 1], i & 1 ? b2.y : b2.x), c0 == 0 ? 0.f : sum[i]);
+            }
+          }
+          __syncwarp();
+          if (lane == 0) mbar_arrive(bar_empty + 8 * prev);
+        } else {
+          if (prev >= 0 && wg_leader) mbar_arrive(bar_empty + 8 * prev);
+          if constexpr (Cfg::REGACC) {
+#pragma unroll
+            for (int i = 0; i < Cfg::ACC; i++) sum[i] = c0 == 0 ? acc[i] : __fadd_rn(sum[i], acc[i]);
+          }
         }
       }
 
-      // ---- this warp's 16 rows of the tile into C: (acc * sa) * sb, then + bias in store_pair ----
+      // ---- this warp's 16 rows of the tile into C: (acc * sa) * sb (BLOCKWISE: sum), then + bias in store_pair ----
       const int row0 = m0 + ew * 16 + (lane >> 2);
       const int col0 = n0 + 2 * (lane & 3);
       float sa[2] = {0.f, 0.f};
+      if constexpr (!BLOCKWISE) {
 #pragma unroll
-      for (int h = 0; h < 2; h++)
-        if (row0 + 8 * h < p.M) sa[h] = __ldg(sc.a + (long long)(row0 + 8 * h) * sc.a_step);
+        for (int h = 0; h < 2; h++)
+          if (row0 + 8 * h < p.M) sa[h] = __ldg(sc.a + (long long)(row0 + 8 * h) * sc.a_step);
+      }
       const int ce[2] = {0, 0};
 #pragma unroll
       for (int j = 0; j < BN / 8; j++) {
@@ -722,7 +828,7 @@ gemm_tc_fp8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
 #pragma unroll
         for (int e = 0; e < 2; e++) {
           if (col + e >= p.N) continue;
-          sb[e] = __ldg(sc.b + (long long)(col + e) * sc.b_step);
+          if constexpr (!BLOCKWISE) sb[e] = __ldg(sc.b + (long long)(col + e) * sc.b_step);
           if (sc.bias != nullptr) {
             if constexpr (std::is_same<OutT, float>::value)
               bi[e] = __ldg(reinterpret_cast<const float*>(sc.bias) + col + e);
@@ -734,9 +840,13 @@ gemm_tc_fp8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
         for (int h = 0; h < 2; h++) {
           const float v0 = Cfg::REGACC ? sum[4 * j + 2 * h] : acc[4 * j + 2 * h];
           const float v1 = Cfg::REGACC ? sum[4 * j + 2 * h + 1] : acc[4 * j + 2 * h + 1];
-          store_pair<OutT, float, ACT_NONE>(p, row0 + 8 * h, col, __fmul_rn(__fmul_rn(v0, sa[h]), sb[0]),
-                                            __fmul_rn(__fmul_rn(v1, sa[h]), sb[1]), false, false, 1.f, 1.f, 0, ce, 0.f,
-                                            0.f, bi[0], bi[1]);
+          if constexpr (BLOCKWISE)
+            store_pair<OutT, float, ACT_NONE>(p, row0 + 8 * h, col, v0, v1, false, false, 1.f, 1.f, 0, ce, 0.f, 0.f, bi[0],
+                                              bi[1]);
+          else
+            store_pair<OutT, float, ACT_NONE>(p, row0 + 8 * h, col, __fmul_rn(__fmul_rn(v0, sa[h]), sb[0]),
+                                              __fmul_rn(__fmul_rn(v1, sa[h]), sb[1]), false, false, 1.f, 1.f, 0, ce, 0.f,
+                                              0.f, bi[0], bi[1]);
         }
       }
     }

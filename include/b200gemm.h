@@ -459,6 +459,38 @@ int b200_gemm_fp8(int op_a, int op_b, int a_type, int b_type, int m, int n, int 
                   const float* dScaleA, int scale_a_rowwise, const float* dScaleB, int scale_b_colwise,
                   const void* dBias, void* dC, int ldc, int out_type, int fast_accum, void* stream);
 
+/* ---- Blockwise-scaled FP8 GEMM (torch._scaled_mm's 1 x 128 / 128 x 128 scales, DeepSeek-V3's recipe) ---------------
+ * K is cut into q = ceil(k / 128) k-blocks; block b covers K elements [128 b, 128 b + 128), the last one possibly
+ * partial.  For each block, in order:
+ *   acc_b(i, j)  the FP8 product over block b, a fresh tensor-core accumulator (b200_gemm_fp8's promoted chain)
+ *   s_b(i, j)  = rn(sa_b(i) * sb_b(j))                  one fp32 multiply
+ *   sum        = fma(acc_b(i, j), s_b(i, j), sum)       one fp32 fused multiply-add, from sum = +0
+ * and C = round_out(rn(sum + bias_j)): the bias add and the output rounding of b200_gemm_fp8, no further scaling.
+ *   dScaleA: fp32 on the device.  scale_a_block = 1: sa_b(i) = dScaleA[i * sa_row_stride + b * sa_kb_stride] (1 x 128:
+ *     one scale per row and k-block); 128: sa_b(i) = dScaleA[(i / 128) * sa_row_stride + b * sa_kb_stride] (128 x 128).
+ *   dScaleB: fp32 on the device.  scale_b_block = 1: sb_b(j) = dScaleB[b * sb_kb_stride + j * sb_col_stride] (1 x 128);
+ *     128: sb_b(j) = dScaleB[b * sb_kb_stride + (j / 128) * sb_col_stride] (128 x 128).
+ *   Strides are in elements, any value >= 0 (0 broadcasts; torch's outer-dim-major, row-major and padded layouts all
+ *   work); the byte offset of the last scale read must fit a signed 64-bit integer.  The recipes are torch's three:
+ *   (1, 128), (1, 1) and (128, 1); (128, 128) is B200_ERR_UNSUPPORTED.  Neither scale is read by the host: the call
+ *   never synchronises and can be captured in a CUDA graph, with the scales rewritten between replays.
+ * Operand pairs, output types, the bias, op_a / op_b, pitches, tails, m == 0 / n == 0 and k == 0 (round_out(+0 +
+ * bias_j), no scale read), the non-finite rules and the routes (and so the workspace) are b200_gemm_fp8's; there is no
+ * fast-accumulation form.  Every block size, stride and pointer is checked before the device is touched: a block size
+ * other than 1 or 128, a negative stride, a null scale when m and n are nonzero or a last index out of range is
+ * B200_ERR_BAD_ARG.
+ * Error: each acc_b is within 8 * 2^-13 * sum_{k in b} |a_k b_k| of the exact block product (b200_gemm_fp8's 128-element
+ * chunk bound); with the rounding of s_b and one fp32 rounding of each FMA,
+ *   |sum - sum_b s_b exact_b| <= sum_b |s_b| (8 * 2^-13 + 2^-24) sum_{k in b} |a_k b_k| + q * 2^-24 * max_b |partial sum|.
+ * On exact-class operands (each acc_b exact) the result is the fp32 chain above bit for bit.  Tiles are 128 x 128, six
+ * stages, each stage's 128 + 128 scales staged in shared memory by the producer warpgroup.  Kernels:
+ * "tc_e4m3_obf16_blk_128x128", "tc_e5m2e4m3_of32_blk_128x128", ... */
+int b200_gemm_fp8_blockwise(int op_a, int op_b, int a_type, int b_type, int m, int n, int k,
+                            const uint8_t* dA, int lda, const uint8_t* dB, int ldb,
+                            const float* dScaleA, int scale_a_block, long long sa_row_stride, long long sa_kb_stride,
+                            const float* dScaleB, int scale_b_block, long long sb_kb_stride, long long sb_col_stride,
+                            const void* dBias, void* dC, int ldc, int out_type, void* stream);
+
 /* Pre-split operands for the split-precision modes (AUTO = the library default): the reference
  * leaves its "packAB interface open" for callers that reuse one operand (README.md:85; PackMatrixA/B,
  * aarch64/MMult_4x4_13.cpp:259,361).  TMA needs no repacking of row-major operands, but the fp32 ->
