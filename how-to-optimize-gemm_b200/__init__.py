@@ -33,6 +33,7 @@ EXPORTS = [
     "b200_gemm_bf16_epi", "b200_gemm_f16_epi", "b200_gemm_bf16_batched", "b200_gemm_f16_batched",
     "b200_gemm_bf16_grouped", "b200_gemm_f16_grouped", "b200_gemm_bf16_grouped_k", "b200_gemm_f16_grouped_k",
     "b200_gemm_s8s32_op", "b200_gemm_workspace_bytes_op", "b200_gemm_fp8", "b200_gemm_fp8_blockwise",
+    "b200_gemm_fp8_grouped", "b200_gemm_fp8_batched",
     "b200_nccl_load", "b200_nccl_last_error", "b200_comm_unique_id", "b200_comm_init_rank",
     "b200_comm_destroy", "b200_rowpanel_create", "b200_rowpanel_destroy", "b200_rowpanel_slices", "b200_rowpanel_set_reserve_sms", "b200_rowpanel_trace", "b200_rowpanel_trace_dump", "b200_gemm_f32_rowpanel",
     "b200_gemm_f32_rowpanel_host", "b200_gemm_f32_pack_a", "b200_gemm_f32_packed_ab", "b200_gemm_f32_pack_free_a",
@@ -103,6 +104,10 @@ lib.b200_gemm_workspace_bytes_op.argtypes = [_i, _i, _i, _i, _i, _i]
 lib.b200_gemm_fp8.argtypes = [_i, _i, _i, _i, _i, _i, _i, _vp, _i, _vp, _i, _vp, _i, _vp, _i, _vp, _vp, _i, _i, _i, _vp]
 lib.b200_gemm_fp8_blockwise.argtypes = [_i, _i, _i, _i, _i, _i, _i, _vp, _i, _vp, _i, _vp, _i, _ll, _ll, _vp, _i, _ll, _ll,
                                         _vp, _vp, _i, _i, _vp]
+lib.b200_gemm_fp8_grouped.argtypes = [_i, _i, _i, _i, _i, _vp, _i, _vp, _i, _ll, _vp, _i, _vp, _vp, _ll, _vp, _i, _i, _i,
+                                      _vp]
+lib.b200_gemm_fp8_batched.argtypes = [_i, _i, _i, _i, _i, _vp, _i, _ll, _vp, _i, _ll, _vp, _ll, _vp, _ll, _vp, _i, _ll,
+                                      _i, _i, _i, _vp]
 lib.b200_gemm_workspace_bytes_op.restype = C.c_size_t
 lib.b200_gemm_f32_pack_b.argtypes = [_i, _i, _vp, _i, _i, C.POINTER(_vp), _vp]
 lib.b200_gemm_f32_packed.argtypes = [_i, _i, _i, _vp, _i, _vp, _vp, _i, _i, _vp]
@@ -586,6 +591,123 @@ def scaled_mm(A, B, scale_a, scale_b, bias=None, out_dtype=None, use_fast_accum=
     _check(lib.b200_gemm_fp8(op_a, op_b, ta, tb, m, n, k, A.data_ptr(), lda, B.data_ptr(), ldb, scale_a.data_ptr(),
                              rows[0], scale_b.data_ptr(), rows[1], bias.data_ptr() if bias is not None else None,
                              out.data_ptr(), _ld(out), ot, int(bool(use_fast_accum)), _stream_ptr(stream)))
+    return out
+
+
+def _fp8_in_place(name, t, ld, entry_stride, entry_elems):
+    """Refuses (ValueError) an FP8 operand the tensor cores cannot read in place: a base or a pitch that is not a
+    multiple of 16 bytes, or an entry stride other than 0 or a 16-byte multiple of at least one entry."""
+    if t.data_ptr() % 16 or ld % 16:
+        raise ValueError(f"{name} must have a 16-byte aligned base and a pitch that is a multiple of 16 bytes "
+                         f"(pitch {ld})")
+    if entry_stride != 0 and (entry_stride % 16 or entry_stride < entry_elems):
+        raise ValueError(f"{name}'s stride(0) must be 0 or a multiple of 16 bytes of at least one entry "
+                         f"({entry_elems} elements), not {entry_stride}")
+
+
+def scaled_grouped_mm(A, B, scale_a, scale_b, offs=None, out_dtype=None, use_fast_accum=False, out=None, stream=None):
+    """torch._scaled_grouped_mm for FP8 mixture-of-experts layers: every group, or every entry of a batch, is one
+    scaled_mm with rowwise scales, all of them in one launch (b200_gemm_fp8_grouped / _batched).
+
+    B is 3-D (G, k, n) and column-major in its last two dimensions: W.transpose(-2, -1) of a (G, n, k) weight, read
+    in place.  scale_b is float32 (G, n), contiguous along n.  Then either
+      A 2-D (total_m, k) row-major, scale_a (total_m,) contiguous, and offs a contiguous 1-D int32 CUDA tensor of G
+        cumulative end rows: rows [offs[g-1], offs[g]) of out are (A[rows] @ B[g]) * scale_a[rows, None] * scale_b[g],
+        with the offsets clamped as in gemm(offs=...) and read on the device; rows from offs[-1] on are not written (a
+        new out is torch.empty there, as in torch);
+      A 3-D (G, m, k) row-major in its last two dimensions (an expand()ed A is broadcast), scale_a (G, m) contiguous
+        along m, and no offs: out[g] = (A[g] @ B[g]) * scale_a[g, :, None] * scale_b[g].
+    Each step is rounded as in scaled_mm, so each group or entry is bit for bit scaled_mm on its own rows, B and
+    scales.  Operands are float8_e4m3fn or float8_e5m2 (not both e5m2).  out_dtype is torch.bfloat16 (the default, as
+    in torch), torch.float16 or torch.float32.  use_fast_accum as in scaled_mm.  The offsets and scales stay on the
+    device: the call never synchronises and can be captured in a CUDA graph.
+    Operands of other dtypes are a TypeError.  A 2-D B (torch's 2-D x 2-D and 3-D x 2-D forms), another layout, an
+    operand the tensor cores cannot read in place (16-byte aligned bases and pitches, entry strides 0 or at least one
+    entry), another scale, offs, out_dtype or out, or a CPU tensor is a ValueError."""
+    import torch
+    out_dtype = out_dtype or (out.dtype if out is not None else torch.bfloat16)
+    ta, tb = _fp8_type(A), _fp8_type(B)
+    if ta is None or tb is None:
+        raise TypeError(f"operands must be float8_e4m3fn or float8_e5m2, not {A.dtype} and {B.dtype}")
+    if ta == FP8_E5M2 and tb == FP8_E5M2:
+        raise TypeError("float8_e5m2 x float8_e5m2 is not supported (as in torch._scaled_mm)")
+    if B.dim() == 2 and A.dim() in (2, 3):
+        raise ValueError(f"the {A.dim()}-D x 2-D form of torch._scaled_grouped_mm is not supported: B must be 3-D")
+    if A.dim() not in (2, 3) or B.dim() != 3:
+        raise ValueError(f"A must be 2-D or 3-D and B 3-D, not {A.dim()}-D and {B.dim()}-D")
+    groups, k, n = B.shape
+    if A.shape[-1] != k:
+        raise ValueError(f"contraction dimensions differ: A is {tuple(A.shape)}, B is {tuple(B.shape)}")
+    if out_dtype not in (torch.bfloat16, torch.float16, torch.float32):
+        raise ValueError(f"out_dtype must be bfloat16, float16 or float32, not {out_dtype}")
+    try:
+        op_a, lda = operand_layout(tuple(A.shape[-2:]), A.stride()[-2:])
+        op_bt, ldb = operand_layout((n, k), (B.stride(2), B.stride(1)))      # B_g^T (n x k) must be row-major
+    except ValueError as e:
+        raise ValueError(f"A must be row-major and B column-major in their last two dimensions: {e}") from None
+    if op_a != OP_N or op_bt != OP_N:
+        raise ValueError(f"A must be row-major and B column-major in their last two dimensions, not of strides "
+                         f"{tuple(A.stride())} and {tuple(B.stride())}")
+    sb = B.stride(0) if groups > 1 else 0
+    for name, s in (("scale_a", scale_a), ("scale_b", scale_b)):
+        if s.dtype != torch.float32:
+            raise ValueError(f"{name} must be float32, not {s.dtype}")
+    if scale_b.dim() != 2 or tuple(scale_b.shape) != (groups, n) or (n > 1 and scale_b.stride(1) != 1):
+        raise ValueError(f"scale_b must be ({groups}, {n}) and contiguous along n, not {tuple(scale_b.shape)} of "
+                         f"strides {tuple(scale_b.stride())}")
+    ssb = scale_b.stride(0) if groups > 1 else 0
+    if A.dim() == 2:
+        if offs is None:
+            raise ValueError("a 2-D A needs offs, the groups' cumulative end rows")
+        _check_offs(offs)
+        if offs.numel() != groups:
+            raise ValueError(f"offs has {offs.numel()} elements for {groups} groups of B")
+        if groups > 1 and sb < n * ldb:
+            raise ValueError(f"the groups of B must not overlap or be broadcast (stride(0) = {B.stride(0)})")
+        total_m = A.shape[0]
+        if scale_a.dim() != 1 or scale_a.shape[0] != total_m or not scale_a.is_contiguous():
+            raise ValueError(f"scale_a must be contiguous and 1-D with {total_m} elements, not {tuple(scale_a.shape)}")
+        shape = (total_m, n)
+    else:
+        if offs is not None:
+            raise ValueError("offs must be None for a 3-D A: every entry has its own rows")
+        if A.shape[0] != groups:
+            raise ValueError(f"batch sizes differ: {A.shape[0]} and {groups}")
+        m = A.shape[1]
+        if scale_a.dim() != 2 or tuple(scale_a.shape) != (groups, m) or (m > 1 and scale_a.stride(1) != 1):
+            raise ValueError(f"scale_a must be ({groups}, {m}) and contiguous along m, not {tuple(scale_a.shape)} of "
+                             f"strides {tuple(scale_a.stride())}")
+        shape = (groups, m, n)
+    if out is not None:
+        if out.dtype != out_dtype or tuple(out.shape) != shape:
+            raise ValueError(f"out must be {out_dtype} of shape {shape}, not {out.dtype} of shape {tuple(out.shape)}")
+        rows, cols = shape[-2:]
+        if (cols > 1 and out.stride(-1) != 1) or (rows > 1 and out.stride(-2) < cols):
+            raise ValueError(f"out must be row-major with rows that do not overlap, not of strides {tuple(out.stride())}")
+        if len(shape) == 3 and groups > 1 and rows * cols > 0 and out.stride(0) < (rows - 1) * out.stride(1) + cols:
+            raise ValueError(f"the entries of out must not overlap (stride(0) = {out.stride(0)})")
+    tensors = [A, B, scale_a, scale_b] + [t for t in (offs, out) if t is not None]
+    if not all(t.is_cuda for t in tensors):
+        raise ValueError("A, B, the scales, offs and out must be CUDA tensors")
+    if out is None:
+        out = torch.empty(shape, dtype=out_dtype, device=A.device)
+    if groups == 0 or out.numel() == 0:
+        return out
+    if k > 0:
+        _fp8_in_place("A", A, lda, A.stride(0) if A.dim() == 3 and groups > 1 else 0, A.shape[-2] * lda)
+        _fp8_in_place("B", B, ldb, sb, n * ldb)
+    ot = {torch.float32: OUT_F32, torch.bfloat16: OUT_BF16, torch.float16: OUT_F16}[out_dtype]
+    fast = int(bool(use_fast_accum))
+    if A.dim() == 2:
+        _check(lib.b200_gemm_fp8_grouped(ta, tb, total_m, n, k, A.data_ptr(), lda, B.data_ptr(), ldb, sb,
+                                         offs.data_ptr(), groups, scale_a.data_ptr(), scale_b.data_ptr(), ssb,
+                                         out.data_ptr(), _ld(out), ot, fast, _stream_ptr(stream)))
+    else:
+        _check(lib.b200_gemm_fp8_batched(ta, tb, m, n, k, A.data_ptr(), lda, A.stride(0) if groups > 1 else 0,
+                                         B.data_ptr(), ldb, sb, scale_a.data_ptr(),
+                                         scale_a.stride(0) if groups > 1 else 0, scale_b.data_ptr(), ssb,
+                                         out.data_ptr(), _ld(out[0]), out.stride(0) if groups > 1 else 0, groups, ot,
+                                         fast, _stream_ptr(stream)))
     return out
 
 

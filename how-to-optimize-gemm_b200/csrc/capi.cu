@@ -394,7 +394,8 @@ int g_ffma_halves = 1;        // strict kernel: split the tail round into half t
 //   broadcast), C_g = C + g * sc, with the ends read on the device.  The tiles are a batch's, with no K split.
 // (Stacking, gemm_tc.cuh, names the forms.)
 // FP8 kinds (KIND_E4M3, ...): gemm_tc_fp8_kernel with the scales and bias *scl; K-major A and B, no K split.  A
-// TcBlockScale (ScaleT) selects its blockwise-scaled form, whose stages carry their scales in shared memory.
+// TcBlockScale (ScaleT) selects its blockwise-scaled form, whose stages carry their scales in shared memory; STACK_GROUP
+// / STACK_BATCH with a TcStackScale its stacked form (the stack as above, the rowwise scales of every entry in *scl).
 struct Stack {
   int count;               // entries of a batch, or groups
   long long sa, sb, sc;    // elements between consecutive entries of A, B and C
@@ -462,13 +463,18 @@ int launch_tc(int m, int n, int k, const void* A, long long lda, int a_rows_tota
   if constexpr (EPI) p.bias = c.bias;            // shares col_max's slot: EPI kernels are never scaled
   p.stream_c = g_stream_c < 0 ? (g_stream_c = (getenv("B200GEMM_STREAM_C") ? atoi(getenv("B200GEMM_STREAM_C")) : kStreamCDefault)) : g_stream_c;
   auto kern = [] {
-    if constexpr (STACK != STACK_NONE) return gemm_tc_stacked_kernel<KIND, BN, STAGES, OutT, AL, BL, STACK>;
-    else if constexpr (FP8) return gemm_tc_fp8_kernel<KIND, BN, STAGES, OutT, Prod, BLK>;
+    if constexpr (FP8) return gemm_tc_fp8_kernel<KIND, BN, STAGES, OutT, Prod, BLK, STACK>;
+    else if constexpr (STACK != STACK_NONE) return gemm_tc_stacked_kernel<KIND, BN, STAGES, OutT, AL, BL, STACK>;
     else return gemm_tc_kernel<KIND, BN, STAGES, OutT, Prod, A_ROW_BYTES, AL, BL, EPI>;
   }();
   if (int arc = ensure_smem_attr(kern, smem)) return arc;
   TcStack ts{1, 0, 0, 0, nullptr};
   if constexpr (STACK != STACK_NONE) ts = TcStack{stk->count, stk->sa ? 1 : 0, stk->sb ? 1 : 0, stk->sc, stk->offs};
+  [[maybe_unused]] ScaleT fp8_scale{};          // a stacked FP8 call's TcStackScale takes the stack here
+  if constexpr (FP8) {
+    fp8_scale = *scl;
+    if constexpr (STACK != STACK_NONE) fp8_scale.st = ts;
+  }
   // the whole batch's tiles, or the grouped call's bound on them (the entry point checked that they and their split
   // parts fit the kernel's int index)
   int tiles = p.tiles_m * p.tiles_n * (STACK == STACK_GROUP ? 1 : ts.count);
@@ -502,8 +508,8 @@ int launch_tc(int m, int n, int k, const void* A, long long lda, int a_rows_tota
   g_ktimer.begin(c.st);
   {
     cudaError_t e;
-    if constexpr (STACK != STACK_NONE) e = launch_pdl(kern, dim3(units), dim3(Cfg::THREADS), smem, c.st, 1, tmA, tmB, p, ts);
-    else if constexpr (FP8) e = launch_pdl(kern, dim3(units), dim3(Cfg::THREADS), smem, c.st, 1, tmA, tmB, p, *scl);
+    if constexpr (FP8) e = launch_pdl(kern, dim3(units), dim3(Cfg::THREADS), smem, c.st, 1, tmA, tmB, p, fp8_scale);
+    else if constexpr (STACK != STACK_NONE) e = launch_pdl(kern, dim3(units), dim3(Cfg::THREADS), smem, c.st, 1, tmA, tmB, p, ts);
     else e = launch_pdl(kern, dim3(units), dim3(Cfg::THREADS), smem, c.st, 1, tmA, tmB, p);
     release_flag_slot(flag_user, c.st);
     if (e != cudaSuccess) { cudaGetLastError(); return (int)e; }
@@ -1572,6 +1578,155 @@ int gemm_fp8_blockwise(int op_a, int op_b, int a_type, int b_type, int m, int n,
                  TcBlockScale{scale_a, scale_b, sa_row, sa_kb, sb_kb, sb_col, a_blk, b_blk, bias}, 0, st);
 }
 
+// ---- grouped and strided-batched FP8 GEMMs (torch._scaled_grouped_mm 2-D x 3-D and 3-D x 3-D) ---------------------------
+// gemm_tc_fp8_kernel over a stack: row-major A, every B_b stored n x k (B^T, torch's column-major mat_b), rowwise
+// scales, no bias, no workspace.  The operands are read in place only (FP8 has no CUDA-core kernel, and staging every
+// expert's weight would copy all of B), so the entry points refuse what TMA cannot describe.
+// Kernel names by [stacking: 0 = grouped, 1 = batch][kind][C type][width index, 3 = promoted].
+#define FP8_STACK_NAMES(P, S)                                                                                           \
+  {{P "_of32_" S "_128x256", P "_of32_" S "_128x192", P "_of32_" S "_128x128", P "_of32_" S "_acc_128x128"},           \
+   {P "_obf16_" S "_128x256", P "_obf16_" S "_128x192", P "_obf16_" S "_128x128", P "_obf16_" S "_acc_128x128"},       \
+   {P "_of16_" S "_128x256", P "_of16_" S "_128x192", P "_of16_" S "_128x128", P "_of16_" S "_acc_128x128"}}
+const char* const kFp8StackNames[2][3][3][4] = {
+    {FP8_STACK_NAMES("tc_e4m3", "grp"), FP8_STACK_NAMES("tc_e4m3e5m2", "grp"), FP8_STACK_NAMES("tc_e5m2e4m3", "grp")},
+    {FP8_STACK_NAMES("tc_e4m3", "bat"), FP8_STACK_NAMES("tc_e4m3e5m2", "bat"), FP8_STACK_NAMES("tc_e5m2e4m3", "bat")}};
+
+// The stacked call *stk (m = total_m for a grouped call) at pick_bn's width over the stack's tiles (fast), or promoted
+// per 128-element k-block at BN = 128, as tc_fp8 chooses for one matrix.
+template <int KIND, typename OutT, int STACK>
+int tc_fp8_stacked(int m, int n, int k, const void* A, int lda, const void* B, int ldb, void* C, int ldc,
+                   const Stack& stk, const TcStackScale& sc, bool fast, const char* const (&names)[4], const Call& c) {
+  // m rows of A per entry (a grouped A is one entry of total_m rows); every B entry is n x k
+  if (fast) {
+    const int bn_m = STACK == STACK_GROUP ? 128 : m;
+    const int bn_batch = STACK == STACK_GROUP ? (int)grouped_tile_rows(m, stk.count) : stk.count;
+    return with_width(bn_m, n, [&](auto W) {
+      using Wd = decltype(W);
+      return launch_tc<KIND, Wd::BN, Wd::STAGES, OutT, ProdSingle, 128, LAYOUT_K, LAYOUT_K, false, STACK>(
+          m, n, k, A, lda, m, 0, B, ldb, n, 0, C, ldc, names[Wd::idx], c, 0, nullptr, nullptr, &stk, &sc);
+    }, bn_batch);
+  }
+  return launch_tc<KIND, 128, Width<128>::STAGES, OutT, ProdPromoted, 128, LAYOUT_K, LAYOUT_K, false, STACK>(
+      m, n, k, A, lda, m, 0, B, ldb, n, 0, C, ldc, names[3], c, 128, nullptr, nullptr, &stk, &sc);
+}
+
+template <int STACK>
+int fp8_stacked_run(int a_type, int b_type, int m, int n, int k, const uint8_t* A, int lda, const uint8_t* B, int ldb,
+                    void* C, int ldc, int out_type, const Stack& stk, const TcStackScale& sc, int fast, cudaStream_t st) {
+  if (int rc = ensure_device()) return rc;
+  Call c{st};
+  if (k == 0) {                                             // +0 over the covered rows / entries, no scale read
+    if (out_type == B200_OUT_F32)
+      return STACK == STACK_GROUP ? degenerate_grouped<float>(m, n, C, ldc, stk, c) : degenerate_batched<float>(m, n, C, ldc, stk, c);
+    return STACK == STACK_GROUP ? degenerate_grouped<uint16_t>(m, n, C, ldc, stk, c)
+                                : degenerate_batched<uint16_t>(m, n, C, ldc, stk, c);
+  }
+  const int kind = a_type == B200_FP8_E5M2 ? 2 : b_type == B200_FP8_E5M2 ? 1 : 0;
+  const auto& names = kFp8StackNames[STACK == STACK_GROUP ? 0 : 1][kind][out_type];
+  auto by_out = [&](auto kd) {
+    constexpr int KIND = decltype(kd)::value;
+    if (out_type == B200_OUT_F32)
+      return tc_fp8_stacked<KIND, float, STACK>(m, n, k, A, lda, B, ldb, C, ldc, stk, sc, fast, names, c);
+    if (out_type == B200_OUT_BF16)
+      return tc_fp8_stacked<KIND, bf16_out, STACK>(m, n, k, A, lda, B, ldb, C, ldc, stk, sc, fast, names, c);
+    return tc_fp8_stacked<KIND, f16_out, STACK>(m, n, k, A, lda, B, ldb, C, ldc, stk, sc, fast, names, c);
+  };
+  if (kind == 2) return by_out(std::integral_constant<int, KIND_E5M2E4M3>());
+  if (kind == 1) return by_out(std::integral_constant<int, KIND_E4M3E5M2>());
+  return by_out(std::integral_constant<int, KIND_E4M3>());
+}
+
+// The checks every stacked FP8 call shares: operand types, output type and fast_accum are B200_ERR_BAD_ARG, and
+// (e5m2, e5m2) is B200_ERR_UNSUPPORTED, as for b200_gemm_fp8.
+int fp8_stacked_types(int a_type, int b_type, int out_type, int fast_accum) {
+  auto fp8 = [](int t) { return t == B200_FP8_E4M3 || t == B200_FP8_E5M2; };
+  if (!fp8(a_type) || !fp8(b_type)) return B200_ERR_BAD_ARG;
+  if (out_type != B200_OUT_F32 && out_type != B200_OUT_BF16 && out_type != B200_OUT_F16) return B200_ERR_BAD_ARG;
+  if (fast_accum != 0 && fast_accum != 1) return B200_ERR_BAD_ARG;
+  return 0;
+}
+// In-place operands: 16-byte aligned bases and 16-byte multiple pitches (FP8 elements are bytes).
+bool fp8_in_place(const void* A, long long lda, const void* B, long long ldb) {
+  return aligned16(A) && aligned16(B) && lda % 16 == 0 && ldb % 16 == 0;
+}
+
+// Rows [end_{g-1}, end_g) of C = round_out((A_rows B_g^T * sa_i) * sb_g[j]), B_g = B + g * stride_b (n x k), sb_g =
+// scale_b + g * scale_b_stride, sa_i = scale_a[i] at the row i of A; the ends are b200_gemm_bf16_grouped's, read on the
+// device.  Argument rules (all before the device is touched): b200_gemm_fp8's on types and flags, b200_gemm_bf16_grouped's
+// on sizes, groups, offsets, overlap and the tile bound for an op_b = T call, negative scale_b_stride or one whose last
+// group's offset exceeds 2^60 elements, null scales with work to do (B200_ERR_BAD_ARG); operands not read in place
+// (B200_ERR_UNSUPPORTED).  groups == 0, total_m == 0 or n == 0 is a no-op.
+int gemm_fp8_grouped(int a_type, int b_type, int total_m, int n, int k, const uint8_t* A, int lda, const uint8_t* B,
+                     int ldb, long long stride_b, const int32_t* offs, int groups, const float* scale_a,
+                     const float* scale_b, long long scale_b_stride, void* C, int ldc, int out_type, int fast_accum,
+                     cudaStream_t st) {
+  if (int rc = fp8_stacked_types(a_type, b_type, out_type, fast_accum)) return rc;
+  if (groups < 0 || stride_b < 0 || scale_b_stride < 0 || groups > kMaxGroups) return B200_ERR_BAD_ARG;
+  if (total_m < 0 || n < 0 || k < 0) return B200_ERR_BAD_ARG;
+  if (a_type == B200_FP8_E5M2 && b_type == B200_FP8_E5M2) return B200_ERR_UNSUPPORTED;
+  if (groups == 0) return 0;
+  int rc = check_args(total_m, n, k, A, lda, B, ldb, C, ldc, B200_OP_N, B200_OP_T);
+  if (rc == 1) return 0;
+  if (rc) return rc;
+  if (!offs || !scale_a || !scale_b) return B200_ERR_BAD_ARG;
+  if (groups > 1) {
+    if (stride_b < (long long)n * ldb) return B200_ERR_BAD_ARG;                          // B_g would overlap
+    if (stride_b > (1LL << 60) / (groups - 1) || scale_b_stride > (1LL << 60) / (groups - 1)) return B200_ERR_BAD_ARG;
+  }
+  const long long tiles_n = (n + 127LL) / 128;
+  if (tiles_n > 0x3FFFFFFFLL / grouped_tile_rows(total_m, groups)) return B200_ERR_BAD_ARG;
+  if (k > 0 && (!fp8_in_place(A, lda, B, ldb) || (groups > 1 && !batch_tma_ok(stride_b, n, ldb, 1))))
+    return B200_ERR_UNSUPPORTED;
+  const Stack gr{groups, 0, groups > 1 ? stride_b : 0, 0, offs};
+  TcStackScale sc{};
+  sc.a = scale_a; sc.b = scale_b; sc.a_step = 1; sc.b_step = 1; sc.bias = nullptr;
+  sc.a_entry_stride = 0; sc.b_entry_stride = scale_b_stride;
+  return fp8_stacked_run<STACK_GROUP>(a_type, b_type, total_m, n, k, A, lda, B, ldb, C, ldc, out_type, gr, sc, fast_accum,
+                                      st);
+}
+
+// C_b = round_out((A_b B_b^T * sa_b[i]) * sb_b[j]) for b < batch, X_b = X + b * stride_x, sa_b = scale_a + b *
+// scale_a_stride, sb_b = scale_b + b * scale_b_stride (elements).  Argument rules (all before the device is touched):
+// b200_gemm_fp8's on types and flags and b200_gemm_bf16_batched's on sizes, strides, C overlap and the tile bound, with
+// the scale strides bounded like the operand strides, null scales with work to do (B200_ERR_BAD_ARG); operands not read
+// in place, an input stride other than 0 or at least one entry included (B200_ERR_UNSUPPORTED).  batch == 0, m == 0 or
+// n == 0 is a no-op; batch == 1 is the (N, T) b200_gemm_fp8 call with rowwise scales.
+int gemm_fp8_batched(int a_type, int b_type, int m, int n, int k, const uint8_t* A, int lda, long long stride_a,
+                     const uint8_t* B, int ldb, long long stride_b, const float* scale_a, long long scale_a_stride,
+                     const float* scale_b, long long scale_b_stride, void* C, int ldc, long long stride_c, int batch,
+                     int out_type, int fast_accum, cudaStream_t st) {
+  if (int rc = fp8_stacked_types(a_type, b_type, out_type, fast_accum)) return rc;
+  if (batch < 0 || stride_a < 0 || stride_b < 0 || stride_c < 0 || scale_a_stride < 0 || scale_b_stride < 0)
+    return B200_ERR_BAD_ARG;
+  if (m < 0 || n < 0 || k < 0) return B200_ERR_BAD_ARG;
+  if (a_type == B200_FP8_E5M2 && b_type == B200_FP8_E5M2) return B200_ERR_UNSUPPORTED;
+  if (batch == 0) return 0;
+  int rc = check_args(m, n, k, A, lda, B, ldb, C, ldc, B200_OP_N, B200_OP_T);
+  if (rc == 1) return 0;
+  if (rc) return rc;
+  if (!scale_a || !scale_b) return B200_ERR_BAD_ARG;
+  if (batch > 1) {
+    if (stride_c < (long long)(m - 1) * ldc + n) return B200_ERR_BAD_ARG;               // entries of C would overlap
+    const long long max_stride = (1LL << 60) / (batch - 1);
+    if (stride_a > max_stride || stride_b > max_stride || stride_c > max_stride || scale_a_stride > max_stride ||
+        scale_b_stride > max_stride)
+      return B200_ERR_BAD_ARG;
+    const long long tiles1 = ((m + 127LL) / 128) * ((n + 127LL) / 128);                  // < 2^48
+    if (tiles1 > 0x7FFFFFFFLL / 4 / batch) return B200_ERR_BAD_ARG;
+  }
+  if (k > 0 && (!fp8_in_place(A, lda, B, ldb) ||
+                (batch > 1 && (!batch_tma_ok(stride_a, m, lda, 1) || !batch_tma_ok(stride_b, n, ldb, 1)))))
+    return B200_ERR_UNSUPPORTED;
+  if (batch == 1)
+    return gemm_fp8(B200_OP_N, B200_OP_T, a_type, b_type, m, n, k, A, lda, B, ldb, scale_a, 1, scale_b, 1, nullptr, C, ldc,
+                    out_type, fast_accum, st);
+  const Stack bt{batch, stride_a, stride_b, stride_c, nullptr};
+  TcStackScale sc{};
+  sc.a = scale_a; sc.b = scale_b; sc.a_step = 1; sc.b_step = 1; sc.bias = nullptr;
+  sc.a_entry_stride = scale_a_stride; sc.b_entry_stride = scale_b_stride;
+  return fp8_stacked_run<STACK_BATCH>(a_type, b_type, m, n, k, A, lda, B, ldb, C, ldc, out_type, bt, sc, fast_accum, st);
+}
+
 }  // namespace
 
 extern "C" {
@@ -1786,6 +1941,22 @@ int b200_gemm_fp8_blockwise(int op_a, int op_b, int a_type, int b_type, int m, i
   return gemm_fp8_blockwise(op_a, op_b, a_type, b_type, m, n, k, dA, lda, dB, ldb, dScaleA, scale_a_block, sa_row_stride,
                             sa_kb_stride, dScaleB, scale_b_block, sb_kb_stride, sb_col_stride, dBias, dC, ldc, out_type,
                             (cudaStream_t)stream);
+}
+
+int b200_gemm_fp8_grouped(int a_type, int b_type, int total_m, int n, int k, const uint8_t* dA, int lda,
+                          const uint8_t* dB, int ldb, long long stride_b, const int32_t* dOffs, int groups,
+                          const float* dScaleA, const float* dScaleB, long long scale_b_stride, void* dC, int ldc,
+                          int out_type, int fast_accum, void* stream) {
+  return gemm_fp8_grouped(a_type, b_type, total_m, n, k, dA, lda, dB, ldb, stride_b, dOffs, groups, dScaleA, dScaleB,
+                          scale_b_stride, dC, ldc, out_type, fast_accum, (cudaStream_t)stream);
+}
+
+int b200_gemm_fp8_batched(int a_type, int b_type, int m, int n, int k, const uint8_t* dA, int lda, long long stride_a,
+                          const uint8_t* dB, int ldb, long long stride_b, const float* dScaleA, long long scale_a_stride,
+                          const float* dScaleB, long long scale_b_stride, void* dC, int ldc, long long stride_c,
+                          int batch, int out_type, int fast_accum, void* stream) {
+  return gemm_fp8_batched(a_type, b_type, m, n, k, dA, lda, stride_a, dB, ldb, stride_b, dScaleA, scale_a_stride, dScaleB,
+                          scale_b_stride, dC, ldc, stride_c, batch, out_type, fast_accum, (cudaStream_t)stream);
 }
 
 int b200_gemm_s8s32_op(int op_a, int op_b, int m, int n, int k, const int8_t* dA, int lda, const int8_t* dB, int ldb,

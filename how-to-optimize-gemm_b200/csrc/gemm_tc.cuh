@@ -592,6 +592,52 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   }
 }
 
+// ---- the entry of a work tile of the stacked kernels (gemm_tc_stacked_kernel, gemm_tc_fp8_kernel with STACK) -----------
+struct StackEntry {
+  int tile0, tiles_m;      // the entry's first work tile and its tile rows (tile_coords)
+  int a_row, a_entry;      // A: row of the entry's first row, entry coordinate
+  int b_entry;             // B: entry coordinate
+  int M;                   // rows of the entry's C
+  long long c_off;         // elements from C to the entry's first row
+  int k0, k_len;           // KGROUP: the group's first K row and its k_g
+  int entry;               // the entry's index (batch entry or group), whatever its operands' entry coordinates
+};
+// The entry of work tile `tile`.  grp_end / grp_tile: the GROUP kernels' tables (group_table), grp_end the KGROUP
+// kernels' K ends, else unused.
+template <int STACK>
+__device__ __forceinline__ StackEntry stack_entry(int tile, const TcParams& p, const TcStack& st, const int* grp_end,
+                                                  const int* grp_tile) {
+  StackEntry se;
+  int e;
+  if constexpr (STACK == STACK_GROUP) {
+    e = group_of(grp_tile, st.count, tile / p.tiles_n);
+    se.tile0 = grp_tile[e] * p.tiles_n;
+    se.tiles_m = grp_tile[e + 1] - grp_tile[e];
+    se.a_row = grp_end[e];
+    se.M = grp_end[e + 1] - grp_end[e];
+    se.c_off = (long long)grp_end[e] * p.ldc;
+  } else {
+    const int per_entry = p.tiles_m * p.tiles_n;
+    e = tile / per_entry;
+    se.tile0 = e * per_entry;
+    se.tiles_m = p.tiles_m;
+    se.a_row = 0;
+    se.M = p.M;
+    se.c_off = (long long)e * st.stride_c;
+  }
+  if constexpr (STACK == STACK_KGROUP) {
+    se.k0 = grp_end[e];
+    se.k_len = grp_end[e + 1] - grp_end[e];
+  } else {
+    se.k0 = 0;
+    se.k_len = p.K;
+  }
+  se.a_entry = e * st.a_step;
+  se.b_entry = e * st.b_step;
+  se.entry = e;
+  return se;
+}
+
 // ---- FP8 GEMM (torch._scaled_mm) ---------------------------------------------------------------------------------------
 // C = round_out((acc * sa_i) * sb_j + bias_j), each step one fp32 round-to-nearest operation (explicit intrinsics: no
 // FMA contraction).  acc is op(A) op(B) of the FP8 operands: with ProdSingle one wgmma accumulator over all of K
@@ -621,6 +667,14 @@ struct TcBlockScale {
   long long b_kb, b_col;   // scale_b strides: per k-block, per column (b_blk = 1) or 128-column block (128)
   int a_blk, b_blk;        // 1 or 128, never both 128
   const void* bias;        // as TcScale::bias
+};
+// Stacked FP8 kernels (STACK_GROUP / STACK_BATCH, torch._scaled_grouped_mm): rowwise scales only (a_step = b_step = 1,
+// no bias), the stack, and the scales' element strides between entries.  Entry e's row i takes a[i_global] (grouped:
+// the row of the stacked A) or a[e * a_entry_stride + i] (batch), and its column j b[e * b_entry_stride + j]: scales
+// follow the entry index, so a broadcast operand (entry coordinate 0) still gets each entry's own scales.
+struct TcStackScale : TcScale {
+  TcStack st;
+  long long a_entry_stride, b_entry_stride;
 };
 // Shared memory of one stage's block scales: 128 floats of A (one per tile row), then 128 of B (one per tile column).
 constexpr int kBlkScaleStageBytes = 2 * 128 * 4;
@@ -667,15 +721,46 @@ __device__ __forceinline__ void fp8_block_scale_loader(const TcParams& p, const 
   asm volatile("cp.async.wait_all;" ::: "memory");
 }
 
+// The stacked FP8 kernels' group tables (group_table: the clamped ends, then each group's first tile row), static
+// shared memory of the GROUPED kernels that read them.
+template <int WHICH>
+__device__ __forceinline__ int* fp8_group_table() {
+  __shared__ int t[kMaxGroups + 1];
+  return t;
+}
+// Work tiles of an FP8 launch: one matrix's, a batch's, or (GROUPED) the table's, built here by every CTA after
+// griddep_wait (group_table ends in __syncthreads; CTAs past the table's tiles have no work).
+template <int STACK, int BM, class Scale>
+__device__ __forceinline__ int fp8_num_tiles(const TcParams& p, const Scale& sc) {
+  if constexpr (STACK == STACK_GROUP) {
+    group_table(sc.st.offs, sc.st.count, p.M, BM, fp8_group_table<0>(), fp8_group_table<1>());
+    return fp8_group_table<1>()[sc.st.count] * p.tiles_n;
+  } else if constexpr (STACK == STACK_BATCH) {
+    return p.tiles_m * p.tiles_n * sc.st.count;
+  } else {
+    return p.tiles_m * p.tiles_n;
+  }
+}
+
 // BLOCKWISE = true: the blockwise-scaled kernels (ProdPromoted, BN = 128, argument TcBlockScale, shared memory
 // Cfg::SMEM_BYTES + STAGES * kBlkScaleStageBytes).  The TMA thread and the MMA chain are unchanged; warps 1 and 2 load
 // the stage's scales (fp8_block_scale_loader), whose copies also arrive on the stage's full barrier, and each consumer
 // warp releases a stage itself (eight arrivals) once its own reads of the stage's scales are done.  false: the code of the
 // tensorwise / rowwise kernels, unchanged.
-template <int KIND, int BN, int STAGES, typename OutT, class Prod, bool BLOCKWISE = false>
+// STACK = STACK_GROUP / STACK_BATCH: the stacked FP8 kernels (argument TcStackScale), gemm_tc_stacked_kernel's schedule
+// over this kernel's MMA chains.  Work items are whole tiles, entry outermost (stack_entry); a grouped CTA builds the
+// clamped group table after griddep_wait.  A and B are 3-D tensor maps read one entry per box (a grouped A is one
+// entry, loaded at row end_g-1 + m0); the store goes through a TcParams whose C and M are the entry's, so rows of a tile
+// that belong to the next group are never stored.  Each entry's C is bit for bit the single-matrix kernel's on that
+// entry at the same width.  STACK_NONE: the single-matrix kernels, unchanged: every stacked path sits in an
+// `if constexpr` branch of its own and the stacking is tested in place (a local constexpr alias for it, like an unused
+// local variable, changed the register assignment of those kernels).
+template <int KIND, int BN, int STAGES, typename OutT, class Prod, bool BLOCKWISE = false, int STACK = STACK_NONE>
 __global__ void __launch_bounds__((TcConfig<KIND, BN, STAGES, Prod, 128>::THREADS), 1)
 gemm_tc_fp8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const TcParams p,
-                   const typename std::conditional<BLOCKWISE, TcBlockScale, TcScale>::type sc) {
+                   const typename std::conditional<BLOCKWISE, TcBlockScale,
+                                                   typename std::conditional<STACK != STACK_NONE, TcStackScale,
+                                                                             TcScale>::type>::type sc) {
   using Cfg = TcConfig<KIND, BN, STAGES, Prod, 128>;
   using MMA = typename Cfg::MMA;
   static_assert(KIND == KIND_E4M3 || KIND == KIND_E4M3E5M2 || KIND == KIND_E5M2E4M3, "FP8 kinds");
@@ -684,6 +769,10 @@ gemm_tc_fp8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
   static_assert(!BLOCKWISE || (std::is_same<Prod, ProdPromoted>::value && BN == 128 && Cfg::BK == 128),
                 "blockwise scales: one 128-element k-block per promotion, tiles on the 128 x 128 scale blocks");
   static_assert(!BLOCKWISE || Cfg::SMEM_BYTES + STAGES * kBlkScaleStageBytes <= 232448, "blockwise: shared memory");
+  static_assert(!(BLOCKWISE && STACK != STACK_NONE), "stacked FP8: rowwise scales only");
+  static_assert(STACK == STACK_NONE || STACK == STACK_GROUP || STACK == STACK_BATCH, "stacked FP8: a batch or a grouped call");
+  static_assert(STACK != STACK_GROUP || Cfg::SMEM_BYTES + 2 * (kMaxGroups + 1) * (int)sizeof(int) <= 232448,
+                "the pipeline and the group tables exceed the 227 KB of shared memory of sm_90");
 
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;   // swizzle atoms need 1 KB
@@ -708,7 +797,7 @@ gemm_tc_fp8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
   griddep_launch();
   griddep_wait();
 
-  const int num_tiles = p.tiles_m * p.tiles_n;
+  const int num_tiles = fp8_num_tiles<STACK, Cfg::BM>(p, sc);   // STACK_GROUP: builds the group table first
   const int num_kb = (p.K + Cfg::BK - 1) / Cfg::BK;
 
   if (warp < 4) {
@@ -717,17 +806,34 @@ gemm_tc_fp8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
     if (warp == 0 && lane == 0) {
       int s = 0;
       uint32_t ph = 0;
-      for (int w = blockIdx.x; w < num_tiles; w += gridDim.x) {
-        int mb, nb;
-        tile_coords(w, p.tiles_m, p.tiles_n, p.group_m, mb, nb);
-        const int m0 = mb * Cfg::BM, n0 = nb * BN;
-        for (int kb = 0; kb < num_kb; kb++) {
-          mbar_wait(bar_empty + 8 * s, ph ^ 1);
-          const uint32_t full = bar_full + 8 * s;
-          mbar_arrive_expect_tx(full, Cfg::STAGE_BYTES);
-          tma_load_2d(sA + s * Cfg::A_STAGE, &tmA, full, kb * Cfg::BK, m0);
-          tma_load_2d(sB + s * Cfg::B_STAGE, &tmB, full, kb * Cfg::BK, n0);
-          if (++s == STAGES) { s = 0; ph ^= 1; }
+      if constexpr (STACK != STACK_NONE) {                       // one entry per 3-D box; a grouped A at row end_{g-1} + m0
+        for (int w = blockIdx.x; w < num_tiles; w += gridDim.x) {
+          const StackEntry se = stack_entry<STACK>(w, p, sc.st, fp8_group_table<0>(), fp8_group_table<1>());
+          int mb, nb;
+          tile_coords(w - se.tile0, se.tiles_m, p.tiles_n, p.group_m, mb, nb);
+          const int m0 = se.a_row + mb * Cfg::BM, n0 = nb * BN;
+          for (int kb = 0; kb < num_kb; kb++) {
+            mbar_wait(bar_empty + 8 * s, ph ^ 1);
+            const uint32_t full = bar_full + 8 * s;
+            mbar_arrive_expect_tx(full, Cfg::STAGE_BYTES);
+            tma_load_3d(sA + s * Cfg::A_STAGE, &tmA, full, kb * Cfg::BK, m0, se.a_entry);
+            tma_load_3d(sB + s * Cfg::B_STAGE, &tmB, full, kb * Cfg::BK, n0, se.b_entry);
+            if (++s == STAGES) { s = 0; ph ^= 1; }
+          }
+        }
+      } else {
+        for (int w = blockIdx.x; w < num_tiles; w += gridDim.x) {
+          int mb, nb;
+          tile_coords(w, p.tiles_m, p.tiles_n, p.group_m, mb, nb);
+          const int m0 = mb * Cfg::BM, n0 = nb * BN;
+          for (int kb = 0; kb < num_kb; kb++) {
+            mbar_wait(bar_empty + 8 * s, ph ^ 1);
+            const uint32_t full = bar_full + 8 * s;
+            mbar_arrive_expect_tx(full, Cfg::STAGE_BYTES);
+            tma_load_2d(sA + s * Cfg::A_STAGE, &tmA, full, kb * Cfg::BK, m0);
+            tma_load_2d(sB + s * Cfg::B_STAGE, &tmB, full, kb * Cfg::BK, n0);
+            if (++s == STAGES) { s = 0; ph ^= 1; }
+          }
         }
       }
     }
@@ -750,8 +856,13 @@ gemm_tc_fp8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
     [[maybe_unused]] float ssa[2] = {0.f, 0.f}, ssb = 0.f;
     for (int w = blockIdx.x; w < num_tiles; w += gridDim.x) {
       int mb, nb;
-      tile_coords(w, p.tiles_m, p.tiles_n, p.group_m, mb, nb);
-      const int m0 = mb * Cfg::BM, n0 = nb * BN;
+      if constexpr (STACK != STACK_NONE) {
+        const StackEntry se = stack_entry<STACK>(w, p, sc.st, fp8_group_table<0>(), fp8_group_table<1>());
+        tile_coords(w - se.tile0, se.tiles_m, p.tiles_n, p.group_m, mb, nb);
+      } else {
+        tile_coords(w, p.tiles_m, p.tiles_n, p.group_m, mb, nb);
+      }
+      const int m0 = mb * Cfg::BM, n0 = nb * BN;      // stacked: m0 is a row inside the entry
       const int chunk = BLOCKWISE ? 1 : Cfg::REGACC ? p.chunk_kb : num_kb;
       for (int c0 = 0; c0 < num_kb; c0 += chunk) {
         const int c1 = min(c0 + chunk, num_kb);
@@ -814,6 +925,39 @@ gemm_tc_fp8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
       // ---- this warp's 16 rows of the tile into C: (acc * sa) * sb (BLOCKWISE: sum), then + bias in store_pair ----
       const int row0 = m0 + ew * 16 + (lane >> 2);
       const int col0 = n0 + 2 * (lane & 3);
+      if constexpr (STACK != STACK_NONE) {
+        // the entry's C and rows (pc; rows of the tile past the entry's are never stored), and its scale vectors: row i
+        // of the entry takes sa_e[i], column j sb_e[j].  No bias.  (A copy of the store below, so that the
+        // single-matrix kernels keep their code.)
+        const StackEntry se = stack_entry<STACK>(w, p, sc.st, fp8_group_table<0>(), fp8_group_table<1>());
+        TcParams pc = p;
+        pc.C = static_cast<uint8_t*>(p.C) + se.c_off * OutBytes<OutT>::V;
+        pc.M = se.M;
+        const float* sa_e = sc.a + (STACK == STACK_GROUP ? (long long)se.a_row : se.entry * sc.a_entry_stride);
+        const float* sb_e = sc.b + se.entry * sc.b_entry_stride;
+        float sa[2] = {0.f, 0.f};
+#pragma unroll
+        for (int h = 0; h < 2; h++)
+          if (row0 + 8 * h < pc.M) sa[h] = __ldg(sa_e + row0 + 8 * h);
+        const int ce[2] = {0, 0};
+#pragma unroll
+        for (int j = 0; j < BN / 8; j++) {
+          const int col = col0 + 8 * j;
+          float sb[2] = {0.f, 0.f};
+#pragma unroll
+          for (int e = 0; e < 2; e++)
+            if (col + e < p.N) sb[e] = __ldg(sb_e + col + e);
+#pragma unroll
+          for (int h = 0; h < 2; h++) {
+            const float v0 = Cfg::REGACC ? sum[4 * j + 2 * h] : acc[4 * j + 2 * h];
+            const float v1 = Cfg::REGACC ? sum[4 * j + 2 * h + 1] : acc[4 * j + 2 * h + 1];
+            store_pair<OutT, float, ACT_NONE>(pc, row0 + 8 * h, col, __fmul_rn(__fmul_rn(v0, sa[h]), sb[0]),
+                                              __fmul_rn(__fmul_rn(v1, sa[h]), sb[1]), false, false, 1.f, 1.f, 0, ce, 0.f,
+                                              0.f);
+          }
+        }
+        continue;
+      }
       float sa[2] = {0.f, 0.f};
       if constexpr (!BLOCKWISE) {
 #pragma unroll
@@ -881,48 +1025,7 @@ gemm_tc_fp8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
 //   the consumers zero its rows >= k_g - 64 kb in shared memory before its MMAs (zero_k_tail).  The MMA count is
 //   unchanged, so every C_g is bit for bit the _ex call with k = k_g, whose TMA zero-fills those rows.  A group with
 //   k_g = 0 issues no loads or MMAs and stores the _ex k == 0 result (store_beta_c).
-struct StackEntry {
-  int tile0, tiles_m;      // the entry's first work tile and its tile rows (tile_coords)
-  int a_row, a_entry;      // A: row of the entry's first row, entry coordinate
-  int b_entry;             // B: entry coordinate
-  int M;                   // rows of the entry's C
-  long long c_off;         // elements from C to the entry's first row
-  int k0, k_len;           // KGROUP: the group's first K row and its k_g
-};
-// The entry of work tile `tile`.  grp_end / grp_tile: the GROUP kernels' tables (group_table), grp_end the KGROUP
-// kernels' K ends, else unused.
-template <int STACK>
-__device__ __forceinline__ StackEntry stack_entry(int tile, const TcParams& p, const TcStack& st, const int* grp_end,
-                                                  const int* grp_tile) {
-  StackEntry se;
-  int e;
-  if constexpr (STACK == STACK_GROUP) {
-    e = group_of(grp_tile, st.count, tile / p.tiles_n);
-    se.tile0 = grp_tile[e] * p.tiles_n;
-    se.tiles_m = grp_tile[e + 1] - grp_tile[e];
-    se.a_row = grp_end[e];
-    se.M = grp_end[e + 1] - grp_end[e];
-    se.c_off = (long long)grp_end[e] * p.ldc;
-  } else {
-    const int per_entry = p.tiles_m * p.tiles_n;
-    e = tile / per_entry;
-    se.tile0 = e * per_entry;
-    se.tiles_m = p.tiles_m;
-    se.a_row = 0;
-    se.M = p.M;
-    se.c_off = (long long)e * st.stride_c;
-  }
-  if constexpr (STACK == STACK_KGROUP) {
-    se.k0 = grp_end[e];
-    se.k_len = grp_end[e + 1] - grp_end[e];
-  } else {
-    se.k0 = 0;
-    se.k_len = p.K;
-  }
-  se.a_entry = e * st.a_step;
-  se.b_entry = e * st.b_step;
-  return se;
-}
+// StackEntry / stack_entry (above gemm_tc_fp8_kernel, which shares them) find a work tile's entry.
 
 // KGROUP: zeroes K rows [r0, BK) of one stage's MN-major boxes (A's, then B's; contiguous in shared memory), where one
 // K row of a SWIZZLE_128B box is one whole 128-byte line, so no swizzle arithmetic is needed.  The 256 consumer threads

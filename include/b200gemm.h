@@ -491,6 +491,42 @@ int b200_gemm_fp8_blockwise(int op_a, int op_b, int a_type, int b_type, int m, i
                             const float* dScaleB, int scale_b_block, long long sb_kb_stride, long long sb_col_stride,
                             const void* dBias, void* dC, int ldc, int out_type, void* stream);
 
+/* ---- Grouped and batched FP8 GEMMs (torch._scaled_grouped_mm 2-D x 3-D and 3-D x 3-D; FP8 mixture-of-experts layers) --
+ * Every entry is one (N, T) b200_gemm_fp8 call with rowwise scales and no bias, all of them in one launch:
+ *   C_e = round_out( (A_e B_e^T * sa_e[i]) * sb_e[j] )
+ * A_e is row-major (lda >= k) and every B_e is stored n x k (ldb >= k): torch's column-major mat_b, the
+ * W.transpose(-2, -1) of a (G, n, k) weight.  Operand pairs, output types, fast_accum, the non-finite rules and the
+ * rounding are b200_gemm_fp8's, and so each entry's C is bit for bit that call's on the entry's rows, B and scales (the
+ * same kernel code at the same tile width; b200_gemm_debug_set_bn forces a fast width for both).
+ *   b200_gemm_fp8_grouped: group g is rows [end_{g-1}, end_g) of A (total_m x k) and C, times B_g = dB + g * stride_b,
+ *     with the ends of b200_gemm_bf16_grouped (end_{-1} = 0, end_g = min(max(dOffs[g], end_{g-1}), total_m), read on
+ *     the device; rows from end_{G-1} on are never written).  sa = dScaleA[row of A] (total_m elements), sb_g =
+ *     dScaleB + g * scale_b_stride (n elements each).
+ *   b200_gemm_fp8_batched: entry b is A_b = dA + b * stride_a (m x k), B_b = dB + b * stride_b, C_b = dC + b * stride_c,
+ *     sa_b = dScaleA + b * scale_a_stride (m elements), sb_b = dScaleB + b * scale_b_stride (n elements).  A stride of
+ *     0 broadcasts an operand; its scales still follow their own stride, so each entry may scale a shared A
+ *     differently.  batch == 1 is the (N, T) b200_gemm_fp8 call with rowwise scales: same kernel, name and bits.
+ * Scales are fp32 on the device and never read by the host, like the offsets: the calls never synchronise and can be
+ * captured in a CUDA graph, with offsets and scales rewritten between replays.  No bias (torch refuses one here), no
+ * workspace, no K-split tail.  k == 0 stores +0 over the covered rows / entries and reads no scale.
+ * Argument rules, all checked before the device is touched: the types and flags of b200_gemm_fp8; the sizes, groups,
+ * offsets, strides, overlap and tile-count bounds of b200_gemm_bf16_grouped / _batched, with the scale strides >= 0 and
+ * bounded like the operand strides; a null scale (or offs) with work to do: B200_ERR_BAD_ARG.  The operands must be
+ * read in place by the tensor cores: 16-byte aligned bases, lda, ldb and the operand strides multiples of 16 bytes, and
+ * every input stride 0 or at least one entry (rows x ld); anything else is B200_ERR_UNSUPPORTED (there is no CUDA-core
+ * FP8 kernel, and staging every entry's B would copy all of it).  Tiles are b200_gemm_fp8's: promoted 128 x 128, or
+ * fast at pick_bn's width over the stack's tiles (a grouped call counts its bound of ceil(total_m / 128) + G tile rows).
+ * Kernels: "tc_e4m3_obf16_grp_128x256", "tc_e4m3_of32_grp_acc_128x128", "tc_e4m3e5m2_of16_bat_128x192", ...; a k == 0
+ * call runs "fill_zero_grp" / "fill_zero_bat". */
+int b200_gemm_fp8_grouped(int a_type, int b_type, int total_m, int n, int k, const uint8_t* dA, int lda,
+                          const uint8_t* dB, int ldb, long long stride_b, const int32_t* dOffs, int groups,
+                          const float* dScaleA, const float* dScaleB, long long scale_b_stride,
+                          void* dC, int ldc, int out_type, int fast_accum, void* stream);
+int b200_gemm_fp8_batched(int a_type, int b_type, int m, int n, int k, const uint8_t* dA, int lda, long long stride_a,
+                          const uint8_t* dB, int ldb, long long stride_b, const float* dScaleA, long long scale_a_stride,
+                          const float* dScaleB, long long scale_b_stride, void* dC, int ldc, long long stride_c,
+                          int batch, int out_type, int fast_accum, void* stream);
+
 /* Pre-split operands for the split-precision modes (AUTO = the library default): the reference
  * leaves its "packAB interface open" for callers that reuse one operand (README.md:85; PackMatrixA/B,
  * aarch64/MMult_4x4_13.cpp:259,361).  TMA needs no repacking of row-major operands, but the fp32 ->
