@@ -33,7 +33,7 @@ EXPORTS = [
     "b200_gemm_bf16_epi", "b200_gemm_f16_epi", "b200_gemm_bf16_batched", "b200_gemm_f16_batched",
     "b200_gemm_bf16_grouped", "b200_gemm_f16_grouped", "b200_gemm_bf16_grouped_k", "b200_gemm_f16_grouped_k",
     "b200_gemm_s8s32_op", "b200_gemm_workspace_bytes_op", "b200_gemm_fp8", "b200_gemm_fp8_blockwise",
-    "b200_gemm_fp8_grouped", "b200_gemm_fp8_batched",
+    "b200_gemm_fp8_grouped", "b200_gemm_fp8_batched", "b200_gemm_fp8_blockwise_grouped", "b200_gemm_fp8_blockwise_batched",
     "b200_nccl_load", "b200_nccl_last_error", "b200_comm_unique_id", "b200_comm_init_rank",
     "b200_comm_destroy", "b200_rowpanel_create", "b200_rowpanel_destroy", "b200_rowpanel_slices", "b200_rowpanel_set_reserve_sms", "b200_rowpanel_trace", "b200_rowpanel_trace_dump", "b200_gemm_f32_rowpanel",
     "b200_gemm_f32_rowpanel_host", "b200_gemm_f32_pack_a", "b200_gemm_f32_packed_ab", "b200_gemm_f32_pack_free_a",
@@ -108,6 +108,10 @@ lib.b200_gemm_fp8_grouped.argtypes = [_i, _i, _i, _i, _i, _vp, _i, _vp, _i, _ll,
                                       _vp]
 lib.b200_gemm_fp8_batched.argtypes = [_i, _i, _i, _i, _i, _vp, _i, _ll, _vp, _i, _ll, _vp, _ll, _vp, _ll, _vp, _i, _ll,
                                       _i, _i, _i, _vp]
+lib.b200_gemm_fp8_blockwise_grouped.argtypes = [_i, _i, _i, _i, _i, _vp, _i, _vp, _i, _ll, _vp, _i, _vp, _ll, _ll, _vp, _i,
+                                                _ll, _ll, _ll, _vp, _i, _i, _vp]
+lib.b200_gemm_fp8_blockwise_batched.argtypes = [_i, _i, _i, _i, _i, _vp, _i, _ll, _vp, _i, _ll, _vp, _i, _ll, _ll, _ll, _vp,
+                                                _i, _ll, _ll, _ll, _vp, _i, _ll, _i, _i, _vp]
 lib.b200_gemm_workspace_bytes_op.restype = C.c_size_t
 lib.b200_gemm_f32_pack_b.argtypes = [_i, _i, _vp, _i, _i, C.POINTER(_vp), _vp]
 lib.b200_gemm_f32_packed.argtypes = [_i, _i, _i, _vp, _i, _vp, _vp, _i, _i, _vp]
@@ -605,9 +609,27 @@ def _fp8_in_place(name, t, ld, entry_stride, entry_elems):
                          f"({entry_elems} elements), not {entry_stride}")
 
 
+def _grouped_blockwise_recipe(A, scale_a, scale_b, groups, n, k):
+    """(scale_a_block, scale_b_block) of a grouped (2-D A) or batched (3-D A) blockwise call, resolved from the
+    scales' shapes in scaled_mm's order, or None.  scale_b is (G, q, ceil(n / 128)) or (G, q, n); scale_a is
+    (total_m, q) for a 2-D A (1 x 128 only), and (G, m, q) or (G, ceil(m / 128), q) for a 3-D A."""
+    q, nb = -(-k // 128), -(-n // 128)
+    if A.dim() == 2:
+        want_a = {1: (A.shape[0], q)}
+    else:
+        m = A.shape[1]
+        want_a = {1: (groups, m, q), 128: (groups, -(-m // 128), q)}
+    want_b = {128: (groups, q, nb), 1: (groups, q, n)}
+    for blocks in ((1, 128), (1, 1), (128, 1)):
+        if blocks[0] in want_a and tuple(scale_a.shape) == want_a[blocks[0]] and tuple(scale_b.shape) == want_b[blocks[1]]:
+            return blocks
+    return None
+
+
 def scaled_grouped_mm(A, B, scale_a, scale_b, offs=None, out_dtype=None, use_fast_accum=False, out=None, stream=None):
     """torch._scaled_grouped_mm for FP8 mixture-of-experts layers: every group, or every entry of a batch, is one
-    scaled_mm with rowwise scales, all of them in one launch (b200_gemm_fp8_grouped / _batched).
+    scaled_mm with rowwise scales, all of them in one launch (b200_gemm_fp8_grouped / _batched), or with blockwise
+    scales one blockwise scaled_mm (b200_gemm_fp8_blockwise_grouped / _batched).
 
     B is 3-D (G, k, n) and column-major in its last two dimensions: W.transpose(-2, -1) of a (G, n, k) weight, read
     in place.  scale_b is float32 (G, n), contiguous along n.  Then either
@@ -617,6 +639,12 @@ def scaled_grouped_mm(A, B, scale_a, scale_b, offs=None, out_dtype=None, use_fas
         new out is torch.empty there, as in torch);
       A 3-D (G, m, k) row-major in its last two dimensions (an expand()ed A is broadcast), scale_a (G, m) contiguous
         along m, and no offs: out[g] = (A[g] @ B[g]) * scale_a[g, :, None] * scale_b[g].
+    Blockwise scales (DeepSeek-V3's recipe), with q = ceil(k / 128): a 3-D scale_b, (G, q, ceil(n / 128)) for 128 x 128
+    weight blocks or (G, q, n) for 1 x 128, with scale_a (total_m, q) for a 2-D A (1 x 128 only: a 128-row block
+    would straddle groups), or (G, m, q) or (G, ceil(m / 128), q) for a 3-D A; the pair of 128 x 128 shapes is
+    refused.  Scales are float32 CUDA tensors of any strides (torch's outer-dim-major layout is read in place).  A
+    shape that fits two recipes resolves in scaled_mm's order, which gives the same result.  Each group or entry is
+    then the blockwise scaled_mm without bias on its rows, B and scales; use_fast_accum=True is refused.
     Each step is rounded as in scaled_mm, so each group or entry is bit for bit scaled_mm on its own rows, B and
     scales.  Operands are float8_e4m3fn or float8_e5m2 (not both e5m2).  out_dtype is torch.bfloat16 (the default, as
     in torch), torch.float16 or torch.float32.  use_fast_accum as in scaled_mm.  The offsets and scales stay on the
@@ -652,10 +680,19 @@ def scaled_grouped_mm(A, B, scale_a, scale_b, offs=None, out_dtype=None, use_fas
     for name, s in (("scale_a", scale_a), ("scale_b", scale_b)):
         if s.dtype != torch.float32:
             raise ValueError(f"{name} must be float32, not {s.dtype}")
-    if scale_b.dim() != 2 or tuple(scale_b.shape) != (groups, n) or (n > 1 and scale_b.stride(1) != 1):
+    if scale_b.dim() == 3:
+        q, mq = -(-k // 128), "total_m" if A.dim() == 2 else "m or ceil(m / 128)"
+        if _grouped_blockwise_recipe(A, scale_a, scale_b, groups, n, k) is None:
+            raise ValueError(f"blockwise scales must be scale_b ({groups}, {q}, {-(-n // 128)}) or ({groups}, {q}, {n}) "
+                             f"with scale_a ({mq}, {q}) (not both 128 x 128), not {tuple(scale_a.shape)} and "
+                             f"{tuple(scale_b.shape)}")
+    elif scale_b.dim() != 2 or tuple(scale_b.shape) != (groups, n) or (n > 1 and scale_b.stride(1) != 1):
         raise ValueError(f"scale_b must be ({groups}, {n}) and contiguous along n, not {tuple(scale_b.shape)} of "
                          f"strides {tuple(scale_b.stride())}")
     ssb = scale_b.stride(0) if groups > 1 else 0
+    blocks = _grouped_blockwise_recipe(A, scale_a, scale_b, groups, n, k) if scale_b.dim() == 3 else None
+    if blocks is not None and use_fast_accum:
+        raise ValueError("use_fast_accum=True is not available with blockwise scales: their scales change every k-block")
     if A.dim() == 2:
         if offs is None:
             raise ValueError("a 2-D A needs offs, the groups' cumulative end rows")
@@ -665,7 +702,7 @@ def scaled_grouped_mm(A, B, scale_a, scale_b, offs=None, out_dtype=None, use_fas
         if groups > 1 and sb < n * ldb:
             raise ValueError(f"the groups of B must not overlap or be broadcast (stride(0) = {B.stride(0)})")
         total_m = A.shape[0]
-        if scale_a.dim() != 1 or scale_a.shape[0] != total_m or not scale_a.is_contiguous():
+        if blocks is None and (scale_a.dim() != 1 or scale_a.shape[0] != total_m or not scale_a.is_contiguous()):
             raise ValueError(f"scale_a must be contiguous and 1-D with {total_m} elements, not {tuple(scale_a.shape)}")
         shape = (total_m, n)
     else:
@@ -674,7 +711,7 @@ def scaled_grouped_mm(A, B, scale_a, scale_b, offs=None, out_dtype=None, use_fas
         if A.shape[0] != groups:
             raise ValueError(f"batch sizes differ: {A.shape[0]} and {groups}")
         m = A.shape[1]
-        if scale_a.dim() != 2 or tuple(scale_a.shape) != (groups, m) or (m > 1 and scale_a.stride(1) != 1):
+        if blocks is None and (scale_a.dim() != 2 or tuple(scale_a.shape) != (groups, m) or (m > 1 and scale_a.stride(1) != 1)):
             raise ValueError(f"scale_a must be ({groups}, {m}) and contiguous along m, not {tuple(scale_a.shape)} of "
                              f"strides {tuple(scale_a.stride())}")
         shape = (groups, m, n)
@@ -698,7 +735,21 @@ def scaled_grouped_mm(A, B, scale_a, scale_b, offs=None, out_dtype=None, use_fas
         _fp8_in_place("B", B, ldb, sb, n * ldb)
     ot = {torch.float32: OUT_F32, torch.bfloat16: OUT_BF16, torch.float16: OUT_F16}[out_dtype]
     fast = int(bool(use_fast_accum))
-    if A.dim() == 2:
+    if blocks is not None and A.dim() == 2:
+        _check(lib.b200_gemm_fp8_blockwise_grouped(ta, tb, total_m, n, k, A.data_ptr(), lda, B.data_ptr(), ldb, sb,
+                                                   offs.data_ptr(), groups, scale_a.data_ptr(), scale_a.stride(0),
+                                                   scale_a.stride(1), scale_b.data_ptr(), blocks[1], scale_b.stride(1),
+                                                   scale_b.stride(2), ssb, out.data_ptr(), _ld(out), ot,
+                                                   _stream_ptr(stream)))
+    elif blocks is not None:
+        _check(lib.b200_gemm_fp8_blockwise_batched(ta, tb, m, n, k, A.data_ptr(), lda, A.stride(0) if groups > 1 else 0,
+                                                   B.data_ptr(), ldb, sb, scale_a.data_ptr(), blocks[0],
+                                                   scale_a.stride(1), scale_a.stride(2),
+                                                   scale_a.stride(0) if groups > 1 else 0, scale_b.data_ptr(), blocks[1],
+                                                   scale_b.stride(1), scale_b.stride(2), ssb, out.data_ptr(),
+                                                   _ld(out[0]), out.stride(0) if groups > 1 else 0, groups, ot,
+                                                   _stream_ptr(stream)))
+    elif A.dim() == 2:
         _check(lib.b200_gemm_fp8_grouped(ta, tb, total_m, n, k, A.data_ptr(), lda, B.data_ptr(), ldb, sb,
                                          offs.data_ptr(), groups, scale_a.data_ptr(), scale_b.data_ptr(), ssb,
                                          out.data_ptr(), _ld(out), ot, fast, _stream_ptr(stream)))

@@ -395,7 +395,8 @@ int g_ffma_halves = 1;        // strict kernel: split the tail round into half t
 // (Stacking, gemm_tc.cuh, names the forms.)
 // FP8 kinds (KIND_E4M3, ...): gemm_tc_fp8_kernel with the scales and bias *scl; K-major A and B, no K split.  A
 // TcBlockScale (ScaleT) selects its blockwise-scaled form, whose stages carry their scales in shared memory; STACK_GROUP
-// / STACK_BATCH with a TcStackScale its stacked form (the stack as above, the rowwise scales of every entry in *scl).
+// / STACK_BATCH with a TcStackScale its stacked form (the stack as above, the rowwise scales of every entry in *scl),
+// and with a TcStackBlockScale its stacked blockwise form.
 struct Stack {
   int count;               // entries of a batch, or groups
   long long sa, sb, sc;    // elements between consecutive entries of A, B and C
@@ -413,7 +414,7 @@ int launch_tc(int m, int n, int k, const void* A, long long lda, int a_rows_tota
   using Cfg = TcConfig<KIND, BN, STAGES, Prod, A_ROW_BYTES, AL, BL>;
   using T = KindTraits<KIND>;
   constexpr bool FP8 = KIND == KIND_E4M3 || KIND == KIND_E4M3E5M2 || KIND == KIND_E5M2E4M3;
-  constexpr bool BLK = std::is_same<ScaleT, TcBlockScale>::value;
+  constexpr bool BLK = std::is_same<ScaleT, TcBlockScale>::value || std::is_same<ScaleT, TcStackBlockScale>::value;
   constexpr int smem = Cfg::SMEM_BYTES + (BLK ? STAGES * kBlkScaleStageBytes : 0);
   constexpr CUtensorMapDataType dt = KIND == KIND_F16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
                                    : KIND == KIND_FP16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16
@@ -470,7 +471,7 @@ int launch_tc(int m, int n, int k, const void* A, long long lda, int a_rows_tota
   if (int arc = ensure_smem_attr(kern, smem)) return arc;
   TcStack ts{1, 0, 0, 0, nullptr};
   if constexpr (STACK != STACK_NONE) ts = TcStack{stk->count, stk->sa ? 1 : 0, stk->sb ? 1 : 0, stk->sc, stk->offs};
-  [[maybe_unused]] ScaleT fp8_scale{};          // a stacked FP8 call's TcStackScale takes the stack here
+  [[maybe_unused]] ScaleT fp8_scale{};          // a stacked FP8 call's TcStackScale / TcStackBlockScale takes the stack here
   if constexpr (FP8) {
     fp8_scale = *scl;
     if constexpr (STACK != STACK_NONE) fp8_scale.st = ts;
@@ -1582,37 +1583,43 @@ int gemm_fp8_blockwise(int op_a, int op_b, int a_type, int b_type, int m, int n,
 // gemm_tc_fp8_kernel over a stack: row-major A, every B_b stored n x k (B^T, torch's column-major mat_b), rowwise
 // scales, no bias, no workspace.  The operands are read in place only (FP8 has no CUDA-core kernel, and staging every
 // expert's weight would copy all of B), so the entry points refuse what TMA cannot describe.
-// Kernel names by [stacking: 0 = grouped, 1 = batch][kind][C type][width index, 3 = promoted].
+// Kernel names by [stacking: 0 = grouped, 1 = batch][kind][C type][width index, 3 = promoted, 4 = blockwise].
 #define FP8_STACK_NAMES(P, S)                                                                                           \
-  {{P "_of32_" S "_128x256", P "_of32_" S "_128x192", P "_of32_" S "_128x128", P "_of32_" S "_acc_128x128"},           \
-   {P "_obf16_" S "_128x256", P "_obf16_" S "_128x192", P "_obf16_" S "_128x128", P "_obf16_" S "_acc_128x128"},       \
-   {P "_of16_" S "_128x256", P "_of16_" S "_128x192", P "_of16_" S "_128x128", P "_of16_" S "_acc_128x128"}}
-const char* const kFp8StackNames[2][3][3][4] = {
+  {{P "_of32_" S "_128x256", P "_of32_" S "_128x192", P "_of32_" S "_128x128", P "_of32_" S "_acc_128x128",            \
+    P "_of32_" S "_blk_128x128"},                                                                                       \
+   {P "_obf16_" S "_128x256", P "_obf16_" S "_128x192", P "_obf16_" S "_128x128", P "_obf16_" S "_acc_128x128",        \
+    P "_obf16_" S "_blk_128x128"},                                                                                      \
+   {P "_of16_" S "_128x256", P "_of16_" S "_128x192", P "_of16_" S "_128x128", P "_of16_" S "_acc_128x128",            \
+    P "_of16_" S "_blk_128x128"}}
+const char* const kFp8StackNames[2][3][3][5] = {
     {FP8_STACK_NAMES("tc_e4m3", "grp"), FP8_STACK_NAMES("tc_e4m3e5m2", "grp"), FP8_STACK_NAMES("tc_e5m2e4m3", "grp")},
     {FP8_STACK_NAMES("tc_e4m3", "bat"), FP8_STACK_NAMES("tc_e4m3e5m2", "bat"), FP8_STACK_NAMES("tc_e5m2e4m3", "bat")}};
 
 // The stacked call *stk (m = total_m for a grouped call) at pick_bn's width over the stack's tiles (fast), or promoted
-// per 128-element k-block at BN = 128, as tc_fp8 chooses for one matrix.
-template <int KIND, typename OutT, int STACK>
+// per 128-element k-block at BN = 128, as tc_fp8 chooses for one matrix.  Blockwise scales (Scale = TcStackBlockScale)
+// are always promoted.
+template <int KIND, typename OutT, int STACK, class Scale>
 int tc_fp8_stacked(int m, int n, int k, const void* A, int lda, const void* B, int ldb, void* C, int ldc,
-                   const Stack& stk, const TcStackScale& sc, bool fast, const char* const (&names)[4], const Call& c) {
+                   const Stack& stk, const Scale& sc, bool fast, const char* const (&names)[5], const Call& c) {
+  constexpr bool blk = std::is_same<Scale, TcStackBlockScale>::value;
   // m rows of A per entry (a grouped A is one entry of total_m rows); every B entry is n x k
-  if (fast) {
-    const int bn_m = STACK == STACK_GROUP ? 128 : m;
-    const int bn_batch = STACK == STACK_GROUP ? (int)grouped_tile_rows(m, stk.count) : stk.count;
-    return with_width(bn_m, n, [&](auto W) {
-      using Wd = decltype(W);
-      return launch_tc<KIND, Wd::BN, Wd::STAGES, OutT, ProdSingle, 128, LAYOUT_K, LAYOUT_K, false, STACK>(
-          m, n, k, A, lda, m, 0, B, ldb, n, 0, C, ldc, names[Wd::idx], c, 0, nullptr, nullptr, &stk, &sc);
-    }, bn_batch);
-  }
+  if constexpr (!blk)
+    if (fast) {
+      const int bn_m = STACK == STACK_GROUP ? 128 : m;
+      const int bn_batch = STACK == STACK_GROUP ? (int)grouped_tile_rows(m, stk.count) : stk.count;
+      return with_width(bn_m, n, [&](auto W) {
+        using Wd = decltype(W);
+        return launch_tc<KIND, Wd::BN, Wd::STAGES, OutT, ProdSingle, 128, LAYOUT_K, LAYOUT_K, false, STACK>(
+            m, n, k, A, lda, m, 0, B, ldb, n, 0, C, ldc, names[Wd::idx], c, 0, nullptr, nullptr, &stk, &sc);
+      }, bn_batch);
+    }
   return launch_tc<KIND, 128, Width<128>::STAGES, OutT, ProdPromoted, 128, LAYOUT_K, LAYOUT_K, false, STACK>(
-      m, n, k, A, lda, m, 0, B, ldb, n, 0, C, ldc, names[3], c, 128, nullptr, nullptr, &stk, &sc);
+      m, n, k, A, lda, m, 0, B, ldb, n, 0, C, ldc, names[blk ? 4 : 3], c, 128, nullptr, nullptr, &stk, &sc);
 }
 
-template <int STACK>
+template <int STACK, class Scale>
 int fp8_stacked_run(int a_type, int b_type, int m, int n, int k, const uint8_t* A, int lda, const uint8_t* B, int ldb,
-                    void* C, int ldc, int out_type, const Stack& stk, const TcStackScale& sc, int fast, cudaStream_t st) {
+                    void* C, int ldc, int out_type, const Stack& stk, const Scale& sc, int fast, cudaStream_t st) {
   if (int rc = ensure_device()) return rc;
   Call c{st};
   if (k == 0) {                                             // +0 over the covered rows / entries, no scale read
@@ -1725,6 +1732,106 @@ int gemm_fp8_batched(int a_type, int b_type, int m, int n, int k, const uint8_t*
   sc.a = scale_a; sc.b = scale_b; sc.a_step = 1; sc.b_step = 1; sc.bias = nullptr;
   sc.a_entry_stride = scale_a_stride; sc.b_entry_stride = scale_b_stride;
   return fp8_stacked_run<STACK_BATCH>(a_type, b_type, m, n, k, A, lda, B, ldb, C, ldc, out_type, bt, sc, fast_accum, st);
+}
+
+// ---- grouped and strided-batched blockwise FP8 GEMMs (DeepSeek-V3-style MoE layers) -----------------------------------
+// Every entry is the (N, T) b200_gemm_fp8_blockwise call with no bias on its rows, B and scales, in one launch of the
+// stacked blockwise kernel.  The checks are those of the rowwise stacked calls above and of gemm_fp8_blockwise, with
+// each scale's last index bound including (count - 1) * its entry stride; all before the device is touched.
+
+// Element index of the last scale of a stack of `count` entries `entry_stride` apart (last_scale_index's rule).
+__int128 last_stacked_scale_index(long long count, long long entry_stride, long long rows, long long q,
+                                  long long row_stride, long long kb_stride) {
+  return (__int128)(count - 1) * entry_stride + last_scale_index(rows, q, row_stride, kb_stride);
+}
+
+// Rows [end_{g-1}, end_g) of C = the blockwise product of those rows of A with B_g = B + g * stride_b (n x k); scale_a
+// is 1 x 128 over the stacked A (row i of A: scale_a[i * sa_row + kb * sa_kb]; a 128-row block would straddle groups),
+// scale_b of group g starts at scale_b + g * scale_b_stride, 1 x 128 or 128 x 128 (b_blk).
+int gemm_fp8_blockwise_grouped(int a_type, int b_type, int total_m, int n, int k, const uint8_t* A, int lda,
+                               const uint8_t* B, int ldb, long long stride_b, const int32_t* offs, int groups,
+                               const float* scale_a, long long sa_row, long long sa_kb, const float* scale_b, int b_blk,
+                               long long sb_kb, long long sb_col, long long scale_b_stride, void* C, int ldc,
+                               int out_type, cudaStream_t st) {
+  if (int rc = fp8_stacked_types(a_type, b_type, out_type, 0)) return rc;
+  if (b_blk != 1 && b_blk != 128) return B200_ERR_BAD_ARG;
+  if (sa_row < 0 || sa_kb < 0 || sb_kb < 0 || sb_col < 0 || scale_b_stride < 0) return B200_ERR_BAD_ARG;
+  if (groups < 0 || stride_b < 0 || groups > kMaxGroups) return B200_ERR_BAD_ARG;
+  if (total_m < 0 || n < 0 || k < 0) return B200_ERR_BAD_ARG;
+  if (a_type == B200_FP8_E5M2 && b_type == B200_FP8_E5M2) return B200_ERR_UNSUPPORTED;
+  if (groups == 0) return 0;
+  int rc = check_args(total_m, n, k, A, lda, B, ldb, C, ldc, B200_OP_N, B200_OP_T);
+  if (rc == 1) return 0;
+  if (rc) return rc;
+  if (!offs || !scale_a || !scale_b) return B200_ERR_BAD_ARG;
+  if (groups > 1) {
+    if (stride_b < (long long)n * ldb) return B200_ERR_BAD_ARG;                          // B_g would overlap
+    if (stride_b > (1LL << 60) / (groups - 1) || scale_b_stride > (1LL << 60) / (groups - 1)) return B200_ERR_BAD_ARG;
+  }
+  const long long tiles_n = (n + 127LL) / 128;
+  if (tiles_n > 0x3FFFFFFFLL / grouped_tile_rows(total_m, groups)) return B200_ERR_BAD_ARG;
+  const long long q = (k + 127LL) / 128;
+  const __int128 max_index = INT64_MAX / 4;
+  if (last_scale_index(total_m, q, sa_row, sa_kb) > max_index ||
+      last_stacked_scale_index(groups, scale_b_stride, b_blk == 1 ? n : tiles_n, q, sb_col, sb_kb) > max_index)
+    return B200_ERR_BAD_ARG;
+  if (k > 0 && (!fp8_in_place(A, lda, B, ldb) || (groups > 1 && !batch_tma_ok(stride_b, n, ldb, 1))))
+    return B200_ERR_UNSUPPORTED;
+  const Stack gr{groups, 0, groups > 1 ? stride_b : 0, 0, offs};
+  TcStackBlockScale sc{};
+  sc.a = scale_a; sc.b = scale_b; sc.a_row = sa_row; sc.a_kb = sa_kb; sc.b_kb = sb_kb; sc.b_col = sb_col;
+  sc.a_blk = 1; sc.b_blk = b_blk; sc.bias = nullptr;
+  sc.a_entry_stride = 0; sc.b_entry_stride = scale_b_stride;
+  return fp8_stacked_run<STACK_GROUP>(a_type, b_type, total_m, n, k, A, lda, B, ldb, C, ldc, out_type, gr, sc, 0, st);
+}
+
+// C_b = the blockwise product of A_b = A + b * stride_a (m x k) and B_b = B + b * stride_b (n x k), C_b = C + b *
+// stride_c, with entry b's scales at scale_a + b * scale_a_stride and scale_b + b * scale_b_stride, each indexed as by
+// gemm_fp8_blockwise.  batch == 1 is the (N, T) b200_gemm_fp8_blockwise call with no bias.
+int gemm_fp8_blockwise_batched(int a_type, int b_type, int m, int n, int k, const uint8_t* A, int lda, long long stride_a,
+                               const uint8_t* B, int ldb, long long stride_b, const float* scale_a, int a_blk,
+                               long long sa_row, long long sa_kb, long long scale_a_stride, const float* scale_b,
+                               int b_blk, long long sb_kb, long long sb_col, long long scale_b_stride, void* C, int ldc,
+                               long long stride_c, int batch, int out_type, cudaStream_t st) {
+  if (int rc = fp8_stacked_types(a_type, b_type, out_type, 0)) return rc;
+  if ((a_blk != 1 && a_blk != 128) || (b_blk != 1 && b_blk != 128)) return B200_ERR_BAD_ARG;
+  if (sa_row < 0 || sa_kb < 0 || sb_kb < 0 || sb_col < 0) return B200_ERR_BAD_ARG;
+  if (batch < 0 || stride_a < 0 || stride_b < 0 || stride_c < 0 || scale_a_stride < 0 || scale_b_stride < 0)
+    return B200_ERR_BAD_ARG;
+  if (m < 0 || n < 0 || k < 0) return B200_ERR_BAD_ARG;
+  if (a_type == B200_FP8_E5M2 && b_type == B200_FP8_E5M2) return B200_ERR_UNSUPPORTED;
+  if (a_blk == 128 && b_blk == 128) return B200_ERR_UNSUPPORTED;      // not a torch recipe
+  if (batch == 0) return 0;
+  int rc = check_args(m, n, k, A, lda, B, ldb, C, ldc, B200_OP_N, B200_OP_T);
+  if (rc == 1) return 0;
+  if (rc) return rc;
+  if (!scale_a || !scale_b) return B200_ERR_BAD_ARG;
+  if (batch > 1) {
+    if (stride_c < (long long)(m - 1) * ldc + n) return B200_ERR_BAD_ARG;               // entries of C would overlap
+    const long long max_stride = (1LL << 60) / (batch - 1);
+    if (stride_a > max_stride || stride_b > max_stride || stride_c > max_stride || scale_a_stride > max_stride ||
+        scale_b_stride > max_stride)
+      return B200_ERR_BAD_ARG;
+    const long long tiles1 = ((m + 127LL) / 128) * ((n + 127LL) / 128);                  // < 2^48
+    if (tiles1 > 0x7FFFFFFFLL / 4 / batch) return B200_ERR_BAD_ARG;
+  }
+  const long long q = (k + 127LL) / 128;
+  const __int128 max_index = INT64_MAX / 4;
+  if (last_stacked_scale_index(batch, scale_a_stride, a_blk == 1 ? m : (m + 127LL) / 128, q, sa_row, sa_kb) > max_index ||
+      last_stacked_scale_index(batch, scale_b_stride, b_blk == 1 ? n : (n + 127LL) / 128, q, sb_col, sb_kb) > max_index)
+    return B200_ERR_BAD_ARG;
+  if (k > 0 && (!fp8_in_place(A, lda, B, ldb) ||
+                (batch > 1 && (!batch_tma_ok(stride_a, m, lda, 1) || !batch_tma_ok(stride_b, n, ldb, 1)))))
+    return B200_ERR_UNSUPPORTED;
+  if (batch == 1)
+    return gemm_fp8_blockwise(B200_OP_N, B200_OP_T, a_type, b_type, m, n, k, A, lda, B, ldb, scale_a, a_blk, sa_row,
+                              sa_kb, scale_b, b_blk, sb_kb, sb_col, nullptr, C, ldc, out_type, st);
+  const Stack bt{batch, stride_a, stride_b, stride_c, nullptr};
+  TcStackBlockScale sc{};
+  sc.a = scale_a; sc.b = scale_b; sc.a_row = sa_row; sc.a_kb = sa_kb; sc.b_kb = sb_kb; sc.b_col = sb_col;
+  sc.a_blk = a_blk; sc.b_blk = b_blk; sc.bias = nullptr;
+  sc.a_entry_stride = scale_a_stride; sc.b_entry_stride = scale_b_stride;
+  return fp8_stacked_run<STACK_BATCH>(a_type, b_type, m, n, k, A, lda, B, ldb, C, ldc, out_type, bt, sc, 0, st);
 }
 
 }  // namespace
@@ -1957,6 +2064,30 @@ int b200_gemm_fp8_batched(int a_type, int b_type, int m, int n, int k, const uin
                           int batch, int out_type, int fast_accum, void* stream) {
   return gemm_fp8_batched(a_type, b_type, m, n, k, dA, lda, stride_a, dB, ldb, stride_b, dScaleA, scale_a_stride, dScaleB,
                           scale_b_stride, dC, ldc, stride_c, batch, out_type, fast_accum, (cudaStream_t)stream);
+}
+
+int b200_gemm_fp8_blockwise_grouped(int a_type, int b_type, int total_m, int n, int k, const uint8_t* dA, int lda,
+                                    const uint8_t* dB, int ldb, long long stride_b, const int32_t* dOffs, int groups,
+                                    const float* dScaleA, long long sa_row_stride, long long sa_kb_stride,
+                                    const float* dScaleB, int scale_b_block, long long sb_kb_stride,
+                                    long long sb_col_stride, long long scale_b_stride, void* dC, int ldc, int out_type,
+                                    void* stream) {
+  return gemm_fp8_blockwise_grouped(a_type, b_type, total_m, n, k, dA, lda, dB, ldb, stride_b, dOffs, groups, dScaleA,
+                                    sa_row_stride, sa_kb_stride, dScaleB, scale_b_block, sb_kb_stride, sb_col_stride,
+                                    scale_b_stride, dC, ldc, out_type, (cudaStream_t)stream);
+}
+
+int b200_gemm_fp8_blockwise_batched(int a_type, int b_type, int m, int n, int k, const uint8_t* dA, int lda,
+                                    long long stride_a, const uint8_t* dB, int ldb, long long stride_b,
+                                    const float* dScaleA, int scale_a_block, long long sa_row_stride,
+                                    long long sa_kb_stride, long long scale_a_stride, const float* dScaleB,
+                                    int scale_b_block, long long sb_kb_stride, long long sb_col_stride,
+                                    long long scale_b_stride, void* dC, int ldc, long long stride_c, int batch,
+                                    int out_type, void* stream) {
+  return gemm_fp8_blockwise_batched(a_type, b_type, m, n, k, dA, lda, stride_a, dB, ldb, stride_b, dScaleA, scale_a_block,
+                                    sa_row_stride, sa_kb_stride, scale_a_stride, dScaleB, scale_b_block, sb_kb_stride,
+                                    sb_col_stride, scale_b_stride, dC, ldc, stride_c, batch, out_type,
+                                    (cudaStream_t)stream);
 }
 
 int b200_gemm_s8s32_op(int op_a, int op_b, int m, int n, int k, const int8_t* dA, int lda, const int8_t* dB, int ldb,

@@ -676,6 +676,14 @@ struct TcStackScale : TcScale {
   TcStack st;
   long long a_entry_stride, b_entry_stride;
 };
+// Stacked blockwise FP8 kernels (BLOCKWISE with STACK_GROUP / STACK_BATCH): TcBlockScale's indexing inside each entry,
+// no bias, plus the stack and the scales' element strides between entries.  Entry e's k-block kb takes, for row i,
+// a[(end_{e-1} + i) * a_row + kb * a_kb] (grouped: the row of the stacked A, a_blk = 1 only) or
+// a[e * a_entry_stride + ia * a_row + kb * a_kb] (batch), and for column j b[e * b_entry_stride + kb * b_kb + jb * b_col].
+struct TcStackBlockScale : TcBlockScale {
+  TcStack st;
+  long long a_entry_stride, b_entry_stride;
+};
 // Shared memory of one stage's block scales: 128 floats of A (one per tile row), then 128 of B (one per tile column).
 constexpr int kBlkScaleStageBytes = 2 * 128 * 4;
 
@@ -728,6 +736,52 @@ __device__ __forceinline__ int* fp8_group_table() {
   __shared__ int t[kMaxGroups + 1];
   return t;
 }
+
+// fp8_block_scale_loader over a stack (TcStackBlockScale): the TMA thread's num_tiles work tiles, each in its entry
+// (stack_entry; the group table is built before the warp split).  Per tile one source pointer per lane, at the entry's
+// scales: a grouped A's rows are the stacked A's (row end_{e-1} + i), a batch's A and every B start at e * entry
+// stride.  A rows >= the entry's M (the next group's, or past the tensor) and B columns >= N are zero-filled without a
+// read, so no load leaves the scale tensors whatever the offsets.  A separate function, so that the single-matrix
+// loader keeps its code.
+template <class Cfg, int BN, int STAGES, int STACK>
+__device__ __forceinline__ void fp8_block_scale_loader_stacked(const TcParams& p, const TcStackBlockScale& sc,
+                                                               int num_tiles, uint32_t slots, uint32_t bar_full,
+                                                               uint32_t bar_empty, bool is_b, int lane) {
+  const float* base = is_b ? sc.b : sc.a;
+  const long long blk_stride = is_b ? sc.b_col : sc.a_row, kb_stride = is_b ? sc.b_kb : sc.a_kb;
+  const bool per_block = (is_b ? sc.b_blk : sc.a_blk) == 128;
+  const int num_kb = (p.K + Cfg::BK - 1) / Cfg::BK;
+  const uint32_t half = slots + (is_b ? 512u : 0u) + 4u * lane;
+  int s = 0;
+  uint32_t ph = 0;
+  for (int w = blockIdx.x; w < num_tiles; w += gridDim.x) {
+    const StackEntry se = stack_entry<STACK>(w, p, sc.st, fp8_group_table<0>(), fp8_group_table<1>());
+    int mb, nb;
+    tile_coords(w - se.tile0, se.tiles_m, p.tiles_n, p.group_m, mb, nb);
+    const int t = is_b ? nb : mb;
+    const int i0 = t * (is_b ? BN : Cfg::BM) + lane;
+    const int valid = (is_b ? p.N : se.M) - i0;               // scale q of this lane exists iff 32 q < valid
+    long long e_off;                                          // elements from base to the entry's first row / column
+    if (is_b) e_off = se.entry * sc.b_entry_stride;
+    else if constexpr (STACK == STACK_GROUP) e_off = se.a_row * sc.a_row;
+    else e_off = se.entry * sc.a_entry_stride;
+    const float* src = base + e_off + (long long)(per_block ? t : i0) * blk_stride;
+    const long long step = per_block ? 0 : 32 * blk_stride;
+    for (int kb = 0; kb < num_kb; kb++, src += kb_stride) {
+      mbar_wait(bar_empty + 8 * s, ph ^ 1);
+      const uint32_t dst = half + s * kBlkScaleStageBytes;
+#pragma unroll
+      for (int q = 0; q < 4; q++) {
+        const bool in = 32 * q < valid;
+        asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;" ::"r"(dst + 128u * q), "l"(in ? src + q * step : base),
+                     "r"(in ? 4 : 0) : "memory");
+      }
+      asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(bar_full + 8 * s) : "memory");
+      if (++s == STAGES) { s = 0; ph ^= 1; }
+    }
+  }
+  asm volatile("cp.async.wait_all;" ::: "memory");
+}
 // Work tiles of an FP8 launch: one matrix's, a batch's, or (GROUPED) the table's, built here by every CTA after
 // griddep_wait (group_table ends in __syncthreads; CTAs past the table's tiles have no work).
 template <int STACK, int BM, class Scale>
@@ -755,12 +809,15 @@ __device__ __forceinline__ int fp8_num_tiles(const TcParams& p, const Scale& sc)
 // entry at the same width.  STACK_NONE: the single-matrix kernels, unchanged: every stacked path sits in an
 // `if constexpr` branch of its own and the stacking is tested in place (a local constexpr alias for it, like an unused
 // local variable, changed the register assignment of those kernels).
+// BLOCKWISE with STACK_GROUP / STACK_BATCH (argument TcStackBlockScale): the stacked schedule with the blockwise
+// stages; warps 1 and 2 run fp8_block_scale_loader_stacked over the same tiles, and each tile's sum is stored through
+// its entry's TcParams with no further scaling and no bias (the single-matrix store's rn(sum + -0) = sum).
 template <int KIND, int BN, int STAGES, typename OutT, class Prod, bool BLOCKWISE = false, int STACK = STACK_NONE>
 __global__ void __launch_bounds__((TcConfig<KIND, BN, STAGES, Prod, 128>::THREADS), 1)
 gemm_tc_fp8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const TcParams p,
-                   const typename std::conditional<BLOCKWISE, TcBlockScale,
-                                                   typename std::conditional<STACK != STACK_NONE, TcStackScale,
-                                                                             TcScale>::type>::type sc) {
+                   const typename std::conditional<
+                       BLOCKWISE, typename std::conditional<STACK != STACK_NONE, TcStackBlockScale, TcBlockScale>::type,
+                       typename std::conditional<STACK != STACK_NONE, TcStackScale, TcScale>::type>::type sc) {
   using Cfg = TcConfig<KIND, BN, STAGES, Prod, 128>;
   using MMA = typename Cfg::MMA;
   static_assert(KIND == KIND_E4M3 || KIND == KIND_E4M3E5M2 || KIND == KIND_E5M2E4M3, "FP8 kinds");
@@ -769,7 +826,9 @@ gemm_tc_fp8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
   static_assert(!BLOCKWISE || (std::is_same<Prod, ProdPromoted>::value && BN == 128 && Cfg::BK == 128),
                 "blockwise scales: one 128-element k-block per promotion, tiles on the 128 x 128 scale blocks");
   static_assert(!BLOCKWISE || Cfg::SMEM_BYTES + STAGES * kBlkScaleStageBytes <= 232448, "blockwise: shared memory");
-  static_assert(!(BLOCKWISE && STACK != STACK_NONE), "stacked FP8: rowwise scales only");
+  static_assert(!(BLOCKWISE && STACK == STACK_GROUP) ||
+                    Cfg::SMEM_BYTES + STAGES * kBlkScaleStageBytes + 2 * (kMaxGroups + 1) * (int)sizeof(int) <= 232448,
+                "grouped blockwise: the pipeline, the scale slots and the group tables exceed 227 KB of shared memory");
   static_assert(STACK == STACK_NONE || STACK == STACK_GROUP || STACK == STACK_BATCH, "stacked FP8: a batch or a grouped call");
   static_assert(STACK != STACK_GROUP || Cfg::SMEM_BYTES + 2 * (kMaxGroups + 1) * (int)sizeof(int) <= 232448,
                 "the pipeline and the group tables exceed the 227 KB of shared memory of sm_90");
@@ -837,9 +896,14 @@ gemm_tc_fp8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
         }
       }
     }
-    if constexpr (BLOCKWISE)
+    if constexpr (BLOCKWISE && STACK != STACK_NONE) {
+      if (warp == 1 || warp == 2)
+        fp8_block_scale_loader_stacked<Cfg, BN, STAGES, STACK>(p, sc, num_tiles, s_scale, bar_full, bar_empty, warp == 2,
+                                                               lane);
+    } else if constexpr (BLOCKWISE) {
       if (warp == 1 || warp == 2)
         fp8_block_scale_loader<Cfg, BN, STAGES>(p, sc, s_scale, bar_full, bar_empty, warp == 2, lane);
+    }
   } else {
     // ===================== consumers (warpgroups 1 and 2): MMA chain + scaled epilogue =====================
     setmaxnreg_inc<232>();
@@ -925,7 +989,22 @@ gemm_tc_fp8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
       // ---- this warp's 16 rows of the tile into C: (acc * sa) * sb (BLOCKWISE: sum), then + bias in store_pair ----
       const int row0 = m0 + ew * 16 + (lane >> 2);
       const int col0 = n0 + 2 * (lane & 3);
-      if constexpr (STACK != STACK_NONE) {
+      if constexpr (BLOCKWISE && STACK != STACK_NONE) {
+        // the entry's C and rows, as below; the blockwise sum is stored as is (no bias)
+        const StackEntry se = stack_entry<STACK>(w, p, sc.st, fp8_group_table<0>(), fp8_group_table<1>());
+        TcParams pc = p;
+        pc.C = static_cast<uint8_t*>(p.C) + se.c_off * OutBytes<OutT>::V;
+        pc.M = se.M;
+        const int ce[2] = {0, 0};
+#pragma unroll
+        for (int j = 0; j < BN / 8; j++)
+#pragma unroll
+          for (int h = 0; h < 2; h++)
+            store_pair<OutT, float, ACT_NONE>(pc, row0 + 8 * h, col0 + 8 * j, sum[4 * j + 2 * h], sum[4 * j + 2 * h + 1],
+                                              false, false, 1.f, 1.f, 0, ce, 0.f, 0.f);
+        continue;
+      }
+      if constexpr (STACK != STACK_NONE && !BLOCKWISE) {
         // the entry's C and rows (pc; rows of the tile past the entry's are never stored), and its scale vectors: row i
         // of the entry takes sa_e[i], column j sb_e[j].  No bias.  (A copy of the store below, so that the
         // single-matrix kernels keep their code.)

@@ -527,6 +527,48 @@ int b200_gemm_fp8_batched(int a_type, int b_type, int m, int n, int k, const uin
                           const float* dScaleB, long long scale_b_stride, void* dC, int ldc, long long stride_c,
                           int batch, int out_type, int fast_accum, void* stream);
 
+/* ---- Grouped and batched blockwise-scaled FP8 GEMMs (DeepSeek-V3-style FP8 mixture-of-experts layers) ---------------
+ * Every entry is one (N, T) b200_gemm_fp8_blockwise call with no bias, all of them in one launch, and equals that call
+ * on the entry's rows, B and scales bit for bit (the same MMA chain, fold and store):
+ *   C_e = round_out(sum_e),  sum_e = fma(acc_b, rn(sa_b(i) * sb_b(j)), sum_e) over the k-blocks b in order, from +0.
+ * A_e is row-major (lda >= k) and every B_e is stored n x k (ldb >= k), as for b200_gemm_fp8_grouped / _batched.
+ *   b200_gemm_fp8_blockwise_grouped: group g is rows [end_{g-1}, end_g) of A (total_m x k) and C, times B_g = dB + g *
+ *     stride_b, with b200_gemm_bf16_grouped's clamped ends read on the device (rows from end_{G-1} on are never
+ *     written).  scale_a is always 1 x 128 (a 128-row block would straddle groups), indexed by the row of A:
+ *     sa_b(i) = dScaleA[i * sa_row_stride + b * sa_kb_stride] (torch's (total_m, q) scale_a).  Group g's scale_b
+ *     starts at dScaleB + g * scale_b_stride and is indexed as b200_gemm_fp8_blockwise's (scale_b_block 1 or 128).
+ *   b200_gemm_fp8_blockwise_batched: entry e is A_e = dA + e * stride_a (m x k), B_e = dB + e * stride_b, C_e = dC + e
+ *     * stride_c; its scales start at dScaleA + e * scale_a_stride and dScaleB + e * scale_b_stride and are indexed as
+ *     b200_gemm_fp8_blockwise's, with any of its three recipes; (128, 128) is B200_ERR_UNSUPPORTED.  An operand stride
+ *     of 0 broadcasts the operand; its scales still follow their own stride.  batch == 1 is the (N, T)
+ *     b200_gemm_fp8_blockwise call with no bias: same kernel, name and bits.
+ * Neither the offsets nor the scales are read by the host: the calls never synchronise and can be captured in a CUDA
+ * graph.  No bias, no fast accumulation, no workspace, no K-split tail.  k == 0 stores +0 over the covered rows /
+ * entries and reads no scale.  A scale row past an entry's rows (a grouped A's next group) and a column past n are
+ * never read, whatever the offsets.
+ * Argument rules, all checked before the device is touched: the types of b200_gemm_fp8; the block sizes (1 or 128),
+ * strides (>= 0) and last-scale-index bound of b200_gemm_fp8_blockwise, that index including (G - 1) times the entry
+ * stride; the sizes, groups, offsets, strides, overlap and tile bounds of b200_gemm_fp8_grouped / _batched, with the
+ * scale entry strides bounded like the operand strides; a null scale (or offs) with work to do: B200_ERR_BAD_ARG.
+ * Operands not read in place, as for b200_gemm_fp8_grouped / _batched: B200_ERR_UNSUPPORTED.  Tiles are 128 x 128,
+ * six stages, as b200_gemm_fp8_blockwise's.  Kernels: "tc_e4m3_obf16_grp_blk_128x128", "tc_e5m2e4m3_of32_bat_blk_128x128",
+ * ...; a k == 0 call runs "fill_zero_grp" / "fill_zero_bat". */
+int b200_gemm_fp8_blockwise_grouped(int a_type, int b_type, int total_m, int n, int k,
+                                    const uint8_t* dA, int lda, const uint8_t* dB, int ldb, long long stride_b,
+                                    const int32_t* dOffs, int groups,
+                                    const float* dScaleA, long long sa_row_stride, long long sa_kb_stride,
+                                    const float* dScaleB, int scale_b_block, long long sb_kb_stride,
+                                    long long sb_col_stride, long long scale_b_stride,
+                                    void* dC, int ldc, int out_type, void* stream);
+int b200_gemm_fp8_blockwise_batched(int a_type, int b_type, int m, int n, int k,
+                                    const uint8_t* dA, int lda, long long stride_a,
+                                    const uint8_t* dB, int ldb, long long stride_b,
+                                    const float* dScaleA, int scale_a_block, long long sa_row_stride,
+                                    long long sa_kb_stride, long long scale_a_stride,
+                                    const float* dScaleB, int scale_b_block, long long sb_kb_stride,
+                                    long long sb_col_stride, long long scale_b_stride,
+                                    void* dC, int ldc, long long stride_c, int batch, int out_type, void* stream);
+
 /* Pre-split operands for the split-precision modes (AUTO = the library default): the reference
  * leaves its "packAB interface open" for callers that reuse one operand (README.md:85; PackMatrixA/B,
  * aarch64/MMult_4x4_13.cpp:259,361).  TMA needs no repacking of row-major operands, but the fp32 ->
