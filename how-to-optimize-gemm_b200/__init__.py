@@ -34,6 +34,7 @@ EXPORTS = [
     "b200_gemm_bf16_grouped", "b200_gemm_f16_grouped", "b200_gemm_bf16_grouped_k", "b200_gemm_f16_grouped_k",
     "b200_gemm_s8s32_op", "b200_gemm_workspace_bytes_op", "b200_gemm_fp8", "b200_gemm_fp8_blockwise",
     "b200_gemm_fp8_grouped", "b200_gemm_fp8_batched", "b200_gemm_fp8_blockwise_grouped", "b200_gemm_fp8_blockwise_batched",
+    "b200_gemm_fp8_q8", "b200_gemm_fp8_blockwise_q8",
     "b200_nccl_load", "b200_nccl_last_error", "b200_comm_unique_id", "b200_comm_init_rank",
     "b200_comm_destroy", "b200_rowpanel_create", "b200_rowpanel_destroy", "b200_rowpanel_slices", "b200_rowpanel_set_reserve_sms", "b200_rowpanel_trace", "b200_rowpanel_trace_dump", "b200_gemm_f32_rowpanel",
     "b200_gemm_f32_rowpanel_host", "b200_gemm_f32_pack_a", "b200_gemm_f32_packed_ab", "b200_gemm_f32_pack_free_a",
@@ -112,6 +113,10 @@ lib.b200_gemm_fp8_blockwise_grouped.argtypes = [_i, _i, _i, _i, _i, _vp, _i, _vp
                                                 _ll, _ll, _ll, _vp, _i, _i, _vp]
 lib.b200_gemm_fp8_blockwise_batched.argtypes = [_i, _i, _i, _i, _i, _vp, _i, _ll, _vp, _i, _ll, _vp, _i, _ll, _ll, _ll, _vp,
                                                 _i, _ll, _ll, _ll, _vp, _i, _ll, _i, _i, _vp]
+lib.b200_gemm_fp8_q8.argtypes = [_i, _i, _i, _i, _i, _i, _i, _vp, _i, _vp, _i, _vp, _i, _vp, _i, _vp, _i, _i, _i, _vp, _i, _vp,
+                                 _vp, _ll, _ll, _vp]
+lib.b200_gemm_fp8_blockwise_q8.argtypes = [_i, _i, _i, _i, _i, _i, _i, _vp, _i, _vp, _i, _vp, _i, _ll, _ll, _vp, _i, _ll,
+                                           _ll, _vp, _i, _i, _vp, _i, _vp, _vp, _ll, _ll, _vp]
 lib.b200_gemm_workspace_bytes_op.restype = C.c_size_t
 lib.b200_gemm_f32_pack_b.argtypes = [_i, _i, _vp, _i, _i, C.POINTER(_vp), _vp]
 lib.b200_gemm_f32_packed.argtypes = [_i, _i, _i, _vp, _i, _vp, _vp, _i, _i, _vp]
@@ -498,6 +503,11 @@ def _fp8_type(t):
     return {torch.float8_e4m3fn: FP8_E4M3, torch.float8_e5m2: FP8_E5M2}.get(t.dtype)
 
 
+def _is_fp8(dtype):
+    import torch
+    return dtype in (torch.float8_e4m3fn, torch.float8_e5m2)
+
+
 def _blockwise_recipe(scale_a, scale_b, m, n, k):
     """(scale_a_block, scale_b_block) of torch._scaled_mm's blockwise recipes, resolved from the scales' shapes in the
     order torch checks them, or None.  Both scales must be 2-D float32 tensors."""
@@ -512,7 +522,8 @@ def _blockwise_recipe(scale_a, scale_b, m, n, k):
     return None
 
 
-def scaled_mm(A, B, scale_a, scale_b, bias=None, out_dtype=None, use_fast_accum=False, out=None, stream=None):
+def scaled_mm(A, B, scale_a, scale_b, bias=None, out_dtype=None, use_fast_accum=False, out=None, stream=None, *,
+              scale_result=None):
     """torch._scaled_mm for FP8 CUDA tensors: out = ((A @ B) * scale_a) * scale_b + bias, each step rounded in fp32 and
     the result rounded once to out_dtype (b200_gemm_fp8), or with blockwise scales the sum over 128-element k-blocks
     of each block's product times its scales (b200_gemm_fp8_blockwise).
@@ -531,10 +542,19 @@ def scaled_mm(A, B, scale_a, scale_b, bias=None, out_dtype=None, use_fast_accum=
     contiguous elements of out_dtype.  out_dtype is torch.bfloat16 (the default), torch.float16 or torch.float32.
     use_fast_accum = False promotes the tensor core's FP8 sums to fp32 every 128 elements of K; True keeps one
     tensor-core accumulator over K (faster, less precise) and is refused with blockwise scales.
+    out_dtype torch.float8_e4m3fn or torch.float8_e5m2 writes FP8: out = fp8(v / scale_result), v the fp32 value the
+    other outputs round, fp8() round to nearest with finite values saturated to the format's largest (b200_gemm_fp8_q8 /
+    b200_gemm_fp8_blockwise_q8, static mode).  scale_result is None (1) or a one-element float32 CUDA tensor, read on the
+    device; the bias is then bf16.  Every input recipe above works with an FP8 out_dtype.
     Operands of other dtypes, or two e5m2 operands, are a TypeError; a scale of another shape or dtype, a CPU tensor,
-    another bias, out_dtype or out (shape, dtype, or rows that overlap) is a ValueError."""
+    another bias, out_dtype, scale_result or out (shape, dtype, or rows that overlap) is a ValueError."""
     import torch
     out_dtype = out_dtype or (out.dtype if out is not None else torch.bfloat16)
+    if _is_fp8(out_dtype):
+        return _scaled_mm_fp8_out(A, B, scale_a, scale_b, bias, None, out_dtype, use_fast_accum, out, None, scale_result,
+                                  stream)[0]
+    if scale_result is not None:
+        raise ValueError("scale_result applies to an FP8 out_dtype only")
     ta, tb = _fp8_type(A), _fp8_type(B)
     if ta is None or tb is None:
         raise TypeError(f"operands must be float8_e4m3fn or float8_e5m2, not {A.dtype} and {B.dtype}")
@@ -546,23 +566,7 @@ def scaled_mm(A, B, scale_a, scale_b, bias=None, out_dtype=None, use_fast_accum=
     n = B.shape[1]
     if out_dtype not in (torch.bfloat16, torch.float16, torch.float32):
         raise ValueError(f"out_dtype must be bfloat16, float16 or float32, not {out_dtype}")
-    rows = []
-    for name, s, length, shape in (("scale_a", scale_a, m, (m, 1)), ("scale_b", scale_b, n, (1, n))):
-        if s.dtype != torch.float32:
-            raise ValueError(f"{name} must be float32, not {s.dtype}")
-        if s.numel() == 1:
-            rows.append(0)
-        elif s.numel() == length and tuple(s.shape) == shape and s.is_contiguous():
-            rows.append(1)
-        else:
-            rows = None
-            break
-    blocks = _blockwise_recipe(scale_a, scale_b, m, n, k) if rows is None else None
-    if rows is None and blocks is None:
-        q = -(-k // 128)
-        raise ValueError(f"scale_a and scale_b must have one element, shapes (m, 1) and (1, n), or blockwise shapes "
-                         f"(({m}, {q}), ({q}, {-(-n // 128)})), (({m}, {q}), ({q}, {n})) or "
-                         f"(({-(-m // 128)}, {q}), ({q}, {n})), not {tuple(scale_a.shape)} and {tuple(scale_b.shape)}")
+    rows, blocks = _resolve_scales(scale_a, scale_b, m, n, k)
     if blocks is not None and use_fast_accum:
         raise ValueError("use_fast_accum=True is not available with blockwise scales: their scales change every k-block")
     if bias is not None:
@@ -596,6 +600,122 @@ def scaled_mm(A, B, scale_a, scale_b, bias=None, out_dtype=None, use_fast_accum=
                              rows[0], scale_b.data_ptr(), rows[1], bias.data_ptr() if bias is not None else None,
                              out.data_ptr(), _ld(out), ot, int(bool(use_fast_accum)), _stream_ptr(stream)))
     return out
+
+
+def _resolve_scales(scale_a, scale_b, m, n, k):
+    """(rows, blocks) of scaled_mm's scale resolution: rows = (scale_a_rowwise, scale_b_colwise) for tensorwise /
+    rowwise scales, else blocks = (scale_a_block, scale_b_block); a ValueError when neither fits."""
+    import torch
+    rows = []
+    for name, s, length, shape in (("scale_a", scale_a, m, (m, 1)), ("scale_b", scale_b, n, (1, n))):
+        if s.dtype != torch.float32:
+            raise ValueError(f"{name} must be float32, not {s.dtype}")
+        if s.numel() == 1:
+            rows.append(0)
+        elif s.numel() == length and tuple(s.shape) == shape and s.is_contiguous():
+            rows.append(1)
+        else:
+            rows = None
+            break
+    blocks = _blockwise_recipe(scale_a, scale_b, m, n, k) if rows is None else None
+    if rows is None and blocks is None:
+        q = -(-k // 128)
+        raise ValueError(f"scale_a and scale_b must have one element, shapes (m, 1) and (1, n), or blockwise shapes "
+                         f"(({m}, {q}), ({q}, {-(-n // 128)})), (({m}, {q}), ({q}, {n})) or "
+                         f"(({-(-m // 128)}, {q}), ({q}, {n})), not {tuple(scale_a.shape)} and {tuple(scale_b.shape)}")
+    return rows, blocks
+
+
+def _scaled_mm_fp8_out(A, B, scale_a, scale_b, bias, activation, out_dtype, use_fast_accum, out, out_scale,
+                       scale_result, stream, dynamic=False):
+    """The FP8-output form of scaled_mm (static: scale_result) and scaled_mm_quant (dynamic: out_scale); returns
+    (out, scale_c or None).  Every check happens before the device is touched."""
+    import torch
+    ta, tb = _fp8_type(A), _fp8_type(B)
+    if ta is None or tb is None:
+        raise TypeError(f"operands must be float8_e4m3fn or float8_e5m2, not {A.dtype} and {B.dtype}")
+    if ta == FP8_E5M2 and tb == FP8_E5M2:
+        raise TypeError("float8_e5m2 x float8_e5m2 is not supported (as in torch._scaled_mm)")
+    if A.dim() != 2 or B.dim() != 2 or A.shape[1] != B.shape[0]:
+        raise ValueError(f"A and B must be 2-D with matching inner dimensions, not {tuple(A.shape)} and {tuple(B.shape)}")
+    m, k = A.shape
+    n = B.shape[1]
+    if not _is_fp8(out_dtype):
+        raise ValueError(f"out_dtype must be float8_e4m3fn or float8_e5m2, not {out_dtype}")
+    if activation not in ACTIVATIONS:
+        raise ValueError(f"activation must be one of {sorted(a for a in ACTIVATIONS if a)} or None, not {activation!r}")
+    rows, blocks = _resolve_scales(scale_a, scale_b, m, n, k)
+    if blocks is not None and use_fast_accum:
+        raise ValueError("use_fast_accum=True is not available with blockwise scales: their scales change every k-block")
+    if bias is not None:
+        if bias.dtype != torch.bfloat16:
+            raise ValueError(f"with an FP8 output the bias must be bfloat16, not {bias.dtype}")
+        if bias.dim() != 1 or bias.shape[0] != n or not bias.is_contiguous():
+            raise ValueError(f"the bias must be contiguous and 1-D with n = {n} elements, not of shape {tuple(bias.shape)}")
+    if scale_result is not None and (scale_result.dtype != torch.float32 or scale_result.numel() != 1):
+        raise ValueError(f"scale_result must be one float32 element, not {scale_result.dtype} of shape "
+                         f"{tuple(scale_result.shape)}")
+    if out is not None:
+        if out.dtype != out_dtype or tuple(out.shape) != (m, n):
+            raise ValueError(f"out must be {out_dtype} of shape {(m, n)}, not {out.dtype} of shape {tuple(out.shape)}")
+        if (n > 1 and out.stride(1) != 1) or (m > 1 and out.stride(0) < n):
+            raise ValueError(f"out must be row-major with rows that do not overlap, not of strides {tuple(out.stride())}")
+    qn = -(-n // 128)
+    if out_scale is not None:
+        if out_scale.dtype != torch.float32 or tuple(out_scale.shape) != (m, qn):
+            raise ValueError(f"out_scale must be float32 of shape {(m, qn)}, not {out_scale.dtype} of shape "
+                             f"{tuple(out_scale.shape)}")
+        sr_, sb_ = out_scale.stride()
+        row_major = (qn == 1 or sb_ == 1) and (m == 1 or sr_ >= qn)
+        col_major = (m == 1 or sr_ == 1) and (qn == 1 or sb_ >= m)
+        if not (row_major or col_major):
+            raise ValueError(f"out_scale must be row-major or outer-dim-major without overlap, not of strides "
+                             f"{tuple(out_scale.stride())}")
+    op_a, lda = operand_layout(tuple(A.shape), A.stride())
+    op_b, ldb = operand_layout(tuple(B.shape), B.stride())
+    tensors = [A, B, scale_a, scale_b] + [t for t in (bias, out, out_scale, scale_result) if t is not None]
+    if not all(t.is_cuda for t in tensors):
+        raise ValueError("A, B, the scales, the bias, scale_result, out and out_scale must be CUDA tensors")
+    if out is None:
+        out = torch.empty((m, n), dtype=out_dtype, device=A.device)
+    if dynamic and out_scale is None:
+        out_scale = torch.empty((m, qn), dtype=torch.float32, device=A.device)
+    if m == 0 or n == 0:
+        return out, out_scale
+    ct = FP8_E4M3 if out_dtype == torch.float8_e4m3fn else FP8_E5M2
+    act = ACTIVATIONS[activation]
+    bi = bias.data_ptr() if bias is not None else None
+    sr = scale_result.data_ptr() if scale_result is not None else None
+    sc, sc_row, sc_blk = (out_scale.data_ptr(), *out_scale.stride()) if dynamic else (None, 0, 0)
+    if blocks is not None:
+        _check(lib.b200_gemm_fp8_blockwise_q8(op_a, op_b, ta, tb, m, n, k, A.data_ptr(), lda, B.data_ptr(), ldb,
+                                              scale_a.data_ptr(), blocks[0], scale_a.stride(0), scale_a.stride(1),
+                                              scale_b.data_ptr(), blocks[1], scale_b.stride(0), scale_b.stride(1), bi,
+                                              act, ct, out.data_ptr(), _ld(out), sr, sc, sc_row, sc_blk,
+                                              _stream_ptr(stream)))
+    else:
+        _check(lib.b200_gemm_fp8_q8(op_a, op_b, ta, tb, m, n, k, A.data_ptr(), lda, B.data_ptr(), ldb, scale_a.data_ptr(),
+                                    rows[0], scale_b.data_ptr(), rows[1], bi, act, int(bool(use_fast_accum)), ct,
+                                    out.data_ptr(), _ld(out), sr, sc, sc_row, sc_blk, _stream_ptr(stream)))
+    return out, out_scale
+
+
+def scaled_mm_quant(A, B, scale_a, scale_b, bias=None, activation=None, out_dtype=None, use_fast_accum=False,
+                    out=None, out_scale=None, stream=None):
+    """scaled_mm with a fused 1 x 128 quantisation of its output: returns (C, scale_c) with C FP8 (out_dtype
+    torch.float8_e4m3fn, the default, or torch.float8_e5m2) and scale_c float32 (m, ceil(n / 128)), so that
+    C[i, j] * scale_c[i, j // 128] ~ act(A @ B * scales + bias)[i, j] (b200_gemm_fp8_q8 / b200_gemm_fp8_blockwise_q8,
+    dynamic mode).  Per row and 128-column block, d = amax / F (F = 448 or 57344; 1 for an all-zero block, NaN for a
+    block holding a NaN or an inf) and C = fp8(v / d).  (C, scale_c) is the (A, scale_a) of a following 1 x 128
+    blockwise scaled_mm: scaled_mm(C, W2.t(), scale_c, sW2) runs the next layer with no conversion in between.
+    A, B, scale_a, scale_b and use_fast_accum are scaled_mm's; bias is None or n contiguous bf16 values; activation
+    takes gemm()'s strings (None, "relu", "gelu", "gelu_tanh").  out_scale may be any (m, ceil(n / 128)) float32 view
+    that is row-major or outer-dim-major (torch's layout for scale_a); a new one is row-major.  The refusals are
+    scaled_mm's, and an out_scale of another shape, dtype or layout is a ValueError."""
+    import torch
+    out_dtype = out_dtype or (out.dtype if out is not None else torch.float8_e4m3fn)
+    return _scaled_mm_fp8_out(A, B, scale_a, scale_b, bias, activation, out_dtype, use_fast_accum, out, out_scale, None,
+                              stream, dynamic=True)
 
 
 def _fp8_in_place(name, t, ld, entry_stride, entry_elems):

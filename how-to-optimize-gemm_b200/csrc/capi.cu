@@ -414,7 +414,8 @@ int launch_tc(int m, int n, int k, const void* A, long long lda, int a_rows_tota
   using Cfg = TcConfig<KIND, BN, STAGES, Prod, A_ROW_BYTES, AL, BL>;
   using T = KindTraits<KIND>;
   constexpr bool FP8 = KIND == KIND_E4M3 || KIND == KIND_E4M3E5M2 || KIND == KIND_E5M2E4M3;
-  constexpr bool BLK = std::is_same<ScaleT, TcBlockScale>::value || std::is_same<ScaleT, TcStackBlockScale>::value;
+  constexpr bool BLK = std::is_same<ScaleT, TcBlockScale>::value || std::is_same<ScaleT, TcStackBlockScale>::value ||
+                      std::is_same<ScaleT, TcBlockScaleQ8>::value;
   constexpr int smem = Cfg::SMEM_BYTES + (BLK ? STAGES * kBlkScaleStageBytes : 0);
   constexpr CUtensorMapDataType dt = KIND == KIND_F16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
                                    : KIND == KIND_FP16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16
@@ -1474,7 +1475,8 @@ const char* const kFp8Names[3][3][5] = {FP8_NAMES("tc_e4m3"), FP8_NAMES("tc_e4m3
 // operands are made K-major and TMA-able in the workspace (stage_kmajor), which holds the same bytes, so every route is
 // bit-identical to the aligned (N, T) call.  fast: one accumulator over K at pick_bn's width; else promoted per
 // 128-element k-block (two 64 x BN fp32 tiles in registers: BN = 128).  Blockwise scales (Scale = TcBlockScale) are
-// always promoted; their indices are logical (row, k-block) / (k-block, column), so staging never touches them.
+// always promoted; their indices are logical (row, k-block) / (k-block, column), so staging never touches them.  An FP8
+// C (TcScaleQ8 / TcBlockScaleQ8) has no 192-wide tile: its 128-column scale blocks must not straddle tiles.
 template <int KIND, typename OutT, class Scale>
 int tc_fp8(int op_a, int op_b, int m, int n, int k, const void* A, long long lda, const void* B, long long ldb, void* C,
            int ldc, const Scale& sc, bool fast, const char* const (&names)[5], const Call& c) {
@@ -1482,10 +1484,10 @@ int tc_fp8(int op_a, int op_b, int m, int n, int k, const void* A, long long lda
   const bool copy_b = op_b && !(aligned16(B) && ldb % 16 == 0);
   const int sa = op_a || copy_a, sb = op_b && !copy_b;          // kmajor_ws_bytes / stage_kmajor's view of the layout
   auto run = [&](const void* a, long long la, const void* b, long long lb) {
-    constexpr bool blk = std::is_same<Scale, TcBlockScale>::value;
+    constexpr bool blk = std::is_same<Scale, TcBlockScale>::value || std::is_same<Scale, TcBlockScaleQ8>::value;
     if constexpr (!blk)
       if (fast)
-        return with_width(m, n, [&](auto W) {
+        return with_width<!Fp8Out<OutT>::V>(m, n, [&](auto W) {
           using Wd = decltype(W);
           return launch_tc<KIND, Wd::BN, Wd::STAGES, OutT>(m, n, k, a, la, m, 0, b, lb, n, 0, C, ldc, names[Wd::idx], c,
                                                            0, nullptr, nullptr, nullptr, &sc);
@@ -1528,20 +1530,30 @@ int fp8_run(int op_a, int op_b, int a_type, int b_type, int m, int n, int k, con
   return gemm_fp8_kind<KIND_E4M3>(op_a, op_b, m, n, k, A, lda, B, ldb, C, ldc, out_type, sc, fast_accum, c);
 }
 
-// C = round_out((op(A) op(B) * sa_i) * sb_j + bias_j); every argument is checked before the device is touched.
-int gemm_fp8(int op_a, int op_b, int a_type, int b_type, int m, int n, int k, const uint8_t* A, int lda, const uint8_t* B,
-             int ldb, const float* scale_a, int scale_a_rowwise, const float* scale_b, int scale_b_colwise,
-             const void* bias, void* C, int ldc, int out_type, int fast_accum, cudaStream_t st) {
+// b200_gemm_fp8's argument checks other than the output type, in its order: < 0 an error, 1 nothing to do, 0 run.
+int fp8_args(int op_a, int op_b, int a_type, int b_type, int m, int n, int k, const uint8_t* A, int lda, const uint8_t* B,
+             int ldb, const float* scale_a, int scale_a_rowwise, const float* scale_b, int scale_b_colwise, const void* C,
+             int ldc, int fast_accum) {
   auto fp8 = [](int t) { return t == B200_FP8_E4M3 || t == B200_FP8_E5M2; };
   if (!fp8(a_type) || !fp8(b_type)) return B200_ERR_BAD_ARG;
-  if (out_type != B200_OUT_F32 && out_type != B200_OUT_BF16 && out_type != B200_OUT_F16) return B200_ERR_BAD_ARG;
   if ((scale_a_rowwise != 0 && scale_a_rowwise != 1) || (scale_b_colwise != 0 && scale_b_colwise != 1)) return B200_ERR_BAD_ARG;
   if (fast_accum != 0 && fast_accum != 1) return B200_ERR_BAD_ARG;
   int rc = check_args(m, n, k, A, lda, B, ldb, C, ldc, op_a, op_b);
   if (rc < 0) return rc;
   if (a_type == B200_FP8_E5M2 && b_type == B200_FP8_E5M2) return B200_ERR_UNSUPPORTED;
-  if (rc == 1) return 0;
+  if (rc == 1) return 1;
   if (!scale_a || !scale_b) return B200_ERR_BAD_ARG;
+  return 0;
+}
+
+// C = round_out((op(A) op(B) * sa_i) * sb_j + bias_j); every argument is checked before the device is touched.
+int gemm_fp8(int op_a, int op_b, int a_type, int b_type, int m, int n, int k, const uint8_t* A, int lda, const uint8_t* B,
+             int ldb, const float* scale_a, int scale_a_rowwise, const float* scale_b, int scale_b_colwise,
+             const void* bias, void* C, int ldc, int out_type, int fast_accum, cudaStream_t st) {
+  if (out_type != B200_OUT_F32 && out_type != B200_OUT_BF16 && out_type != B200_OUT_F16) return B200_ERR_BAD_ARG;
+  if (int rc = fp8_args(op_a, op_b, a_type, b_type, m, n, k, A, lda, B, ldb, scale_a, scale_a_rowwise, scale_b,
+                        scale_b_colwise, C, ldc, fast_accum))
+    return rc < 0 ? rc : 0;
   return fp8_run(op_a, op_b, a_type, b_type, m, n, k, A, lda, B, ldb, C, ldc, out_type,
                  TcScale{scale_a, scale_b, scale_a_rowwise, scale_b_colwise, bias}, fast_accum, st);
 }
@@ -1553,30 +1565,130 @@ __int128 last_scale_index(long long rows, long long q, long long row_stride, lon
   return (__int128)(rows - 1) * row_stride + (__int128)(q > 0 ? q - 1 : 0) * kb_stride;
 }
 
-// C = round_out(sum + bias_j), sum = fma(acc_kb, rn(sa_kb(i) * sb_kb(j)), sum) over the k-blocks in order from +0;
-// every argument is checked before the device is touched.
-int gemm_fp8_blockwise(int op_a, int op_b, int a_type, int b_type, int m, int n, int k, const uint8_t* A, int lda,
+// b200_gemm_fp8_blockwise's argument checks other than the output type, in its order: < 0 an error, 1 nothing to do,
+// 0 run.
+int fp8_blockwise_args(int op_a, int op_b, int a_type, int b_type, int m, int n, int k, const uint8_t* A, int lda,
                        const uint8_t* B, int ldb, const float* scale_a, int a_blk, long long sa_row, long long sa_kb,
-                       const float* scale_b, int b_blk, long long sb_kb, long long sb_col, const void* bias, void* C,
-                       int ldc, int out_type, cudaStream_t st) {
+                       const float* scale_b, int b_blk, long long sb_kb, long long sb_col, const void* C, int ldc) {
   auto fp8 = [](int t) { return t == B200_FP8_E4M3 || t == B200_FP8_E5M2; };
   if (!fp8(a_type) || !fp8(b_type)) return B200_ERR_BAD_ARG;
-  if (out_type != B200_OUT_F32 && out_type != B200_OUT_BF16 && out_type != B200_OUT_F16) return B200_ERR_BAD_ARG;
   if ((a_blk != 1 && a_blk != 128) || (b_blk != 1 && b_blk != 128)) return B200_ERR_BAD_ARG;
   if (sa_row < 0 || sa_kb < 0 || sb_kb < 0 || sb_col < 0) return B200_ERR_BAD_ARG;
   int rc = check_args(m, n, k, A, lda, B, ldb, C, ldc, op_a, op_b);
   if (rc < 0) return rc;
   if (a_type == B200_FP8_E5M2 && b_type == B200_FP8_E5M2) return B200_ERR_UNSUPPORTED;
   if (a_blk == 128 && b_blk == 128) return B200_ERR_UNSUPPORTED;      // not a torch recipe
-  if (rc == 1) return 0;
+  if (rc == 1) return 1;
   if (!scale_a || !scale_b) return B200_ERR_BAD_ARG;
   const long long q = (k + 127LL) / 128;
   const __int128 max_index = INT64_MAX / 4;                           // the byte offset fits a signed 64-bit integer
   if (last_scale_index(a_blk == 1 ? m : (m + 127LL) / 128, q, sa_row, sa_kb) > max_index ||
       last_scale_index(b_blk == 1 ? n : (n + 127LL) / 128, q, sb_col, sb_kb) > max_index)
     return B200_ERR_BAD_ARG;
+  return 0;
+}
+
+// C = round_out(sum + bias_j), sum = fma(acc_kb, rn(sa_kb(i) * sb_kb(j)), sum) over the k-blocks in order from +0;
+// every argument is checked before the device is touched.
+int gemm_fp8_blockwise(int op_a, int op_b, int a_type, int b_type, int m, int n, int k, const uint8_t* A, int lda,
+                       const uint8_t* B, int ldb, const float* scale_a, int a_blk, long long sa_row, long long sa_kb,
+                       const float* scale_b, int b_blk, long long sb_kb, long long sb_col, const void* bias, void* C,
+                       int ldc, int out_type, cudaStream_t st) {
+  if (out_type != B200_OUT_F32 && out_type != B200_OUT_BF16 && out_type != B200_OUT_F16) return B200_ERR_BAD_ARG;
+  if (int rc = fp8_blockwise_args(op_a, op_b, a_type, b_type, m, n, k, A, lda, B, ldb, scale_a, a_blk, sa_row, sa_kb,
+                                  scale_b, b_blk, sb_kb, sb_col, C, ldc))
+    return rc < 0 ? rc : 0;
   return fp8_run(op_a, op_b, a_type, b_type, m, n, k, A, lda, B, ldb, C, ldc, out_type,
                  TcBlockScale{scale_a, scale_b, sa_row, sa_kb, sb_kb, sb_col, a_blk, b_blk, bias}, 0, st);
+}
+
+// ---- FP8 output (torch._scaled_mm's scale_result; the fused 1 x 128 quantisation of C) --------------------------------
+// Kernel names by [kind][C type: 0 = e4m3, 1 = e5m2][width index as kFp8Names; no 192-wide tile].
+#define FP8_Q8_NAMES(P)                                                                                               \
+  {{P "_oe4m3_128x256", nullptr, P "_oe4m3_128x128", P "_oe4m3_acc_128x128", P "_oe4m3_blk_128x128"},                 \
+   {P "_oe5m2_128x256", nullptr, P "_oe5m2_128x128", P "_oe5m2_acc_128x128", P "_oe5m2_blk_128x128"}}
+const char* const kFp8Q8Names[3][2][5] = {FP8_Q8_NAMES("tc_e4m3"), FP8_Q8_NAMES("tc_e4m3e5m2"),
+                                          FP8_Q8_NAMES("tc_e5m2e4m3")};
+
+// The output arguments of the _q8 entry points that need no sizes: C type, activation, mode and strides.
+int fp8_q8_out_args(int c_type, int act, const float* scale_result, const float* scale_c, long long sc_row,
+                    long long sc_blk) {
+  if (c_type != B200_FP8_E4M3 && c_type != B200_FP8_E5M2) return B200_ERR_BAD_ARG;
+  if (act < B200_ACT_NONE || act > B200_ACT_GELU_TANH) return B200_ERR_BAD_ARG;
+  if (scale_c && (scale_result || sc_row < 0 || sc_blk < 0)) return B200_ERR_BAD_ARG;
+  return 0;
+}
+// Dynamic mode with work to do: scale_c is row-major (m, q_n) (sc_blk == 1, sc_row >= q_n) or outer-dim-major
+// (sc_row == 1, sc_blk >= m), the stride of an extent-1 dimension being free; anything else could overlap.  The last
+// index's byte offset fits a signed 64-bit integer.
+bool fp8_q8_scale_layout_ok(int m, int n, long long sc_row, long long sc_blk) {
+  const long long qn = (n + 127LL) / 128;
+  const bool row_major = (qn == 1 || sc_blk == 1) && (m == 1 || sc_row >= qn);
+  const bool col_major = (m == 1 || sc_row == 1) && (qn == 1 || sc_blk >= m);
+  return (row_major || col_major) && last_scale_index(m, qn, sc_row, sc_blk) <= INT64_MAX / 4;
+}
+
+// k == 0: the element-wise pass (fp8_q8_k0_kernel), no operand and no input scale read.
+template <typename OutT>
+int fp8_q8_k0(int m, int n, void* C, int ldc, const void* bias, const TcQ8& q, cudaStream_t st) {
+  const long long items = (long long)m * ((n + 127) / 128);
+  const int blocks = (int)(items < 4096LL * 128 ? (items + 127) / 128 : 4096);
+  fp8_q8_k0_kernel<OutT><<<blocks, 128, 0, st>>>(m, n, static_cast<uint8_t*>(C), ldc,
+                                                 static_cast<const uint16_t*>(bias), q);
+  g_launches++;
+  t_last_kernel = "fp8_q8_k0";
+  return last_launch_status();
+}
+
+// Every FP8-output call after its argument checks (Scale = TcScaleQ8 or TcBlockScaleQ8): the routes of fp8_run.
+template <class Scale>
+int fp8_q8_run(int op_a, int op_b, int a_type, int b_type, int m, int n, int k, const uint8_t* A, int lda,
+               const uint8_t* B, int ldb, void* C, int ldc, int c_type, const Scale& sc, int fast_accum, cudaStream_t st) {
+  if (int rc = ensure_device()) return rc;
+  Call c{st};
+  const bool e4 = c_type == B200_FP8_E4M3;
+  if (k == 0)
+    return e4 ? fp8_q8_k0<e4m3_out>(m, n, C, ldc, sc.bias, sc.q, st) : fp8_q8_k0<e5m2_out>(m, n, C, ldc, sc.bias, sc.q, st);
+  auto kind = [&](auto K) {
+    constexpr int KIND = decltype(K)::value;
+    const auto& names = kFp8Q8Names[KIND - KIND_E4M3][e4 ? 0 : 1];
+    if (e4) return tc_fp8<KIND, e4m3_out>(op_a, op_b, m, n, k, A, lda, B, ldb, C, ldc, sc, fast_accum, names, c);
+    return tc_fp8<KIND, e5m2_out>(op_a, op_b, m, n, k, A, lda, B, ldb, C, ldc, sc, fast_accum, names, c);
+  };
+  if (a_type == B200_FP8_E5M2) return kind(std::integral_constant<int, KIND_E5M2E4M3>());
+  if (b_type == B200_FP8_E5M2) return kind(std::integral_constant<int, KIND_E4M3E5M2>());
+  return kind(std::integral_constant<int, KIND_E4M3>());
+}
+
+int gemm_fp8_q8(int op_a, int op_b, int a_type, int b_type, int m, int n, int k, const uint8_t* A, int lda,
+                const uint8_t* B, int ldb, const float* scale_a, int scale_a_rowwise, const float* scale_b,
+                int scale_b_colwise, const uint16_t* bias, int act, int fast_accum, int c_type, uint8_t* C, int ldc,
+                const float* scale_result, float* scale_c, long long sc_row, long long sc_blk, cudaStream_t st) {
+  if (int rc = fp8_q8_out_args(c_type, act, scale_result, scale_c, sc_row, sc_blk)) return rc;
+  if (int rc = fp8_args(op_a, op_b, a_type, b_type, m, n, k, A, lda, B, ldb, scale_a, scale_a_rowwise, scale_b,
+                        scale_b_colwise, C, ldc, fast_accum))
+    return rc < 0 ? rc : 0;
+  if (scale_c && !fp8_q8_scale_layout_ok(m, n, sc_row, sc_blk)) return B200_ERR_BAD_ARG;
+  TcScaleQ8 sc;
+  static_cast<TcScale&>(sc) = TcScale{scale_a, scale_b, scale_a_rowwise, scale_b_colwise, bias};
+  sc.q = TcQ8{scale_result, scale_c, sc_row, sc_blk, act};
+  return fp8_q8_run(op_a, op_b, a_type, b_type, m, n, k, A, lda, B, ldb, C, ldc, c_type, sc, fast_accum, st);
+}
+
+int gemm_fp8_blockwise_q8(int op_a, int op_b, int a_type, int b_type, int m, int n, int k, const uint8_t* A, int lda,
+                          const uint8_t* B, int ldb, const float* scale_a, int a_blk, long long sa_row, long long sa_kb,
+                          const float* scale_b, int b_blk, long long sb_kb, long long sb_col, const uint16_t* bias,
+                          int act, int c_type, uint8_t* C, int ldc, const float* scale_result, float* scale_c,
+                          long long sc_row, long long sc_blk, cudaStream_t st) {
+  if (int rc = fp8_q8_out_args(c_type, act, scale_result, scale_c, sc_row, sc_blk)) return rc;
+  if (int rc = fp8_blockwise_args(op_a, op_b, a_type, b_type, m, n, k, A, lda, B, ldb, scale_a, a_blk, sa_row, sa_kb,
+                                  scale_b, b_blk, sb_kb, sb_col, C, ldc))
+    return rc < 0 ? rc : 0;
+  if (scale_c && !fp8_q8_scale_layout_ok(m, n, sc_row, sc_blk)) return B200_ERR_BAD_ARG;
+  TcBlockScaleQ8 sc;
+  static_cast<TcBlockScale&>(sc) = TcBlockScale{scale_a, scale_b, sa_row, sa_kb, sb_kb, sb_col, a_blk, b_blk, bias};
+  sc.q = TcQ8{scale_result, scale_c, sc_row, sc_blk, act};
+  return fp8_q8_run(op_a, op_b, a_type, b_type, m, n, k, A, lda, B, ldb, C, ldc, c_type, sc, 0, st);
 }
 
 // ---- grouped and strided-batched FP8 GEMMs (torch._scaled_grouped_mm 2-D x 3-D and 3-D x 3-D) ---------------------------
@@ -2048,6 +2160,28 @@ int b200_gemm_fp8_blockwise(int op_a, int op_b, int a_type, int b_type, int m, i
   return gemm_fp8_blockwise(op_a, op_b, a_type, b_type, m, n, k, dA, lda, dB, ldb, dScaleA, scale_a_block, sa_row_stride,
                             sa_kb_stride, dScaleB, scale_b_block, sb_kb_stride, sb_col_stride, dBias, dC, ldc, out_type,
                             (cudaStream_t)stream);
+}
+
+int b200_gemm_fp8_q8(int op_a, int op_b, int a_type, int b_type, int m, int n, int k, const uint8_t* dA, int lda,
+                     const uint8_t* dB, int ldb, const float* dScaleA, int scale_a_rowwise, const float* dScaleB,
+                     int scale_b_colwise, const uint16_t* dBiasBf16, int act, int fast_accum, int c_type, uint8_t* dC,
+                     int ldc, const float* dScaleResult, float* dScaleC, long long sc_row_stride,
+                     long long sc_blk_stride, void* stream) {
+  return gemm_fp8_q8(op_a, op_b, a_type, b_type, m, n, k, dA, lda, dB, ldb, dScaleA, scale_a_rowwise, dScaleB,
+                     scale_b_colwise, dBiasBf16, act, fast_accum, c_type, dC, ldc, dScaleResult, dScaleC, sc_row_stride,
+                     sc_blk_stride, (cudaStream_t)stream);
+}
+
+int b200_gemm_fp8_blockwise_q8(int op_a, int op_b, int a_type, int b_type, int m, int n, int k, const uint8_t* dA,
+                               int lda, const uint8_t* dB, int ldb, const float* dScaleA, int scale_a_block,
+                               long long sa_row_stride, long long sa_kb_stride, const float* dScaleB, int scale_b_block,
+                               long long sb_kb_stride, long long sb_col_stride, const uint16_t* dBiasBf16, int act,
+                               int c_type, uint8_t* dC, int ldc, const float* dScaleResult, float* dScaleC,
+                               long long sc_row_stride, long long sc_blk_stride, void* stream) {
+  return gemm_fp8_blockwise_q8(op_a, op_b, a_type, b_type, m, n, k, dA, lda, dB, ldb, dScaleA, scale_a_block,
+                               sa_row_stride, sa_kb_stride, dScaleB, scale_b_block, sb_kb_stride, sb_col_stride,
+                               dBiasBf16, act, c_type, dC, ldc, dScaleResult, dScaleC, sc_row_stride, sc_blk_stride,
+                               (cudaStream_t)stream);
 }
 
 int b200_gemm_fp8_grouped(int a_type, int b_type, int total_m, int n, int k, const uint8_t* dA, int lda,

@@ -240,10 +240,17 @@ struct bf16_out {};   // tag: C stored as bf16 (RNE from the fp32 accumulator)
 struct f16_out {};    // tag: C stored as fp16 (RNE from the fp32 accumulator; beyond 65504 rounds to +-inf)
 struct s8_out {};     // tag: C stored as int8 through requant_s8 (TcParams::row_max = per-row scale,
                       // TcParams::col_max = per-row bias or null); int8 kernels only
+struct e4m3_out {};   // tag: C stored as FP8 E4M3 bytes (FP8 kernels: cvt.rn.satfinite, see fp8_q8_tile)
+struct e5m2_out {};   // tag: C stored as FP8 E5M2 bytes
 template <typename OutT> struct OutBytes { static constexpr int V = 4; };
 template <> struct OutBytes<bf16_out> { static constexpr int V = 2; };
 template <> struct OutBytes<f16_out> { static constexpr int V = 2; };
 template <> struct OutBytes<s8_out> { static constexpr int V = 1; };
+template <> struct OutBytes<e4m3_out> { static constexpr int V = 1; };
+template <> struct OutBytes<e5m2_out> { static constexpr int V = 1; };
+template <typename OutT> struct Fp8Out { static constexpr bool V = false; };
+template <> struct Fp8Out<e4m3_out> { static constexpr bool V = true; static constexpr float MAX = 448.f; };
+template <> struct Fp8Out<e5m2_out> { static constexpr bool V = true; static constexpr float MAX = 57344.f; };
 
 __device__ __forceinline__ uint32_t cvt_bf16x2(float lo, float hi) {
   uint32_t r;
@@ -651,7 +658,7 @@ struct TcScale {
   const float* a;          // [m] or [1]
   const float* b;          // [n] or [1]
   int a_step, b_step;      // 0 = tensorwise, 1 = one scale per row of A / column of B
-  const void* bias;        // [n] of C's type (bf16 / fp16 bits, or fp32), null = none
+  const void* bias;        // [n] of C's type (bf16 / fp16 bits, or fp32; bf16 for an FP8 C), null = none
 };
 
 // Blockwise scales (BLOCKWISE kernels, torch._scaled_mm's 1 x 128 / 128 x 128 recipes): k-block kb (K elements
@@ -684,6 +691,89 @@ struct TcStackBlockScale : TcBlockScale {
   TcStack st;
   long long a_entry_stride, b_entry_stride;
 };
+// FP8 output (OutT e4m3_out / e5m2_out, single-matrix kernels): each element's fp32 value v is the existing kernels'
+// value before round_out (tensorwise / rowwise: act(rn(rn(rn(acc * sa_i) * sb_j) + bias_j)); blockwise:
+// act(rn(sum + bias_j))), with a bf16 bias (TcScale::bias / TcBlockScale::bias, n bf16 values, null = none).  Then
+//   static (scale_c null):  c = fp8(rn(v / s_r)), s_r = *scale_result read on the device, null = 1;
+//   dynamic 1 x 128:        d = rn(amax / F) over the row's 128-column block (1 when that is 0, NaN when the block holds
+//                           a NaN or an inf), c = fp8(rn(v / d)), d stored at scale_c[i * sc_row + blk * sc_blk].
+// fp8() is cvt.rn.satfinite: a finite value past the format's largest F (448, 57344) becomes +-F, NaN stays NaN.
+// Their own argument types, so that TcScale and TcBlockScale, and the existing FP8 kernels, keep their layout and code.
+struct TcQ8 {
+  const float* scale_result;
+  float* scale_c;
+  long long sc_row, sc_blk;  // element strides of scale_c per row and per 128-column block
+  int act;                   // an EpiAct, uniform per launch
+};
+struct TcScaleQ8 : TcScale { TcQ8 q; };
+struct TcBlockScaleQ8 : TcBlockScale { TcQ8 q; };
+
+// Two fp32 values as two FP8 bytes (lo in the low byte), round to nearest even, finite values saturated.
+template <typename OutT>
+__device__ __forceinline__ uint32_t cvt_fp8x2(float lo, float hi) {
+  uint16_t r;
+  if constexpr (std::is_same<OutT, e4m3_out>::value)
+    asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(r) : "f"(hi), "f"(lo));
+  else
+    asm("cvt.rn.satfinite.e5m2x2.f32 %0, %1, %2;" : "=h"(r) : "f"(hi), "f"(lo));
+  return r;
+}
+// max that returns NaN when either input is NaN (fmaxf drops it): a block's amax carries its NaN
+__device__ __forceinline__ float fmax_nan(float a, float b) {
+  float r;
+  asm("max.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
+  return r;
+}
+// The dynamic scale of a block from its amax: NaN for a NaN or inf amax, else rn(amax / F), 1 when that is 0.
+template <typename OutT>
+__device__ __forceinline__ float q8_block_scale(float amax) {
+  const float d = __fdiv_rn(amax, Fp8Out<OutT>::MAX);
+  return !(amax <= 3.402823466e38f) ? __uint_as_float(0x7FC00000u) : d == 0.f ? 1.f : d;
+}
+// One FP8 pair (col, col + 1) of row `row` into C at byte pitch p.ldc: a 2-byte store where the address allows (any
+// base and pitch work).
+template <typename OutT>
+__device__ __forceinline__ void store_fp8_pair(const TcParams& p, int row, int col, float y0, float y1) {
+  const uint32_t w = cvt_fp8x2<OutT>(y0, y1);
+  uint8_t* dst = static_cast<uint8_t*>(p.C) + (long long)row * p.ldc + col;
+  if (col + 1 < p.N && (reinterpret_cast<uintptr_t>(dst) & 1) == 0) {
+    *reinterpret_cast<uint16_t*>(dst) = (uint16_t)w;
+  } else {
+    dst[0] = (uint8_t)w;
+    if (col + 1 < p.N) dst[1] = (uint8_t)(w >> 8);
+  }
+}
+
+// k == 0 with an FP8 output: v = act(rn(+0 + bias_j)) quantised as fp8_q8_tile does, one thread per row and 128-column
+// block, reading no operand and no input scale.
+template <typename OutT>
+__global__ void fp8_q8_k0_kernel(int m, int n, uint8_t* C, long long ldc, const uint16_t* bias, TcQ8 q) {
+  const int qn = (n + 127) / 128;
+  const long long items = (long long)m * qn;
+  const bool dyn = q.scale_c != nullptr;
+  const float sr = !dyn && q.scale_result != nullptr ? *q.scale_result : 1.f;
+  TcParams p;
+  p.C = C; p.ldc = ldc; p.N = n;
+  for (long long it = blockIdx.x * (long long)blockDim.x + threadIdx.x; it < items; it += (long long)gridDim.x * blockDim.x) {
+    const int row = (int)(it / qn), blk = (int)(it % qn);
+    const int c0 = 128 * blk, c1 = min(c0 + 128, n);
+    auto val = [&](int j) {
+      const float t = __fadd_rn(0.f, bias != nullptr ? __uint_as_float((uint32_t)bias[j] << 16) : -0.f);
+      switch (q.act) {
+        case ACT_RELU: return epi_act<ACT_RELU>(t);
+        case ACT_GELU: return epi_act<ACT_GELU>(t);
+        case ACT_GELU_TANH: return epi_act<ACT_GELU_TANH>(t);
+        default: return t;
+      }
+    };
+    float amax = 0.f;
+    for (int j = c0; j < c1; j++) amax = fmax_nan(amax, fabsf(val(j)));
+    const float d = dyn ? q8_block_scale<OutT>(amax) : sr;
+    for (int j = c0; j < c1; j += 2)
+      store_fp8_pair<OutT>(p, row, j, __fdiv_rn(val(j), d), j + 1 < c1 ? __fdiv_rn(val(j + 1), d) : 0.f);
+    if (dyn) q.scale_c[row * q.sc_row + blk * q.sc_blk] = d;
+  }
+}
 // Shared memory of one stage's block scales: 128 floats of A (one per tile row), then 128 of B (one per tile column).
 constexpr int kBlkScaleStageBytes = 2 * 128 * 4;
 
@@ -796,6 +886,112 @@ __device__ __forceinline__ int fp8_num_tiles(const TcParams& p, const Scale& sc)
   }
 }
 
+// The GELUs of fp8_q8_tile on the thread's NX values, rolled: each trip applies epi_act to x[0 .. 3] and rotates the
+// array by four, so after NX / 4 trips every value has its activation and is back in place.  Fully unrolled (NX
+// inlined erfcf / tanhf evaluations), the scheduler's interleaving of the evaluations ran the blockwise kernels out of
+// registers; rolled, every FP8-output kernel has 0 spill bytes, at the same time per tile (DESIGN §9).
+template <int ACT, int NX>
+__device__ __forceinline__ void q8_gelu_rolled(float (&x)[NX]) {
+  static_assert(NX % 4 == 0, "groups of four");
+#pragma unroll 1
+  for (int r = 0; r < NX / 4; r++) {
+    float y[4];
+#pragma unroll
+    for (int i = 0; i < 4; i++) y[i] = epi_act<ACT>(x[i]);
+#pragma unroll
+    for (int i = 0; i < NX - 4; i++) x[i] = x[i + 4];
+#pragma unroll
+    for (int i = 0; i < 4; i++) x[NX - 4 + i] = y[i];
+  }
+}
+
+// The FP8-output store of one consumer thread's part of a tile (TcQ8).  x holds the thread's accumulators (wgmma's
+// m64nN layout: x[4j + 2h + e] is row row0 + 8h, column col0 + 8j + e, and the quad of lanes 4r .. 4r + 3 holds all
+// columns of its rows), so each 128-column block of a row lies in one quad: j in [16 cb, 16 cb + 16).  Pass 1
+// overwrites x with v: the scaling, the bias and ReLU unrolled, the GELUs rolled (q8_gelu_rolled).  Each row-block's
+// NaN-carrying amax is then taken over columns < N only; the quad's amax is two shfl.xor steps.  Pass 2 divides,
+// converts and stores rows < M and columns < N; lane 4r writes its rows' scales.  The activation is the launch's
+// run-time code, tested once per tile: the store is one copy, not one per activation.
+template <int BN, typename OutT, bool BLOCKWISE, class Scale, int NX>
+__device__ __forceinline__ void fp8_q8_tile(const TcParams& p, const Scale& sc, float (&x)[NX], int row0, int col0,
+                                            int lane) {
+  constexpr int NB = BN / 128;
+  static_assert(BN % 128 == 0 && NX == BN / 2, "whole 128-column blocks per tile");
+  const int act = sc.q.act;
+  float sa[2] = {0.f, 0.f};
+  if constexpr (!BLOCKWISE) {
+#pragma unroll
+    for (int h = 0; h < 2; h++)
+      if (row0 + 8 * h < p.M) sa[h] = __ldg(sc.a + (long long)(row0 + 8 * h) * sc.a_step);
+  }
+  const unsigned short* bias = static_cast<const unsigned short*>(sc.bias);
+#pragma unroll
+  for (int j = 0; j < BN / 8; j++) {
+    const int col = col0 + 8 * j;
+    float sb[2] = {0.f, 0.f}, bi[2] = {-0.f, -0.f};
+#pragma unroll
+    for (int e = 0; e < 2; e++) {
+      if (col + e >= p.N) continue;
+      if constexpr (!BLOCKWISE) sb[e] = __ldg(sc.b + (long long)(col + e) * sc.b_step);
+      if (bias != nullptr) bi[e] = __uint_as_float((uint32_t)__ldg(bias + col + e) << 16);
+    }
+#pragma unroll
+    for (int h = 0; h < 2; h++)
+#pragma unroll
+      for (int e = 0; e < 2; e++) {
+        const int i = 4 * j + 2 * h + e;
+        const float t = __fadd_rn(BLOCKWISE ? x[i] : __fmul_rn(__fmul_rn(x[i], sa[h]), sb[e]), bi[e]);
+        x[i] = act == ACT_RELU && t < 0.f ? 0.f : t;                      // epi_act<ACT_RELU>, bit for bit
+      }
+  }
+  if (act == ACT_GELU) q8_gelu_rolled<ACT_GELU>(x);
+  else if (act == ACT_GELU_TANH) q8_gelu_rolled<ACT_GELU_TANH>(x);
+  float amax[NB][2];
+#pragma unroll
+  for (int cb = 0; cb < NB; cb++) amax[cb][0] = amax[cb][1] = 0.f;
+#pragma unroll
+  for (int j = 0; j < BN / 8; j++)
+#pragma unroll
+    for (int h = 0; h < 2; h++)
+#pragma unroll
+      for (int e = 0; e < 2; e++)
+        if (col0 + 8 * j + e < p.N) amax[j / 16][h] = fmax_nan(amax[j / 16][h], fabsf(x[4 * j + 2 * h + e]));
+  const bool dyn = sc.q.scale_c != nullptr;
+  float d[NB][2];
+  if (dyn) {
+#pragma unroll
+    for (int cb = 0; cb < NB; cb++)
+#pragma unroll
+      for (int h = 0; h < 2; h++) {
+        float a = amax[cb][h];
+        a = fmax_nan(a, __shfl_xor_sync(0xFFFFFFFFu, a, 1));
+        a = fmax_nan(a, __shfl_xor_sync(0xFFFFFFFFu, a, 2));
+        d[cb][h] = q8_block_scale<OutT>(a);
+      }
+  } else {
+    const float sr = sc.q.scale_result != nullptr ? __ldg(sc.q.scale_result) : 1.f;
+#pragma unroll
+    for (int cb = 0; cb < NB; cb++) d[cb][0] = d[cb][1] = sr;
+  }
+#pragma unroll
+  for (int j = 0; j < BN / 8; j++)
+#pragma unroll
+    for (int h = 0; h < 2; h++) {
+      const int row = row0 + 8 * h, col = col0 + 8 * j;
+      if (row >= p.M || col >= p.N) continue;
+      const float dd = d[j / 16][h];
+      store_fp8_pair<OutT>(p, row, col, __fdiv_rn(x[4 * j + 2 * h], dd), __fdiv_rn(x[4 * j + 2 * h + 1], dd));
+    }
+  if (dyn && (lane & 3) == 0) {
+#pragma unroll
+    for (int cb = 0; cb < NB; cb++)
+#pragma unroll
+      for (int h = 0; h < 2; h++)
+        if (row0 + 8 * h < p.M && col0 + 128 * cb < p.N)
+          sc.q.scale_c[(long long)(row0 + 8 * h) * sc.q.sc_row + (long long)(col0 / 128 + cb) * sc.q.sc_blk] = d[cb][h];
+  }
+}
+
 // BLOCKWISE = true: the blockwise-scaled kernels (ProdPromoted, BN = 128, argument TcBlockScale, shared memory
 // Cfg::SMEM_BYTES + STAGES * kBlkScaleStageBytes).  The TMA thread and the MMA chain are unchanged; warps 1 and 2 load
 // the stage's scales (fp8_block_scale_loader), whose copies also arrive on the stage's full barrier, and each consumer
@@ -816,13 +1012,17 @@ template <int KIND, int BN, int STAGES, typename OutT, class Prod, bool BLOCKWIS
 __global__ void __launch_bounds__((TcConfig<KIND, BN, STAGES, Prod, 128>::THREADS), 1)
 gemm_tc_fp8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const TcParams p,
                    const typename std::conditional<
-                       BLOCKWISE, typename std::conditional<STACK != STACK_NONE, TcStackBlockScale, TcBlockScale>::type,
-                       typename std::conditional<STACK != STACK_NONE, TcStackScale, TcScale>::type>::type sc) {
+                       Fp8Out<OutT>::V, typename std::conditional<BLOCKWISE, TcBlockScaleQ8, TcScaleQ8>::type,
+                       typename std::conditional<
+                           BLOCKWISE, typename std::conditional<STACK != STACK_NONE, TcStackBlockScale, TcBlockScale>::type,
+                           typename std::conditional<STACK != STACK_NONE, TcStackScale, TcScale>::type>::type>::type sc) {
   using Cfg = TcConfig<KIND, BN, STAGES, Prod, 128>;
   using MMA = typename Cfg::MMA;
   static_assert(KIND == KIND_E4M3 || KIND == KIND_E4M3E5M2 || KIND == KIND_E5M2E4M3, "FP8 kinds");
   static_assert(!Cfg::A_MN && !Cfg::B_MN && Prod::NPA == 1 && Prod::NPB == 1, "FP8: K-major A and B, one plane");
-  static_assert(std::is_same<OutT, float>::value || OutBytes<OutT>::V == 2, "FP8: fp32, bf16 or fp16 C");
+  static_assert(std::is_same<OutT, float>::value || OutBytes<OutT>::V == 2 || Fp8Out<OutT>::V, "FP8: fp32, 16-bit or FP8 C");
+  static_assert(!Fp8Out<OutT>::V || (STACK == STACK_NONE && BN % 128 == 0),
+                "FP8 C: single-matrix kernels, tiles of whole 128-column scale blocks");
   static_assert(!BLOCKWISE || (std::is_same<Prod, ProdPromoted>::value && BN == 128 && Cfg::BK == 128),
                 "blockwise scales: one 128-element k-block per promotion, tiles on the 128 x 128 scale blocks");
   static_assert(!BLOCKWISE || Cfg::SMEM_BYTES + STAGES * kBlkScaleStageBytes <= 232448, "blockwise: shared memory");
@@ -989,6 +1189,12 @@ gemm_tc_fp8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
       // ---- this warp's 16 rows of the tile into C: (acc * sa) * sb (BLOCKWISE: sum), then + bias in store_pair ----
       const int row0 = m0 + ew * 16 + (lane >> 2);
       const int col0 = n0 + 2 * (lane & 3);
+      if constexpr (Fp8Out<OutT>::V) {
+        // FP8 C (TcQ8): v, then the static or dynamic quantisation, in fp8_q8_tile
+        if constexpr (Cfg::REGACC) fp8_q8_tile<BN, OutT, BLOCKWISE>(p, sc, sum, row0, col0, lane);
+        else fp8_q8_tile<BN, OutT, BLOCKWISE>(p, sc, acc, row0, col0, lane);
+        continue;
+      }
       if constexpr (BLOCKWISE && STACK != STACK_NONE) {
         // the entry's C and rows, as below; the blockwise sum is stored as is (no bias)
         const StackEntry se = stack_entry<STACK>(w, p, sc.st, fp8_group_table<0>(), fp8_group_table<1>());

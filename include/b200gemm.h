@@ -491,6 +491,43 @@ int b200_gemm_fp8_blockwise(int op_a, int op_b, int a_type, int b_type, int m, i
                             const float* dScaleB, int scale_b_block, long long sb_kb_stride, long long sb_col_stride,
                             const void* dBias, void* dC, int ldc, int out_type, void* stream);
 
+/* ---- FP8 outputs of the FP8 GEMMs (torch._scaled_mm's scale_result; a fused 1 x 128 quantisation of C) ------------
+ * Each element first gets the fp32 value v that b200_gemm_fp8 / b200_gemm_fp8_blockwise form before round_out:
+ *   b200_gemm_fp8_q8:            v = act(rn(rn(rn(acc * sa_i) * sb_j) + bias_j))
+ *   b200_gemm_fp8_blockwise_q8:  v = act(rn(sum + bias_j)), sum the blockwise FMA fold
+ * dBiasBf16 is null (then -0 is added) or n bf16 values; act is a B200_ACT_* code, the fp32 activation of the 16-bit
+ * epilogue.  c_type is B200_FP8_E4M3 (F = 448) or B200_FP8_E5M2 (F = 57344); C is m rows of ldc >= n bytes, any base
+ * and any pitch.  fp8() below is round to nearest even with finite values past +-F saturated to +-F and NaN kept NaN.
+ *   Static mode (dScaleC null): c_ij = fp8(rn(v_ij / s_r)), s_r = *dScaleResult (fp32 on the device, never read by the
+ *     host), null = 1.  The rule is torch._scaled_mm's scale_result: torch's CPU kernel divides by it, and torch on CUDA
+ *     saturates an FP8 output (measured with torch 2.11+cu128 on an H100 80GB HBM3; that build ignores scale_result on
+ *     CUDA with tensorwise scales, so it equals this call only for s_r = 1.  DESIGN §9).
+ *   Dynamic 1 x 128 mode (dScaleC non-null, dScaleResult must be null): for row i and column block c (columns
+ *     [128 c, min(128 c + 128, n))), amax = max |v| over the block, d = rn(amax / F), d = 1 when that is 0, d = NaN when
+ *     the block holds a NaN or an inf (all its elements are then NaN); c_ij = fp8(rn(v_ij / d)) and
+ *     dScaleC[i * sc_row_stride + c * sc_blk_stride] = d.  (C, dScaleC) is then the (A, scale_a) of a following
+ *     b200_gemm_fp8_blockwise call with scale_a_block = 1 and k = n.  The scale layout is row-major (m, q_n)
+ *     (sc_blk_stride == 1, sc_row_stride >= q_n) or outer-dim-major (sc_row_stride == 1, sc_blk_stride >= m), q_n =
+ *     ceil(n / 128), the stride of an extent-1 dimension being free; anything else is B200_ERR_BAD_ARG.
+ * Everything else (operand pairs, input scales, op_a / op_b, pitches, routes and workspace, fast_accum, the argument
+ * checks before the device is touched) is b200_gemm_fp8's / b200_gemm_fp8_blockwise's.  m == 0 or n == 0 is a no-op;
+ * k == 0 quantises v = act(rn(+0 + bias_j)) in an element-wise pass that reads no operand and no input scale.  Tiles:
+ * promoted 128 x 128, fast 128 x 256 or 128 x 128 (no 192-wide tile: it would split a 128-column block), blockwise
+ * 128 x 128.  Kernels: "tc_e4m3_oe4m3_acc_128x128", "tc_e4m3e5m2_oe5m2_128x256", "tc_e4m3_oe4m3_blk_128x128", ... */
+int b200_gemm_fp8_q8(int op_a, int op_b, int a_type, int b_type, int m, int n, int k,
+                     const uint8_t* dA, int lda, const uint8_t* dB, int ldb,
+                     const float* dScaleA, int scale_a_rowwise, const float* dScaleB, int scale_b_colwise,
+                     const uint16_t* dBiasBf16, int act, int fast_accum, int c_type, uint8_t* dC, int ldc,
+                     const float* dScaleResult, float* dScaleC, long long sc_row_stride, long long sc_blk_stride,
+                     void* stream);
+int b200_gemm_fp8_blockwise_q8(int op_a, int op_b, int a_type, int b_type, int m, int n, int k,
+                               const uint8_t* dA, int lda, const uint8_t* dB, int ldb,
+                               const float* dScaleA, int scale_a_block, long long sa_row_stride, long long sa_kb_stride,
+                               const float* dScaleB, int scale_b_block, long long sb_kb_stride, long long sb_col_stride,
+                               const uint16_t* dBiasBf16, int act, int c_type, uint8_t* dC, int ldc,
+                               const float* dScaleResult, float* dScaleC, long long sc_row_stride,
+                               long long sc_blk_stride, void* stream);
+
 /* ---- Grouped and batched FP8 GEMMs (torch._scaled_grouped_mm 2-D x 3-D and 3-D x 3-D; FP8 mixture-of-experts layers) --
  * Every entry is one (N, T) b200_gemm_fp8 call with rowwise scales and no bias, all of them in one launch:
  *   C_e = round_out( (A_e B_e^T * sa_e[i]) * sb_e[j] )
