@@ -34,7 +34,8 @@ EXPORTS = [
     "b200_gemm_bf16_grouped", "b200_gemm_f16_grouped", "b200_gemm_bf16_grouped_k", "b200_gemm_f16_grouped_k",
     "b200_gemm_s8s32_op", "b200_gemm_workspace_bytes_op", "b200_gemm_fp8", "b200_gemm_fp8_blockwise",
     "b200_gemm_fp8_grouped", "b200_gemm_fp8_batched", "b200_gemm_fp8_blockwise_grouped", "b200_gemm_fp8_blockwise_batched",
-    "b200_gemm_fp8_q8", "b200_gemm_fp8_blockwise_q8",
+    "b200_gemm_fp8_q8", "b200_gemm_fp8_blockwise_q8", "b200_gemm_fp8_grouped_q8", "b200_gemm_fp8_batched_q8",
+    "b200_gemm_fp8_blockwise_grouped_q8", "b200_gemm_fp8_blockwise_batched_q8",
     "b200_nccl_load", "b200_nccl_last_error", "b200_comm_unique_id", "b200_comm_init_rank",
     "b200_comm_destroy", "b200_rowpanel_create", "b200_rowpanel_destroy", "b200_rowpanel_slices", "b200_rowpanel_set_reserve_sms", "b200_rowpanel_trace", "b200_rowpanel_trace_dump", "b200_gemm_f32_rowpanel",
     "b200_gemm_f32_rowpanel_host", "b200_gemm_f32_pack_a", "b200_gemm_f32_packed_ab", "b200_gemm_f32_pack_free_a",
@@ -117,6 +118,15 @@ lib.b200_gemm_fp8_q8.argtypes = [_i, _i, _i, _i, _i, _i, _i, _vp, _i, _vp, _i, _
                                  _vp, _ll, _ll, _vp]
 lib.b200_gemm_fp8_blockwise_q8.argtypes = [_i, _i, _i, _i, _i, _i, _i, _vp, _i, _vp, _i, _vp, _i, _ll, _ll, _vp, _i, _ll,
                                            _ll, _vp, _i, _i, _vp, _i, _vp, _vp, _ll, _ll, _vp]
+lib.b200_gemm_fp8_grouped_q8.argtypes = [_i, _i, _i, _i, _i, _vp, _i, _vp, _i, _ll, _vp, _i, _vp, _vp, _ll, _i, _i, _i, _vp,
+                                         _i, _vp, _ll, _ll, _vp]
+lib.b200_gemm_fp8_batched_q8.argtypes = [_i, _i, _i, _i, _i, _vp, _i, _ll, _vp, _i, _ll, _vp, _ll, _vp, _ll, _i, _i, _i,
+                                         _vp, _i, _ll, _vp, _ll, _ll, _ll, _i, _vp]
+lib.b200_gemm_fp8_blockwise_grouped_q8.argtypes = [_i, _i, _i, _i, _i, _vp, _i, _vp, _i, _ll, _vp, _i, _vp, _ll, _ll, _vp,
+                                                   _i, _ll, _ll, _ll, _i, _i, _vp, _i, _vp, _ll, _ll, _vp]
+lib.b200_gemm_fp8_blockwise_batched_q8.argtypes = [_i, _i, _i, _i, _i, _vp, _i, _ll, _vp, _i, _ll, _vp, _i, _ll, _ll, _ll,
+                                                   _vp, _i, _ll, _ll, _ll, _i, _i, _vp, _i, _ll, _vp, _ll, _ll, _ll, _i,
+                                                   _vp]
 lib.b200_gemm_workspace_bytes_op.restype = C.c_size_t
 lib.b200_gemm_f32_pack_b.argtypes = [_i, _i, _vp, _i, _i, C.POINTER(_vp), _vp]
 lib.b200_gemm_f32_packed.argtypes = [_i, _i, _i, _vp, _i, _vp, _vp, _i, _i, _vp]
@@ -774,6 +784,62 @@ def scaled_grouped_mm(A, B, scale_a, scale_b, offs=None, out_dtype=None, use_fas
     entry), another scale, offs, out_dtype or out, or a CPU tensor is a ValueError."""
     import torch
     out_dtype = out_dtype or (out.dtype if out is not None else torch.bfloat16)
+    g = _scaled_grouped_args(A, B, scale_a, scale_b, offs, out_dtype, use_fast_accum, out, fp8_out=False)
+    tensors = [A, B, scale_a, scale_b] + [t for t in (offs, out) if t is not None]
+    if not all(t.is_cuda for t in tensors):
+        raise ValueError("A, B, the scales, offs and out must be CUDA tensors")
+    if out is None:
+        out = torch.empty(g.shape, dtype=out_dtype, device=A.device)
+    if g.groups == 0 or out.numel() == 0:
+        return out
+    g.check_in_place(A, B)
+    ta, tb, groups, n, k, lda, ldb, sb, ssb, blocks = g.ta, g.tb, g.groups, g.n, g.k, g.lda, g.ldb, g.sb, g.ssb, g.blocks
+    ot = {torch.float32: OUT_F32, torch.bfloat16: OUT_BF16, torch.float16: OUT_F16}[out_dtype]
+    fast = int(bool(use_fast_accum))
+    if blocks is not None and A.dim() == 2:
+        _check(lib.b200_gemm_fp8_blockwise_grouped(ta, tb, g.m, n, k, A.data_ptr(), lda, B.data_ptr(), ldb, sb,
+                                                   offs.data_ptr(), groups, scale_a.data_ptr(), scale_a.stride(0),
+                                                   scale_a.stride(1), scale_b.data_ptr(), blocks[1], scale_b.stride(1),
+                                                   scale_b.stride(2), ssb, out.data_ptr(), _ld(out), ot,
+                                                   _stream_ptr(stream)))
+    elif blocks is not None:
+        _check(lib.b200_gemm_fp8_blockwise_batched(ta, tb, g.m, n, k, A.data_ptr(), lda, A.stride(0) if groups > 1 else 0,
+                                                   B.data_ptr(), ldb, sb, scale_a.data_ptr(), blocks[0],
+                                                   scale_a.stride(1), scale_a.stride(2),
+                                                   scale_a.stride(0) if groups > 1 else 0, scale_b.data_ptr(), blocks[1],
+                                                   scale_b.stride(1), scale_b.stride(2), ssb, out.data_ptr(),
+                                                   _ld(out[0]), out.stride(0) if groups > 1 else 0, groups, ot,
+                                                   _stream_ptr(stream)))
+    elif A.dim() == 2:
+        _check(lib.b200_gemm_fp8_grouped(ta, tb, g.m, n, k, A.data_ptr(), lda, B.data_ptr(), ldb, sb,
+                                         offs.data_ptr(), groups, scale_a.data_ptr(), scale_b.data_ptr(), ssb,
+                                         out.data_ptr(), _ld(out), ot, fast, _stream_ptr(stream)))
+    else:
+        _check(lib.b200_gemm_fp8_batched(ta, tb, g.m, n, k, A.data_ptr(), lda, A.stride(0) if groups > 1 else 0,
+                                         B.data_ptr(), ldb, sb, scale_a.data_ptr(),
+                                         scale_a.stride(0) if groups > 1 else 0, scale_b.data_ptr(), ssb,
+                                         out.data_ptr(), _ld(out[0]), out.stride(0) if groups > 1 else 0, groups, ot,
+                                         fast, _stream_ptr(stream)))
+    return out
+
+
+class _GroupedArgs:
+    """The operands of a scaled_grouped_mm / scaled_grouped_mm_quant call as the C ABI reads them."""
+
+    def __init__(self, **kw):
+        self.__dict__.update(kw)
+
+    def check_in_place(self, A, B):
+        if self.k > 0:
+            _fp8_in_place("A", A, self.lda, A.stride(0) if A.dim() == 3 and self.groups > 1 else 0, A.shape[-2] * self.lda)
+            _fp8_in_place("B", B, self.ldb, self.sb, self.n * self.ldb)
+
+
+def _scaled_grouped_args(A, B, scale_a, scale_b, offs, out_dtype, use_fast_accum, out, fp8_out):
+    """scaled_grouped_mm's shape resolution and refusals, in its order, for a 16-bit / fp32 (fp8_out False) or an FP8
+    out_dtype; every check but the operands' in-place rule (check_in_place), which applies only with work to do, and
+    the callers' check that every tensor is on the GPU."""
+    import torch
     ta, tb = _fp8_type(A), _fp8_type(B)
     if ta is None or tb is None:
         raise TypeError(f"operands must be float8_e4m3fn or float8_e5m2, not {A.dtype} and {B.dtype}")
@@ -786,7 +852,9 @@ def scaled_grouped_mm(A, B, scale_a, scale_b, offs=None, out_dtype=None, use_fas
     groups, k, n = B.shape
     if A.shape[-1] != k:
         raise ValueError(f"contraction dimensions differ: A is {tuple(A.shape)}, B is {tuple(B.shape)}")
-    if out_dtype not in (torch.bfloat16, torch.float16, torch.float32):
+    if fp8_out and not _is_fp8(out_dtype):
+        raise ValueError(f"out_dtype must be float8_e4m3fn or float8_e5m2, not {out_dtype}")
+    if not fp8_out and out_dtype not in (torch.bfloat16, torch.float16, torch.float32):
         raise ValueError(f"out_dtype must be bfloat16, float16 or float32, not {out_dtype}")
     try:
         op_a, lda = operand_layout(tuple(A.shape[-2:]), A.stride()[-2:])
@@ -821,10 +889,10 @@ def scaled_grouped_mm(A, B, scale_a, scale_b, offs=None, out_dtype=None, use_fas
             raise ValueError(f"offs has {offs.numel()} elements for {groups} groups of B")
         if groups > 1 and sb < n * ldb:
             raise ValueError(f"the groups of B must not overlap or be broadcast (stride(0) = {B.stride(0)})")
-        total_m = A.shape[0]
-        if blocks is None and (scale_a.dim() != 1 or scale_a.shape[0] != total_m or not scale_a.is_contiguous()):
-            raise ValueError(f"scale_a must be contiguous and 1-D with {total_m} elements, not {tuple(scale_a.shape)}")
-        shape = (total_m, n)
+        m = A.shape[0]
+        if blocks is None and (scale_a.dim() != 1 or scale_a.shape[0] != m or not scale_a.is_contiguous()):
+            raise ValueError(f"scale_a must be contiguous and 1-D with {m} elements, not {tuple(scale_a.shape)}")
+        shape = (m, n)
     else:
         if offs is not None:
             raise ValueError("offs must be None for a 3-D A: every entry has its own rows")
@@ -843,43 +911,87 @@ def scaled_grouped_mm(A, B, scale_a, scale_b, offs=None, out_dtype=None, use_fas
             raise ValueError(f"out must be row-major with rows that do not overlap, not of strides {tuple(out.stride())}")
         if len(shape) == 3 and groups > 1 and rows * cols > 0 and out.stride(0) < (rows - 1) * out.stride(1) + cols:
             raise ValueError(f"the entries of out must not overlap (stride(0) = {out.stride(0)})")
-    tensors = [A, B, scale_a, scale_b] + [t for t in (offs, out) if t is not None]
+    return _GroupedArgs(ta=ta, tb=tb, groups=groups, m=m, n=n, k=k, lda=lda, ldb=ldb, sb=sb, ssb=ssb, blocks=blocks,
+                        shape=shape)
+
+
+def scaled_grouped_mm_quant(A, B, scale_a, scale_b, offs=None, activation=None, out_dtype=None, use_fast_accum=False,
+                            out=None, out_scale=None, stream=None):
+    """scaled_grouped_mm with a fused 1 x 128 quantisation of every group's or entry's output: returns (C, scale_c)
+    with C FP8 (out_dtype torch.float8_e4m3fn, the default, or torch.float8_e5m2) and scale_c float32, (total_m,
+    ceil(n / 128)) for a 2-D A and (G, m, ceil(n / 128)) for a 3-D A (b200_gemm_fp8_grouped_q8 / _batched_q8 /
+    _blockwise_grouped_q8 / _blockwise_batched_q8).  Each group or entry is bit for bit scaled_mm_quant on its own
+    rows, B and scales without bias: per row and 128-column block d = amax / F (F = 448 or 57344; 1 for an all-zero
+    block, NaN for a block holding a NaN or an inf) and C = fp8(v / d), v = act(the fp32 value scaled_grouped_mm rounds).
+    A 2-D A's scale_c is indexed by the row of C, so scaled_grouped_mm(C, W2.transpose(-2, -1), scale_c, sW2, offs)
+    runs the next layer with no conversion; rows from offs[-1] on are written in neither.
+    A, B, scale_a, scale_b, offs, use_fast_accum, out and the refusals are scaled_grouped_mm's; activation takes
+    gemm()'s strings (None, "relu", "gelu", "gelu_tanh").  out_scale may be any float32 view of scale_c's shape whose
+    last two dimensions are row-major or outer-dim-major (for a 3-D A, entries that do not overlap); a new one is
+    row-major.  Another out_scale or activation is a ValueError."""
+    import torch
+    out_dtype = out_dtype or (out.dtype if out is not None else torch.float8_e4m3fn)
+    if activation not in ACTIVATIONS:
+        raise ValueError(f"activation must be one of {sorted(a for a in ACTIVATIONS if a)} or None, not {activation!r}")
+    g = _scaled_grouped_args(A, B, scale_a, scale_b, offs, out_dtype, use_fast_accum, out, fp8_out=True)
+    groups, n, k = g.groups, g.n, g.k
+    qn = -(-n // 128)
+    sc_shape = g.shape[:-1] + (qn,)
+    if out_scale is not None:
+        if out_scale.dtype != torch.float32 or tuple(out_scale.shape) != sc_shape:
+            raise ValueError(f"out_scale must be float32 of shape {sc_shape}, not {out_scale.dtype} of shape "
+                             f"{tuple(out_scale.shape)}")
+        rows = sc_shape[-2]
+        sr_, sb_ = out_scale.stride()[-2:]
+        row_major = (qn == 1 or sb_ == 1) and (rows == 1 or sr_ >= qn)
+        col_major = (rows == 1 or sr_ == 1) and (qn == 1 or sb_ >= rows)
+        if not (row_major or col_major):
+            raise ValueError(f"out_scale must be row-major or outer-dim-major without overlap in its last two "
+                             f"dimensions, not of strides {tuple(out_scale.stride())}")
+        if (len(sc_shape) == 3 and groups > 1 and rows * qn > 0 and
+                out_scale.stride(0) < (rows - 1) * sr_ + (qn - 1) * sb_ + 1):
+            raise ValueError(f"the entries of out_scale must not overlap (stride(0) = {out_scale.stride(0)})")
+    tensors = [A, B, scale_a, scale_b] + [t for t in (offs, out, out_scale) if t is not None]
     if not all(t.is_cuda for t in tensors):
-        raise ValueError("A, B, the scales, offs and out must be CUDA tensors")
+        raise ValueError("A, B, the scales, offs, out and out_scale must be CUDA tensors")
     if out is None:
-        out = torch.empty(shape, dtype=out_dtype, device=A.device)
+        out = torch.empty(g.shape, dtype=out_dtype, device=A.device)
+    if out_scale is None:
+        out_scale = torch.empty(sc_shape, dtype=torch.float32, device=A.device)
     if groups == 0 or out.numel() == 0:
-        return out
-    if k > 0:
-        _fp8_in_place("A", A, lda, A.stride(0) if A.dim() == 3 and groups > 1 else 0, A.shape[-2] * lda)
-        _fp8_in_place("B", B, ldb, sb, n * ldb)
-    ot = {torch.float32: OUT_F32, torch.bfloat16: OUT_BF16, torch.float16: OUT_F16}[out_dtype]
+        return out, out_scale
+    g.check_in_place(A, B)
+    ta, tb, lda, ldb, sb, ssb, blocks = g.ta, g.tb, g.lda, g.ldb, g.sb, g.ssb, g.blocks
+    ct = FP8_E4M3 if out_dtype == torch.float8_e4m3fn else FP8_E5M2
+    act = ACTIVATIONS[activation]
     fast = int(bool(use_fast_accum))
-    if blocks is not None and A.dim() == 2:
-        _check(lib.b200_gemm_fp8_blockwise_grouped(ta, tb, total_m, n, k, A.data_ptr(), lda, B.data_ptr(), ldb, sb,
-                                                   offs.data_ptr(), groups, scale_a.data_ptr(), scale_a.stride(0),
-                                                   scale_a.stride(1), scale_b.data_ptr(), blocks[1], scale_b.stride(1),
-                                                   scale_b.stride(2), ssb, out.data_ptr(), _ld(out), ot,
-                                                   _stream_ptr(stream)))
-    elif blocks is not None:
-        _check(lib.b200_gemm_fp8_blockwise_batched(ta, tb, m, n, k, A.data_ptr(), lda, A.stride(0) if groups > 1 else 0,
-                                                   B.data_ptr(), ldb, sb, scale_a.data_ptr(), blocks[0],
-                                                   scale_a.stride(1), scale_a.stride(2),
-                                                   scale_a.stride(0) if groups > 1 else 0, scale_b.data_ptr(), blocks[1],
-                                                   scale_b.stride(1), scale_b.stride(2), ssb, out.data_ptr(),
-                                                   _ld(out[0]), out.stride(0) if groups > 1 else 0, groups, ot,
-                                                   _stream_ptr(stream)))
-    elif A.dim() == 2:
-        _check(lib.b200_gemm_fp8_grouped(ta, tb, total_m, n, k, A.data_ptr(), lda, B.data_ptr(), ldb, sb,
-                                         offs.data_ptr(), groups, scale_a.data_ptr(), scale_b.data_ptr(), ssb,
-                                         out.data_ptr(), _ld(out), ot, fast, _stream_ptr(stream)))
+    sc_row, sc_blk = out_scale.stride()[-2:]
+    st = _stream_ptr(stream)
+    if A.dim() == 2:
+        if blocks is not None:
+            _check(lib.b200_gemm_fp8_blockwise_grouped_q8(
+                ta, tb, g.m, n, k, A.data_ptr(), lda, B.data_ptr(), ldb, sb, offs.data_ptr(), groups, scale_a.data_ptr(),
+                scale_a.stride(0), scale_a.stride(1), scale_b.data_ptr(), blocks[1], scale_b.stride(1), scale_b.stride(2),
+                ssb, act, ct, out.data_ptr(), _ld(out), out_scale.data_ptr(), sc_row, sc_blk, st))
+        else:
+            _check(lib.b200_gemm_fp8_grouped_q8(ta, tb, g.m, n, k, A.data_ptr(), lda, B.data_ptr(), ldb, sb,
+                                                offs.data_ptr(), groups, scale_a.data_ptr(), scale_b.data_ptr(), ssb, act,
+                                                fast, ct, out.data_ptr(), _ld(out), out_scale.data_ptr(), sc_row, sc_blk,
+                                                st))
+        return out, out_scale
+    sa_e, c_e, sc_e = ((A.stride(0), out.stride(0), out_scale.stride(0)) if groups > 1 else (0, 0, 0))
+    if blocks is not None:
+        _check(lib.b200_gemm_fp8_blockwise_batched_q8(
+            ta, tb, g.m, n, k, A.data_ptr(), lda, sa_e, B.data_ptr(), ldb, sb, scale_a.data_ptr(), blocks[0],
+            scale_a.stride(1), scale_a.stride(2), scale_a.stride(0) if groups > 1 else 0, scale_b.data_ptr(), blocks[1],
+            scale_b.stride(1), scale_b.stride(2), ssb, act, ct, out.data_ptr(), _ld(out[0]), c_e, out_scale.data_ptr(),
+            sc_row, sc_blk, sc_e, groups, st))
     else:
-        _check(lib.b200_gemm_fp8_batched(ta, tb, m, n, k, A.data_ptr(), lda, A.stride(0) if groups > 1 else 0,
-                                         B.data_ptr(), ldb, sb, scale_a.data_ptr(),
-                                         scale_a.stride(0) if groups > 1 else 0, scale_b.data_ptr(), ssb,
-                                         out.data_ptr(), _ld(out[0]), out.stride(0) if groups > 1 else 0, groups, ot,
-                                         fast, _stream_ptr(stream)))
-    return out
+        _check(lib.b200_gemm_fp8_batched_q8(ta, tb, g.m, n, k, A.data_ptr(), lda, sa_e, B.data_ptr(), ldb, sb,
+                                            scale_a.data_ptr(), scale_a.stride(0) if groups > 1 else 0,
+                                            scale_b.data_ptr(), ssb, act, fast, ct, out.data_ptr(), _ld(out[0]), c_e,
+                                            out_scale.data_ptr(), sc_row, sc_blk, sc_e, groups, st))
+    return out, out_scale
 
 
 def gemm_f32(A, B, out=None, mode=F32_AUTO, stream=None, accumulate=False):

@@ -396,7 +396,8 @@ int g_ffma_halves = 1;        // strict kernel: split the tail round into half t
 // FP8 kinds (KIND_E4M3, ...): gemm_tc_fp8_kernel with the scales and bias *scl; K-major A and B, no K split.  A
 // TcBlockScale (ScaleT) selects its blockwise-scaled form, whose stages carry their scales in shared memory; STACK_GROUP
 // / STACK_BATCH with a TcStackScale its stacked form (the stack as above, the rowwise scales of every entry in *scl),
-// and with a TcStackBlockScale its stacked blockwise form.
+// and with a TcStackBlockScale its stacked blockwise form.  A TcStackScaleQ8 / TcStackBlockScaleQ8 (FP8 C) selects
+// gemm_tc_fp8_q8_stacked_kernel, the same body.
 struct Stack {
   int count;               // entries of a batch, or groups
   long long sa, sb, sc;    // elements between consecutive entries of A, B and C
@@ -415,7 +416,8 @@ int launch_tc(int m, int n, int k, const void* A, long long lda, int a_rows_tota
   using T = KindTraits<KIND>;
   constexpr bool FP8 = KIND == KIND_E4M3 || KIND == KIND_E4M3E5M2 || KIND == KIND_E5M2E4M3;
   constexpr bool BLK = std::is_same<ScaleT, TcBlockScale>::value || std::is_same<ScaleT, TcStackBlockScale>::value ||
-                      std::is_same<ScaleT, TcBlockScaleQ8>::value;
+                      std::is_same<ScaleT, TcBlockScaleQ8>::value || std::is_same<ScaleT, TcStackBlockScaleQ8>::value;
+  constexpr bool STACK_Q8 = std::is_same<ScaleT, TcStackScaleQ8>::value || std::is_same<ScaleT, TcStackBlockScaleQ8>::value;
   constexpr int smem = Cfg::SMEM_BYTES + (BLK ? STAGES * kBlkScaleStageBytes : 0);
   constexpr CUtensorMapDataType dt = KIND == KIND_F16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
                                    : KIND == KIND_FP16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16
@@ -465,7 +467,8 @@ int launch_tc(int m, int n, int k, const void* A, long long lda, int a_rows_tota
   if constexpr (EPI) p.bias = c.bias;            // shares col_max's slot: EPI kernels are never scaled
   p.stream_c = g_stream_c < 0 ? (g_stream_c = (getenv("B200GEMM_STREAM_C") ? atoi(getenv("B200GEMM_STREAM_C")) : kStreamCDefault)) : g_stream_c;
   auto kern = [] {
-    if constexpr (FP8) return gemm_tc_fp8_kernel<KIND, BN, STAGES, OutT, Prod, BLK, STACK>;
+    if constexpr (STACK_Q8) return gemm_tc_fp8_q8_stacked_kernel<KIND, BN, STAGES, OutT, Prod, BLK, STACK>;
+    else if constexpr (FP8) return gemm_tc_fp8_kernel<KIND, BN, STAGES, OutT, Prod, BLK, STACK>;
     else if constexpr (STACK != STACK_NONE) return gemm_tc_stacked_kernel<KIND, BN, STAGES, OutT, AL, BL, STACK>;
     else return gemm_tc_kernel<KIND, BN, STAGES, OutT, Prod, A_ROW_BYTES, AL, BL, EPI>;
   }();
@@ -1708,18 +1711,18 @@ const char* const kFp8StackNames[2][3][3][5] = {
     {FP8_STACK_NAMES("tc_e4m3", "bat"), FP8_STACK_NAMES("tc_e4m3e5m2", "bat"), FP8_STACK_NAMES("tc_e5m2e4m3", "bat")}};
 
 // The stacked call *stk (m = total_m for a grouped call) at pick_bn's width over the stack's tiles (fast), or promoted
-// per 128-element k-block at BN = 128, as tc_fp8 chooses for one matrix.  Blockwise scales (Scale = TcStackBlockScale)
-// are always promoted.
+// per 128-element k-block at BN = 128, as tc_fp8 chooses for one matrix.  Blockwise scales (Scale = TcStackBlockScale
+// / TcStackBlockScaleQ8) are always promoted.  An FP8 C has no 192-wide tile, as in tc_fp8.
 template <int KIND, typename OutT, int STACK, class Scale>
 int tc_fp8_stacked(int m, int n, int k, const void* A, int lda, const void* B, int ldb, void* C, int ldc,
                    const Stack& stk, const Scale& sc, bool fast, const char* const (&names)[5], const Call& c) {
-  constexpr bool blk = std::is_same<Scale, TcStackBlockScale>::value;
+  constexpr bool blk = std::is_same<Scale, TcStackBlockScale>::value || std::is_same<Scale, TcStackBlockScaleQ8>::value;
   // m rows of A per entry (a grouped A is one entry of total_m rows); every B entry is n x k
   if constexpr (!blk)
     if (fast) {
       const int bn_m = STACK == STACK_GROUP ? 128 : m;
       const int bn_batch = STACK == STACK_GROUP ? (int)grouped_tile_rows(m, stk.count) : stk.count;
-      return with_width(bn_m, n, [&](auto W) {
+      return with_width<!Fp8Out<OutT>::V>(bn_m, n, [&](auto W) {
         using Wd = decltype(W);
         return launch_tc<KIND, Wd::BN, Wd::STAGES, OutT, ProdSingle, 128, LAYOUT_K, LAYOUT_K, false, STACK>(
             m, n, k, A, lda, m, 0, B, ldb, n, 0, C, ldc, names[Wd::idx], c, 0, nullptr, nullptr, &stk, &sc);
@@ -1756,11 +1759,14 @@ int fp8_stacked_run(int a_type, int b_type, int m, int n, int k, const uint8_t* 
 }
 
 // The checks every stacked FP8 call shares: operand types, output type and fast_accum are B200_ERR_BAD_ARG, and
-// (e5m2, e5m2) is B200_ERR_UNSUPPORTED, as for b200_gemm_fp8.
-int fp8_stacked_types(int a_type, int b_type, int out_type, int fast_accum) {
+// (e5m2, e5m2) is B200_ERR_UNSUPPORTED, as for b200_gemm_fp8.  The output type is checked by the entry points (the
+// _q8 ones take an FP8 C type instead); the rest here.
+bool fp8_out_type_ok(int out_type) {
+  return out_type == B200_OUT_F32 || out_type == B200_OUT_BF16 || out_type == B200_OUT_F16;
+}
+int fp8_stacked_types(int a_type, int b_type, int fast_accum) {
   auto fp8 = [](int t) { return t == B200_FP8_E4M3 || t == B200_FP8_E5M2; };
   if (!fp8(a_type) || !fp8(b_type)) return B200_ERR_BAD_ARG;
-  if (out_type != B200_OUT_F32 && out_type != B200_OUT_BF16 && out_type != B200_OUT_F16) return B200_ERR_BAD_ARG;
   if (fast_accum != 0 && fast_accum != 1) return B200_ERR_BAD_ARG;
   return 0;
 }
@@ -1775,17 +1781,17 @@ bool fp8_in_place(const void* A, long long lda, const void* B, long long ldb) {
 // on sizes, groups, offsets, overlap and the tile bound for an op_b = T call, negative scale_b_stride or one whose last
 // group's offset exceeds 2^60 elements, null scales with work to do (B200_ERR_BAD_ARG); operands not read in place
 // (B200_ERR_UNSUPPORTED).  groups == 0, total_m == 0 or n == 0 is a no-op.
-int gemm_fp8_grouped(int a_type, int b_type, int total_m, int n, int k, const uint8_t* A, int lda, const uint8_t* B,
+// fp8_grouped_args: b200_gemm_fp8_grouped's checks other than the output type, in its order: < 0 an error, 1 nothing
+// to do, 0 run.
+int fp8_grouped_args(int a_type, int b_type, int total_m, int n, int k, const uint8_t* A, int lda, const uint8_t* B,
                      int ldb, long long stride_b, const int32_t* offs, int groups, const float* scale_a,
-                     const float* scale_b, long long scale_b_stride, void* C, int ldc, int out_type, int fast_accum,
-                     cudaStream_t st) {
-  if (int rc = fp8_stacked_types(a_type, b_type, out_type, fast_accum)) return rc;
+                     const float* scale_b, long long scale_b_stride, const void* C, int ldc, int fast_accum) {
+  if (int rc = fp8_stacked_types(a_type, b_type, fast_accum)) return rc;
   if (groups < 0 || stride_b < 0 || scale_b_stride < 0 || groups > kMaxGroups) return B200_ERR_BAD_ARG;
   if (total_m < 0 || n < 0 || k < 0) return B200_ERR_BAD_ARG;
   if (a_type == B200_FP8_E5M2 && b_type == B200_FP8_E5M2) return B200_ERR_UNSUPPORTED;
-  if (groups == 0) return 0;
+  if (groups == 0) return 1;
   int rc = check_args(total_m, n, k, A, lda, B, ldb, C, ldc, B200_OP_N, B200_OP_T);
-  if (rc == 1) return 0;
   if (rc) return rc;
   if (!offs || !scale_a || !scale_b) return B200_ERR_BAD_ARG;
   if (groups > 1) {
@@ -1796,12 +1802,29 @@ int gemm_fp8_grouped(int a_type, int b_type, int total_m, int n, int k, const ui
   if (tiles_n > 0x3FFFFFFFLL / grouped_tile_rows(total_m, groups)) return B200_ERR_BAD_ARG;
   if (k > 0 && (!fp8_in_place(A, lda, B, ldb) || (groups > 1 && !batch_tma_ok(stride_b, n, ldb, 1))))
     return B200_ERR_UNSUPPORTED;
-  const Stack gr{groups, 0, groups > 1 ? stride_b : 0, 0, offs};
+  return 0;
+}
+TcStackScale fp8_grouped_scale(const float* scale_a, const float* scale_b, long long scale_b_stride) {
   TcStackScale sc{};
   sc.a = scale_a; sc.b = scale_b; sc.a_step = 1; sc.b_step = 1; sc.bias = nullptr;
   sc.a_entry_stride = 0; sc.b_entry_stride = scale_b_stride;
-  return fp8_stacked_run<STACK_GROUP>(a_type, b_type, total_m, n, k, A, lda, B, ldb, C, ldc, out_type, gr, sc, fast_accum,
-                                      st);
+  return sc;
+}
+Stack fp8_grouped_stack(int groups, long long stride_b, const int32_t* offs) {
+  return Stack{groups, 0, groups > 1 ? stride_b : 0, 0, offs};
+}
+
+int gemm_fp8_grouped(int a_type, int b_type, int total_m, int n, int k, const uint8_t* A, int lda, const uint8_t* B,
+                     int ldb, long long stride_b, const int32_t* offs, int groups, const float* scale_a,
+                     const float* scale_b, long long scale_b_stride, void* C, int ldc, int out_type, int fast_accum,
+                     cudaStream_t st) {
+  if (!fp8_out_type_ok(out_type)) return B200_ERR_BAD_ARG;
+  if (int rc = fp8_grouped_args(a_type, b_type, total_m, n, k, A, lda, B, ldb, stride_b, offs, groups, scale_a, scale_b,
+                                scale_b_stride, C, ldc, fast_accum))
+    return rc < 0 ? rc : 0;
+  return fp8_stacked_run<STACK_GROUP>(a_type, b_type, total_m, n, k, A, lda, B, ldb, C, ldc, out_type,
+                                      fp8_grouped_stack(groups, stride_b, offs),
+                                      fp8_grouped_scale(scale_a, scale_b, scale_b_stride), fast_accum, st);
 }
 
 // C_b = round_out((A_b B_b^T * sa_b[i]) * sb_b[j]) for b < batch, X_b = X + b * stride_x, sa_b = scale_a + b *
@@ -1810,18 +1833,19 @@ int gemm_fp8_grouped(int a_type, int b_type, int total_m, int n, int k, const ui
 // the scale strides bounded like the operand strides, null scales with work to do (B200_ERR_BAD_ARG); operands not read
 // in place, an input stride other than 0 or at least one entry included (B200_ERR_UNSUPPORTED).  batch == 0, m == 0 or
 // n == 0 is a no-op; batch == 1 is the (N, T) b200_gemm_fp8 call with rowwise scales.
-int gemm_fp8_batched(int a_type, int b_type, int m, int n, int k, const uint8_t* A, int lda, long long stride_a,
+// fp8_batched_args: b200_gemm_fp8_batched's checks other than the output type, in its order: < 0 an error, 1 nothing
+// to do, 0 run.
+int fp8_batched_args(int a_type, int b_type, int m, int n, int k, const uint8_t* A, int lda, long long stride_a,
                      const uint8_t* B, int ldb, long long stride_b, const float* scale_a, long long scale_a_stride,
-                     const float* scale_b, long long scale_b_stride, void* C, int ldc, long long stride_c, int batch,
-                     int out_type, int fast_accum, cudaStream_t st) {
-  if (int rc = fp8_stacked_types(a_type, b_type, out_type, fast_accum)) return rc;
+                     const float* scale_b, long long scale_b_stride, const void* C, int ldc, long long stride_c,
+                     int batch, int fast_accum) {
+  if (int rc = fp8_stacked_types(a_type, b_type, fast_accum)) return rc;
   if (batch < 0 || stride_a < 0 || stride_b < 0 || stride_c < 0 || scale_a_stride < 0 || scale_b_stride < 0)
     return B200_ERR_BAD_ARG;
   if (m < 0 || n < 0 || k < 0) return B200_ERR_BAD_ARG;
   if (a_type == B200_FP8_E5M2 && b_type == B200_FP8_E5M2) return B200_ERR_UNSUPPORTED;
-  if (batch == 0) return 0;
+  if (batch == 0) return 1;
   int rc = check_args(m, n, k, A, lda, B, ldb, C, ldc, B200_OP_N, B200_OP_T);
-  if (rc == 1) return 0;
   if (rc) return rc;
   if (!scale_a || !scale_b) return B200_ERR_BAD_ARG;
   if (batch > 1) {
@@ -1836,14 +1860,30 @@ int gemm_fp8_batched(int a_type, int b_type, int m, int n, int k, const uint8_t*
   if (k > 0 && (!fp8_in_place(A, lda, B, ldb) ||
                 (batch > 1 && (!batch_tma_ok(stride_a, m, lda, 1) || !batch_tma_ok(stride_b, n, ldb, 1)))))
     return B200_ERR_UNSUPPORTED;
-  if (batch == 1)
-    return gemm_fp8(B200_OP_N, B200_OP_T, a_type, b_type, m, n, k, A, lda, B, ldb, scale_a, 1, scale_b, 1, nullptr, C, ldc,
-                    out_type, fast_accum, st);
-  const Stack bt{batch, stride_a, stride_b, stride_c, nullptr};
+  return 0;
+}
+TcStackScale fp8_batched_scale(const float* scale_a, long long scale_a_stride, const float* scale_b,
+                               long long scale_b_stride) {
   TcStackScale sc{};
   sc.a = scale_a; sc.b = scale_b; sc.a_step = 1; sc.b_step = 1; sc.bias = nullptr;
   sc.a_entry_stride = scale_a_stride; sc.b_entry_stride = scale_b_stride;
-  return fp8_stacked_run<STACK_BATCH>(a_type, b_type, m, n, k, A, lda, B, ldb, C, ldc, out_type, bt, sc, fast_accum, st);
+  return sc;
+}
+
+int gemm_fp8_batched(int a_type, int b_type, int m, int n, int k, const uint8_t* A, int lda, long long stride_a,
+                     const uint8_t* B, int ldb, long long stride_b, const float* scale_a, long long scale_a_stride,
+                     const float* scale_b, long long scale_b_stride, void* C, int ldc, long long stride_c, int batch,
+                     int out_type, int fast_accum, cudaStream_t st) {
+  if (!fp8_out_type_ok(out_type)) return B200_ERR_BAD_ARG;
+  if (int rc = fp8_batched_args(a_type, b_type, m, n, k, A, lda, stride_a, B, ldb, stride_b, scale_a, scale_a_stride,
+                                scale_b, scale_b_stride, C, ldc, stride_c, batch, fast_accum))
+    return rc < 0 ? rc : 0;
+  if (batch == 1)
+    return gemm_fp8(B200_OP_N, B200_OP_T, a_type, b_type, m, n, k, A, lda, B, ldb, scale_a, 1, scale_b, 1, nullptr, C, ldc,
+                    out_type, fast_accum, st);
+  return fp8_stacked_run<STACK_BATCH>(a_type, b_type, m, n, k, A, lda, B, ldb, C, ldc, out_type,
+                                      Stack{batch, stride_a, stride_b, stride_c, nullptr},
+                                      fp8_batched_scale(scale_a, scale_a_stride, scale_b, scale_b_stride), fast_accum, st);
 }
 
 // ---- grouped and strided-batched blockwise FP8 GEMMs (DeepSeek-V3-style MoE layers) -----------------------------------
@@ -1860,20 +1900,19 @@ __int128 last_stacked_scale_index(long long count, long long entry_stride, long 
 // Rows [end_{g-1}, end_g) of C = the blockwise product of those rows of A with B_g = B + g * stride_b (n x k); scale_a
 // is 1 x 128 over the stacked A (row i of A: scale_a[i * sa_row + kb * sa_kb]; a 128-row block would straddle groups),
 // scale_b of group g starts at scale_b + g * scale_b_stride, 1 x 128 or 128 x 128 (b_blk).
-int gemm_fp8_blockwise_grouped(int a_type, int b_type, int total_m, int n, int k, const uint8_t* A, int lda,
+// fp8_blockwise_grouped_args: its checks other than the output type, in its order: < 0 an error, 1 nothing to do, 0 run.
+int fp8_blockwise_grouped_args(int a_type, int b_type, int total_m, int n, int k, const uint8_t* A, int lda,
                                const uint8_t* B, int ldb, long long stride_b, const int32_t* offs, int groups,
                                const float* scale_a, long long sa_row, long long sa_kb, const float* scale_b, int b_blk,
-                               long long sb_kb, long long sb_col, long long scale_b_stride, void* C, int ldc,
-                               int out_type, cudaStream_t st) {
-  if (int rc = fp8_stacked_types(a_type, b_type, out_type, 0)) return rc;
+                               long long sb_kb, long long sb_col, long long scale_b_stride, const void* C, int ldc) {
+  if (int rc = fp8_stacked_types(a_type, b_type, 0)) return rc;
   if (b_blk != 1 && b_blk != 128) return B200_ERR_BAD_ARG;
   if (sa_row < 0 || sa_kb < 0 || sb_kb < 0 || sb_col < 0 || scale_b_stride < 0) return B200_ERR_BAD_ARG;
   if (groups < 0 || stride_b < 0 || groups > kMaxGroups) return B200_ERR_BAD_ARG;
   if (total_m < 0 || n < 0 || k < 0) return B200_ERR_BAD_ARG;
   if (a_type == B200_FP8_E5M2 && b_type == B200_FP8_E5M2) return B200_ERR_UNSUPPORTED;
-  if (groups == 0) return 0;
+  if (groups == 0) return 1;
   int rc = check_args(total_m, n, k, A, lda, B, ldb, C, ldc, B200_OP_N, B200_OP_T);
-  if (rc == 1) return 0;
   if (rc) return rc;
   if (!offs || !scale_a || !scale_b) return B200_ERR_BAD_ARG;
   if (groups > 1) {
@@ -1889,23 +1928,42 @@ int gemm_fp8_blockwise_grouped(int a_type, int b_type, int total_m, int n, int k
     return B200_ERR_BAD_ARG;
   if (k > 0 && (!fp8_in_place(A, lda, B, ldb) || (groups > 1 && !batch_tma_ok(stride_b, n, ldb, 1))))
     return B200_ERR_UNSUPPORTED;
-  const Stack gr{groups, 0, groups > 1 ? stride_b : 0, 0, offs};
+  return 0;
+}
+TcStackBlockScale fp8_blockwise_stack_scale(const float* scale_a, int a_blk, long long sa_row, long long sa_kb,
+                                            long long scale_a_stride, const float* scale_b, int b_blk, long long sb_kb,
+                                            long long sb_col, long long scale_b_stride) {
   TcStackBlockScale sc{};
   sc.a = scale_a; sc.b = scale_b; sc.a_row = sa_row; sc.a_kb = sa_kb; sc.b_kb = sb_kb; sc.b_col = sb_col;
-  sc.a_blk = 1; sc.b_blk = b_blk; sc.bias = nullptr;
-  sc.a_entry_stride = 0; sc.b_entry_stride = scale_b_stride;
-  return fp8_stacked_run<STACK_GROUP>(a_type, b_type, total_m, n, k, A, lda, B, ldb, C, ldc, out_type, gr, sc, 0, st);
+  sc.a_blk = a_blk; sc.b_blk = b_blk; sc.bias = nullptr;
+  sc.a_entry_stride = scale_a_stride; sc.b_entry_stride = scale_b_stride;
+  return sc;
+}
+
+int gemm_fp8_blockwise_grouped(int a_type, int b_type, int total_m, int n, int k, const uint8_t* A, int lda,
+                               const uint8_t* B, int ldb, long long stride_b, const int32_t* offs, int groups,
+                               const float* scale_a, long long sa_row, long long sa_kb, const float* scale_b, int b_blk,
+                               long long sb_kb, long long sb_col, long long scale_b_stride, void* C, int ldc,
+                               int out_type, cudaStream_t st) {
+  if (!fp8_out_type_ok(out_type)) return B200_ERR_BAD_ARG;
+  if (int rc = fp8_blockwise_grouped_args(a_type, b_type, total_m, n, k, A, lda, B, ldb, stride_b, offs, groups, scale_a,
+                                          sa_row, sa_kb, scale_b, b_blk, sb_kb, sb_col, scale_b_stride, C, ldc))
+    return rc < 0 ? rc : 0;
+  return fp8_stacked_run<STACK_GROUP>(
+      a_type, b_type, total_m, n, k, A, lda, B, ldb, C, ldc, out_type, fp8_grouped_stack(groups, stride_b, offs),
+      fp8_blockwise_stack_scale(scale_a, 1, sa_row, sa_kb, 0, scale_b, b_blk, sb_kb, sb_col, scale_b_stride), 0, st);
 }
 
 // C_b = the blockwise product of A_b = A + b * stride_a (m x k) and B_b = B + b * stride_b (n x k), C_b = C + b *
 // stride_c, with entry b's scales at scale_a + b * scale_a_stride and scale_b + b * scale_b_stride, each indexed as by
 // gemm_fp8_blockwise.  batch == 1 is the (N, T) b200_gemm_fp8_blockwise call with no bias.
-int gemm_fp8_blockwise_batched(int a_type, int b_type, int m, int n, int k, const uint8_t* A, int lda, long long stride_a,
+// fp8_blockwise_batched_args: its checks other than the output type, in its order: < 0 an error, 1 nothing to do, 0 run.
+int fp8_blockwise_batched_args(int a_type, int b_type, int m, int n, int k, const uint8_t* A, int lda, long long stride_a,
                                const uint8_t* B, int ldb, long long stride_b, const float* scale_a, int a_blk,
                                long long sa_row, long long sa_kb, long long scale_a_stride, const float* scale_b,
-                               int b_blk, long long sb_kb, long long sb_col, long long scale_b_stride, void* C, int ldc,
-                               long long stride_c, int batch, int out_type, cudaStream_t st) {
-  if (int rc = fp8_stacked_types(a_type, b_type, out_type, 0)) return rc;
+                               int b_blk, long long sb_kb, long long sb_col, long long scale_b_stride, const void* C,
+                               int ldc, long long stride_c, int batch) {
+  if (int rc = fp8_stacked_types(a_type, b_type, 0)) return rc;
   if ((a_blk != 1 && a_blk != 128) || (b_blk != 1 && b_blk != 128)) return B200_ERR_BAD_ARG;
   if (sa_row < 0 || sa_kb < 0 || sb_kb < 0 || sb_col < 0) return B200_ERR_BAD_ARG;
   if (batch < 0 || stride_a < 0 || stride_b < 0 || stride_c < 0 || scale_a_stride < 0 || scale_b_stride < 0)
@@ -1913,9 +1971,8 @@ int gemm_fp8_blockwise_batched(int a_type, int b_type, int m, int n, int k, cons
   if (m < 0 || n < 0 || k < 0) return B200_ERR_BAD_ARG;
   if (a_type == B200_FP8_E5M2 && b_type == B200_FP8_E5M2) return B200_ERR_UNSUPPORTED;
   if (a_blk == 128 && b_blk == 128) return B200_ERR_UNSUPPORTED;      // not a torch recipe
-  if (batch == 0) return 0;
+  if (batch == 0) return 1;
   int rc = check_args(m, n, k, A, lda, B, ldb, C, ldc, B200_OP_N, B200_OP_T);
-  if (rc == 1) return 0;
   if (rc) return rc;
   if (!scale_a || !scale_b) return B200_ERR_BAD_ARG;
   if (batch > 1) {
@@ -1935,15 +1992,180 @@ int gemm_fp8_blockwise_batched(int a_type, int b_type, int m, int n, int k, cons
   if (k > 0 && (!fp8_in_place(A, lda, B, ldb) ||
                 (batch > 1 && (!batch_tma_ok(stride_a, m, lda, 1) || !batch_tma_ok(stride_b, n, ldb, 1)))))
     return B200_ERR_UNSUPPORTED;
+  return 0;
+}
+
+int gemm_fp8_blockwise_batched(int a_type, int b_type, int m, int n, int k, const uint8_t* A, int lda, long long stride_a,
+                               const uint8_t* B, int ldb, long long stride_b, const float* scale_a, int a_blk,
+                               long long sa_row, long long sa_kb, long long scale_a_stride, const float* scale_b,
+                               int b_blk, long long sb_kb, long long sb_col, long long scale_b_stride, void* C, int ldc,
+                               long long stride_c, int batch, int out_type, cudaStream_t st) {
+  if (!fp8_out_type_ok(out_type)) return B200_ERR_BAD_ARG;
+  if (int rc = fp8_blockwise_batched_args(a_type, b_type, m, n, k, A, lda, stride_a, B, ldb, stride_b, scale_a, a_blk,
+                                          sa_row, sa_kb, scale_a_stride, scale_b, b_blk, sb_kb, sb_col, scale_b_stride,
+                                          C, ldc, stride_c, batch))
+    return rc < 0 ? rc : 0;
   if (batch == 1)
     return gemm_fp8_blockwise(B200_OP_N, B200_OP_T, a_type, b_type, m, n, k, A, lda, B, ldb, scale_a, a_blk, sa_row,
                               sa_kb, scale_b, b_blk, sb_kb, sb_col, nullptr, C, ldc, out_type, st);
-  const Stack bt{batch, stride_a, stride_b, stride_c, nullptr};
-  TcStackBlockScale sc{};
-  sc.a = scale_a; sc.b = scale_b; sc.a_row = sa_row; sc.a_kb = sa_kb; sc.b_kb = sb_kb; sc.b_col = sb_col;
-  sc.a_blk = a_blk; sc.b_blk = b_blk; sc.bias = nullptr;
-  sc.a_entry_stride = scale_a_stride; sc.b_entry_stride = scale_b_stride;
-  return fp8_stacked_run<STACK_BATCH>(a_type, b_type, m, n, k, A, lda, B, ldb, C, ldc, out_type, bt, sc, 0, st);
+  return fp8_stacked_run<STACK_BATCH>(
+      a_type, b_type, m, n, k, A, lda, B, ldb, C, ldc, out_type, Stack{batch, stride_a, stride_b, stride_c, nullptr},
+      fp8_blockwise_stack_scale(scale_a, a_blk, sa_row, sa_kb, scale_a_stride, scale_b, b_blk, sb_kb, sb_col,
+                                scale_b_stride),
+      0, st);
+}
+
+// ---- FP8 outputs of the grouped and batched FP8 GEMMs (the fused 1 x 128 quantisation of each entry's C) -------------
+// Every entry's C and scale_c are those of the (N, T) single-matrix _q8 / _blockwise_q8 call in dynamic mode with no
+// bias on its rows, B and scales, at the same tile width; one launch of gemm_tc_fp8_q8_stacked_kernel.  The checks are
+// the parent stacked call's and fp8_q8_out_args, then scale_c's layout over (total_m, q_n), or (m, q_n) per entry with
+// entries that do not overlap; all before the device is touched.
+// Kernel names by [stacking: 0 = grouped, 1 = batch][kind][C type: 0 = e4m3, 1 = e5m2][width index as kFp8Q8Names].
+#define FP8_STACK_Q8_NAMES(P, S)                                                                                         \
+  {{P "_oe4m3_" S "_128x256", nullptr, P "_oe4m3_" S "_128x128", P "_oe4m3_" S "_acc_128x128",                          \
+    P "_oe4m3_" S "_blk_128x128"},                                                                                      \
+   {P "_oe5m2_" S "_128x256", nullptr, P "_oe5m2_" S "_128x128", P "_oe5m2_" S "_acc_128x128",                          \
+    P "_oe5m2_" S "_blk_128x128"}}
+const char* const kFp8StackQ8Names[2][3][2][5] = {
+    {FP8_STACK_Q8_NAMES("tc_e4m3", "grp"), FP8_STACK_Q8_NAMES("tc_e4m3e5m2", "grp"),
+     FP8_STACK_Q8_NAMES("tc_e5m2e4m3", "grp")},
+    {FP8_STACK_Q8_NAMES("tc_e4m3", "bat"), FP8_STACK_Q8_NAMES("tc_e4m3e5m2", "bat"),
+     FP8_STACK_Q8_NAMES("tc_e5m2e4m3", "bat")}};
+
+// k == 0: act(+0) quantised and d = 1 over the covered rows / entries (fp8_q8_k0_stacked_kernel), no scale read.
+template <typename OutT, int STACK>
+int fp8_q8_k0_stacked(int m, int n, void* C, int ldc, const Stack& stk, const TcQ8& q, long long sc_entry_stride,
+                      cudaStream_t st) {
+  const long long items = (STACK == STACK_GROUP ? m : (long long)m * stk.count) * ((n + 127) / 128);
+  const int blocks = (int)(items < 4096LL * 128 ? (items + 127) / 128 : 4096);
+  fp8_q8_k0_stacked_kernel<OutT, STACK><<<blocks, 128, 0, st>>>(stk.offs, stk.count, m, n, static_cast<uint8_t*>(C), ldc,
+                                                                stk.sc, q, sc_entry_stride);
+  g_launches++;
+  t_last_kernel = STACK == STACK_GROUP ? "fp8_q8_k0_grp" : "fp8_q8_k0_bat";
+  return last_launch_status();
+}
+
+// Every stacked FP8-output call after its argument checks (Scale = TcStackScaleQ8 or TcStackBlockScaleQ8).
+template <int STACK, class Scale>
+int fp8_q8_stacked_run(int a_type, int b_type, int m, int n, int k, const uint8_t* A, int lda, const uint8_t* B, int ldb,
+                       void* C, int ldc, int c_type, const Stack& stk, const Scale& sc, int fast, cudaStream_t st) {
+  if (int rc = ensure_device()) return rc;
+  Call c{st};
+  const bool e4 = c_type == B200_FP8_E4M3;
+  if (k == 0)
+    return e4 ? fp8_q8_k0_stacked<e4m3_out, STACK>(m, n, C, ldc, stk, sc.q, sc.sc_entry_stride, st)
+              : fp8_q8_k0_stacked<e5m2_out, STACK>(m, n, C, ldc, stk, sc.q, sc.sc_entry_stride, st);
+  const int kind = a_type == B200_FP8_E5M2 ? 2 : b_type == B200_FP8_E5M2 ? 1 : 0;
+  const auto& names = kFp8StackQ8Names[STACK == STACK_GROUP ? 0 : 1][kind][e4 ? 0 : 1];
+  auto by_out = [&](auto kd) {
+    constexpr int KIND = decltype(kd)::value;
+    if (e4) return tc_fp8_stacked<KIND, e4m3_out, STACK>(m, n, k, A, lda, B, ldb, C, ldc, stk, sc, fast, names, c);
+    return tc_fp8_stacked<KIND, e5m2_out, STACK>(m, n, k, A, lda, B, ldb, C, ldc, stk, sc, fast, names, c);
+  };
+  if (kind == 2) return by_out(std::integral_constant<int, KIND_E5M2E4M3>());
+  if (kind == 1) return by_out(std::integral_constant<int, KIND_E4M3E5M2>());
+  return by_out(std::integral_constant<int, KIND_E4M3>());
+}
+
+// The output checks of a stacked _q8 call with work to do (the parent's checks passed): scale_c present, and laid out
+// as fp8_q8_scale_layout_ok requires over one entry's (rows, q_n); batch > 1: entries sc_entry_stride apart that do
+// not overlap, the stride bounded as the other entry strides and the last index's byte offset a signed 64-bit integer.
+int fp8_q8_stacked_scale_args(int rows, int n, const float* scale_c, long long sc_row, long long sc_blk,
+                              long long sc_entry_stride, int batch) {
+  if (!scale_c || !fp8_q8_scale_layout_ok(rows, n, sc_row, sc_blk)) return B200_ERR_BAD_ARG;
+  if (batch > 1) {
+    const long long qn = (n + 127LL) / 128;
+    const __int128 last = last_scale_index(rows, qn, sc_row, sc_blk);
+    if (sc_entry_stride < last + 1 || sc_entry_stride > (1LL << 60) / (batch - 1)) return B200_ERR_BAD_ARG;
+    if (last_stacked_scale_index(batch, sc_entry_stride, rows, qn, sc_row, sc_blk) > INT64_MAX / 4) return B200_ERR_BAD_ARG;
+  }
+  return 0;
+}
+
+int gemm_fp8_grouped_q8(int a_type, int b_type, int total_m, int n, int k, const uint8_t* A, int lda, const uint8_t* B,
+                        int ldb, long long stride_b, const int32_t* offs, int groups, const float* scale_a,
+                        const float* scale_b, long long scale_b_stride, int act, int fast_accum, int c_type, uint8_t* C,
+                        int ldc, float* scale_c, long long sc_row, long long sc_blk, cudaStream_t st) {
+  if (int rc = fp8_q8_out_args(c_type, act, nullptr, scale_c, sc_row, sc_blk)) return rc;
+  if (int rc = fp8_grouped_args(a_type, b_type, total_m, n, k, A, lda, B, ldb, stride_b, offs, groups, scale_a, scale_b,
+                                scale_b_stride, C, ldc, fast_accum))
+    return rc < 0 ? rc : 0;
+  if (int rc = fp8_q8_stacked_scale_args(total_m, n, scale_c, sc_row, sc_blk, 0, 1)) return rc;
+  TcStackScaleQ8 sc;
+  static_cast<TcStackScale&>(sc) = fp8_grouped_scale(scale_a, scale_b, scale_b_stride);
+  sc.q = TcQ8{nullptr, scale_c, sc_row, sc_blk, act};
+  sc.sc_entry_stride = 0;
+  return fp8_q8_stacked_run<STACK_GROUP>(a_type, b_type, total_m, n, k, A, lda, B, ldb, C, ldc, c_type,
+                                         fp8_grouped_stack(groups, stride_b, offs), sc, fast_accum, st);
+}
+
+int gemm_fp8_batched_q8(int a_type, int b_type, int m, int n, int k, const uint8_t* A, int lda, long long stride_a,
+                        const uint8_t* B, int ldb, long long stride_b, const float* scale_a, long long scale_a_stride,
+                        const float* scale_b, long long scale_b_stride, int act, int fast_accum, int c_type, uint8_t* C,
+                        int ldc, long long stride_c, float* scale_c, long long sc_row, long long sc_blk,
+                        long long sc_entry_stride, int batch, cudaStream_t st) {
+  if (int rc = fp8_q8_out_args(c_type, act, nullptr, scale_c, sc_row, sc_blk)) return rc;
+  if (sc_entry_stride < 0) return B200_ERR_BAD_ARG;
+  if (int rc = fp8_batched_args(a_type, b_type, m, n, k, A, lda, stride_a, B, ldb, stride_b, scale_a, scale_a_stride,
+                                scale_b, scale_b_stride, C, ldc, stride_c, batch, fast_accum))
+    return rc < 0 ? rc : 0;
+  if (int rc = fp8_q8_stacked_scale_args(m, n, scale_c, sc_row, sc_blk, sc_entry_stride, batch)) return rc;
+  if (batch == 1)
+    return gemm_fp8_q8(B200_OP_N, B200_OP_T, a_type, b_type, m, n, k, A, lda, B, ldb, scale_a, 1, scale_b, 1, nullptr, act,
+                       fast_accum, c_type, C, ldc, nullptr, scale_c, sc_row, sc_blk, st);
+  TcStackScaleQ8 sc;
+  static_cast<TcStackScale&>(sc) = fp8_batched_scale(scale_a, scale_a_stride, scale_b, scale_b_stride);
+  sc.q = TcQ8{nullptr, scale_c, sc_row, sc_blk, act};
+  sc.sc_entry_stride = sc_entry_stride;
+  return fp8_q8_stacked_run<STACK_BATCH>(a_type, b_type, m, n, k, A, lda, B, ldb, C, ldc, c_type,
+                                         Stack{batch, stride_a, stride_b, stride_c, nullptr}, sc, fast_accum, st);
+}
+
+int gemm_fp8_blockwise_grouped_q8(int a_type, int b_type, int total_m, int n, int k, const uint8_t* A, int lda,
+                                  const uint8_t* B, int ldb, long long stride_b, const int32_t* offs, int groups,
+                                  const float* scale_a, long long sa_row, long long sa_kb, const float* scale_b,
+                                  int b_blk, long long sb_kb, long long sb_col, long long scale_b_stride, int act,
+                                  int c_type, uint8_t* C, int ldc, float* scale_c, long long sc_row, long long sc_blk,
+                                  cudaStream_t st) {
+  if (int rc = fp8_q8_out_args(c_type, act, nullptr, scale_c, sc_row, sc_blk)) return rc;
+  if (int rc = fp8_blockwise_grouped_args(a_type, b_type, total_m, n, k, A, lda, B, ldb, stride_b, offs, groups, scale_a,
+                                          sa_row, sa_kb, scale_b, b_blk, sb_kb, sb_col, scale_b_stride, C, ldc))
+    return rc < 0 ? rc : 0;
+  if (int rc = fp8_q8_stacked_scale_args(total_m, n, scale_c, sc_row, sc_blk, 0, 1)) return rc;
+  TcStackBlockScaleQ8 sc;
+  static_cast<TcStackBlockScale&>(sc) =
+      fp8_blockwise_stack_scale(scale_a, 1, sa_row, sa_kb, 0, scale_b, b_blk, sb_kb, sb_col, scale_b_stride);
+  sc.q = TcQ8{nullptr, scale_c, sc_row, sc_blk, act};
+  sc.sc_entry_stride = 0;
+  return fp8_q8_stacked_run<STACK_GROUP>(a_type, b_type, total_m, n, k, A, lda, B, ldb, C, ldc, c_type,
+                                         fp8_grouped_stack(groups, stride_b, offs), sc, 0, st);
+}
+
+int gemm_fp8_blockwise_batched_q8(int a_type, int b_type, int m, int n, int k, const uint8_t* A, int lda,
+                                  long long stride_a, const uint8_t* B, int ldb, long long stride_b, const float* scale_a,
+                                  int a_blk, long long sa_row, long long sa_kb, long long scale_a_stride,
+                                  const float* scale_b, int b_blk, long long sb_kb, long long sb_col,
+                                  long long scale_b_stride, int act, int c_type, uint8_t* C, int ldc, long long stride_c,
+                                  float* scale_c, long long sc_row, long long sc_blk, long long sc_entry_stride,
+                                  int batch, cudaStream_t st) {
+  if (int rc = fp8_q8_out_args(c_type, act, nullptr, scale_c, sc_row, sc_blk)) return rc;
+  if (sc_entry_stride < 0) return B200_ERR_BAD_ARG;
+  if (int rc = fp8_blockwise_batched_args(a_type, b_type, m, n, k, A, lda, stride_a, B, ldb, stride_b, scale_a, a_blk,
+                                          sa_row, sa_kb, scale_a_stride, scale_b, b_blk, sb_kb, sb_col, scale_b_stride,
+                                          C, ldc, stride_c, batch))
+    return rc < 0 ? rc : 0;
+  if (int rc = fp8_q8_stacked_scale_args(m, n, scale_c, sc_row, sc_blk, sc_entry_stride, batch)) return rc;
+  if (batch == 1)
+    return gemm_fp8_blockwise_q8(B200_OP_N, B200_OP_T, a_type, b_type, m, n, k, A, lda, B, ldb, scale_a, a_blk, sa_row,
+                                 sa_kb, scale_b, b_blk, sb_kb, sb_col, nullptr, act, c_type, C, ldc, nullptr, scale_c,
+                                 sc_row, sc_blk, st);
+  TcStackBlockScaleQ8 sc;
+  static_cast<TcStackBlockScale&>(sc) = fp8_blockwise_stack_scale(scale_a, a_blk, sa_row, sa_kb, scale_a_stride, scale_b,
+                                                                  b_blk, sb_kb, sb_col, scale_b_stride);
+  sc.q = TcQ8{nullptr, scale_c, sc_row, sc_blk, act};
+  sc.sc_entry_stride = sc_entry_stride;
+  return fp8_q8_stacked_run<STACK_BATCH>(a_type, b_type, m, n, k, A, lda, B, ldb, C, ldc, c_type,
+                                         Stack{batch, stride_a, stride_b, stride_c, nullptr}, sc, 0, st);
 }
 
 }  // namespace
@@ -2222,6 +2444,55 @@ int b200_gemm_fp8_blockwise_batched(int a_type, int b_type, int m, int n, int k,
                                     sa_row_stride, sa_kb_stride, scale_a_stride, dScaleB, scale_b_block, sb_kb_stride,
                                     sb_col_stride, scale_b_stride, dC, ldc, stride_c, batch, out_type,
                                     (cudaStream_t)stream);
+}
+
+int b200_gemm_fp8_grouped_q8(int a_type, int b_type, int total_m, int n, int k, const uint8_t* dA, int lda,
+                             const uint8_t* dB, int ldb, long long stride_b, const int32_t* dOffs, int groups,
+                             const float* dScaleA, const float* dScaleB, long long scale_b_stride, int act,
+                             int fast_accum, int c_type, uint8_t* dC, int ldc, float* dScaleC, long long sc_row_stride,
+                             long long sc_blk_stride, void* stream) {
+  return gemm_fp8_grouped_q8(a_type, b_type, total_m, n, k, dA, lda, dB, ldb, stride_b, dOffs, groups, dScaleA, dScaleB,
+                             scale_b_stride, act, fast_accum, c_type, dC, ldc, dScaleC, sc_row_stride, sc_blk_stride,
+                             (cudaStream_t)stream);
+}
+
+int b200_gemm_fp8_batched_q8(int a_type, int b_type, int m, int n, int k, const uint8_t* dA, int lda, long long stride_a,
+                             const uint8_t* dB, int ldb, long long stride_b, const float* dScaleA,
+                             long long scale_a_stride, const float* dScaleB, long long scale_b_stride, int act,
+                             int fast_accum, int c_type, uint8_t* dC, int ldc, long long stride_c, float* dScaleC,
+                             long long sc_row_stride, long long sc_blk_stride, long long sc_entry_stride, int batch,
+                             void* stream) {
+  return gemm_fp8_batched_q8(a_type, b_type, m, n, k, dA, lda, stride_a, dB, ldb, stride_b, dScaleA, scale_a_stride,
+                             dScaleB, scale_b_stride, act, fast_accum, c_type, dC, ldc, stride_c, dScaleC, sc_row_stride,
+                             sc_blk_stride, sc_entry_stride, batch, (cudaStream_t)stream);
+}
+
+int b200_gemm_fp8_blockwise_grouped_q8(int a_type, int b_type, int total_m, int n, int k, const uint8_t* dA, int lda,
+                                       const uint8_t* dB, int ldb, long long stride_b, const int32_t* dOffs, int groups,
+                                       const float* dScaleA, long long sa_row_stride, long long sa_kb_stride,
+                                       const float* dScaleB, int scale_b_block, long long sb_kb_stride,
+                                       long long sb_col_stride, long long scale_b_stride, int act, int c_type,
+                                       uint8_t* dC, int ldc, float* dScaleC, long long sc_row_stride,
+                                       long long sc_blk_stride, void* stream) {
+  return gemm_fp8_blockwise_grouped_q8(a_type, b_type, total_m, n, k, dA, lda, dB, ldb, stride_b, dOffs, groups, dScaleA,
+                                       sa_row_stride, sa_kb_stride, dScaleB, scale_b_block, sb_kb_stride, sb_col_stride,
+                                       scale_b_stride, act, c_type, dC, ldc, dScaleC, sc_row_stride, sc_blk_stride,
+                                       (cudaStream_t)stream);
+}
+
+int b200_gemm_fp8_blockwise_batched_q8(int a_type, int b_type, int m, int n, int k, const uint8_t* dA, int lda,
+                                       long long stride_a, const uint8_t* dB, int ldb, long long stride_b,
+                                       const float* dScaleA, int scale_a_block, long long sa_row_stride,
+                                       long long sa_kb_stride, long long scale_a_stride, const float* dScaleB,
+                                       int scale_b_block, long long sb_kb_stride, long long sb_col_stride,
+                                       long long scale_b_stride, int act, int c_type, uint8_t* dC, int ldc,
+                                       long long stride_c, float* dScaleC, long long sc_row_stride,
+                                       long long sc_blk_stride, long long sc_entry_stride, int batch, void* stream) {
+  return gemm_fp8_blockwise_batched_q8(a_type, b_type, m, n, k, dA, lda, stride_a, dB, ldb, stride_b, dScaleA,
+                                       scale_a_block, sa_row_stride, sa_kb_stride, scale_a_stride, dScaleB,
+                                       scale_b_block, sb_kb_stride, sb_col_stride, scale_b_stride, act, c_type, dC, ldc,
+                                       stride_c, dScaleC, sc_row_stride, sc_blk_stride, sc_entry_stride, batch,
+                                       (cudaStream_t)stream);
 }
 
 int b200_gemm_s8s32_op(int op_a, int op_b, int m, int n, int k, const int8_t* dA, int lda, const int8_t* dB, int ldb,

@@ -707,6 +707,12 @@ struct TcQ8 {
 };
 struct TcScaleQ8 : TcScale { TcQ8 q; };
 struct TcBlockScaleQ8 : TcBlockScale { TcQ8 q; };
+// Stacked FP8 output (gemm_tc_fp8_q8_stacked_kernel, dynamic 1 x 128 mode only, no bias): the stacked argument plus
+// TcQ8 and scale_c's element stride between entries.  Entry e's row i (of the entry) and 128-column block c store
+// their scale at scale_c[i_global * sc_row + c * sc_blk] (grouped: i_global the row of the stacked C) or
+// scale_c[e * sc_entry_stride + i * sc_row + c * sc_blk] (batch).
+struct TcStackScaleQ8 : TcStackScale { TcQ8 q; long long sc_entry_stride; };
+struct TcStackBlockScaleQ8 : TcStackBlockScale { TcQ8 q; long long sc_entry_stride; };
 
 // Two fp32 values as two FP8 bytes (lo in the low byte), round to nearest even, finite values saturated.
 template <typename OutT>
@@ -772,6 +778,50 @@ __global__ void fp8_q8_k0_kernel(int m, int n, uint8_t* C, long long ldc, const 
     for (int j = c0; j < c1; j += 2)
       store_fp8_pair<OutT>(p, row, j, __fdiv_rn(val(j), d), j + 1 < c1 ? __fdiv_rn(val(j + 1), d) : 0.f);
     if (dyn) q.scale_c[row * q.sc_row + blk * q.sc_blk] = d;
+  }
+}
+// k == 0 of the stacked FP8-output calls: every covered row stores act(rn(+0 + -0)) quantised as fp8_q8_tile does
+// (d = 1 for its all-zero blocks) and d.  GROUP: rows [0, end of the last group) of the stacked C, found from the
+// clamped offsets (grouped_rows), scales by the row of C.  BATCH: count entries of m rows, C_e = C + e * stride_c,
+// scale_c_e = scale_c + e * sc_entry_stride.  One thread per row and 128-column block; no operand, no input scale read.
+template <typename OutT, int STACK>
+__global__ void fp8_q8_k0_stacked_kernel(const int* __restrict__ offs, int count, int m, int n, uint8_t* C,
+                                         long long ldc, long long stride_c, TcQ8 q, long long sc_entry_stride) {
+  __shared__ int s_max;
+  const int qn = (n + 127) / 128;
+  long long rows;
+  if constexpr (STACK == STACK_GROUP) rows = grouped_rows(offs, count, m, &s_max);
+  else rows = (long long)m * count;
+  const long long items = rows * qn;
+  TcParams p;
+  p.ldc = ldc; p.N = n;
+  float v = __fadd_rn(0.f, -0.f);
+  switch (q.act) {
+    case ACT_RELU: v = epi_act<ACT_RELU>(v); break;
+    case ACT_GELU: v = epi_act<ACT_GELU>(v); break;
+    case ACT_GELU_TANH: v = epi_act<ACT_GELU_TANH>(v); break;
+    default: break;
+  }
+  const float d = q8_block_scale<OutT>(fabsf(v));
+  const float c = __fdiv_rn(v, d);
+  for (long long it = blockIdx.x * (long long)blockDim.x + threadIdx.x; it < items; it += (long long)gridDim.x * blockDim.x) {
+    const long long r = it / qn;
+    const int blk = (int)(it % qn);
+    int row;
+    float* sc;
+    if constexpr (STACK == STACK_GROUP) {
+      row = (int)r;
+      p.C = C;
+      sc = q.scale_c;
+    } else {
+      const long long e = r / m;
+      row = (int)(r % m);
+      p.C = C + e * stride_c;
+      sc = q.scale_c + e * sc_entry_stride;
+    }
+    const int c0 = 128 * blk, c1 = min(c0 + 128, n);
+    for (int j = c0; j < c1; j += 2) store_fp8_pair<OutT>(p, row, j, c, j + 1 < c1 ? c : 0.f);
+    sc[row * q.sc_row + blk * q.sc_blk] = d;
   }
 }
 // Shared memory of one stage's block scales: 128 floats of A (one per tile row), then 128 of B (one per tile column).
@@ -1008,21 +1058,17 @@ __device__ __forceinline__ void fp8_q8_tile(const TcParams& p, const Scale& sc, 
 // BLOCKWISE with STACK_GROUP / STACK_BATCH (argument TcStackBlockScale): the stacked schedule with the blockwise
 // stages; warps 1 and 2 run fp8_block_scale_loader_stacked over the same tiles, and each tile's sum is stored through
 // its entry's TcParams with no further scaling and no bias (the single-matrix store's rn(sum + -0) = sum).
-template <int KIND, int BN, int STAGES, typename OutT, class Prod, bool BLOCKWISE = false, int STACK = STACK_NONE>
-__global__ void __launch_bounds__((TcConfig<KIND, BN, STAGES, Prod, 128>::THREADS), 1)
-gemm_tc_fp8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const TcParams p,
-                   const typename std::conditional<
-                       Fp8Out<OutT>::V, typename std::conditional<BLOCKWISE, TcBlockScaleQ8, TcScaleQ8>::type,
-                       typename std::conditional<
-                           BLOCKWISE, typename std::conditional<STACK != STACK_NONE, TcStackBlockScale, TcBlockScale>::type,
-                           typename std::conditional<STACK != STACK_NONE, TcStackScale, TcScale>::type>::type>::type sc) {
+// The body is gemm_tc_fp8_body, shared with gemm_tc_fp8_q8_stacked_kernel (below), the stacked FP8-output kernels.
+// Its parameters are taken by value: with references the tensorwise / rowwise kernels' register assignment changed.
+template <int KIND, int BN, int STAGES, typename OutT, class Prod, bool BLOCKWISE, int STACK, class Scale>
+__device__ __forceinline__ void gemm_tc_fp8_body(const CUtensorMap& tmA, const CUtensorMap& tmB, const TcParams p,
+                                                 const Scale sc) {
   using Cfg = TcConfig<KIND, BN, STAGES, Prod, 128>;
   using MMA = typename Cfg::MMA;
   static_assert(KIND == KIND_E4M3 || KIND == KIND_E4M3E5M2 || KIND == KIND_E5M2E4M3, "FP8 kinds");
   static_assert(!Cfg::A_MN && !Cfg::B_MN && Prod::NPA == 1 && Prod::NPB == 1, "FP8: K-major A and B, one plane");
   static_assert(std::is_same<OutT, float>::value || OutBytes<OutT>::V == 2 || Fp8Out<OutT>::V, "FP8: fp32, 16-bit or FP8 C");
-  static_assert(!Fp8Out<OutT>::V || (STACK == STACK_NONE && BN % 128 == 0),
-                "FP8 C: single-matrix kernels, tiles of whole 128-column scale blocks");
+  static_assert(!Fp8Out<OutT>::V || BN % 128 == 0, "FP8 C: tiles of whole 128-column scale blocks");
   static_assert(!BLOCKWISE || (std::is_same<Prod, ProdPromoted>::value && BN == 128 && Cfg::BK == 128),
                 "blockwise scales: one 128-element k-block per promotion, tiles on the 128 x 128 scale blocks");
   static_assert(!BLOCKWISE || Cfg::SMEM_BYTES + STAGES * kBlkScaleStageBytes <= 232448, "blockwise: shared memory");
@@ -1189,7 +1235,34 @@ gemm_tc_fp8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
       // ---- this warp's 16 rows of the tile into C: (acc * sa) * sb (BLOCKWISE: sum), then + bias in store_pair ----
       const int row0 = m0 + ew * 16 + (lane >> 2);
       const int col0 = n0 + 2 * (lane & 3);
-      if constexpr (Fp8Out<OutT>::V) {
+      if constexpr (Fp8Out<OutT>::V && STACK != STACK_NONE) {
+        // stacked FP8 C (TcStackScaleQ8 / TcStackBlockScaleQ8): the entry's C and rows, and its scales as a
+        // single-matrix argument (B's at its entry, no bias), then fp8_q8_tile stores exactly what the single-matrix
+        // kernel stores for that entry.  A group is rows [a_row, a_row + M) of the stacked C, of A's scales and of
+        // scale_c, all indexed by that row: its tile rows are shifted by a_row and masked at the group's end (fewer live
+        // registers than rebased pointers, which spilled at BN = 256).  A batch entry's C, A scales and scale_c start
+        // at its entry strides.
+        const StackEntry se = stack_entry<STACK>(w, p, sc.st, fp8_group_table<0>(), fp8_group_table<1>());
+        TcParams pc = p;
+        typename std::conditional<BLOCKWISE, TcBlockScaleQ8, TcScaleQ8>::type ve;
+        static_cast<typename std::conditional<BLOCKWISE, TcBlockScale, TcScale>::type&>(ve) = sc;
+        ve.b = sc.b + se.entry * sc.b_entry_stride;
+        ve.bias = nullptr;
+        ve.q = sc.q;
+        int r0 = row0;
+        if constexpr (STACK == STACK_GROUP) {
+          pc.M = se.a_row + se.M;
+          r0 += se.a_row;
+        } else {
+          pc.C = static_cast<uint8_t*>(p.C) + se.c_off;
+          pc.M = se.M;
+          ve.a = sc.a + se.entry * sc.a_entry_stride;
+          ve.q.scale_c = sc.q.scale_c + se.entry * sc.sc_entry_stride;
+        }
+        if constexpr (Cfg::REGACC) fp8_q8_tile<BN, OutT, BLOCKWISE>(pc, ve, sum, r0, col0, lane);
+        else fp8_q8_tile<BN, OutT, BLOCKWISE>(pc, ve, acc, r0, col0, lane);
+        continue;
+      } else if constexpr (Fp8Out<OutT>::V) {
         // FP8 C (TcQ8): v, then the static or dynamic quantisation, in fp8_q8_tile
         if constexpr (Cfg::REGACC) fp8_q8_tile<BN, OutT, BLOCKWISE>(p, sc, sum, row0, col0, lane);
         else fp8_q8_tile<BN, OutT, BLOCKWISE>(p, sc, acc, row0, col0, lane);
@@ -1280,6 +1353,31 @@ gemm_tc_fp8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
       }
     }
   }
+}
+
+template <int KIND, int BN, int STAGES, typename OutT, class Prod, bool BLOCKWISE = false, int STACK = STACK_NONE>
+__global__ void __launch_bounds__((TcConfig<KIND, BN, STAGES, Prod, 128>::THREADS), 1)
+gemm_tc_fp8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const TcParams p,
+                   const typename std::conditional<
+                       Fp8Out<OutT>::V, typename std::conditional<BLOCKWISE, TcBlockScaleQ8, TcScaleQ8>::type,
+                       typename std::conditional<
+                           BLOCKWISE, typename std::conditional<STACK != STACK_NONE, TcStackBlockScale, TcBlockScale>::type,
+                           typename std::conditional<STACK != STACK_NONE, TcStackScale, TcScale>::type>::type>::type sc) {
+  static_assert(!Fp8Out<OutT>::V || STACK == STACK_NONE, "stacked FP8 C: gemm_tc_fp8_q8_stacked_kernel");
+  gemm_tc_fp8_body<KIND, BN, STAGES, OutT, Prod, BLOCKWISE, STACK>(tmA, tmB, p, sc);
+}
+
+// The stacked FP8-output kernels (STACK_GROUP / STACK_BATCH, OutT e4m3_out / e5m2_out, dynamic 1 x 128 mode): every
+// entry's C and scale_c are the single-matrix FP8-output kernel's on that entry at the same width.  A __global__ of
+// their own over the same body, so that gemm_tc_fp8_kernel's instantiations stay the FP8 kernels with an fp32 or
+// 16-bit C, or one FP8 C matrix.
+template <int KIND, int BN, int STAGES, typename OutT, class Prod, bool BLOCKWISE, int STACK>
+__global__ void __launch_bounds__((TcConfig<KIND, BN, STAGES, Prod, 128>::THREADS), 1)
+gemm_tc_fp8_q8_stacked_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                              const TcParams p,
+                              const typename std::conditional<BLOCKWISE, TcStackBlockScaleQ8, TcStackScaleQ8>::type sc) {
+  static_assert(Fp8Out<OutT>::V && STACK != STACK_NONE, "stacked FP8 C");
+  gemm_tc_fp8_body<KIND, BN, STAGES, OutT, Prod, BLOCKWISE, STACK>(tmA, tmB, p, sc);
 }
 
 // ---- stacked 16-bit GEMMs: strided batch and grouped (torch._grouped_mm) --------------------------------------------

@@ -606,6 +606,61 @@ int b200_gemm_fp8_blockwise_batched(int a_type, int b_type, int m, int n, int k,
                                     long long sb_col_stride, long long scale_b_stride,
                                     void* dC, int ldc, long long stride_c, int batch, int out_type, void* stream);
 
+/* ---- FP8 outputs of the grouped and batched FP8 GEMMs (a fused 1 x 128 quantisation of each entry's C) -------------
+ * Each call is its stacked parent above with the output type replaced by the dynamic 1 x 128 mode of b200_gemm_fp8_q8:
+ * every group or entry's C and scales are bit for bit the (N, T) single-matrix call in dynamic mode with a null bias
+ * and a null dScaleResult on the entry's rows, B and scales, at the same tile width:
+ *   b200_gemm_fp8_grouped_q8 / _batched_q8:                      b200_gemm_fp8_q8,  v = act(rn(rn(rn(acc * sa_i) * sb_j) + -0))
+ *   b200_gemm_fp8_blockwise_grouped_q8 / _blockwise_batched_q8:  b200_gemm_fp8_blockwise_q8,  v = act(rn(sum + -0))
+ * then per row and 128-column block d = rn(amax / F) (1 when that is 0, NaN for a NaN or an inf in the block), c =
+ * fp8(rn(v / d)), and d is stored.  act is a B200_ACT_* code, c_type B200_FP8_E4M3 or B200_FP8_E5M2; C is any base
+ * and pitch (bytes = elements), as for b200_gemm_fp8_q8.
+ *   Grouped: dScaleC is indexed by the row of C, dScaleC[i * sc_row_stride + c * sc_blk_stride] over (total_m, q_n),
+ *     q_n = ceil(n / 128): exactly the (total_m, q) scale_a that b200_gemm_fp8_blockwise_grouped reads, so (C, dScaleC)
+ *     is the next grouped blockwise GEMM's (A, scale_a).  Rows from end_{G-1} on are written neither in C nor in
+ *     dScaleC.
+ *   Batched: entry e's C starts at dC + e * stride_c and its scales at dScaleC + e * sc_entry_stride, each indexed as
+ *     b200_gemm_fp8_q8's over (m, q_n).  batch == 1 is the single-matrix call itself: same kernel, name and bits.
+ * Argument rules, all checked before the device is touched: the parent's, and c_type, act and the strides of
+ * b200_gemm_fp8_q8; a null dScaleC with work to do; a scale layout that is neither row-major nor outer-dim-major over
+ * (total_m, q_n) or (m, q_n) (b200_gemm_fp8_q8's rule); batch > 1 with sc_entry_stride below one entry's last scale
+ * index + 1 (entries would overlap), above 2^60 / (batch - 1), or with a last index, entry term included, whose byte
+ * offset does not fit a signed 64-bit integer: B200_ERR_BAD_ARG.  No bias, no static scale_result, no 128 x 128 output
+ * blocks.  k == 0 stores act(+0) quantised (the FP8 +0 byte) and d = 1 over the covered rows or entries, reading no
+ * operand and no scale; the grouped form finds its rows from the clamped offsets on the device.  The calls never
+ * synchronise and can be captured in a CUDA graph.  Tiles: promoted 128 x 128, fast 128 x 256 or 128 x 128 (no
+ * 192-wide tile), blockwise 128 x 128.  Kernels: "tc_e4m3_oe4m3_grp_128x256", "tc_e4m3e5m2_oe5m2_bat_acc_128x128",
+ * "tc_e5m2e4m3_oe4m3_grp_blk_128x128", ...; a k == 0 call runs "fp8_q8_k0_grp" / "fp8_q8_k0_bat". */
+int b200_gemm_fp8_grouped_q8(int a_type, int b_type, int total_m, int n, int k, const uint8_t* dA, int lda,
+                             const uint8_t* dB, int ldb, long long stride_b, const int32_t* dOffs, int groups,
+                             const float* dScaleA, const float* dScaleB, long long scale_b_stride, int act,
+                             int fast_accum, int c_type, uint8_t* dC, int ldc, float* dScaleC, long long sc_row_stride,
+                             long long sc_blk_stride, void* stream);
+int b200_gemm_fp8_batched_q8(int a_type, int b_type, int m, int n, int k, const uint8_t* dA, int lda, long long stride_a,
+                             const uint8_t* dB, int ldb, long long stride_b, const float* dScaleA,
+                             long long scale_a_stride, const float* dScaleB, long long scale_b_stride, int act,
+                             int fast_accum, int c_type, uint8_t* dC, int ldc, long long stride_c, float* dScaleC,
+                             long long sc_row_stride, long long sc_blk_stride, long long sc_entry_stride, int batch,
+                             void* stream);
+int b200_gemm_fp8_blockwise_grouped_q8(int a_type, int b_type, int total_m, int n, int k,
+                                       const uint8_t* dA, int lda, const uint8_t* dB, int ldb, long long stride_b,
+                                       const int32_t* dOffs, int groups,
+                                       const float* dScaleA, long long sa_row_stride, long long sa_kb_stride,
+                                       const float* dScaleB, int scale_b_block, long long sb_kb_stride,
+                                       long long sb_col_stride, long long scale_b_stride, int act, int c_type,
+                                       uint8_t* dC, int ldc, float* dScaleC, long long sc_row_stride,
+                                       long long sc_blk_stride, void* stream);
+int b200_gemm_fp8_blockwise_batched_q8(int a_type, int b_type, int m, int n, int k,
+                                       const uint8_t* dA, int lda, long long stride_a,
+                                       const uint8_t* dB, int ldb, long long stride_b,
+                                       const float* dScaleA, int scale_a_block, long long sa_row_stride,
+                                       long long sa_kb_stride, long long scale_a_stride,
+                                       const float* dScaleB, int scale_b_block, long long sb_kb_stride,
+                                       long long sb_col_stride, long long scale_b_stride, int act, int c_type,
+                                       uint8_t* dC, int ldc, long long stride_c, float* dScaleC,
+                                       long long sc_row_stride, long long sc_blk_stride, long long sc_entry_stride,
+                                       int batch, void* stream);
+
 /* Pre-split operands for the split-precision modes (AUTO = the library default): the reference
  * leaves its "packAB interface open" for callers that reuse one operand (README.md:85; PackMatrixA/B,
  * aarch64/MMult_4x4_13.cpp:259,361).  TMA needs no repacking of row-major operands, but the fp32 ->
