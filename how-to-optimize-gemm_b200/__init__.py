@@ -565,35 +565,8 @@ def scaled_mm(A, B, scale_a, scale_b, bias=None, out_dtype=None, use_fast_accum=
                                   stream)[0]
     if scale_result is not None:
         raise ValueError("scale_result applies to an FP8 out_dtype only")
-    ta, tb = _fp8_type(A), _fp8_type(B)
-    if ta is None or tb is None:
-        raise TypeError(f"operands must be float8_e4m3fn or float8_e5m2, not {A.dtype} and {B.dtype}")
-    if ta == FP8_E5M2 and tb == FP8_E5M2:
-        raise TypeError("float8_e5m2 x float8_e5m2 is not supported (as in torch._scaled_mm)")
-    if A.dim() != 2 or B.dim() != 2 or A.shape[1] != B.shape[0]:
-        raise ValueError(f"A and B must be 2-D with matching inner dimensions, not {tuple(A.shape)} and {tuple(B.shape)}")
-    m, k = A.shape
-    n = B.shape[1]
-    if out_dtype not in (torch.bfloat16, torch.float16, torch.float32):
-        raise ValueError(f"out_dtype must be bfloat16, float16 or float32, not {out_dtype}")
-    rows, blocks = _resolve_scales(scale_a, scale_b, m, n, k)
-    if blocks is not None and use_fast_accum:
-        raise ValueError("use_fast_accum=True is not available with blockwise scales: their scales change every k-block")
-    if bias is not None:
-        if bias.dtype != out_dtype:
-            raise ValueError(f"the bias must have dtype {out_dtype}, not {bias.dtype}")
-        if bias.dim() != 1 or bias.shape[0] != n or not bias.is_contiguous():
-            raise ValueError(f"the bias must be contiguous and 1-D with n = {n} elements, not of shape {tuple(bias.shape)}")
-    if out is not None:
-        if out.dtype != out_dtype or tuple(out.shape) != (m, n):
-            raise ValueError(f"out must be {out_dtype} of shape {(m, n)}, not {out.dtype} of shape {tuple(out.shape)}")
-        if (n > 1 and out.stride(1) != 1) or (m > 1 and out.stride(0) < n):
-            raise ValueError(f"out must be row-major with rows that do not overlap, not of strides {tuple(out.stride())}")
-    op_a, lda = operand_layout(tuple(A.shape), A.stride())
-    op_b, ldb = operand_layout(tuple(B.shape), B.stride())
-    tensors = [A, B, scale_a, scale_b] + [t for t in (bias, out) if t is not None]
-    if not all(t.is_cuda for t in tensors):
-        raise ValueError("A, B, the scales, the bias and out must be CUDA tensors")
+    ta, tb, m, n, k, op_a, lda, op_b, ldb, rows, blocks = _scaled_mm_args(A, B, scale_a, scale_b, bias, out_dtype,
+                                                                          use_fast_accum, out, fp8_out=False)
     if out is None:
         out = torch.empty((m, n), dtype=out_dtype, device=A.device)
     if m == 0 or n == 0:
@@ -636,10 +609,11 @@ def _resolve_scales(scale_a, scale_b, m, n, k):
     return rows, blocks
 
 
-def _scaled_mm_fp8_out(A, B, scale_a, scale_b, bias, activation, out_dtype, use_fast_accum, out, out_scale,
-                       scale_result, stream, dynamic=False):
-    """The FP8-output form of scaled_mm (static: scale_result) and scaled_mm_quant (dynamic: out_scale); returns
-    (out, scale_c or None).  Every check happens before the device is touched."""
+def _scaled_mm_args(A, B, scale_a, scale_b, bias, out_dtype, use_fast_accum, out, fp8_out, activation=None,
+                    scale_result=None, out_scale=None):
+    """scaled_mm's operand, shape and scale resolution and its refusals, in its order, for a 16-bit / fp32 (fp8_out
+    False) or an FP8 out_dtype (with scaled_mm_quant's activation and out_scale, and scale_result); returns
+    (ta, tb, m, n, k, op_a, lda, op_b, ldb, rows, blocks), rows and blocks as _resolve_scales gives them."""
     import torch
     ta, tb = _fp8_type(A), _fp8_type(B)
     if ta is None or tb is None:
@@ -650,16 +624,20 @@ def _scaled_mm_fp8_out(A, B, scale_a, scale_b, bias, activation, out_dtype, use_
         raise ValueError(f"A and B must be 2-D with matching inner dimensions, not {tuple(A.shape)} and {tuple(B.shape)}")
     m, k = A.shape
     n = B.shape[1]
-    if not _is_fp8(out_dtype):
+    if fp8_out and not _is_fp8(out_dtype):
         raise ValueError(f"out_dtype must be float8_e4m3fn or float8_e5m2, not {out_dtype}")
-    if activation not in ACTIVATIONS:
+    if not fp8_out and out_dtype not in (torch.bfloat16, torch.float16, torch.float32):
+        raise ValueError(f"out_dtype must be bfloat16, float16 or float32, not {out_dtype}")
+    if fp8_out and activation not in ACTIVATIONS:
         raise ValueError(f"activation must be one of {sorted(a for a in ACTIVATIONS if a)} or None, not {activation!r}")
     rows, blocks = _resolve_scales(scale_a, scale_b, m, n, k)
     if blocks is not None and use_fast_accum:
         raise ValueError("use_fast_accum=True is not available with blockwise scales: their scales change every k-block")
     if bias is not None:
-        if bias.dtype != torch.bfloat16:
+        if fp8_out and bias.dtype != torch.bfloat16:
             raise ValueError(f"with an FP8 output the bias must be bfloat16, not {bias.dtype}")
+        if not fp8_out and bias.dtype != out_dtype:
+            raise ValueError(f"the bias must have dtype {out_dtype}, not {bias.dtype}")
         if bias.dim() != 1 or bias.shape[0] != n or not bias.is_contiguous():
             raise ValueError(f"the bias must be contiguous and 1-D with n = {n} elements, not of shape {tuple(bias.shape)}")
     if scale_result is not None and (scale_result.dtype != torch.float32 or scale_result.numel() != 1):
@@ -685,11 +663,23 @@ def _scaled_mm_fp8_out(A, B, scale_a, scale_b, bias, activation, out_dtype, use_
     op_b, ldb = operand_layout(tuple(B.shape), B.stride())
     tensors = [A, B, scale_a, scale_b] + [t for t in (bias, out, out_scale, scale_result) if t is not None]
     if not all(t.is_cuda for t in tensors):
-        raise ValueError("A, B, the scales, the bias, scale_result, out and out_scale must be CUDA tensors")
+        raise ValueError("A, B, the scales, the bias, scale_result, out and out_scale must be CUDA tensors" if fp8_out
+                         else "A, B, the scales, the bias and out must be CUDA tensors")
+    return ta, tb, m, n, k, op_a, lda, op_b, ldb, rows, blocks
+
+
+def _scaled_mm_fp8_out(A, B, scale_a, scale_b, bias, activation, out_dtype, use_fast_accum, out, out_scale,
+                       scale_result, stream, dynamic=False):
+    """The FP8-output form of scaled_mm (static: scale_result) and scaled_mm_quant (dynamic: out_scale); returns
+    (out, scale_c or None).  Every check happens before the device is touched."""
+    import torch
+    ta, tb, m, n, k, op_a, lda, op_b, ldb, rows, blocks = _scaled_mm_args(
+        A, B, scale_a, scale_b, bias, out_dtype, use_fast_accum, out, fp8_out=True, activation=activation,
+        scale_result=scale_result, out_scale=out_scale)
     if out is None:
         out = torch.empty((m, n), dtype=out_dtype, device=A.device)
     if dynamic and out_scale is None:
-        out_scale = torch.empty((m, qn), dtype=torch.float32, device=A.device)
+        out_scale = torch.empty((m, -(-n // 128)), dtype=torch.float32, device=A.device)
     if m == 0 or n == 0:
         return out, out_scale
     ct = FP8_E4M3 if out_dtype == torch.float8_e4m3fn else FP8_E5M2

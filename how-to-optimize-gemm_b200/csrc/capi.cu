@@ -1466,172 +1466,197 @@ int gemm_s8(int op_a, int op_b, int m, int n, int k, const int8_t* A, int lda, c
   return tc_s8(op_a, op_b, m, n, k, A, lda, B, ldb, C, ldc, c);
 }
 
-// ---- FP8 (torch._scaled_mm) ------------------------------------------------------------------------------------------
-// Kernel names by [kind][C type][width index, 3 = promoted, 4 = blockwise].
-#define FP8_NAMES(P)                                                                                                  \
-  {{P "_of32_128x256", P "_of32_128x192", P "_of32_128x128", P "_of32_acc_128x128", P "_of32_blk_128x128"},           \
-   {P "_obf16_128x256", P "_obf16_128x192", P "_obf16_128x128", P "_obf16_acc_128x128", P "_obf16_blk_128x128"},      \
-   {P "_of16_128x256", P "_of16_128x192", P "_of16_128x128", P "_of16_acc_128x128", P "_of16_blk_128x128"}}
-const char* const kFp8Names[3][3][5] = {FP8_NAMES("tc_e4m3"), FP8_NAMES("tc_e4m3e5m2"), FP8_NAMES("tc_e5m2e4m3")};
-
-// Every layout and pitch runs on the tensor cores: (N, T) with TMA-able operands is read in place; otherwise the
-// operands are made K-major and TMA-able in the workspace (stage_kmajor), which holds the same bytes, so every route is
-// bit-identical to the aligned (N, T) call.  fast: one accumulator over K at pick_bn's width; else promoted per
-// 128-element k-block (two 64 x BN fp32 tiles in registers: BN = 128).  Blockwise scales (Scale = TcBlockScale) are
-// always promoted; their indices are logical (row, k-block) / (k-block, column), so staging never touches them.  An FP8
-// C (TcScaleQ8 / TcBlockScaleQ8) has no 192-wide tile: its 128-column scale blocks must not straddle tiles.
-template <int KIND, typename OutT, class Scale>
-int tc_fp8(int op_a, int op_b, int m, int n, int k, const void* A, long long lda, const void* B, long long ldb, void* C,
-           int ldc, const Scale& sc, bool fast, const char* const (&names)[5], const Call& c) {
-  const bool copy_a = !op_a && !(aligned16(A) && lda % 16 == 0);
-  const bool copy_b = op_b && !(aligned16(B) && ldb % 16 == 0);
-  const int sa = op_a || copy_a, sb = op_b && !copy_b;          // kmajor_ws_bytes / stage_kmajor's view of the layout
-  auto run = [&](const void* a, long long la, const void* b, long long lb) {
-    constexpr bool blk = std::is_same<Scale, TcBlockScale>::value || std::is_same<Scale, TcBlockScaleQ8>::value;
-    if constexpr (!blk)
-      if (fast)
-        return with_width<!Fp8Out<OutT>::V>(m, n, [&](auto W) {
-          using Wd = decltype(W);
-          return launch_tc<KIND, Wd::BN, Wd::STAGES, OutT>(m, n, k, a, la, m, 0, b, lb, n, 0, C, ldc, names[Wd::idx], c,
-                                                           0, nullptr, nullptr, nullptr, &sc);
-        });
-    return launch_tc<KIND, 128, Width<128>::STAGES, OutT, ProdPromoted>(m, n, k, a, la, m, 0, b, lb, n, 0, C, ldc,
-                                                                          names[blk ? 4 : 3], c, 128, nullptr, nullptr,
-                                                                          nullptr, &sc);
-  };
-  if (!sa && sb) return run(A, lda, B, ldb);
-  WsLease ws(kmajor_ws_bytes(sa, sb, m, n, k, 1), c.st);
-  if (ws.rc) return ws.rc;
-  if (int rc = stage_kmajor<uint8_t>(sa, sb, m, n, k, A, lda, B, ldb, ws.base(), c.st, copy_a, copy_b)) return rc;
-  return run(A, lda, B, ldb);
-}
-
-template <int KIND, class Scale>
-int gemm_fp8_kind(int op_a, int op_b, int m, int n, int k, const void* A, int lda, const void* B, int ldb, void* C, int ldc,
-                  int out_type, const Scale& sc, bool fast, const Call& c) {
-  const auto& names = kFp8Names[KIND - KIND_E4M3][out_type];
-  if (out_type == B200_OUT_F32) return tc_fp8<KIND, float>(op_a, op_b, m, n, k, A, lda, B, ldb, C, ldc, sc, fast, names, c);
-  if (out_type == B200_OUT_BF16) return tc_fp8<KIND, bf16_out>(op_a, op_b, m, n, k, A, lda, B, ldb, C, ldc, sc, fast, names, c);
-  return tc_fp8<KIND, f16_out>(op_a, op_b, m, n, k, A, lda, B, ldb, C, ldc, sc, fast, names, c);
-}
-
-// Every FP8 call after its argument checks: k == 0 stores round_out(+0 + bias_j) (or +0) through the bias pass with
-// beta = 0 or the zero fill, reading no scale; otherwise the kind and C type select the kernel.
-template <class Scale>
-int fp8_run(int op_a, int op_b, int a_type, int b_type, int m, int n, int k, const uint8_t* A, int lda, const uint8_t* B,
-            int ldb, void* C, int ldc, int out_type, const Scale& sc, int fast_accum, cudaStream_t st) {
-  if (int rc = ensure_device()) return rc;
-  Call c{st};
-  if (k == 0) {
-    if (sc.bias) { c.bias = sc.bias; c.act = ACT_NONE; }
-    if (out_type == B200_OUT_F32) return degenerate<float, float>(m, n, C, ldc, c);
-    if (out_type == B200_OUT_BF16) return degenerate<uint16_t, uint16_t>(m, n, C, ldc, c);
-    return degenerate<__half, __half>(m, n, C, ldc, c);
-  }
-  if (a_type == B200_FP8_E5M2) return gemm_fp8_kind<KIND_E5M2E4M3>(op_a, op_b, m, n, k, A, lda, B, ldb, C, ldc, out_type, sc, fast_accum, c);
-  if (b_type == B200_FP8_E5M2) return gemm_fp8_kind<KIND_E4M3E5M2>(op_a, op_b, m, n, k, A, lda, B, ldb, C, ldc, out_type, sc, fast_accum, c);
-  return gemm_fp8_kind<KIND_E4M3>(op_a, op_b, m, n, k, A, lda, B, ldb, C, ldc, out_type, sc, fast_accum, c);
-}
-
-// b200_gemm_fp8's argument checks other than the output type, in its order: < 0 an error, 1 nothing to do, 0 run.
-int fp8_args(int op_a, int op_b, int a_type, int b_type, int m, int n, int k, const uint8_t* A, int lda, const uint8_t* B,
-             int ldb, const float* scale_a, int scale_a_rowwise, const float* scale_b, int scale_b_colwise, const void* C,
-             int ldc, int fast_accum) {
-  auto fp8 = [](int t) { return t == B200_FP8_E4M3 || t == B200_FP8_E5M2; };
-  if (!fp8(a_type) || !fp8(b_type)) return B200_ERR_BAD_ARG;
-  if ((scale_a_rowwise != 0 && scale_a_rowwise != 1) || (scale_b_colwise != 0 && scale_b_colwise != 1)) return B200_ERR_BAD_ARG;
-  if (fast_accum != 0 && fast_accum != 1) return B200_ERR_BAD_ARG;
-  int rc = check_args(m, n, k, A, lda, B, ldb, C, ldc, op_a, op_b);
-  if (rc < 0) return rc;
-  if (a_type == B200_FP8_E5M2 && b_type == B200_FP8_E5M2) return B200_ERR_UNSUPPORTED;
-  if (rc == 1) return 1;
-  if (!scale_a || !scale_b) return B200_ERR_BAD_ARG;
-  return 0;
-}
-
-// C = round_out((op(A) op(B) * sa_i) * sb_j + bias_j); every argument is checked before the device is touched.
-int gemm_fp8(int op_a, int op_b, int a_type, int b_type, int m, int n, int k, const uint8_t* A, int lda, const uint8_t* B,
-             int ldb, const float* scale_a, int scale_a_rowwise, const float* scale_b, int scale_b_colwise,
-             const void* bias, void* C, int ldc, int out_type, int fast_accum, cudaStream_t st) {
-  if (out_type != B200_OUT_F32 && out_type != B200_OUT_BF16 && out_type != B200_OUT_F16) return B200_ERR_BAD_ARG;
-  if (int rc = fp8_args(op_a, op_b, a_type, b_type, m, n, k, A, lda, B, ldb, scale_a, scale_a_rowwise, scale_b,
-                        scale_b_colwise, C, ldc, fast_accum))
-    return rc < 0 ? rc : 0;
-  return fp8_run(op_a, op_b, a_type, b_type, m, n, k, A, lda, B, ldb, C, ldc, out_type,
-                 TcScale{scale_a, scale_b, scale_a_rowwise, scale_b_colwise, bias}, fast_accum, st);
-}
+// ---- FP8 (torch._scaled_mm, torch._scaled_grouped_mm) ----------------------------------------------------------------
+// Each FP8 entry point describes its call in an Fp8Call, and fp8_gemm checks it (fp8_check) and runs it.
+// Kernel names by [stacking][kind][C type: fp32, bf16, fp16, e4m3, e5m2][width index, 3 = promoted, 4 = blockwise].
+#define FP8_NAMES(P, S)                                                                                                 \
+  {{P "_of32" S "_128x256", P "_of32" S "_128x192", P "_of32" S "_128x128", P "_of32" S "_acc_128x128",                  \
+    P "_of32" S "_blk_128x128"},                                                                                         \
+   {P "_obf16" S "_128x256", P "_obf16" S "_128x192", P "_obf16" S "_128x128", P "_obf16" S "_acc_128x128",              \
+    P "_obf16" S "_blk_128x128"},                                                                                        \
+   {P "_of16" S "_128x256", P "_of16" S "_128x192", P "_of16" S "_128x128", P "_of16" S "_acc_128x128",                  \
+    P "_of16" S "_blk_128x128"},                                                                                         \
+   {P "_oe4m3" S "_128x256", nullptr, P "_oe4m3" S "_128x128", P "_oe4m3" S "_acc_128x128", P "_oe4m3" S "_blk_128x128"}, \
+   {P "_oe5m2" S "_128x256", nullptr, P "_oe5m2" S "_128x128", P "_oe5m2" S "_acc_128x128", P "_oe5m2" S "_blk_128x128"}}
+const char* const kFp8Names[3][3][5][5] = {
+    {FP8_NAMES("tc_e4m3", ""), FP8_NAMES("tc_e4m3e5m2", ""), FP8_NAMES("tc_e5m2e4m3", "")},
+    {FP8_NAMES("tc_e4m3", "_bat"), FP8_NAMES("tc_e4m3e5m2", "_bat"), FP8_NAMES("tc_e5m2e4m3", "_bat")},
+    {FP8_NAMES("tc_e4m3", "_grp"), FP8_NAMES("tc_e4m3e5m2", "_grp"), FP8_NAMES("tc_e5m2e4m3", "_grp")}};
+static_assert(STACK_NONE == 0 && STACK_BATCH == 1 && STACK_GROUP == 2, "kFp8Names is indexed by the stacking");
 static_assert(KIND_E4M3E5M2 == KIND_E4M3 + 1 && KIND_E5M2E4M3 == KIND_E4M3 + 2, "kFp8Names rows follow the kinds");
 
-// Element index of the last scale a blockwise operand reads, (rows - 1) * row_stride + (q - 1) * kb_stride, in 128
-// bits: the C ABI refuses one whose byte offset does not fit a signed 64-bit integer.
-__int128 last_scale_index(long long rows, long long q, long long row_stride, long long kb_stride) {
-  return (__int128)(rows - 1) * row_stride + (__int128)(q > 0 ? q - 1 : 0) * kb_stride;
+// One FP8 call.  A stacked call (torch._scaled_grouped_mm 2-D x 3-D and 3-D x 3-D) is (N, T): a row-major A (m = total_m
+// rows for a grouped call) and every B entry stored n x k (B^T); it has no bias and its rowwise scales are per row and
+// per column.
+struct Fp8Call {
+  Fp8Call(int at, int bt, int m_, int n_, int k_, const uint8_t* a, int la, const uint8_t* b, int lb, void* c, int lc)
+      : a_type(at), b_type(bt), m(m_), n(n_), k(k_), A(a), lda(la), B(b), ldb(lb), C(c), ldc(lc) {}
+  int a_type, b_type, op_a = B200_OP_N, op_b = B200_OP_T;
+  int m, n, k;
+  const uint8_t* A; int lda;
+  const uint8_t* B; int ldb;
+  void* C; int ldc;
+  int stack = STACK_NONE, count = 1;                    // STACK_GROUP: groups, stride_b, offs; STACK_BATCH: entries
+  long long stride_a = 0, stride_b = 0, stride_c = 0;   // elements between entries
+  const int32_t* offs = nullptr;                        // [count] cumulative ends of the groups, on the device
+  const float* scale_a = nullptr; const float* scale_b = nullptr;
+  bool blockwise = false;
+  int a_step = 1, b_step = 1;                           // tensorwise (0) or rowwise (1)
+  int a_blk = 1, b_blk = 1;                             // blockwise: 1 x 128 or 128 x 128, with TcBlockScale's strides
+  long long sa_row = 0, sa_kb = 0, sb_kb = 0, sb_col = 0;
+  long long sa_entry = 0, sb_entry = 0;                 // elements between entries' scales
+  const void* bias = nullptr;
+  int fast = 0;
+  bool q8 = false;                                      // C: out_type (B200_OUT_*), or FP8 (c_type) with its quantisation
+  int out_type = B200_OUT_F32, c_type = B200_FP8_E4M3, act = B200_ACT_NONE;
+  const float* scale_result = nullptr;
+  float* scale_c = nullptr;
+  long long sc_row = 0, sc_blk = 0, sc_entry = 0;       // scale_c's strides per row, 128-column block and entry
+};
+
+// Element index of the last scale of `count` entries `entry_stride` apart, each (rows - 1) * row_stride + (q - 1) *
+// kb_stride long, in 128 bits: the C ABI refuses one whose byte offset does not fit a signed 64-bit integer.
+__int128 last_scale_index(long long count, long long entry_stride, long long rows, long long q, long long row_stride,
+                          long long kb_stride) {
+  return (__int128)(count - 1) * entry_stride + (__int128)(rows - 1) * row_stride +
+         (__int128)(q > 0 ? q - 1 : 0) * kb_stride;
 }
 
-// b200_gemm_fp8_blockwise's argument checks other than the output type, in its order: < 0 an error, 1 nothing to do,
-// 0 run.
-int fp8_blockwise_args(int op_a, int op_b, int a_type, int b_type, int m, int n, int k, const uint8_t* A, int lda,
-                       const uint8_t* B, int ldb, const float* scale_a, int a_blk, long long sa_row, long long sa_kb,
-                       const float* scale_b, int b_blk, long long sb_kb, long long sb_col, const void* C, int ldc) {
+// Every FP8 call's argument checks, all before the device is touched: < 0 an error, 1 nothing to do, 0 run.  The
+// families have always checked in different orders, kept so that every call returns the code it always has: an FP8 C's
+// own arguments come first; a single-matrix call checks its sizes and pointers (check_args) before the type pair, a
+// stacked call after the type pair and its count.  Stacked calls also refuse (B200_ERR_BAD_ARG) groups > kMaxGroups,
+// B_g that overlap (grouped) or entries of C that overlap (batch), an entry stride above 2^60 / (count - 1), more tiles
+// than the kernel's int index counts and null offsets, and (B200_ERR_UNSUPPORTED) operands not read in place: FP8 has
+// no CUDA-core kernel, and staging every expert's weight would copy all of B.  The last index of each blockwise scale,
+// and of a dynamic-mode scale_c, has a byte offset that fits a signed 64-bit integer.
+int fp8_check(const Fp8Call& f) {
   auto fp8 = [](int t) { return t == B200_FP8_E4M3 || t == B200_FP8_E5M2; };
-  if (!fp8(a_type) || !fp8(b_type)) return B200_ERR_BAD_ARG;
-  if ((a_blk != 1 && a_blk != 128) || (b_blk != 1 && b_blk != 128)) return B200_ERR_BAD_ARG;
-  if (sa_row < 0 || sa_kb < 0 || sb_kb < 0 || sb_col < 0) return B200_ERR_BAD_ARG;
-  int rc = check_args(m, n, k, A, lda, B, ldb, C, ldc, op_a, op_b);
-  if (rc < 0) return rc;
-  if (a_type == B200_FP8_E5M2 && b_type == B200_FP8_E5M2) return B200_ERR_UNSUPPORTED;
-  if (a_blk == 128 && b_blk == 128) return B200_ERR_UNSUPPORTED;      // not a torch recipe
-  if (rc == 1) return 1;
-  if (!scale_a || !scale_b) return B200_ERR_BAD_ARG;
-  const long long q = (k + 127LL) / 128;
-  const __int128 max_index = INT64_MAX / 4;                           // the byte offset fits a signed 64-bit integer
-  if (last_scale_index(a_blk == 1 ? m : (m + 127LL) / 128, q, sa_row, sa_kb) > max_index ||
-      last_scale_index(b_blk == 1 ? n : (n + 127LL) / 128, q, sb_col, sb_kb) > max_index)
+  if (f.q8) {
+    if (!fp8(f.c_type) || f.act < B200_ACT_NONE || f.act > B200_ACT_GELU_TANH) return B200_ERR_BAD_ARG;
+    if ((f.scale_c && (f.scale_result || f.sc_row < 0 || f.sc_blk < 0)) || f.sc_entry < 0) return B200_ERR_BAD_ARG;
+  } else if (f.out_type != B200_OUT_F32 && f.out_type != B200_OUT_BF16 && f.out_type != B200_OUT_F16) {
     return B200_ERR_BAD_ARG;
+  }
+  if (!fp8(f.a_type) || !fp8(f.b_type) || (f.fast != 0 && f.fast != 1)) return B200_ERR_BAD_ARG;
+  if ((f.a_step != 0 && f.a_step != 1) || (f.b_step != 0 && f.b_step != 1)) return B200_ERR_BAD_ARG;
+  if ((f.a_blk != 1 && f.a_blk != 128) || (f.b_blk != 1 && f.b_blk != 128)) return B200_ERR_BAD_ARG;
+  if (f.sa_row < 0 || f.sa_kb < 0 || f.sb_kb < 0 || f.sb_col < 0 || f.sa_entry < 0 || f.sb_entry < 0)
+    return B200_ERR_BAD_ARG;
+  if (f.count < 0 || f.stride_a < 0 || f.stride_b < 0 || f.stride_c < 0) return B200_ERR_BAD_ARG;
+  if (f.stack == STACK_GROUP && f.count > kMaxGroups) return B200_ERR_BAD_ARG;
+  const bool stacked = f.stack != STACK_NONE;
+  int rc = 0;
+  if (!stacked && (rc = check_args(f.m, f.n, f.k, f.A, f.lda, f.B, f.ldb, f.C, f.ldc, f.op_a, f.op_b)) < 0) return rc;
+  if (stacked && (f.m < 0 || f.n < 0 || f.k < 0)) return B200_ERR_BAD_ARG;
+  if (f.a_type == B200_FP8_E5M2 && f.b_type == B200_FP8_E5M2) return B200_ERR_UNSUPPORTED;
+  if (f.a_blk == 128 && f.b_blk == 128) return B200_ERR_UNSUPPORTED;      // not a torch recipe
+  if (stacked && f.count == 0) return 1;
+  if (stacked) rc = check_args(f.m, f.n, f.k, f.A, f.lda, f.B, f.ldb, f.C, f.ldc, f.op_a, f.op_b);
+  if (rc) return rc;
+  if (!f.scale_a || !f.scale_b || (f.stack == STACK_GROUP && !f.offs)) return B200_ERR_BAD_ARG;
+  const long long qn = (f.n + 127LL) / 128, q = (f.k + 127LL) / 128;
+  if (f.count > 1) {
+    const long long max_stride = (1LL << 60) / (f.count - 1);
+    if (f.stride_a > max_stride || f.stride_b > max_stride || f.stride_c > max_stride || f.sa_entry > max_stride ||
+        f.sb_entry > max_stride)
+      return B200_ERR_BAD_ARG;
+    if (f.stack == STACK_GROUP && f.stride_b < (long long)f.n * f.ldb) return B200_ERR_BAD_ARG;
+    if (f.stack == STACK_BATCH && (f.stride_c < (long long)(f.m - 1) * f.ldc + f.n ||
+                                   ((f.m + 127LL) / 128) * qn > 0x7FFFFFFFLL / 4 / f.count))    // tiles of one entry < 2^48
+      return B200_ERR_BAD_ARG;
+  }
+  if (f.stack == STACK_GROUP && qn > 0x3FFFFFFFLL / grouped_tile_rows(f.m, f.count)) return B200_ERR_BAD_ARG;
+  const __int128 max_index = INT64_MAX / 4;
+  if (f.blockwise && (last_scale_index(f.count, f.sa_entry, f.a_blk == 1 ? f.m : (f.m + 127LL) / 128, q, f.sa_row,
+                                       f.sa_kb) > max_index ||
+                      last_scale_index(f.count, f.sb_entry, f.b_blk == 1 ? f.n : qn, q, f.sb_col, f.sb_kb) > max_index))
+    return B200_ERR_BAD_ARG;
+  if (stacked && f.k > 0 &&
+      (!aligned16(f.A) || !aligned16(f.B) || f.lda % 16 || f.ldb % 16 ||
+       (f.count > 1 && (!batch_tma_ok(f.stride_a, f.m, f.lda, 1) || !batch_tma_ok(f.stride_b, f.n, f.ldb, 1)))))
+    return B200_ERR_UNSUPPORTED;
+  if (f.q8 && (f.scale_c || stacked)) {
+    // Dynamic mode: scale_c is row-major (m, q_n) (sc_blk == 1, sc_row >= q_n) or outer-dim-major (sc_row == 1,
+    // sc_blk >= m), the stride of an extent-1 dimension being free; anything else could overlap.  A batch's entries,
+    // sc_entry apart, do not overlap either.  Static mode (no scale_c) is single-matrix only.
+    const bool row_major = (qn == 1 || f.sc_blk == 1) && (f.m == 1 || f.sc_row >= qn);
+    const bool col_major = (f.m == 1 || f.sc_row == 1) && (qn == 1 || f.sc_blk >= f.m);
+    const __int128 last = last_scale_index(1, 0, f.m, qn, f.sc_row, f.sc_blk);
+    if (!f.scale_c || !(row_major || col_major) || last > max_index) return B200_ERR_BAD_ARG;
+    if (f.stack == STACK_BATCH && f.count > 1 &&
+        (f.sc_entry < last + 1 || f.sc_entry > (1LL << 60) / (f.count - 1) ||
+         last_scale_index(f.count, f.sc_entry, f.m, qn, f.sc_row, f.sc_blk) > max_index))
+      return B200_ERR_BAD_ARG;
+  }
   return 0;
 }
 
-// C = round_out(sum + bias_j), sum = fma(acc_kb, rn(sa_kb(i) * sb_kb(j)), sum) over the k-blocks in order from +0;
-// every argument is checked before the device is touched.
-int gemm_fp8_blockwise(int op_a, int op_b, int a_type, int b_type, int m, int n, int k, const uint8_t* A, int lda,
-                       const uint8_t* B, int ldb, const float* scale_a, int a_blk, long long sa_row, long long sa_kb,
-                       const float* scale_b, int b_blk, long long sb_kb, long long sb_col, const void* bias, void* C,
-                       int ldc, int out_type, cudaStream_t st) {
-  if (out_type != B200_OUT_F32 && out_type != B200_OUT_BF16 && out_type != B200_OUT_F16) return B200_ERR_BAD_ARG;
-  if (int rc = fp8_blockwise_args(op_a, op_b, a_type, b_type, m, n, k, A, lda, B, ldb, scale_a, a_blk, sa_row, sa_kb,
-                                  scale_b, b_blk, sb_kb, sb_col, C, ldc))
-    return rc < 0 ? rc : 0;
-  return fp8_run(op_a, op_b, a_type, b_type, m, n, k, A, lda, B, ldb, C, ldc, out_type,
-                 TcBlockScale{scale_a, scale_b, sa_row, sa_kb, sb_kb, sb_col, a_blk, b_blk, bias}, 0, st);
+// The kernel's argument for the call's scale recipe (BLK), C (Q8) and stacking: TcScale ... TcStackBlockScaleQ8.  A
+// stacked one takes the stack (st) in launch_tc.
+template <bool BLK, bool Q8, int STACK>
+using Fp8Arg = std::conditional_t<
+    STACK == STACK_NONE,
+    std::conditional_t<BLK, std::conditional_t<Q8, TcBlockScaleQ8, TcBlockScale>, std::conditional_t<Q8, TcScaleQ8, TcScale>>,
+    std::conditional_t<BLK, std::conditional_t<Q8, TcStackBlockScaleQ8, TcStackBlockScale>,
+                       std::conditional_t<Q8, TcStackScaleQ8, TcStackScale>>>;
+template <bool BLK, bool Q8, int STACK>
+Fp8Arg<BLK, Q8, STACK> fp8_arg(const Fp8Call& f) {
+  Fp8Arg<BLK, Q8, STACK> s{};
+  s.a = f.scale_a; s.b = f.scale_b; s.bias = f.bias;
+  if constexpr (BLK) {
+    s.a_row = f.sa_row; s.a_kb = f.sa_kb; s.b_kb = f.sb_kb; s.b_col = f.sb_col; s.a_blk = f.a_blk; s.b_blk = f.b_blk;
+  } else {
+    s.a_step = f.a_step; s.b_step = f.b_step;
+  }
+  if constexpr (STACK != STACK_NONE) { s.a_entry_stride = f.sa_entry; s.b_entry_stride = f.sb_entry; }
+  if constexpr (Q8) s.q = TcQ8{f.scale_result, f.scale_c, f.sc_row, f.sc_blk, f.act};
+  if constexpr (Q8 && STACK != STACK_NONE) s.sc_entry_stride = f.sc_entry;
+  return s;
 }
 
-// ---- FP8 output (torch._scaled_mm's scale_result; the fused 1 x 128 quantisation of C) --------------------------------
-// Kernel names by [kind][C type: 0 = e4m3, 1 = e5m2][width index as kFp8Names; no 192-wide tile].
-#define FP8_Q8_NAMES(P)                                                                                               \
-  {{P "_oe4m3_128x256", nullptr, P "_oe4m3_128x128", P "_oe4m3_acc_128x128", P "_oe4m3_blk_128x128"},                 \
-   {P "_oe5m2_128x256", nullptr, P "_oe5m2_128x128", P "_oe5m2_acc_128x128", P "_oe5m2_blk_128x128"}}
-const char* const kFp8Q8Names[3][2][5] = {FP8_Q8_NAMES("tc_e4m3"), FP8_Q8_NAMES("tc_e4m3e5m2"),
-                                          FP8_Q8_NAMES("tc_e5m2e4m3")};
-
-// The output arguments of the _q8 entry points that need no sizes: C type, activation, mode and strides.
-int fp8_q8_out_args(int c_type, int act, const float* scale_result, const float* scale_c, long long sc_row,
-                    long long sc_blk) {
-  if (c_type != B200_FP8_E4M3 && c_type != B200_FP8_E5M2) return B200_ERR_BAD_ARG;
-  if (act < B200_ACT_NONE || act > B200_ACT_GELU_TANH) return B200_ERR_BAD_ARG;
-  if (scale_c && (scale_result || sc_row < 0 || sc_blk < 0)) return B200_ERR_BAD_ARG;
-  return 0;
+// fast: one accumulator over K at pick_bn's width (a batch counts the tiles of all its entries, a grouped call its
+// bound of tile rows); else promoted per 128-element k-block (two 64 x BN fp32 tiles in registers: BN = 128).
+// Blockwise scales are always promoted; their indices are logical (row, k-block) / (k-block, column), so staging never
+// touches them.  An FP8 C has no 192-wide tile: its 128-column scale blocks must not straddle tiles.
+// Every layout and pitch of a single matrix runs on the tensor cores: (N, T) with TMA-able operands is read in place;
+// otherwise the operands are made K-major and TMA-able in the workspace (stage_kmajor), which holds the same bytes, so
+// every route is bit-identical to the aligned (N, T) call.  A stacked call is read in place (fp8_check).
+template <int KIND, typename OutT, int STACK, class Scale>
+int tc_fp8(const Fp8Call& f, const Stack& stk, const Scale& sc, const char* const (&names)[5], const Call& c) {
+  constexpr bool blk = std::is_base_of<TcBlockScale, Scale>::value;
+  const int m = f.m, n = f.n, k = f.k;
+  auto run = [&](const void* a, long long la, const void* b, long long lb) {
+    if constexpr (!blk)
+      if (f.fast) {
+        const int bn_m = STACK == STACK_GROUP ? 128 : m;
+        const int bn_batch = STACK == STACK_GROUP ? (int)grouped_tile_rows(m, stk.count) : stk.count;
+        return with_width<!Fp8Out<OutT>::V>(bn_m, n, [&](auto W) {
+          using Wd = decltype(W);
+          return launch_tc<KIND, Wd::BN, Wd::STAGES, OutT, ProdSingle, 128, LAYOUT_K, LAYOUT_K, false, STACK>(
+              m, n, k, a, la, m, 0, b, lb, n, 0, f.C, f.ldc, names[Wd::idx], c, 0, nullptr, nullptr, &stk, &sc);
+        }, bn_batch);
+      }
+    return launch_tc<KIND, 128, Width<128>::STAGES, OutT, ProdPromoted, 128, LAYOUT_K, LAYOUT_K, false, STACK>(
+        m, n, k, a, la, m, 0, b, lb, n, 0, f.C, f.ldc, names[blk ? 4 : 3], c, 128, nullptr, nullptr, &stk, &sc);
+  };
+  if constexpr (STACK == STACK_NONE) {
+    const bool copy_a = !f.op_a && !(aligned16(f.A) && f.lda % 16 == 0);
+    const bool copy_b = f.op_b && !(aligned16(f.B) && f.ldb % 16 == 0);
+    const int sa = f.op_a || copy_a, sb = f.op_b && !copy_b;      // kmajor_ws_bytes / stage_kmajor's view of the layout
+    if (sa || !sb) {
+      const void* A = f.A; const void* B = f.B;
+      long long lda = f.lda, ldb = f.ldb;
+      WsLease ws(kmajor_ws_bytes(sa, sb, m, n, k, 1), c.st);
+      if (ws.rc) return ws.rc;
+      if (int rc = stage_kmajor<uint8_t>(sa, sb, m, n, k, A, lda, B, ldb, ws.base(), c.st, copy_a, copy_b)) return rc;
+      return run(A, lda, B, ldb);
+    }
+  }
+  return run(f.A, f.lda, f.B, f.ldb);
 }
-// Dynamic mode with work to do: scale_c is row-major (m, q_n) (sc_blk == 1, sc_row >= q_n) or outer-dim-major
-// (sc_row == 1, sc_blk >= m), the stride of an extent-1 dimension being free; anything else could overlap.  The last
-// index's byte offset fits a signed 64-bit integer.
-bool fp8_q8_scale_layout_ok(int m, int n, long long sc_row, long long sc_blk) {
-  const long long qn = (n + 127LL) / 128;
-  const bool row_major = (qn == 1 || sc_blk == 1) && (m == 1 || sc_row >= qn);
-  const bool col_major = (m == 1 || sc_row == 1) && (qn == 1 || sc_blk >= m);
-  return (row_major || col_major) && last_scale_index(m, qn, sc_row, sc_blk) <= INT64_MAX / 4;
-}
 
-// k == 0: the element-wise pass (fp8_q8_k0_kernel), no operand and no input scale read.
+// k == 0, FP8 C: the element-wise pass (fp8_q8_k0_kernel), no operand and no input scale read.
 template <typename OutT>
 int fp8_q8_k0(int m, int n, void* C, int ldc, const void* bias, const TcQ8& q, cudaStream_t st) {
   const long long items = (long long)m * ((n + 127) / 128);
@@ -1643,396 +1668,8 @@ int fp8_q8_k0(int m, int n, void* C, int ldc, const void* bias, const TcQ8& q, c
   return last_launch_status();
 }
 
-// Every FP8-output call after its argument checks (Scale = TcScaleQ8 or TcBlockScaleQ8): the routes of fp8_run.
-template <class Scale>
-int fp8_q8_run(int op_a, int op_b, int a_type, int b_type, int m, int n, int k, const uint8_t* A, int lda,
-               const uint8_t* B, int ldb, void* C, int ldc, int c_type, const Scale& sc, int fast_accum, cudaStream_t st) {
-  if (int rc = ensure_device()) return rc;
-  Call c{st};
-  const bool e4 = c_type == B200_FP8_E4M3;
-  if (k == 0)
-    return e4 ? fp8_q8_k0<e4m3_out>(m, n, C, ldc, sc.bias, sc.q, st) : fp8_q8_k0<e5m2_out>(m, n, C, ldc, sc.bias, sc.q, st);
-  auto kind = [&](auto K) {
-    constexpr int KIND = decltype(K)::value;
-    const auto& names = kFp8Q8Names[KIND - KIND_E4M3][e4 ? 0 : 1];
-    if (e4) return tc_fp8<KIND, e4m3_out>(op_a, op_b, m, n, k, A, lda, B, ldb, C, ldc, sc, fast_accum, names, c);
-    return tc_fp8<KIND, e5m2_out>(op_a, op_b, m, n, k, A, lda, B, ldb, C, ldc, sc, fast_accum, names, c);
-  };
-  if (a_type == B200_FP8_E5M2) return kind(std::integral_constant<int, KIND_E5M2E4M3>());
-  if (b_type == B200_FP8_E5M2) return kind(std::integral_constant<int, KIND_E4M3E5M2>());
-  return kind(std::integral_constant<int, KIND_E4M3>());
-}
-
-int gemm_fp8_q8(int op_a, int op_b, int a_type, int b_type, int m, int n, int k, const uint8_t* A, int lda,
-                const uint8_t* B, int ldb, const float* scale_a, int scale_a_rowwise, const float* scale_b,
-                int scale_b_colwise, const uint16_t* bias, int act, int fast_accum, int c_type, uint8_t* C, int ldc,
-                const float* scale_result, float* scale_c, long long sc_row, long long sc_blk, cudaStream_t st) {
-  if (int rc = fp8_q8_out_args(c_type, act, scale_result, scale_c, sc_row, sc_blk)) return rc;
-  if (int rc = fp8_args(op_a, op_b, a_type, b_type, m, n, k, A, lda, B, ldb, scale_a, scale_a_rowwise, scale_b,
-                        scale_b_colwise, C, ldc, fast_accum))
-    return rc < 0 ? rc : 0;
-  if (scale_c && !fp8_q8_scale_layout_ok(m, n, sc_row, sc_blk)) return B200_ERR_BAD_ARG;
-  TcScaleQ8 sc;
-  static_cast<TcScale&>(sc) = TcScale{scale_a, scale_b, scale_a_rowwise, scale_b_colwise, bias};
-  sc.q = TcQ8{scale_result, scale_c, sc_row, sc_blk, act};
-  return fp8_q8_run(op_a, op_b, a_type, b_type, m, n, k, A, lda, B, ldb, C, ldc, c_type, sc, fast_accum, st);
-}
-
-int gemm_fp8_blockwise_q8(int op_a, int op_b, int a_type, int b_type, int m, int n, int k, const uint8_t* A, int lda,
-                          const uint8_t* B, int ldb, const float* scale_a, int a_blk, long long sa_row, long long sa_kb,
-                          const float* scale_b, int b_blk, long long sb_kb, long long sb_col, const uint16_t* bias,
-                          int act, int c_type, uint8_t* C, int ldc, const float* scale_result, float* scale_c,
-                          long long sc_row, long long sc_blk, cudaStream_t st) {
-  if (int rc = fp8_q8_out_args(c_type, act, scale_result, scale_c, sc_row, sc_blk)) return rc;
-  if (int rc = fp8_blockwise_args(op_a, op_b, a_type, b_type, m, n, k, A, lda, B, ldb, scale_a, a_blk, sa_row, sa_kb,
-                                  scale_b, b_blk, sb_kb, sb_col, C, ldc))
-    return rc < 0 ? rc : 0;
-  if (scale_c && !fp8_q8_scale_layout_ok(m, n, sc_row, sc_blk)) return B200_ERR_BAD_ARG;
-  TcBlockScaleQ8 sc;
-  static_cast<TcBlockScale&>(sc) = TcBlockScale{scale_a, scale_b, sa_row, sa_kb, sb_kb, sb_col, a_blk, b_blk, bias};
-  sc.q = TcQ8{scale_result, scale_c, sc_row, sc_blk, act};
-  return fp8_q8_run(op_a, op_b, a_type, b_type, m, n, k, A, lda, B, ldb, C, ldc, c_type, sc, 0, st);
-}
-
-// ---- grouped and strided-batched FP8 GEMMs (torch._scaled_grouped_mm 2-D x 3-D and 3-D x 3-D) ---------------------------
-// gemm_tc_fp8_kernel over a stack: row-major A, every B_b stored n x k (B^T, torch's column-major mat_b), rowwise
-// scales, no bias, no workspace.  The operands are read in place only (FP8 has no CUDA-core kernel, and staging every
-// expert's weight would copy all of B), so the entry points refuse what TMA cannot describe.
-// Kernel names by [stacking: 0 = grouped, 1 = batch][kind][C type][width index, 3 = promoted, 4 = blockwise].
-#define FP8_STACK_NAMES(P, S)                                                                                           \
-  {{P "_of32_" S "_128x256", P "_of32_" S "_128x192", P "_of32_" S "_128x128", P "_of32_" S "_acc_128x128",            \
-    P "_of32_" S "_blk_128x128"},                                                                                       \
-   {P "_obf16_" S "_128x256", P "_obf16_" S "_128x192", P "_obf16_" S "_128x128", P "_obf16_" S "_acc_128x128",        \
-    P "_obf16_" S "_blk_128x128"},                                                                                      \
-   {P "_of16_" S "_128x256", P "_of16_" S "_128x192", P "_of16_" S "_128x128", P "_of16_" S "_acc_128x128",            \
-    P "_of16_" S "_blk_128x128"}}
-const char* const kFp8StackNames[2][3][3][5] = {
-    {FP8_STACK_NAMES("tc_e4m3", "grp"), FP8_STACK_NAMES("tc_e4m3e5m2", "grp"), FP8_STACK_NAMES("tc_e5m2e4m3", "grp")},
-    {FP8_STACK_NAMES("tc_e4m3", "bat"), FP8_STACK_NAMES("tc_e4m3e5m2", "bat"), FP8_STACK_NAMES("tc_e5m2e4m3", "bat")}};
-
-// The stacked call *stk (m = total_m for a grouped call) at pick_bn's width over the stack's tiles (fast), or promoted
-// per 128-element k-block at BN = 128, as tc_fp8 chooses for one matrix.  Blockwise scales (Scale = TcStackBlockScale
-// / TcStackBlockScaleQ8) are always promoted.  An FP8 C has no 192-wide tile, as in tc_fp8.
-template <int KIND, typename OutT, int STACK, class Scale>
-int tc_fp8_stacked(int m, int n, int k, const void* A, int lda, const void* B, int ldb, void* C, int ldc,
-                   const Stack& stk, const Scale& sc, bool fast, const char* const (&names)[5], const Call& c) {
-  constexpr bool blk = std::is_same<Scale, TcStackBlockScale>::value || std::is_same<Scale, TcStackBlockScaleQ8>::value;
-  // m rows of A per entry (a grouped A is one entry of total_m rows); every B entry is n x k
-  if constexpr (!blk)
-    if (fast) {
-      const int bn_m = STACK == STACK_GROUP ? 128 : m;
-      const int bn_batch = STACK == STACK_GROUP ? (int)grouped_tile_rows(m, stk.count) : stk.count;
-      return with_width<!Fp8Out<OutT>::V>(bn_m, n, [&](auto W) {
-        using Wd = decltype(W);
-        return launch_tc<KIND, Wd::BN, Wd::STAGES, OutT, ProdSingle, 128, LAYOUT_K, LAYOUT_K, false, STACK>(
-            m, n, k, A, lda, m, 0, B, ldb, n, 0, C, ldc, names[Wd::idx], c, 0, nullptr, nullptr, &stk, &sc);
-      }, bn_batch);
-    }
-  return launch_tc<KIND, 128, Width<128>::STAGES, OutT, ProdPromoted, 128, LAYOUT_K, LAYOUT_K, false, STACK>(
-      m, n, k, A, lda, m, 0, B, ldb, n, 0, C, ldc, names[blk ? 4 : 3], c, 128, nullptr, nullptr, &stk, &sc);
-}
-
-template <int STACK, class Scale>
-int fp8_stacked_run(int a_type, int b_type, int m, int n, int k, const uint8_t* A, int lda, const uint8_t* B, int ldb,
-                    void* C, int ldc, int out_type, const Stack& stk, const Scale& sc, int fast, cudaStream_t st) {
-  if (int rc = ensure_device()) return rc;
-  Call c{st};
-  if (k == 0) {                                             // +0 over the covered rows / entries, no scale read
-    if (out_type == B200_OUT_F32)
-      return STACK == STACK_GROUP ? degenerate_grouped<float>(m, n, C, ldc, stk, c) : degenerate_batched<float>(m, n, C, ldc, stk, c);
-    return STACK == STACK_GROUP ? degenerate_grouped<uint16_t>(m, n, C, ldc, stk, c)
-                                : degenerate_batched<uint16_t>(m, n, C, ldc, stk, c);
-  }
-  const int kind = a_type == B200_FP8_E5M2 ? 2 : b_type == B200_FP8_E5M2 ? 1 : 0;
-  const auto& names = kFp8StackNames[STACK == STACK_GROUP ? 0 : 1][kind][out_type];
-  auto by_out = [&](auto kd) {
-    constexpr int KIND = decltype(kd)::value;
-    if (out_type == B200_OUT_F32)
-      return tc_fp8_stacked<KIND, float, STACK>(m, n, k, A, lda, B, ldb, C, ldc, stk, sc, fast, names, c);
-    if (out_type == B200_OUT_BF16)
-      return tc_fp8_stacked<KIND, bf16_out, STACK>(m, n, k, A, lda, B, ldb, C, ldc, stk, sc, fast, names, c);
-    return tc_fp8_stacked<KIND, f16_out, STACK>(m, n, k, A, lda, B, ldb, C, ldc, stk, sc, fast, names, c);
-  };
-  if (kind == 2) return by_out(std::integral_constant<int, KIND_E5M2E4M3>());
-  if (kind == 1) return by_out(std::integral_constant<int, KIND_E4M3E5M2>());
-  return by_out(std::integral_constant<int, KIND_E4M3>());
-}
-
-// The checks every stacked FP8 call shares: operand types, output type and fast_accum are B200_ERR_BAD_ARG, and
-// (e5m2, e5m2) is B200_ERR_UNSUPPORTED, as for b200_gemm_fp8.  The output type is checked by the entry points (the
-// _q8 ones take an FP8 C type instead); the rest here.
-bool fp8_out_type_ok(int out_type) {
-  return out_type == B200_OUT_F32 || out_type == B200_OUT_BF16 || out_type == B200_OUT_F16;
-}
-int fp8_stacked_types(int a_type, int b_type, int fast_accum) {
-  auto fp8 = [](int t) { return t == B200_FP8_E4M3 || t == B200_FP8_E5M2; };
-  if (!fp8(a_type) || !fp8(b_type)) return B200_ERR_BAD_ARG;
-  if (fast_accum != 0 && fast_accum != 1) return B200_ERR_BAD_ARG;
-  return 0;
-}
-// In-place operands: 16-byte aligned bases and 16-byte multiple pitches (FP8 elements are bytes).
-bool fp8_in_place(const void* A, long long lda, const void* B, long long ldb) {
-  return aligned16(A) && aligned16(B) && lda % 16 == 0 && ldb % 16 == 0;
-}
-
-// Rows [end_{g-1}, end_g) of C = round_out((A_rows B_g^T * sa_i) * sb_g[j]), B_g = B + g * stride_b (n x k), sb_g =
-// scale_b + g * scale_b_stride, sa_i = scale_a[i] at the row i of A; the ends are b200_gemm_bf16_grouped's, read on the
-// device.  Argument rules (all before the device is touched): b200_gemm_fp8's on types and flags, b200_gemm_bf16_grouped's
-// on sizes, groups, offsets, overlap and the tile bound for an op_b = T call, negative scale_b_stride or one whose last
-// group's offset exceeds 2^60 elements, null scales with work to do (B200_ERR_BAD_ARG); operands not read in place
-// (B200_ERR_UNSUPPORTED).  groups == 0, total_m == 0 or n == 0 is a no-op.
-// fp8_grouped_args: b200_gemm_fp8_grouped's checks other than the output type, in its order: < 0 an error, 1 nothing
-// to do, 0 run.
-int fp8_grouped_args(int a_type, int b_type, int total_m, int n, int k, const uint8_t* A, int lda, const uint8_t* B,
-                     int ldb, long long stride_b, const int32_t* offs, int groups, const float* scale_a,
-                     const float* scale_b, long long scale_b_stride, const void* C, int ldc, int fast_accum) {
-  if (int rc = fp8_stacked_types(a_type, b_type, fast_accum)) return rc;
-  if (groups < 0 || stride_b < 0 || scale_b_stride < 0 || groups > kMaxGroups) return B200_ERR_BAD_ARG;
-  if (total_m < 0 || n < 0 || k < 0) return B200_ERR_BAD_ARG;
-  if (a_type == B200_FP8_E5M2 && b_type == B200_FP8_E5M2) return B200_ERR_UNSUPPORTED;
-  if (groups == 0) return 1;
-  int rc = check_args(total_m, n, k, A, lda, B, ldb, C, ldc, B200_OP_N, B200_OP_T);
-  if (rc) return rc;
-  if (!offs || !scale_a || !scale_b) return B200_ERR_BAD_ARG;
-  if (groups > 1) {
-    if (stride_b < (long long)n * ldb) return B200_ERR_BAD_ARG;                          // B_g would overlap
-    if (stride_b > (1LL << 60) / (groups - 1) || scale_b_stride > (1LL << 60) / (groups - 1)) return B200_ERR_BAD_ARG;
-  }
-  const long long tiles_n = (n + 127LL) / 128;
-  if (tiles_n > 0x3FFFFFFFLL / grouped_tile_rows(total_m, groups)) return B200_ERR_BAD_ARG;
-  if (k > 0 && (!fp8_in_place(A, lda, B, ldb) || (groups > 1 && !batch_tma_ok(stride_b, n, ldb, 1))))
-    return B200_ERR_UNSUPPORTED;
-  return 0;
-}
-TcStackScale fp8_grouped_scale(const float* scale_a, const float* scale_b, long long scale_b_stride) {
-  TcStackScale sc{};
-  sc.a = scale_a; sc.b = scale_b; sc.a_step = 1; sc.b_step = 1; sc.bias = nullptr;
-  sc.a_entry_stride = 0; sc.b_entry_stride = scale_b_stride;
-  return sc;
-}
-Stack fp8_grouped_stack(int groups, long long stride_b, const int32_t* offs) {
-  return Stack{groups, 0, groups > 1 ? stride_b : 0, 0, offs};
-}
-
-int gemm_fp8_grouped(int a_type, int b_type, int total_m, int n, int k, const uint8_t* A, int lda, const uint8_t* B,
-                     int ldb, long long stride_b, const int32_t* offs, int groups, const float* scale_a,
-                     const float* scale_b, long long scale_b_stride, void* C, int ldc, int out_type, int fast_accum,
-                     cudaStream_t st) {
-  if (!fp8_out_type_ok(out_type)) return B200_ERR_BAD_ARG;
-  if (int rc = fp8_grouped_args(a_type, b_type, total_m, n, k, A, lda, B, ldb, stride_b, offs, groups, scale_a, scale_b,
-                                scale_b_stride, C, ldc, fast_accum))
-    return rc < 0 ? rc : 0;
-  return fp8_stacked_run<STACK_GROUP>(a_type, b_type, total_m, n, k, A, lda, B, ldb, C, ldc, out_type,
-                                      fp8_grouped_stack(groups, stride_b, offs),
-                                      fp8_grouped_scale(scale_a, scale_b, scale_b_stride), fast_accum, st);
-}
-
-// C_b = round_out((A_b B_b^T * sa_b[i]) * sb_b[j]) for b < batch, X_b = X + b * stride_x, sa_b = scale_a + b *
-// scale_a_stride, sb_b = scale_b + b * scale_b_stride (elements).  Argument rules (all before the device is touched):
-// b200_gemm_fp8's on types and flags and b200_gemm_bf16_batched's on sizes, strides, C overlap and the tile bound, with
-// the scale strides bounded like the operand strides, null scales with work to do (B200_ERR_BAD_ARG); operands not read
-// in place, an input stride other than 0 or at least one entry included (B200_ERR_UNSUPPORTED).  batch == 0, m == 0 or
-// n == 0 is a no-op; batch == 1 is the (N, T) b200_gemm_fp8 call with rowwise scales.
-// fp8_batched_args: b200_gemm_fp8_batched's checks other than the output type, in its order: < 0 an error, 1 nothing
-// to do, 0 run.
-int fp8_batched_args(int a_type, int b_type, int m, int n, int k, const uint8_t* A, int lda, long long stride_a,
-                     const uint8_t* B, int ldb, long long stride_b, const float* scale_a, long long scale_a_stride,
-                     const float* scale_b, long long scale_b_stride, const void* C, int ldc, long long stride_c,
-                     int batch, int fast_accum) {
-  if (int rc = fp8_stacked_types(a_type, b_type, fast_accum)) return rc;
-  if (batch < 0 || stride_a < 0 || stride_b < 0 || stride_c < 0 || scale_a_stride < 0 || scale_b_stride < 0)
-    return B200_ERR_BAD_ARG;
-  if (m < 0 || n < 0 || k < 0) return B200_ERR_BAD_ARG;
-  if (a_type == B200_FP8_E5M2 && b_type == B200_FP8_E5M2) return B200_ERR_UNSUPPORTED;
-  if (batch == 0) return 1;
-  int rc = check_args(m, n, k, A, lda, B, ldb, C, ldc, B200_OP_N, B200_OP_T);
-  if (rc) return rc;
-  if (!scale_a || !scale_b) return B200_ERR_BAD_ARG;
-  if (batch > 1) {
-    if (stride_c < (long long)(m - 1) * ldc + n) return B200_ERR_BAD_ARG;               // entries of C would overlap
-    const long long max_stride = (1LL << 60) / (batch - 1);
-    if (stride_a > max_stride || stride_b > max_stride || stride_c > max_stride || scale_a_stride > max_stride ||
-        scale_b_stride > max_stride)
-      return B200_ERR_BAD_ARG;
-    const long long tiles1 = ((m + 127LL) / 128) * ((n + 127LL) / 128);                  // < 2^48
-    if (tiles1 > 0x7FFFFFFFLL / 4 / batch) return B200_ERR_BAD_ARG;
-  }
-  if (k > 0 && (!fp8_in_place(A, lda, B, ldb) ||
-                (batch > 1 && (!batch_tma_ok(stride_a, m, lda, 1) || !batch_tma_ok(stride_b, n, ldb, 1)))))
-    return B200_ERR_UNSUPPORTED;
-  return 0;
-}
-TcStackScale fp8_batched_scale(const float* scale_a, long long scale_a_stride, const float* scale_b,
-                               long long scale_b_stride) {
-  TcStackScale sc{};
-  sc.a = scale_a; sc.b = scale_b; sc.a_step = 1; sc.b_step = 1; sc.bias = nullptr;
-  sc.a_entry_stride = scale_a_stride; sc.b_entry_stride = scale_b_stride;
-  return sc;
-}
-
-int gemm_fp8_batched(int a_type, int b_type, int m, int n, int k, const uint8_t* A, int lda, long long stride_a,
-                     const uint8_t* B, int ldb, long long stride_b, const float* scale_a, long long scale_a_stride,
-                     const float* scale_b, long long scale_b_stride, void* C, int ldc, long long stride_c, int batch,
-                     int out_type, int fast_accum, cudaStream_t st) {
-  if (!fp8_out_type_ok(out_type)) return B200_ERR_BAD_ARG;
-  if (int rc = fp8_batched_args(a_type, b_type, m, n, k, A, lda, stride_a, B, ldb, stride_b, scale_a, scale_a_stride,
-                                scale_b, scale_b_stride, C, ldc, stride_c, batch, fast_accum))
-    return rc < 0 ? rc : 0;
-  if (batch == 1)
-    return gemm_fp8(B200_OP_N, B200_OP_T, a_type, b_type, m, n, k, A, lda, B, ldb, scale_a, 1, scale_b, 1, nullptr, C, ldc,
-                    out_type, fast_accum, st);
-  return fp8_stacked_run<STACK_BATCH>(a_type, b_type, m, n, k, A, lda, B, ldb, C, ldc, out_type,
-                                      Stack{batch, stride_a, stride_b, stride_c, nullptr},
-                                      fp8_batched_scale(scale_a, scale_a_stride, scale_b, scale_b_stride), fast_accum, st);
-}
-
-// ---- grouped and strided-batched blockwise FP8 GEMMs (DeepSeek-V3-style MoE layers) -----------------------------------
-// Every entry is the (N, T) b200_gemm_fp8_blockwise call with no bias on its rows, B and scales, in one launch of the
-// stacked blockwise kernel.  The checks are those of the rowwise stacked calls above and of gemm_fp8_blockwise, with
-// each scale's last index bound including (count - 1) * its entry stride; all before the device is touched.
-
-// Element index of the last scale of a stack of `count` entries `entry_stride` apart (last_scale_index's rule).
-__int128 last_stacked_scale_index(long long count, long long entry_stride, long long rows, long long q,
-                                  long long row_stride, long long kb_stride) {
-  return (__int128)(count - 1) * entry_stride + last_scale_index(rows, q, row_stride, kb_stride);
-}
-
-// Rows [end_{g-1}, end_g) of C = the blockwise product of those rows of A with B_g = B + g * stride_b (n x k); scale_a
-// is 1 x 128 over the stacked A (row i of A: scale_a[i * sa_row + kb * sa_kb]; a 128-row block would straddle groups),
-// scale_b of group g starts at scale_b + g * scale_b_stride, 1 x 128 or 128 x 128 (b_blk).
-// fp8_blockwise_grouped_args: its checks other than the output type, in its order: < 0 an error, 1 nothing to do, 0 run.
-int fp8_blockwise_grouped_args(int a_type, int b_type, int total_m, int n, int k, const uint8_t* A, int lda,
-                               const uint8_t* B, int ldb, long long stride_b, const int32_t* offs, int groups,
-                               const float* scale_a, long long sa_row, long long sa_kb, const float* scale_b, int b_blk,
-                               long long sb_kb, long long sb_col, long long scale_b_stride, const void* C, int ldc) {
-  if (int rc = fp8_stacked_types(a_type, b_type, 0)) return rc;
-  if (b_blk != 1 && b_blk != 128) return B200_ERR_BAD_ARG;
-  if (sa_row < 0 || sa_kb < 0 || sb_kb < 0 || sb_col < 0 || scale_b_stride < 0) return B200_ERR_BAD_ARG;
-  if (groups < 0 || stride_b < 0 || groups > kMaxGroups) return B200_ERR_BAD_ARG;
-  if (total_m < 0 || n < 0 || k < 0) return B200_ERR_BAD_ARG;
-  if (a_type == B200_FP8_E5M2 && b_type == B200_FP8_E5M2) return B200_ERR_UNSUPPORTED;
-  if (groups == 0) return 1;
-  int rc = check_args(total_m, n, k, A, lda, B, ldb, C, ldc, B200_OP_N, B200_OP_T);
-  if (rc) return rc;
-  if (!offs || !scale_a || !scale_b) return B200_ERR_BAD_ARG;
-  if (groups > 1) {
-    if (stride_b < (long long)n * ldb) return B200_ERR_BAD_ARG;                          // B_g would overlap
-    if (stride_b > (1LL << 60) / (groups - 1) || scale_b_stride > (1LL << 60) / (groups - 1)) return B200_ERR_BAD_ARG;
-  }
-  const long long tiles_n = (n + 127LL) / 128;
-  if (tiles_n > 0x3FFFFFFFLL / grouped_tile_rows(total_m, groups)) return B200_ERR_BAD_ARG;
-  const long long q = (k + 127LL) / 128;
-  const __int128 max_index = INT64_MAX / 4;
-  if (last_scale_index(total_m, q, sa_row, sa_kb) > max_index ||
-      last_stacked_scale_index(groups, scale_b_stride, b_blk == 1 ? n : tiles_n, q, sb_col, sb_kb) > max_index)
-    return B200_ERR_BAD_ARG;
-  if (k > 0 && (!fp8_in_place(A, lda, B, ldb) || (groups > 1 && !batch_tma_ok(stride_b, n, ldb, 1))))
-    return B200_ERR_UNSUPPORTED;
-  return 0;
-}
-TcStackBlockScale fp8_blockwise_stack_scale(const float* scale_a, int a_blk, long long sa_row, long long sa_kb,
-                                            long long scale_a_stride, const float* scale_b, int b_blk, long long sb_kb,
-                                            long long sb_col, long long scale_b_stride) {
-  TcStackBlockScale sc{};
-  sc.a = scale_a; sc.b = scale_b; sc.a_row = sa_row; sc.a_kb = sa_kb; sc.b_kb = sb_kb; sc.b_col = sb_col;
-  sc.a_blk = a_blk; sc.b_blk = b_blk; sc.bias = nullptr;
-  sc.a_entry_stride = scale_a_stride; sc.b_entry_stride = scale_b_stride;
-  return sc;
-}
-
-int gemm_fp8_blockwise_grouped(int a_type, int b_type, int total_m, int n, int k, const uint8_t* A, int lda,
-                               const uint8_t* B, int ldb, long long stride_b, const int32_t* offs, int groups,
-                               const float* scale_a, long long sa_row, long long sa_kb, const float* scale_b, int b_blk,
-                               long long sb_kb, long long sb_col, long long scale_b_stride, void* C, int ldc,
-                               int out_type, cudaStream_t st) {
-  if (!fp8_out_type_ok(out_type)) return B200_ERR_BAD_ARG;
-  if (int rc = fp8_blockwise_grouped_args(a_type, b_type, total_m, n, k, A, lda, B, ldb, stride_b, offs, groups, scale_a,
-                                          sa_row, sa_kb, scale_b, b_blk, sb_kb, sb_col, scale_b_stride, C, ldc))
-    return rc < 0 ? rc : 0;
-  return fp8_stacked_run<STACK_GROUP>(
-      a_type, b_type, total_m, n, k, A, lda, B, ldb, C, ldc, out_type, fp8_grouped_stack(groups, stride_b, offs),
-      fp8_blockwise_stack_scale(scale_a, 1, sa_row, sa_kb, 0, scale_b, b_blk, sb_kb, sb_col, scale_b_stride), 0, st);
-}
-
-// C_b = the blockwise product of A_b = A + b * stride_a (m x k) and B_b = B + b * stride_b (n x k), C_b = C + b *
-// stride_c, with entry b's scales at scale_a + b * scale_a_stride and scale_b + b * scale_b_stride, each indexed as by
-// gemm_fp8_blockwise.  batch == 1 is the (N, T) b200_gemm_fp8_blockwise call with no bias.
-// fp8_blockwise_batched_args: its checks other than the output type, in its order: < 0 an error, 1 nothing to do, 0 run.
-int fp8_blockwise_batched_args(int a_type, int b_type, int m, int n, int k, const uint8_t* A, int lda, long long stride_a,
-                               const uint8_t* B, int ldb, long long stride_b, const float* scale_a, int a_blk,
-                               long long sa_row, long long sa_kb, long long scale_a_stride, const float* scale_b,
-                               int b_blk, long long sb_kb, long long sb_col, long long scale_b_stride, const void* C,
-                               int ldc, long long stride_c, int batch) {
-  if (int rc = fp8_stacked_types(a_type, b_type, 0)) return rc;
-  if ((a_blk != 1 && a_blk != 128) || (b_blk != 1 && b_blk != 128)) return B200_ERR_BAD_ARG;
-  if (sa_row < 0 || sa_kb < 0 || sb_kb < 0 || sb_col < 0) return B200_ERR_BAD_ARG;
-  if (batch < 0 || stride_a < 0 || stride_b < 0 || stride_c < 0 || scale_a_stride < 0 || scale_b_stride < 0)
-    return B200_ERR_BAD_ARG;
-  if (m < 0 || n < 0 || k < 0) return B200_ERR_BAD_ARG;
-  if (a_type == B200_FP8_E5M2 && b_type == B200_FP8_E5M2) return B200_ERR_UNSUPPORTED;
-  if (a_blk == 128 && b_blk == 128) return B200_ERR_UNSUPPORTED;      // not a torch recipe
-  if (batch == 0) return 1;
-  int rc = check_args(m, n, k, A, lda, B, ldb, C, ldc, B200_OP_N, B200_OP_T);
-  if (rc) return rc;
-  if (!scale_a || !scale_b) return B200_ERR_BAD_ARG;
-  if (batch > 1) {
-    if (stride_c < (long long)(m - 1) * ldc + n) return B200_ERR_BAD_ARG;               // entries of C would overlap
-    const long long max_stride = (1LL << 60) / (batch - 1);
-    if (stride_a > max_stride || stride_b > max_stride || stride_c > max_stride || scale_a_stride > max_stride ||
-        scale_b_stride > max_stride)
-      return B200_ERR_BAD_ARG;
-    const long long tiles1 = ((m + 127LL) / 128) * ((n + 127LL) / 128);                  // < 2^48
-    if (tiles1 > 0x7FFFFFFFLL / 4 / batch) return B200_ERR_BAD_ARG;
-  }
-  const long long q = (k + 127LL) / 128;
-  const __int128 max_index = INT64_MAX / 4;
-  if (last_stacked_scale_index(batch, scale_a_stride, a_blk == 1 ? m : (m + 127LL) / 128, q, sa_row, sa_kb) > max_index ||
-      last_stacked_scale_index(batch, scale_b_stride, b_blk == 1 ? n : (n + 127LL) / 128, q, sb_col, sb_kb) > max_index)
-    return B200_ERR_BAD_ARG;
-  if (k > 0 && (!fp8_in_place(A, lda, B, ldb) ||
-                (batch > 1 && (!batch_tma_ok(stride_a, m, lda, 1) || !batch_tma_ok(stride_b, n, ldb, 1)))))
-    return B200_ERR_UNSUPPORTED;
-  return 0;
-}
-
-int gemm_fp8_blockwise_batched(int a_type, int b_type, int m, int n, int k, const uint8_t* A, int lda, long long stride_a,
-                               const uint8_t* B, int ldb, long long stride_b, const float* scale_a, int a_blk,
-                               long long sa_row, long long sa_kb, long long scale_a_stride, const float* scale_b,
-                               int b_blk, long long sb_kb, long long sb_col, long long scale_b_stride, void* C, int ldc,
-                               long long stride_c, int batch, int out_type, cudaStream_t st) {
-  if (!fp8_out_type_ok(out_type)) return B200_ERR_BAD_ARG;
-  if (int rc = fp8_blockwise_batched_args(a_type, b_type, m, n, k, A, lda, stride_a, B, ldb, stride_b, scale_a, a_blk,
-                                          sa_row, sa_kb, scale_a_stride, scale_b, b_blk, sb_kb, sb_col, scale_b_stride,
-                                          C, ldc, stride_c, batch))
-    return rc < 0 ? rc : 0;
-  if (batch == 1)
-    return gemm_fp8_blockwise(B200_OP_N, B200_OP_T, a_type, b_type, m, n, k, A, lda, B, ldb, scale_a, a_blk, sa_row,
-                              sa_kb, scale_b, b_blk, sb_kb, sb_col, nullptr, C, ldc, out_type, st);
-  return fp8_stacked_run<STACK_BATCH>(
-      a_type, b_type, m, n, k, A, lda, B, ldb, C, ldc, out_type, Stack{batch, stride_a, stride_b, stride_c, nullptr},
-      fp8_blockwise_stack_scale(scale_a, a_blk, sa_row, sa_kb, scale_a_stride, scale_b, b_blk, sb_kb, sb_col,
-                                scale_b_stride),
-      0, st);
-}
-
-// ---- FP8 outputs of the grouped and batched FP8 GEMMs (the fused 1 x 128 quantisation of each entry's C) -------------
-// Every entry's C and scale_c are those of the (N, T) single-matrix _q8 / _blockwise_q8 call in dynamic mode with no
-// bias on its rows, B and scales, at the same tile width; one launch of gemm_tc_fp8_q8_stacked_kernel.  The checks are
-// the parent stacked call's and fp8_q8_out_args, then scale_c's layout over (total_m, q_n), or (m, q_n) per entry with
-// entries that do not overlap; all before the device is touched.
-// Kernel names by [stacking: 0 = grouped, 1 = batch][kind][C type: 0 = e4m3, 1 = e5m2][width index as kFp8Q8Names].
-#define FP8_STACK_Q8_NAMES(P, S)                                                                                         \
-  {{P "_oe4m3_" S "_128x256", nullptr, P "_oe4m3_" S "_128x128", P "_oe4m3_" S "_acc_128x128",                          \
-    P "_oe4m3_" S "_blk_128x128"},                                                                                      \
-   {P "_oe5m2_" S "_128x256", nullptr, P "_oe5m2_" S "_128x128", P "_oe5m2_" S "_acc_128x128",                          \
-    P "_oe5m2_" S "_blk_128x128"}}
-const char* const kFp8StackQ8Names[2][3][2][5] = {
-    {FP8_STACK_Q8_NAMES("tc_e4m3", "grp"), FP8_STACK_Q8_NAMES("tc_e4m3e5m2", "grp"),
-     FP8_STACK_Q8_NAMES("tc_e5m2e4m3", "grp")},
-    {FP8_STACK_Q8_NAMES("tc_e4m3", "bat"), FP8_STACK_Q8_NAMES("tc_e4m3e5m2", "bat"),
-     FP8_STACK_Q8_NAMES("tc_e5m2e4m3", "bat")}};
-
-// k == 0: act(+0) quantised and d = 1 over the covered rows / entries (fp8_q8_k0_stacked_kernel), no scale read.
+// k == 0, stacked FP8 C: act(+0) quantised and d = 1 over the covered rows / entries (fp8_q8_k0_stacked_kernel), no
+// scale read.
 template <typename OutT, int STACK>
 int fp8_q8_k0_stacked(int m, int n, void* C, int ldc, const Stack& stk, const TcQ8& q, long long sc_entry_stride,
                       cudaStream_t st) {
@@ -2045,127 +1682,63 @@ int fp8_q8_k0_stacked(int m, int n, void* C, int ldc, const Stack& stk, const Tc
   return last_launch_status();
 }
 
-// Every stacked FP8-output call after its argument checks (Scale = TcStackScaleQ8 or TcStackBlockScaleQ8).
-template <int STACK, class Scale>
-int fp8_q8_stacked_run(int a_type, int b_type, int m, int n, int k, const uint8_t* A, int lda, const uint8_t* B, int ldb,
-                       void* C, int ldc, int c_type, const Stack& stk, const Scale& sc, int fast, cudaStream_t st) {
+// Every FP8 call: its checks, then one launch.  A batch of one is the single-matrix (N, T) call: the same kernel, name
+// and bits.  k == 0 reads no operand and no scale: C = round_out(+0 + bias_j) (or +0) through the bias pass with beta =
+// 0 or the zero fill over the rows or entries the call covers, or an FP8 C's element-wise pass.  Otherwise the type
+// pair selects the kind, the C type the kernel's OutT, and the stacking and scale recipe the kernel.
+int fp8_gemm(Fp8Call f, void* stream) {
+  if (int rc = fp8_check(f)) return rc < 0 ? rc : 0;
+  if (f.stack == STACK_BATCH && f.count == 1) f.stack = STACK_NONE;
   if (int rc = ensure_device()) return rc;
+  const cudaStream_t st = (cudaStream_t)stream;
   Call c{st};
-  const bool e4 = c_type == B200_FP8_E4M3;
-  if (k == 0)
-    return e4 ? fp8_q8_k0_stacked<e4m3_out, STACK>(m, n, C, ldc, stk, sc.q, sc.sc_entry_stride, st)
-              : fp8_q8_k0_stacked<e5m2_out, STACK>(m, n, C, ldc, stk, sc.q, sc.sc_entry_stride, st);
-  const int kind = a_type == B200_FP8_E5M2 ? 2 : b_type == B200_FP8_E5M2 ? 1 : 0;
-  const auto& names = kFp8StackQ8Names[STACK == STACK_GROUP ? 0 : 1][kind][e4 ? 0 : 1];
-  auto by_out = [&](auto kd) {
-    constexpr int KIND = decltype(kd)::value;
-    if (e4) return tc_fp8_stacked<KIND, e4m3_out, STACK>(m, n, k, A, lda, B, ldb, C, ldc, stk, sc, fast, names, c);
-    return tc_fp8_stacked<KIND, e5m2_out, STACK>(m, n, k, A, lda, B, ldb, C, ldc, stk, sc, fast, names, c);
-  };
-  if (kind == 2) return by_out(std::integral_constant<int, KIND_E5M2E4M3>());
-  if (kind == 1) return by_out(std::integral_constant<int, KIND_E4M3E5M2>());
-  return by_out(std::integral_constant<int, KIND_E4M3>());
-}
-
-// The output checks of a stacked _q8 call with work to do (the parent's checks passed): scale_c present, and laid out
-// as fp8_q8_scale_layout_ok requires over one entry's (rows, q_n); batch > 1: entries sc_entry_stride apart that do
-// not overlap, the stride bounded as the other entry strides and the last index's byte offset a signed 64-bit integer.
-int fp8_q8_stacked_scale_args(int rows, int n, const float* scale_c, long long sc_row, long long sc_blk,
-                              long long sc_entry_stride, int batch) {
-  if (!scale_c || !fp8_q8_scale_layout_ok(rows, n, sc_row, sc_blk)) return B200_ERR_BAD_ARG;
-  if (batch > 1) {
-    const long long qn = (n + 127LL) / 128;
-    const __int128 last = last_scale_index(rows, qn, sc_row, sc_blk);
-    if (sc_entry_stride < last + 1 || sc_entry_stride > (1LL << 60) / (batch - 1)) return B200_ERR_BAD_ARG;
-    if (last_stacked_scale_index(batch, sc_entry_stride, rows, qn, sc_row, sc_blk) > INT64_MAX / 4) return B200_ERR_BAD_ARG;
+  const Stack stk{f.count, f.stride_a, f.count > 1 ? f.stride_b : 0, f.stride_c, f.offs};
+  if (f.k == 0 && f.q8) {
+    const TcQ8 q{f.scale_result, f.scale_c, f.sc_row, f.sc_blk, f.act};
+    auto k0 = [&](auto out) {
+      using O = decltype(out);
+      if (f.stack == STACK_GROUP) return fp8_q8_k0_stacked<O, STACK_GROUP>(f.m, f.n, f.C, f.ldc, stk, q, f.sc_entry, st);
+      if (f.stack == STACK_BATCH) return fp8_q8_k0_stacked<O, STACK_BATCH>(f.m, f.n, f.C, f.ldc, stk, q, f.sc_entry, st);
+      return fp8_q8_k0<O>(f.m, f.n, f.C, f.ldc, f.bias, q, st);
+    };
+    return f.c_type == B200_FP8_E4M3 ? k0(e4m3_out()) : k0(e5m2_out());
   }
-  return 0;
-}
-
-int gemm_fp8_grouped_q8(int a_type, int b_type, int total_m, int n, int k, const uint8_t* A, int lda, const uint8_t* B,
-                        int ldb, long long stride_b, const int32_t* offs, int groups, const float* scale_a,
-                        const float* scale_b, long long scale_b_stride, int act, int fast_accum, int c_type, uint8_t* C,
-                        int ldc, float* scale_c, long long sc_row, long long sc_blk, cudaStream_t st) {
-  if (int rc = fp8_q8_out_args(c_type, act, nullptr, scale_c, sc_row, sc_blk)) return rc;
-  if (int rc = fp8_grouped_args(a_type, b_type, total_m, n, k, A, lda, B, ldb, stride_b, offs, groups, scale_a, scale_b,
-                                scale_b_stride, C, ldc, fast_accum))
-    return rc < 0 ? rc : 0;
-  if (int rc = fp8_q8_stacked_scale_args(total_m, n, scale_c, sc_row, sc_blk, 0, 1)) return rc;
-  TcStackScaleQ8 sc;
-  static_cast<TcStackScale&>(sc) = fp8_grouped_scale(scale_a, scale_b, scale_b_stride);
-  sc.q = TcQ8{nullptr, scale_c, sc_row, sc_blk, act};
-  sc.sc_entry_stride = 0;
-  return fp8_q8_stacked_run<STACK_GROUP>(a_type, b_type, total_m, n, k, A, lda, B, ldb, C, ldc, c_type,
-                                         fp8_grouped_stack(groups, stride_b, offs), sc, fast_accum, st);
-}
-
-int gemm_fp8_batched_q8(int a_type, int b_type, int m, int n, int k, const uint8_t* A, int lda, long long stride_a,
-                        const uint8_t* B, int ldb, long long stride_b, const float* scale_a, long long scale_a_stride,
-                        const float* scale_b, long long scale_b_stride, int act, int fast_accum, int c_type, uint8_t* C,
-                        int ldc, long long stride_c, float* scale_c, long long sc_row, long long sc_blk,
-                        long long sc_entry_stride, int batch, cudaStream_t st) {
-  if (int rc = fp8_q8_out_args(c_type, act, nullptr, scale_c, sc_row, sc_blk)) return rc;
-  if (sc_entry_stride < 0) return B200_ERR_BAD_ARG;
-  if (int rc = fp8_batched_args(a_type, b_type, m, n, k, A, lda, stride_a, B, ldb, stride_b, scale_a, scale_a_stride,
-                                scale_b, scale_b_stride, C, ldc, stride_c, batch, fast_accum))
-    return rc < 0 ? rc : 0;
-  if (int rc = fp8_q8_stacked_scale_args(m, n, scale_c, sc_row, sc_blk, sc_entry_stride, batch)) return rc;
-  if (batch == 1)
-    return gemm_fp8_q8(B200_OP_N, B200_OP_T, a_type, b_type, m, n, k, A, lda, B, ldb, scale_a, 1, scale_b, 1, nullptr, act,
-                       fast_accum, c_type, C, ldc, nullptr, scale_c, sc_row, sc_blk, st);
-  TcStackScaleQ8 sc;
-  static_cast<TcStackScale&>(sc) = fp8_batched_scale(scale_a, scale_a_stride, scale_b, scale_b_stride);
-  sc.q = TcQ8{nullptr, scale_c, sc_row, sc_blk, act};
-  sc.sc_entry_stride = sc_entry_stride;
-  return fp8_q8_stacked_run<STACK_BATCH>(a_type, b_type, m, n, k, A, lda, B, ldb, C, ldc, c_type,
-                                         Stack{batch, stride_a, stride_b, stride_c, nullptr}, sc, fast_accum, st);
-}
-
-int gemm_fp8_blockwise_grouped_q8(int a_type, int b_type, int total_m, int n, int k, const uint8_t* A, int lda,
-                                  const uint8_t* B, int ldb, long long stride_b, const int32_t* offs, int groups,
-                                  const float* scale_a, long long sa_row, long long sa_kb, const float* scale_b,
-                                  int b_blk, long long sb_kb, long long sb_col, long long scale_b_stride, int act,
-                                  int c_type, uint8_t* C, int ldc, float* scale_c, long long sc_row, long long sc_blk,
-                                  cudaStream_t st) {
-  if (int rc = fp8_q8_out_args(c_type, act, nullptr, scale_c, sc_row, sc_blk)) return rc;
-  if (int rc = fp8_blockwise_grouped_args(a_type, b_type, total_m, n, k, A, lda, B, ldb, stride_b, offs, groups, scale_a,
-                                          sa_row, sa_kb, scale_b, b_blk, sb_kb, sb_col, scale_b_stride, C, ldc))
-    return rc < 0 ? rc : 0;
-  if (int rc = fp8_q8_stacked_scale_args(total_m, n, scale_c, sc_row, sc_blk, 0, 1)) return rc;
-  TcStackBlockScaleQ8 sc;
-  static_cast<TcStackBlockScale&>(sc) =
-      fp8_blockwise_stack_scale(scale_a, 1, sa_row, sa_kb, 0, scale_b, b_blk, sb_kb, sb_col, scale_b_stride);
-  sc.q = TcQ8{nullptr, scale_c, sc_row, sc_blk, act};
-  sc.sc_entry_stride = 0;
-  return fp8_q8_stacked_run<STACK_GROUP>(a_type, b_type, total_m, n, k, A, lda, B, ldb, C, ldc, c_type,
-                                         fp8_grouped_stack(groups, stride_b, offs), sc, 0, st);
-}
-
-int gemm_fp8_blockwise_batched_q8(int a_type, int b_type, int m, int n, int k, const uint8_t* A, int lda,
-                                  long long stride_a, const uint8_t* B, int ldb, long long stride_b, const float* scale_a,
-                                  int a_blk, long long sa_row, long long sa_kb, long long scale_a_stride,
-                                  const float* scale_b, int b_blk, long long sb_kb, long long sb_col,
-                                  long long scale_b_stride, int act, int c_type, uint8_t* C, int ldc, long long stride_c,
-                                  float* scale_c, long long sc_row, long long sc_blk, long long sc_entry_stride,
-                                  int batch, cudaStream_t st) {
-  if (int rc = fp8_q8_out_args(c_type, act, nullptr, scale_c, sc_row, sc_blk)) return rc;
-  if (sc_entry_stride < 0) return B200_ERR_BAD_ARG;
-  if (int rc = fp8_blockwise_batched_args(a_type, b_type, m, n, k, A, lda, stride_a, B, ldb, stride_b, scale_a, a_blk,
-                                          sa_row, sa_kb, scale_a_stride, scale_b, b_blk, sb_kb, sb_col, scale_b_stride,
-                                          C, ldc, stride_c, batch))
-    return rc < 0 ? rc : 0;
-  if (int rc = fp8_q8_stacked_scale_args(m, n, scale_c, sc_row, sc_blk, sc_entry_stride, batch)) return rc;
-  if (batch == 1)
-    return gemm_fp8_blockwise_q8(B200_OP_N, B200_OP_T, a_type, b_type, m, n, k, A, lda, B, ldb, scale_a, a_blk, sa_row,
-                                 sa_kb, scale_b, b_blk, sb_kb, sb_col, nullptr, act, c_type, C, ldc, nullptr, scale_c,
-                                 sc_row, sc_blk, st);
-  TcStackBlockScaleQ8 sc;
-  static_cast<TcStackBlockScale&>(sc) = fp8_blockwise_stack_scale(scale_a, a_blk, sa_row, sa_kb, scale_a_stride, scale_b,
-                                                                  b_blk, sb_kb, sb_col, scale_b_stride);
-  sc.q = TcQ8{nullptr, scale_c, sc_row, sc_blk, act};
-  sc.sc_entry_stride = sc_entry_stride;
-  return fp8_q8_stacked_run<STACK_BATCH>(a_type, b_type, m, n, k, A, lda, B, ldb, C, ldc, c_type,
-                                         Stack{batch, stride_a, stride_b, stride_c, nullptr}, sc, 0, st);
+  if (f.k == 0) {
+    const bool c32 = f.out_type == B200_OUT_F32;
+    if (f.stack == STACK_GROUP)
+      return c32 ? degenerate_grouped<float>(f.m, f.n, f.C, f.ldc, stk, c) : degenerate_grouped<uint16_t>(f.m, f.n, f.C, f.ldc, stk, c);
+    if (f.stack == STACK_BATCH)
+      return c32 ? degenerate_batched<float>(f.m, f.n, f.C, f.ldc, stk, c) : degenerate_batched<uint16_t>(f.m, f.n, f.C, f.ldc, stk, c);
+    if (f.bias) { c.bias = f.bias; c.act = ACT_NONE; }
+    if (c32) return degenerate<float, float>(f.m, f.n, f.C, f.ldc, c);
+    if (f.out_type == B200_OUT_BF16) return degenerate<uint16_t, uint16_t>(f.m, f.n, f.C, f.ldc, c);
+    return degenerate<__half, __half>(f.m, f.n, f.C, f.ldc, c);
+  }
+  const int ci = f.q8 ? 3 + (f.c_type == B200_FP8_E5M2) : f.out_type;      // kFp8Names' C type
+  auto launch = [&](auto kind, auto out) {
+    constexpr int KIND = decltype(kind)::value;
+    using OutT = decltype(out);
+    auto stacked = [&](auto stack) {
+      constexpr int STACK = decltype(stack)::value;
+      constexpr bool Q8 = Fp8Out<OutT>::V;
+      const auto& names = kFp8Names[STACK][KIND - KIND_E4M3][ci];
+      if (f.blockwise) return tc_fp8<KIND, OutT, STACK>(f, stk, fp8_arg<true, Q8, STACK>(f), names, c);
+      return tc_fp8<KIND, OutT, STACK>(f, stk, fp8_arg<false, Q8, STACK>(f), names, c);
+    };
+    if (f.stack == STACK_GROUP) return stacked(std::integral_constant<int, STACK_GROUP>());
+    if (f.stack == STACK_BATCH) return stacked(std::integral_constant<int, STACK_BATCH>());
+    return stacked(std::integral_constant<int, STACK_NONE>());
+  };
+  auto by_c = [&](auto kind) {
+    if (ci == 0) return launch(kind, float());
+    if (ci == 1) return launch(kind, bf16_out());
+    if (ci == 2) return launch(kind, f16_out());
+    if (ci == 3) return launch(kind, e4m3_out());
+    return launch(kind, e5m2_out());
+  };
+  if (f.a_type == B200_FP8_E5M2) return by_c(std::integral_constant<int, KIND_E5M2E4M3>());
+  if (f.b_type == B200_FP8_E5M2) return by_c(std::integral_constant<int, KIND_E4M3E5M2>());
+  return by_c(std::integral_constant<int, KIND_E4M3>());
 }
 
 }  // namespace
@@ -2371,17 +1944,24 @@ int b200_gemm_s8s32(int m, int n, int k, const int8_t* dA, int lda, const int8_t
 int b200_gemm_fp8(int op_a, int op_b, int a_type, int b_type, int m, int n, int k, const uint8_t* dA, int lda,
                   const uint8_t* dB, int ldb, const float* dScaleA, int scale_a_rowwise, const float* dScaleB,
                   int scale_b_colwise, const void* dBias, void* dC, int ldc, int out_type, int fast_accum, void* stream) {
-  return gemm_fp8(op_a, op_b, a_type, b_type, m, n, k, dA, lda, dB, ldb, dScaleA, scale_a_rowwise, dScaleB,
-                  scale_b_colwise, dBias, dC, ldc, out_type, fast_accum, (cudaStream_t)stream);
+  Fp8Call f(a_type, b_type, m, n, k, dA, lda, dB, ldb, dC, ldc);
+  f.op_a = op_a; f.op_b = op_b;
+  f.scale_a = dScaleA; f.a_step = scale_a_rowwise; f.scale_b = dScaleB; f.b_step = scale_b_colwise;
+  f.bias = dBias; f.fast = fast_accum; f.out_type = out_type;
+  return fp8_gemm(f, stream);
 }
 
 int b200_gemm_fp8_blockwise(int op_a, int op_b, int a_type, int b_type, int m, int n, int k, const uint8_t* dA, int lda,
                             const uint8_t* dB, int ldb, const float* dScaleA, int scale_a_block, long long sa_row_stride,
                             long long sa_kb_stride, const float* dScaleB, int scale_b_block, long long sb_kb_stride,
                             long long sb_col_stride, const void* dBias, void* dC, int ldc, int out_type, void* stream) {
-  return gemm_fp8_blockwise(op_a, op_b, a_type, b_type, m, n, k, dA, lda, dB, ldb, dScaleA, scale_a_block, sa_row_stride,
-                            sa_kb_stride, dScaleB, scale_b_block, sb_kb_stride, sb_col_stride, dBias, dC, ldc, out_type,
-                            (cudaStream_t)stream);
+  Fp8Call f(a_type, b_type, m, n, k, dA, lda, dB, ldb, dC, ldc);
+  f.op_a = op_a; f.op_b = op_b;
+  f.blockwise = true;
+  f.scale_a = dScaleA; f.a_blk = scale_a_block; f.sa_row = sa_row_stride; f.sa_kb = sa_kb_stride;
+  f.scale_b = dScaleB; f.b_blk = scale_b_block; f.sb_kb = sb_kb_stride; f.sb_col = sb_col_stride;
+  f.bias = dBias; f.out_type = out_type;
+  return fp8_gemm(f, stream);
 }
 
 int b200_gemm_fp8_q8(int op_a, int op_b, int a_type, int b_type, int m, int n, int k, const uint8_t* dA, int lda,
@@ -2389,9 +1969,13 @@ int b200_gemm_fp8_q8(int op_a, int op_b, int a_type, int b_type, int m, int n, i
                      int scale_b_colwise, const uint16_t* dBiasBf16, int act, int fast_accum, int c_type, uint8_t* dC,
                      int ldc, const float* dScaleResult, float* dScaleC, long long sc_row_stride,
                      long long sc_blk_stride, void* stream) {
-  return gemm_fp8_q8(op_a, op_b, a_type, b_type, m, n, k, dA, lda, dB, ldb, dScaleA, scale_a_rowwise, dScaleB,
-                     scale_b_colwise, dBiasBf16, act, fast_accum, c_type, dC, ldc, dScaleResult, dScaleC, sc_row_stride,
-                     sc_blk_stride, (cudaStream_t)stream);
+  Fp8Call f(a_type, b_type, m, n, k, dA, lda, dB, ldb, dC, ldc);
+  f.op_a = op_a; f.op_b = op_b;
+  f.scale_a = dScaleA; f.a_step = scale_a_rowwise; f.scale_b = dScaleB; f.b_step = scale_b_colwise;
+  f.bias = dBiasBf16; f.fast = fast_accum;
+  f.q8 = true; f.c_type = c_type; f.act = act; f.scale_result = dScaleResult;
+  f.scale_c = dScaleC; f.sc_row = sc_row_stride; f.sc_blk = sc_blk_stride;
+  return fp8_gemm(f, stream);
 }
 
 int b200_gemm_fp8_blockwise_q8(int op_a, int op_b, int a_type, int b_type, int m, int n, int k, const uint8_t* dA,
@@ -2400,26 +1984,37 @@ int b200_gemm_fp8_blockwise_q8(int op_a, int op_b, int a_type, int b_type, int m
                                long long sb_kb_stride, long long sb_col_stride, const uint16_t* dBiasBf16, int act,
                                int c_type, uint8_t* dC, int ldc, const float* dScaleResult, float* dScaleC,
                                long long sc_row_stride, long long sc_blk_stride, void* stream) {
-  return gemm_fp8_blockwise_q8(op_a, op_b, a_type, b_type, m, n, k, dA, lda, dB, ldb, dScaleA, scale_a_block,
-                               sa_row_stride, sa_kb_stride, dScaleB, scale_b_block, sb_kb_stride, sb_col_stride,
-                               dBiasBf16, act, c_type, dC, ldc, dScaleResult, dScaleC, sc_row_stride, sc_blk_stride,
-                               (cudaStream_t)stream);
+  Fp8Call f(a_type, b_type, m, n, k, dA, lda, dB, ldb, dC, ldc);
+  f.op_a = op_a; f.op_b = op_b;
+  f.blockwise = true;
+  f.scale_a = dScaleA; f.a_blk = scale_a_block; f.sa_row = sa_row_stride; f.sa_kb = sa_kb_stride;
+  f.scale_b = dScaleB; f.b_blk = scale_b_block; f.sb_kb = sb_kb_stride; f.sb_col = sb_col_stride;
+  f.bias = dBiasBf16;
+  f.q8 = true; f.c_type = c_type; f.act = act; f.scale_result = dScaleResult;
+  f.scale_c = dScaleC; f.sc_row = sc_row_stride; f.sc_blk = sc_blk_stride;
+  return fp8_gemm(f, stream);
 }
 
 int b200_gemm_fp8_grouped(int a_type, int b_type, int total_m, int n, int k, const uint8_t* dA, int lda,
                           const uint8_t* dB, int ldb, long long stride_b, const int32_t* dOffs, int groups,
                           const float* dScaleA, const float* dScaleB, long long scale_b_stride, void* dC, int ldc,
                           int out_type, int fast_accum, void* stream) {
-  return gemm_fp8_grouped(a_type, b_type, total_m, n, k, dA, lda, dB, ldb, stride_b, dOffs, groups, dScaleA, dScaleB,
-                          scale_b_stride, dC, ldc, out_type, fast_accum, (cudaStream_t)stream);
+  Fp8Call f(a_type, b_type, total_m, n, k, dA, lda, dB, ldb, dC, ldc);
+  f.stack = STACK_GROUP; f.count = groups; f.stride_b = stride_b; f.offs = dOffs;
+  f.scale_a = dScaleA; f.scale_b = dScaleB; f.sb_entry = scale_b_stride;
+  f.fast = fast_accum; f.out_type = out_type;
+  return fp8_gemm(f, stream);
 }
 
 int b200_gemm_fp8_batched(int a_type, int b_type, int m, int n, int k, const uint8_t* dA, int lda, long long stride_a,
                           const uint8_t* dB, int ldb, long long stride_b, const float* dScaleA, long long scale_a_stride,
                           const float* dScaleB, long long scale_b_stride, void* dC, int ldc, long long stride_c,
                           int batch, int out_type, int fast_accum, void* stream) {
-  return gemm_fp8_batched(a_type, b_type, m, n, k, dA, lda, stride_a, dB, ldb, stride_b, dScaleA, scale_a_stride, dScaleB,
-                          scale_b_stride, dC, ldc, stride_c, batch, out_type, fast_accum, (cudaStream_t)stream);
+  Fp8Call f(a_type, b_type, m, n, k, dA, lda, dB, ldb, dC, ldc);
+  f.stack = STACK_BATCH; f.count = batch; f.stride_a = stride_a; f.stride_b = stride_b; f.stride_c = stride_c;
+  f.scale_a = dScaleA; f.sa_entry = scale_a_stride; f.scale_b = dScaleB; f.sb_entry = scale_b_stride;
+  f.fast = fast_accum; f.out_type = out_type;
+  return fp8_gemm(f, stream);
 }
 
 int b200_gemm_fp8_blockwise_grouped(int a_type, int b_type, int total_m, int n, int k, const uint8_t* dA, int lda,
@@ -2428,9 +2023,14 @@ int b200_gemm_fp8_blockwise_grouped(int a_type, int b_type, int total_m, int n, 
                                     const float* dScaleB, int scale_b_block, long long sb_kb_stride,
                                     long long sb_col_stride, long long scale_b_stride, void* dC, int ldc, int out_type,
                                     void* stream) {
-  return gemm_fp8_blockwise_grouped(a_type, b_type, total_m, n, k, dA, lda, dB, ldb, stride_b, dOffs, groups, dScaleA,
-                                    sa_row_stride, sa_kb_stride, dScaleB, scale_b_block, sb_kb_stride, sb_col_stride,
-                                    scale_b_stride, dC, ldc, out_type, (cudaStream_t)stream);
+  Fp8Call f(a_type, b_type, total_m, n, k, dA, lda, dB, ldb, dC, ldc);
+  f.stack = STACK_GROUP; f.count = groups; f.stride_b = stride_b; f.offs = dOffs;
+  f.blockwise = true;
+  f.scale_a = dScaleA; f.sa_row = sa_row_stride; f.sa_kb = sa_kb_stride;
+  f.scale_b = dScaleB; f.b_blk = scale_b_block; f.sb_kb = sb_kb_stride; f.sb_col = sb_col_stride;
+  f.sb_entry = scale_b_stride;
+  f.out_type = out_type;
+  return fp8_gemm(f, stream);
 }
 
 int b200_gemm_fp8_blockwise_batched(int a_type, int b_type, int m, int n, int k, const uint8_t* dA, int lda,
@@ -2440,10 +2040,15 @@ int b200_gemm_fp8_blockwise_batched(int a_type, int b_type, int m, int n, int k,
                                     int scale_b_block, long long sb_kb_stride, long long sb_col_stride,
                                     long long scale_b_stride, void* dC, int ldc, long long stride_c, int batch,
                                     int out_type, void* stream) {
-  return gemm_fp8_blockwise_batched(a_type, b_type, m, n, k, dA, lda, stride_a, dB, ldb, stride_b, dScaleA, scale_a_block,
-                                    sa_row_stride, sa_kb_stride, scale_a_stride, dScaleB, scale_b_block, sb_kb_stride,
-                                    sb_col_stride, scale_b_stride, dC, ldc, stride_c, batch, out_type,
-                                    (cudaStream_t)stream);
+  Fp8Call f(a_type, b_type, m, n, k, dA, lda, dB, ldb, dC, ldc);
+  f.stack = STACK_BATCH; f.count = batch; f.stride_a = stride_a; f.stride_b = stride_b; f.stride_c = stride_c;
+  f.blockwise = true;
+  f.scale_a = dScaleA; f.a_blk = scale_a_block; f.sa_row = sa_row_stride; f.sa_kb = sa_kb_stride;
+  f.sa_entry = scale_a_stride;
+  f.scale_b = dScaleB; f.b_blk = scale_b_block; f.sb_kb = sb_kb_stride; f.sb_col = sb_col_stride;
+  f.sb_entry = scale_b_stride;
+  f.out_type = out_type;
+  return fp8_gemm(f, stream);
 }
 
 int b200_gemm_fp8_grouped_q8(int a_type, int b_type, int total_m, int n, int k, const uint8_t* dA, int lda,
@@ -2451,9 +2056,12 @@ int b200_gemm_fp8_grouped_q8(int a_type, int b_type, int total_m, int n, int k, 
                              const float* dScaleA, const float* dScaleB, long long scale_b_stride, int act,
                              int fast_accum, int c_type, uint8_t* dC, int ldc, float* dScaleC, long long sc_row_stride,
                              long long sc_blk_stride, void* stream) {
-  return gemm_fp8_grouped_q8(a_type, b_type, total_m, n, k, dA, lda, dB, ldb, stride_b, dOffs, groups, dScaleA, dScaleB,
-                             scale_b_stride, act, fast_accum, c_type, dC, ldc, dScaleC, sc_row_stride, sc_blk_stride,
-                             (cudaStream_t)stream);
+  Fp8Call f(a_type, b_type, total_m, n, k, dA, lda, dB, ldb, dC, ldc);
+  f.stack = STACK_GROUP; f.count = groups; f.stride_b = stride_b; f.offs = dOffs;
+  f.scale_a = dScaleA; f.scale_b = dScaleB; f.sb_entry = scale_b_stride;
+  f.fast = fast_accum;
+  f.q8 = true; f.c_type = c_type; f.act = act; f.scale_c = dScaleC; f.sc_row = sc_row_stride; f.sc_blk = sc_blk_stride;
+  return fp8_gemm(f, stream);
 }
 
 int b200_gemm_fp8_batched_q8(int a_type, int b_type, int m, int n, int k, const uint8_t* dA, int lda, long long stride_a,
@@ -2462,9 +2070,13 @@ int b200_gemm_fp8_batched_q8(int a_type, int b_type, int m, int n, int k, const 
                              int fast_accum, int c_type, uint8_t* dC, int ldc, long long stride_c, float* dScaleC,
                              long long sc_row_stride, long long sc_blk_stride, long long sc_entry_stride, int batch,
                              void* stream) {
-  return gemm_fp8_batched_q8(a_type, b_type, m, n, k, dA, lda, stride_a, dB, ldb, stride_b, dScaleA, scale_a_stride,
-                             dScaleB, scale_b_stride, act, fast_accum, c_type, dC, ldc, stride_c, dScaleC, sc_row_stride,
-                             sc_blk_stride, sc_entry_stride, batch, (cudaStream_t)stream);
+  Fp8Call f(a_type, b_type, m, n, k, dA, lda, dB, ldb, dC, ldc);
+  f.stack = STACK_BATCH; f.count = batch; f.stride_a = stride_a; f.stride_b = stride_b; f.stride_c = stride_c;
+  f.scale_a = dScaleA; f.sa_entry = scale_a_stride; f.scale_b = dScaleB; f.sb_entry = scale_b_stride;
+  f.fast = fast_accum;
+  f.q8 = true; f.c_type = c_type; f.act = act; f.scale_c = dScaleC; f.sc_row = sc_row_stride; f.sc_blk = sc_blk_stride;
+  f.sc_entry = sc_entry_stride;
+  return fp8_gemm(f, stream);
 }
 
 int b200_gemm_fp8_blockwise_grouped_q8(int a_type, int b_type, int total_m, int n, int k, const uint8_t* dA, int lda,
@@ -2474,10 +2086,14 @@ int b200_gemm_fp8_blockwise_grouped_q8(int a_type, int b_type, int total_m, int 
                                        long long sb_col_stride, long long scale_b_stride, int act, int c_type,
                                        uint8_t* dC, int ldc, float* dScaleC, long long sc_row_stride,
                                        long long sc_blk_stride, void* stream) {
-  return gemm_fp8_blockwise_grouped_q8(a_type, b_type, total_m, n, k, dA, lda, dB, ldb, stride_b, dOffs, groups, dScaleA,
-                                       sa_row_stride, sa_kb_stride, dScaleB, scale_b_block, sb_kb_stride, sb_col_stride,
-                                       scale_b_stride, act, c_type, dC, ldc, dScaleC, sc_row_stride, sc_blk_stride,
-                                       (cudaStream_t)stream);
+  Fp8Call f(a_type, b_type, total_m, n, k, dA, lda, dB, ldb, dC, ldc);
+  f.stack = STACK_GROUP; f.count = groups; f.stride_b = stride_b; f.offs = dOffs;
+  f.blockwise = true;
+  f.scale_a = dScaleA; f.sa_row = sa_row_stride; f.sa_kb = sa_kb_stride;
+  f.scale_b = dScaleB; f.b_blk = scale_b_block; f.sb_kb = sb_kb_stride; f.sb_col = sb_col_stride;
+  f.sb_entry = scale_b_stride;
+  f.q8 = true; f.c_type = c_type; f.act = act; f.scale_c = dScaleC; f.sc_row = sc_row_stride; f.sc_blk = sc_blk_stride;
+  return fp8_gemm(f, stream);
 }
 
 int b200_gemm_fp8_blockwise_batched_q8(int a_type, int b_type, int m, int n, int k, const uint8_t* dA, int lda,
@@ -2488,11 +2104,16 @@ int b200_gemm_fp8_blockwise_batched_q8(int a_type, int b_type, int m, int n, int
                                        long long scale_b_stride, int act, int c_type, uint8_t* dC, int ldc,
                                        long long stride_c, float* dScaleC, long long sc_row_stride,
                                        long long sc_blk_stride, long long sc_entry_stride, int batch, void* stream) {
-  return gemm_fp8_blockwise_batched_q8(a_type, b_type, m, n, k, dA, lda, stride_a, dB, ldb, stride_b, dScaleA,
-                                       scale_a_block, sa_row_stride, sa_kb_stride, scale_a_stride, dScaleB,
-                                       scale_b_block, sb_kb_stride, sb_col_stride, scale_b_stride, act, c_type, dC, ldc,
-                                       stride_c, dScaleC, sc_row_stride, sc_blk_stride, sc_entry_stride, batch,
-                                       (cudaStream_t)stream);
+  Fp8Call f(a_type, b_type, m, n, k, dA, lda, dB, ldb, dC, ldc);
+  f.stack = STACK_BATCH; f.count = batch; f.stride_a = stride_a; f.stride_b = stride_b; f.stride_c = stride_c;
+  f.blockwise = true;
+  f.scale_a = dScaleA; f.a_blk = scale_a_block; f.sa_row = sa_row_stride; f.sa_kb = sa_kb_stride;
+  f.sa_entry = scale_a_stride;
+  f.scale_b = dScaleB; f.b_blk = scale_b_block; f.sb_kb = sb_kb_stride; f.sb_col = sb_col_stride;
+  f.sb_entry = scale_b_stride;
+  f.q8 = true; f.c_type = c_type; f.act = act; f.scale_c = dScaleC; f.sc_row = sc_row_stride; f.sc_blk = sc_blk_stride;
+  f.sc_entry = sc_entry_stride;
+  return fp8_gemm(f, stream);
 }
 
 int b200_gemm_s8s32_op(int op_a, int op_b, int m, int n, int k, const int8_t* dA, int lda, const int8_t* dB, int ldb,

@@ -161,7 +161,7 @@ def test_grouped_q8_argument_validation(gemm):
     """Refusals before the device is touched, each at its bound: they hold with or without a GPU."""
     for call in CALLS:
         rows = SIZE[call]
-        # the output arguments (fp8_q8_out_args)
+        # the output arguments (fp8_check's first checks)
         assert call(gemm, ct=2) == ERR_BAD_ARG and call(gemm, ct=-1) == ERR_BAD_ARG
         assert call(gemm, act=4) == ERR_BAD_ARG and call(gemm, act=-1) == ERR_BAD_ARG
         assert call(gemm, sc_row=-1) == ERR_BAD_ARG and call(gemm, sc_blk=-1) == ERR_BAD_ARG

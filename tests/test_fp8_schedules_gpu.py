@@ -59,7 +59,7 @@ cdiv = ts.cdiv
 
 # ==== schedule model ====================================================================================================
 # A restatement of the FP8 host choices of csrc/capi.cu:
-#   tc_fp8 / tc_fp8_stacked  -> fp8_width()   fast: pick_bn over {256, 192, 128} (FP8 C: {256, 128}; a forced 192 falls
+#   tc_fp8                   -> fp8_width()   fast: pick_bn over {256, 192, 128} (FP8 C: {256, 128}; a forced 192 falls
 #                                             back to the heuristic); promoted and blockwise: always 128
 #   Width<BN>                -> STAGES         4, 5 and 6 stages at BN = 256, 192 and 128
 #   launch_tc                -> schedule()     one CTA per SM, grid = min(tiles, SMs); FP8 never splits K; a grouped
