@@ -296,6 +296,12 @@ cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t sme
   return cudaLaunchKernelEx(&cfg, kern, std::forward<Args>(args)...);
 }
 
+// gridDim.y may not exceed 65535.  A y extent sized from a problem dimension (rows of C, K of a transposed operand) is
+// capped here and its kernel walks y with a grid stride, so every size the ABI accepts launches; below the cap the
+// grid is the uncapped one and the kernel's loop runs once.
+constexpr long long kMaxGridY = 65535;
+inline unsigned grid_y(long long blocks) { return (unsigned)(blocks < kMaxGridY ? blocks : kMaxGridY); }
+
 template <typename T>
 int launch_zero(int m, int n, T* C, int ldc, cudaStream_t st) {
   dim3 grid((n + 255) / 256, m < 4096 ? m : 4096);
@@ -309,12 +315,13 @@ int launch_zero(int m, int n, T* C, int ldc, cudaStream_t st) {
 template <typename InT, typename OutT>
 int launch_generic(int op_a, int op_b, int m, int n, int k, const void* A, int lda, const void* B, int ldb, void* C,
                    int ldc, const char* name, const Call& c) {
-  dim3 grid((n + 63) / 64, (m + 63) / 64);
+  const long long mblocks = (m + 63LL) / 64;
+  dim3 grid((n + 63) / 64, grid_y(mblocks));
   const long long a_rs = op_a ? 1 : lda, a_cs = op_a ? lda : 1, b_rs = op_b ? 1 : ldb, b_cs = op_b ? ldb : 1;
-  gemm_generic_kernel<InT, OutT><<<grid, 256, 0, c.st>>>(m, n, k, static_cast<const InT*>(A), a_rs, a_cs,
-                                                         static_cast<const InT*>(B), b_rs, b_cs, static_cast<OutT*>(C), ldc,
-                                                         c.acc, nullptr, nullptr, c.axpby, c.alpha, c.beta,
-                                                         static_cast<const InT*>(c.bias), c.act);
+  auto kern = mblocks > kMaxGridY ? gemm_generic_kernel<InT, OutT, true> : gemm_generic_kernel<InT, OutT>;
+  kern<<<grid, 256, 0, c.st>>>(m, n, k, static_cast<const InT*>(A), a_rs, a_cs, static_cast<const InT*>(B), b_rs, b_cs,
+                               static_cast<OutT*>(C), ldc, c.acc, nullptr, nullptr, c.axpby, c.alpha, c.beta,
+                               static_cast<const InT*>(c.bias), c.act);
   g_launches++;
   t_last_kernel = name;
   return last_launch_status();
@@ -322,8 +329,10 @@ int launch_generic(int op_a, int op_b, int m, int n, int k, const void* A, int l
 
 int launch_generic_requant(int m, int n, int k, const int8_t* A, int lda, const int8_t* B, int ldb, int8_t* C,
                            int ldc, const float* scales, const float* bias, cudaStream_t st) {
-  dim3 grid((n + 63) / 64, (m + 63) / 64);
-  gemm_generic_kernel<int8_t, int8_t><<<grid, 256, 0, st>>>(m, n, k, A, lda, 1, B, ldb, 1, C, ldc, 0, scales, bias);
+  const long long mblocks = (m + 63LL) / 64;
+  dim3 grid((n + 63) / 64, grid_y(mblocks));
+  auto kern = mblocks > kMaxGridY ? gemm_generic_kernel<int8_t, int8_t, true> : gemm_generic_kernel<int8_t, int8_t>;
+  kern<<<grid, 256, 0, st>>>(m, n, k, A, lda, 1, B, ldb, 1, C, ldc, 0, scales, bias, 0, 1.f, 0.f, nullptr, -1);
   g_launches++;
   t_last_kernel = "generic_s8_requant_64x64";
   return last_launch_status();
@@ -690,8 +699,10 @@ struct WsLease {
 // src (rows x cols, pitch ld) -> dst (cols x rows, pitch dld): one launch.
 template <typename E>
 int launch_transpose(const E* src, long long ld, int rows, int cols, E* dst, long long dld, cudaStream_t st) {
-  launch_pdl(transpose_kernel<E>, dim3((cols + 31) / 32, (rows + 31) / 32), dim3(256), 0, st, 1, src, ld, rows, cols, dst, dld);
+  const cudaError_t e = launch_pdl(transpose_kernel<E>, dim3((cols + 31) / 32, grid_y((rows + 31LL) / 32)), dim3(256), 0,
+                                   st, 1, src, ld, rows, cols, dst, dld);
   g_launches++;
+  if (e != cudaSuccess) { cudaGetLastError(); return (int)e; }
   return last_launch_status();
 }
 
@@ -871,12 +882,13 @@ int launch_f16_split_rows(const float* A, long long lda, int rows, int cols, flo
   return last_launch_status();
 }
 
-// B (rows x cols, scaled by column) -> planes + cmax (must be zero on entry).  Two launches.  zero_buf:
+// B (rows x cols, scaled by column) -> planes + cmax (must be zero on entry).  Two launches, both made even when the
+// first fails (the second clears zero_buf, which the caller counts on), and the first failure returned.  zero_buf:
 // another buffer to clear on the way (the idle half of the double-buffered maxima), or null.
 int launch_f16_split_cols(const float* B, long long ldb, int rows, int cols, float* cmax, uint16_t* planes,
                           long long pitch, int plane_rows, float* zero_buf, int zero_n, cudaStream_t st) {
-  launch_pdl(col_absmax_kernel, dim3((cols + 1023) / 1024, (rows + 15) / 16), dim3(256), 0, st, 1, B, (long long)ldb, rows, cols,
-             reinterpret_cast<unsigned int*>(cmax));
+  const cudaError_t e1 = launch_pdl(col_absmax_kernel, dim3((cols + 1023) / 1024, grid_y((rows + 15LL) / 16)), dim3(256), 0,
+                                    st, 1, B, (long long)ldb, rows, cols, reinterpret_cast<unsigned int*>(cmax));
   const int gx = (int)((pitch + 2047) / 2048);
   int gy = (t_ctx->sms * 8 + gx - 1) / gx;
   if (gy > (plane_rows + 1) / 2) gy = (plane_rows + 1) / 2;
@@ -885,8 +897,9 @@ int launch_f16_split_cols(const float* B, long long ldb, int rows, int cols, flo
     cudaMemsetAsync(zero_buf, 0, (size_t)zero_n * 4, st);
     zero_buf = nullptr;
   }
-  launch_pdl(split_f16_cols_kernel, dim3(gx, gy), dim3(256), 0, st, 1, B, (long long)ldb, rows, cols, (const float*)cmax, planes, pitch, plane_rows, zero_buf, zero_n);
+  const cudaError_t e2 = launch_pdl(split_f16_cols_kernel, dim3(gx, gy), dim3(256), 0, st, 1, B, (long long)ldb, rows, cols, (const float*)cmax, planes, pitch, plane_rows, zero_buf, zero_n);
   g_launches += 2;
+  if (e1 != cudaSuccess || e2 != cudaSuccess) { cudaGetLastError(); return (int)(e1 != cudaSuccess ? e1 : e2); }
   return last_launch_status();
 }
 
@@ -1242,7 +1255,7 @@ int degenerate_batched(int m, int n, void* C, int ldc, const Stack& bt, const Ca
 template <typename InT, typename OutT>
 int launch_generic_batched(int op_a, int op_b, int m, int n, int k, const void* A, int lda, const void* B, int ldb,
                            void* C, int ldc, const Stack& bt, const char* name, const Call& c) {
-  dim3 grid((n + 63) / 64, (m + 63) / 64, bt.count < kMaxGridZ ? bt.count : kMaxGridZ);
+  dim3 grid((n + 63) / 64, grid_y((m + 63LL) / 64), bt.count < kMaxGridZ ? bt.count : kMaxGridZ);
   const long long a_rs = op_a ? 1 : lda, a_cs = op_a ? lda : 1, b_rs = op_b ? 1 : ldb, b_cs = op_b ? ldb : 1;
   gemm_generic_batched_kernel<InT, OutT><<<grid, 256, 0, c.st>>>(
       bt.count, m, n, k, static_cast<const InT*>(A), a_rs, a_cs, bt.sa, static_cast<const InT*>(B), b_rs, b_cs, bt.sb,
@@ -2278,7 +2291,7 @@ int b200_mxf4_quantize_b(int k, int n, const float* dB, int ldb, uint8_t* dQ, ui
   int rc = ensure_device();
   if (rc) return rc;
   const int kpad = (k + 127) & ~127, n_pad = (n + 127) & ~127;
-  mxf4_quantize_cols_t_kernel<<<dim3((n_pad + 255) / 256, kpad / 32), 256, 0, (cudaStream_t)stream>>>(dB, ldb, k, n, dQ, kpad, dSF, n_pad);
+  mxf4_quantize_cols_t_kernel<<<dim3((n_pad + 255) / 256, grid_y(kpad / 32)), 256, 0, (cudaStream_t)stream>>>(dB, ldb, k, n, dQ, kpad, dSF, n_pad);
   g_launches++;
   t_last_kernel = "mxf4_quantize_cols_t";
   return last_launch_status();
@@ -2305,7 +2318,7 @@ int b200_gemm_mxf4(int m, int n, int k, const uint8_t* dAq, const uint8_t* dSFA,
   long long blocks = ((long long)m * (kpad / 32) + 255) / 256;
   if (blocks > t_ctx->sms * 16) blocks = t_ctx->sms * 16;
   launch_pdl(mxf4_expand_rows_kernel, dim3((unsigned)blocks), dim3(256), 0, st, 1, dAq, dSFA, m, kpad, a16);
-  launch_pdl(mxf4_expand_cols_t_kernel, dim3((n + 255) / 256, kpad / 32), dim3(256), 0, st, 1, dBq, dSFB, n, kpad, b16, npitch);
+  launch_pdl(mxf4_expand_cols_t_kernel, dim3((n + 255) / 256, grid_y(kpad / 32)), dim3(256), 0, st, 1, dBq, dSFB, n, kpad, b16, npitch);
   g_launches += 2;
   if ((rc = last_launch_status())) return rc;
   Call c{st};

@@ -51,7 +51,10 @@ __device__ __forceinline__ float act_bias(float t, float b, int act) {
 // a 16-bit C, and C is read only when beta != 0.
 // bias / act (16-bit operands, b200_gemm_bf16_epi / _f16_epi; needs axpby): after the alpha / beta step, t + bias[j]
 // (skipped for a null bias) goes through epi_act (ptx.cuh), the tensor-core kernel's activation.  act = -1: none.
-template <typename InT, typename OutT>
+// WALK_Y: a block computes the row blocks blockIdx.y, + gridDim.y, ... (launched when M needs more than gridDim.y's
+// 65535 blocks).  Without it a block computes row block blockIdx.y only: a loop back-edge alone raises the 16-bit
+// kernels from 40 registers to as many as 63, which would cost them occupancy on every call.
+template <typename InT, typename OutT, bool WALK_Y = false>
 __global__ void __launch_bounds__(256)
 gemm_generic_kernel(int M, int N, int K, const InT* __restrict__ A, long long a_rs, long long a_cs,
                     const InT* __restrict__ B, long long b_rs, long long b_cs, OutT* __restrict__ C, long long ldc,
@@ -62,82 +65,88 @@ gemm_generic_kernel(int M, int N, int K, const InT* __restrict__ A, long long a_
   __shared__ Acc As[16][64 + 4];
   __shared__ Acc Bs[16][64 + 4];
   const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
-  const int m0 = blockIdx.y * 64, n0 = blockIdx.x * 64;
-  Acc acc[4][4];
+  const int n0 = blockIdx.x * 64, mblocks = (int)(((long long)M + 63) / 64);
+  // With WALK_Y, the k loop's closing __syncthreads (K > 0) orders one row block's last reads of As / Bs before the
+  // next one's loads.
+  for (int mb = blockIdx.y; mb < mblocks; mb += gridDim.y) {
+    const int m0 = mb * 64;
+    Acc acc[4][4];
 #pragma unroll
-  for (int i = 0; i < 4; i++)
+    for (int i = 0; i < 4; i++)
 #pragma unroll
-    for (int j = 0; j < 4; j++) acc[i][j] = 0;
-  if constexpr (std::is_same<Acc, OutT>::value) {
-    if (accumulate) {          // chain starts from C(i,j): the CPU harness contract C += A*B
+      for (int j = 0; j < 4; j++) acc[i][j] = 0;
+    if constexpr (std::is_same<Acc, OutT>::value) {
+      if (accumulate) {          // chain starts from C(i,j): the CPU harness contract C += A*B
 #pragma unroll
-      for (int i = 0; i < 4; i++)
+        for (int i = 0; i < 4; i++)
 #pragma unroll
-        for (int j = 0; j < 4; j++) {
-          const int gm = m0 + ty + 16 * i, gn = n0 + tx + 16 * j;
-          if (gm < M && gn < N) acc[i][j] = C[(long long)gm * ldc + gn];
-        }
+          for (int j = 0; j < 4; j++) {
+            const int gm = m0 + ty + 16 * i, gn = n0 + tx + 16 * j;
+            if (gm < M && gn < N) acc[i][j] = C[(long long)gm * ldc + gn];
+          }
+      }
     }
-  }
 
-  for (int k0 = 0; k0 < K; k0 += 16) {
+    for (int k0 = 0; k0 < K; k0 += 16) {
 #pragma unroll
-    for (int r = 0; r < 4; r++) {
-      const int idx = threadIdx.x + r * 256;          // 0..1023
-      const int am = idx >> 4, ak = idx & 15;          // A tile 64 x 16, k fastest
-      const int gm = m0 + am, gk = k0 + ak;
-      As[ak][am] = (gm < M && gk < K) ? LoadAs<InT>::ld(A + (long long)gm * a_rs + (long long)gk * a_cs) : (Acc)0;
-      const int bk = idx >> 6, bn = idx & 63;          // B tile 16 x 64, n fastest
-      const int gk2 = k0 + bk, gn = n0 + bn;
-      Bs[bk][bn] = (gk2 < K && gn < N) ? LoadAs<InT>::ld(B + (long long)gk2 * b_rs + (long long)gn * b_cs) : (Acc)0;
-    }
-    __syncthreads();
+      for (int r = 0; r < 4; r++) {
+        const int idx = threadIdx.x + r * 256;          // 0..1023
+        const int am = idx >> 4, ak = idx & 15;          // A tile 64 x 16, k fastest
+        const int gm = m0 + am, gk = k0 + ak;
+        As[ak][am] = (gm < M && gk < K) ? LoadAs<InT>::ld(A + (long long)gm * a_rs + (long long)gk * a_cs) : (Acc)0;
+        const int bk = idx >> 6, bn = idx & 63;          // B tile 16 x 64, n fastest
+        const int gk2 = k0 + bk, gn = n0 + bn;
+        Bs[bk][bn] = (gk2 < K && gn < N) ? LoadAs<InT>::ld(B + (long long)gk2 * b_rs + (long long)gn * b_cs) : (Acc)0;
+      }
+      __syncthreads();
 #pragma unroll
-    for (int kk = 0; kk < 16; kk++) {
-      Acc a[4], b[4];
+      for (int kk = 0; kk < 16; kk++) {
+        Acc a[4], b[4];
 #pragma unroll
-      for (int i = 0; i < 4; i++) a[i] = As[kk][ty + 16 * i];
+        for (int i = 0; i < 4; i++) a[i] = As[kk][ty + 16 * i];
 #pragma unroll
-      for (int j = 0; j < 4; j++) b[j] = Bs[kk][tx + 16 * j];
+        for (int j = 0; j < 4; j++) b[j] = Bs[kk][tx + 16 * j];
 #pragma unroll
-      for (int i = 0; i < 4; i++)
+        for (int i = 0; i < 4; i++)
 #pragma unroll
-        for (int j = 0; j < 4; j++) {
-          if constexpr (sizeof(Acc) == 4 && !std::is_same<Acc, int32_t>::value)
-            acc[i][j] = fmaf(a[i], b[j], acc[i][j]);
-          else
-            acc[i][j] += a[i] * b[j];
-        }
-    }
-    __syncthreads();
-  }
-#pragma unroll
-  for (int i = 0; i < 4; i++) {
-    const int gm = m0 + ty + 16 * i;
-    if (gm >= M) continue;
-#pragma unroll
-    for (int j = 0; j < 4; j++) {
-      const int gn = n0 + tx + 16 * j;
-      if (gn < N) {
-        if constexpr (std::is_same<OutT, int8_t>::value && std::is_same<Acc, int32_t>::value) {
-          // requantising store (int8 C): per-row scale and optional per-row bias
-          C[(long long)gm * ldc + gn] = (int8_t)requant_s8(acc[i][j], rq_scale[gm], rq_bias ? rq_bias[gm] : 0.0f,
-                                                            rq_bias != nullptr);
-        } else if constexpr (std::is_same<Acc, float>::value) {        // fp32, bf16 or fp16 C
-          float v = acc[i][j];
-          if (axpby) {
-            v *= alpha;
-            if (beta != 0.f) v = fmaf(beta, LoadAs<OutT>::ld(C + (long long)gm * ldc + gn), v);
+          for (int j = 0; j < 4; j++) {
+            if constexpr (sizeof(Acc) == 4 && !std::is_same<Acc, int32_t>::value)
+              acc[i][j] = fmaf(a[i], b[j], acc[i][j]);
+            else
+              acc[i][j] += a[i] * b[j];
           }
-          if constexpr (sizeof(InT) == 2) {
-            if (act >= 0) v = act_bias(v, bias != nullptr ? LoadAs<InT>::ld(bias + gn) : -0.f, act);
+      }
+      __syncthreads();
+    }
+#pragma unroll
+    for (int i = 0; i < 4; i++) {
+      const int gm = m0 + ty + 16 * i;
+      if (gm >= M) continue;
+#pragma unroll
+      for (int j = 0; j < 4; j++) {
+        const int gn = n0 + tx + 16 * j;
+        if (gn < N) {
+          if constexpr (std::is_same<OutT, int8_t>::value && std::is_same<Acc, int32_t>::value) {
+            // requantising store (int8 C): per-row scale and optional per-row bias
+            C[(long long)gm * ldc + gn] = (int8_t)requant_s8(acc[i][j], rq_scale[gm], rq_bias ? rq_bias[gm] : 0.0f,
+                                                              rq_bias != nullptr);
+          } else if constexpr (std::is_same<Acc, float>::value) {        // fp32, bf16 or fp16 C
+            float v = acc[i][j];
+            if (axpby) {
+              v *= alpha;
+              if (beta != 0.f) v = fmaf(beta, LoadAs<OutT>::ld(C + (long long)gm * ldc + gn), v);
+            }
+            if constexpr (sizeof(InT) == 2) {
+              if (act >= 0) v = act_bias(v, bias != nullptr ? LoadAs<InT>::ld(bias + gn) : -0.f, act);
+            }
+            store_out<float, OutT>(C + (long long)gm * ldc + gn, v);
+          } else {
+            store_out<Acc, OutT>(C + (long long)gm * ldc + gn, acc[i][j]);
           }
-          store_out<float, OutT>(C + (long long)gm * ldc + gn, v);
-        } else {
-          store_out<Acc, OutT>(C + (long long)gm * ldc + gn, acc[i][j]);
         }
       }
     }
+    if constexpr (!WALK_Y) break;
   }
 }
 
@@ -248,16 +257,18 @@ __device__ __forceinline__ void generic_tile16(GenericTile& As, GenericTile& Bs,
 }
 
 // Strided batch: entry z of each operand at X + z * x_bs (elements; 0 broadcasts A or B), the entries over
-// blockIdx.z, gridDim.z at a time.
+// blockIdx.z, gridDim.z at a time, and the row blocks over blockIdx.y, gridDim.y at a time.
 template <typename InT, typename OutT>
 __global__ void __launch_bounds__(256)
 gemm_generic_batched_kernel(int batch, int M, int N, int K, const InT* __restrict__ A, long long a_rs, long long a_cs,
                             long long a_bs, const InT* __restrict__ B, long long b_rs, long long b_cs, long long b_bs,
                             OutT* __restrict__ C, long long ldc, long long c_bs, int axpby, float alpha, float beta) {
   __shared__ GenericTile As, Bs;
+  const int mblocks = (int)(((long long)M + 63) / 64);
   for (int z = blockIdx.z; z < batch; z += gridDim.z)
-    generic_tile16(As, Bs, blockIdx.y * 64, blockIdx.x * 64, M, N, K, A + z * a_bs, a_rs, a_cs, B + z * b_bs, b_rs,
-                   b_cs, C + z * c_bs, ldc, axpby, alpha, beta);
+    for (int mb = blockIdx.y; mb < mblocks; mb += gridDim.y)
+      generic_tile16(As, Bs, mb * 64, blockIdx.x * 64, M, N, K, A + z * a_bs, a_rs, a_cs, B + z * b_bs, b_rs, b_cs,
+                     C + z * c_bs, ldc, axpby, alpha, beta);
 }
 
 // scale_inplace_kernel (s != 0) and fill_zero_kernel (s == 0) over every entry: the k == 0 / alpha == 0 pass.

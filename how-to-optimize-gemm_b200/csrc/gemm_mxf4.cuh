@@ -83,39 +83,43 @@ __global__ void __launch_bounds__(256) mxf4_quantize_rows_kernel(const float* __
 }
 
 // Transposing quantiser for a row-major B (k x n): block = 32 k-rows x 256 n-columns through shared memory,
-// then thread = one column: its 32 values along K are one scale block.  Output rows are the COLUMNS of B.
+// then thread = one column: its 32 values along K are one scale block.  Output rows are the COLUMNS of B.  A block
+// takes the K-blocks blockIdx.y, + gridDim.y, ... (gridDim.y is capped at 65535: one unless kpad > 2097120).
 __global__ void __launch_bounds__(256) mxf4_quantize_cols_t_kernel(const float* __restrict__ src, long long ld, int krows,
                                                                    int ncols, uint8_t* __restrict__ q, int kpad,
                                                                    uint8_t* __restrict__ sf, int n_pad) {
   __shared__ float tile[32][257];
-  const int kb = blockIdx.y, n0 = blockIdx.x * 256, katoms = kpad >> 7;
-  for (int rr = threadIdx.x >> 6; rr < 32; rr += 4) {
-    const int kr = kb * 32 + rr;
-#pragma unroll
-    for (int cc = 0; cc < 4; cc++) {
-      const int c = (threadIdx.x & 63) + cc * 64;
-      tile[rr][c] = (kr < krows && n0 + c < ncols) ? src[(long long)kr * ld + n0 + c] : 0.f;
-    }
-  }
-  __syncthreads();
+  const int n0 = blockIdx.x * 256, katoms = kpad >> 7, kblocks = kpad >> 5;
   const int n = n0 + threadIdx.x;
-  if (n >= n_pad) return;
-  float mx = 0.f;
+  for (int kb = blockIdx.y; kb < kblocks; kb += gridDim.y) {
+    if (kb != (int)blockIdx.y) __syncthreads();        // the previous K-block's reads of `tile` are done
+    for (int rr = threadIdx.x >> 6; rr < 32; rr += 4) {
+      const int kr = kb * 32 + rr;
 #pragma unroll
-  for (int e = 0; e < 32; e++) mx = fmaxf(mx, fabsf(tile[e][threadIdx.x]));
-  const uint32_t se = ue8m0_from_max(mx);
-  const float inv = ue8m0_inv(se);
-  sf[mxf4_sf_offset(n, kb, katoms)] = (uint8_t)se;
-  if (n < ncols) {
-    uint32_t w[4];
-#pragma unroll
-    for (int j = 0; j < 4; j++) {
-      uint32_t v = 0;
-#pragma unroll
-      for (int e = 0; e < 8; e++) v |= e2m1_encode(tile[j * 8 + e][threadIdx.x] * inv) << (4 * e);
-      w[j] = v;
+      for (int cc = 0; cc < 4; cc++) {
+        const int c = (threadIdx.x & 63) + cc * 64;
+        tile[rr][c] = (kr < krows && n0 + c < ncols) ? src[(long long)kr * ld + n0 + c] : 0.f;
+      }
     }
-    *reinterpret_cast<uint4*>(q + (long long)n * (kpad >> 1) + kb * 16) = make_uint4(w[0], w[1], w[2], w[3]);
+    __syncthreads();
+    if (n >= n_pad) continue;
+    float mx = 0.f;
+#pragma unroll
+    for (int e = 0; e < 32; e++) mx = fmaxf(mx, fabsf(tile[e][threadIdx.x]));
+    const uint32_t se = ue8m0_from_max(mx);
+    const float inv = ue8m0_inv(se);
+    sf[mxf4_sf_offset(n, kb, katoms)] = (uint8_t)se;
+    if (n < ncols) {
+      uint32_t w[4];
+#pragma unroll
+      for (int j = 0; j < 4; j++) {
+        uint32_t v = 0;
+#pragma unroll
+        for (int e = 0; e < 8; e++) v |= e2m1_encode(tile[j * 8 + e][threadIdx.x] * inv) << (4 * e);
+        w[j] = v;
+      }
+      *reinterpret_cast<uint4*>(q + (long long)n * (kpad >> 1) + kb * 16) = make_uint4(w[0], w[1], w[2], w[3]);
+    }
   }
 }
 
@@ -168,18 +172,21 @@ __global__ void __launch_bounds__(256) mxf4_expand_rows_kernel(const uint8_t* __
   }
 }
 
-// B^T: n x kpad/2 bytes -> row-major kpad x n bf16 (pitch dld).  Thread = one column n and one 32-row K-block;
-// neighbouring threads write neighbouring columns.
+// B^T: n x kpad/2 bytes -> row-major kpad x n bf16 (pitch dld).  Thread = one column n and the 32-row K-blocks
+// blockIdx.y, + gridDim.y, ... (gridDim.y is capped at 65535: one unless kpad > 2097120); neighbouring threads write
+// neighbouring columns.
 __global__ void __launch_bounds__(256) mxf4_expand_cols_t_kernel(const uint8_t* __restrict__ q, const uint8_t* __restrict__ sf,
                                                                  int n, int kpad, uint16_t* __restrict__ dst, long long dld) {
   griddep_launch();
   griddep_wait();
-  const int c = blockIdx.x * blockDim.x + threadIdx.x, kb = blockIdx.y, katoms = kpad >> 7;
+  const int c = blockIdx.x * blockDim.x + threadIdx.x, katoms = kpad >> 7, kblocks = kpad >> 5;
   if (c >= n) return;
-  float x[32];
-  mxf4_expand32(q + (long long)c * (kpad >> 1) + kb * 16, sf[mxf4_sf_offset(c, kb, katoms)], x);
+  for (int kb = blockIdx.y; kb < kblocks; kb += gridDim.y) {
+    float x[32];
+    mxf4_expand32(q + (long long)c * (kpad >> 1) + kb * 16, sf[mxf4_sf_offset(c, kb, katoms)], x);
 #pragma unroll
-  for (int e = 0; e < 32; e++) dst[(long long)(kb * 32 + e) * dld + c] = __bfloat16_as_ushort(__float2bfloat16_rn(x[e]));
+    for (int e = 0; e < 32; e++) dst[(long long)(kb * 32 + e) * dld + c] = __bfloat16_as_ushort(__float2bfloat16_rn(x[e]));
+  }
 }
 
 }  // namespace b200

@@ -1650,25 +1650,30 @@ gemm_tc_stacked_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
 }
 
 // ---- B^T for the K-major operands of tf32 / int8 ------------------------------------------------------
-// src: rows x cols (pitch ld), dst: cols x rows (pitch dld).  32 x 32 tiles through shared memory.
+// src: rows x cols (pitch ld), dst: cols x rows (pitch dld).  32 x 32 tiles through shared memory; a block takes
+// the row tiles blockIdx.y, + gridDim.y, ... (gridDim.y is capped at 65535: one tile unless rows > 2097120).
 template <typename E>
 __global__ void __launch_bounds__(256) transpose_kernel(const E* __restrict__ src, long long ld, int rows, int cols,
                                                         E* __restrict__ dst, long long dld) {
   __shared__ E tile[32][33];
   griddep_launch();
   griddep_wait();
-  const int c0 = blockIdx.x * 32, r0 = blockIdx.y * 32;
+  const int c0 = blockIdx.x * 32, rtiles = (int)(((long long)rows + 31) / 32);
   const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
+  for (int rt = blockIdx.y; rt < rtiles; rt += gridDim.y) {
+    const int r0 = rt * 32;
+    if (rt != (int)blockIdx.y) __syncthreads();        // the previous tile's reads of `tile` are done
 #pragma unroll
-  for (int i = 0; i < 32; i += 8) {
-    const int r = r0 + ty + i, c = c0 + tx;
-    if (r < rows && c < cols) tile[ty + i][tx] = src[(long long)r * ld + c];
-  }
-  __syncthreads();
+    for (int i = 0; i < 32; i += 8) {
+      const int r = r0 + ty + i, c = c0 + tx;
+      if (r < rows && c < cols) tile[ty + i][tx] = src[(long long)r * ld + c];
+    }
+    __syncthreads();
 #pragma unroll
-  for (int i = 0; i < 32; i += 8) {
-    const int c = c0 + ty + i, r = r0 + tx;
-    if (c < cols && r < rows) dst[(long long)c * dld + r] = tile[tx][ty + i];
+    for (int i = 0; i < 32; i += 8) {
+      const int c = c0 + ty + i, r = r0 + tx;
+      if (c < cols && r < rows) dst[(long long)c * dld + r] = tile[tx][ty + i];
+    }
   }
 }
 
@@ -1879,7 +1884,8 @@ __global__ void __launch_bounds__(256) split_f16_rows_kernel(const float* __rest
 // Column maxima of B into out[cols] (zero on entry; non-negative floats order like their bit patterns,
 // so atomicMax on the uint view works).  A block walks 16 rows of a 1024-column strip: every row read is one
 // contiguous 4 KB segment (DRAM page locality; the first version read 512-byte pieces of eight rows at a time
-// and reached 3 TB/s), a thread keeps its 4 columns' maxima in registers, no cross-thread reduction.
+// and reached 3 TB/s), a thread keeps its 4 columns' maxima in registers, no cross-thread reduction.  gridDim.y is
+// capped at 65535, so a block takes the row blocks blockIdx.y, + gridDim.y, ... (one unless rows > 1048560).
 __global__ void __launch_bounds__(256) col_absmax_kernel(const float* __restrict__ src, long long ld, int rows,
                                                          int cols, unsigned int* __restrict__ out) {
   constexpr int ROWS = 16;      // all 16 row loads of a thread in flight at once (ncu: 32 rows in 4 batches of 8 reached 3 TB/s)
@@ -1887,23 +1893,26 @@ __global__ void __launch_bounds__(256) col_absmax_kernel(const float* __restrict
   griddep_wait();
   const int c = blockIdx.x * 1024 + threadIdx.x * 4;
   if (c >= cols) return;
-  const int r0 = blockIdx.y * ROWS, r1 = min(r0 + ROWS, rows);
+  const int rblocks = (int)(((long long)rows + ROWS - 1) / ROWS);
   const bool vec = (ld & 3) == 0 && (reinterpret_cast<uintptr_t>(src) & 15) == 0 && c + 4 <= cols;
   float4 mx = make_float4(0.f, 0.f, 0.f, 0.f);
-  if (vec) {
+  for (int rb = blockIdx.y; rb < rblocks; rb += gridDim.y) {
+    const int r0 = rb * ROWS, r1 = min(r0 + ROWS, rows);
+    if (vec) {
 #pragma unroll 16
-    for (int r = r0; r < r1; r++) {
-      const float4 v = __ldg(reinterpret_cast<const float4*>(src + (long long)r * ld + c));
-      mx.x = fmaxf(mx.x, fabsf(v.x)); mx.y = fmaxf(mx.y, fabsf(v.y));
-      mx.z = fmaxf(mx.z, fabsf(v.z)); mx.w = fmaxf(mx.w, fabsf(v.w));
-    }
-  } else {
-    for (int r = r0; r < r1; r++) {
-      const float* s = src + (long long)r * ld + c;
-      mx.x = fmaxf(mx.x, fabsf(s[0]));
-      if (c + 1 < cols) mx.y = fmaxf(mx.y, fabsf(s[1]));
-      if (c + 2 < cols) mx.z = fmaxf(mx.z, fabsf(s[2]));
-      if (c + 3 < cols) mx.w = fmaxf(mx.w, fabsf(s[3]));
+      for (int r = r0; r < r1; r++) {
+        const float4 v = __ldg(reinterpret_cast<const float4*>(src + (long long)r * ld + c));
+        mx.x = fmaxf(mx.x, fabsf(v.x)); mx.y = fmaxf(mx.y, fabsf(v.y));
+        mx.z = fmaxf(mx.z, fabsf(v.z)); mx.w = fmaxf(mx.w, fabsf(v.w));
+      }
+    } else {
+      for (int r = r0; r < r1; r++) {
+        const float* s = src + (long long)r * ld + c;
+        mx.x = fmaxf(mx.x, fabsf(s[0]));
+        if (c + 1 < cols) mx.y = fmaxf(mx.y, fabsf(s[1]));
+        if (c + 2 < cols) mx.z = fmaxf(mx.z, fabsf(s[2]));
+        if (c + 3 < cols) mx.w = fmaxf(mx.w, fabsf(s[3]));
+      }
     }
   }
   // Only a block that can raise the running maximum touches it: hundreds of row blocks hit the same 4 addresses and
