@@ -35,7 +35,7 @@ EXPORTS = [
     "b200_gemm_s8s32_op", "b200_gemm_workspace_bytes_op", "b200_gemm_fp8", "b200_gemm_fp8_blockwise",
     "b200_gemm_fp8_grouped", "b200_gemm_fp8_batched", "b200_gemm_fp8_blockwise_grouped", "b200_gemm_fp8_blockwise_batched",
     "b200_gemm_fp8_q8", "b200_gemm_fp8_blockwise_q8", "b200_gemm_fp8_grouped_q8", "b200_gemm_fp8_batched_q8",
-    "b200_gemm_fp8_blockwise_grouped_q8", "b200_gemm_fp8_blockwise_batched_q8",
+    "b200_gemm_fp8_blockwise_grouped_q8", "b200_gemm_fp8_blockwise_batched_q8", "b200_fp8_quantize",
     "b200_nccl_load", "b200_nccl_last_error", "b200_comm_unique_id", "b200_comm_init_rank",
     "b200_comm_destroy", "b200_rowpanel_create", "b200_rowpanel_destroy", "b200_rowpanel_slices", "b200_rowpanel_set_reserve_sms", "b200_rowpanel_trace", "b200_rowpanel_trace_dump", "b200_gemm_f32_rowpanel",
     "b200_gemm_f32_rowpanel_host", "b200_gemm_f32_pack_a", "b200_gemm_f32_packed_ab", "b200_gemm_f32_pack_free_a",
@@ -127,6 +127,8 @@ lib.b200_gemm_fp8_blockwise_grouped_q8.argtypes = [_i, _i, _i, _i, _i, _vp, _i, 
 lib.b200_gemm_fp8_blockwise_batched_q8.argtypes = [_i, _i, _i, _i, _i, _vp, _i, _ll, _vp, _i, _ll, _vp, _i, _ll, _ll, _ll,
                                                    _vp, _i, _ll, _ll, _ll, _i, _i, _vp, _i, _ll, _vp, _ll, _ll, _ll, _i,
                                                    _vp]
+lib.b200_fp8_quantize.argtypes = [_i, _i, _i, _i, _i, _i, _vp, _i, _ll, _vp, _i, _ll, _vp, _ll, _ll, _ll, _vp, _i, _ll, _vp,
+                                  _ll, _ll, _ll, _vp]
 lib.b200_gemm_workspace_bytes_op.restype = C.c_size_t
 lib.b200_gemm_f32_pack_b.argtypes = [_i, _i, _vp, _i, _i, C.POINTER(_vp), _vp]
 lib.b200_gemm_f32_packed.argtypes = [_i, _i, _i, _vp, _i, _vp, _vp, _i, _i, _vp]
@@ -982,6 +984,100 @@ def scaled_grouped_mm_quant(A, B, scale_a, scale_b, offs=None, activation=None, 
                                             scale_b.data_ptr(), ssb, act, fast, ct, out.data_ptr(), _ld(out[0]), c_e,
                                             out_scale.data_ptr(), sc_row, sc_blk, sc_e, groups, st))
     return out, out_scale
+
+
+def _scale_layout_ok(rows, blks, s_row, s_blk):
+    """b200_gemm_fp8_q8's rule for a scale matrix: row-major or outer-dim-major, an extent-1 dimension's stride free."""
+    row_major = (blks == 1 or s_blk == 1) and (rows == 1 or s_row >= blks)
+    col_major = (rows == 1 or s_row == 1) and (blks == 1 or s_blk >= rows)
+    return row_major or col_major
+
+
+def quantize_fp8(x, block=(1, 128), dtype=None, transpose=False, out=None, out_scale=None, stream=None):
+    """Blockwise FP8 quantisation of x on the device (b200_fp8_quantize): returns (q, s), or (q, s, qt, st) with
+    transpose=True, the operands and scales that scaled_mm / scaled_grouped_mm take with blockwise scales.
+
+    x is a 2-D (m, k) or 3-D (G, m, k) CUDA tensor of bfloat16, float16 or float32 with unit last stride, rows at any
+    pitch.  dtype is torch.float8_e4m3fn (the default, F = 448) or torch.float8_e5m2 (F = 57344).  For each block,
+    d = amax / F (amax the largest |x| in the block; 1 for an all-zero block, NaN for a block holding a NaN or an inf)
+    and q = fp8(x / d), rounded to nearest even with finite values saturated to +-F: the rule of scaled_mm_quant's
+    epilogue, bit for bit.  block is
+      (1, 128)    activations and gradients: s (..., m, ceil(k / 128)), one scale per row and 128 columns.  qt (..., k,
+                  m) is the (1, 128) quantisation of x^T, with st (..., k, ceil(m / 128)): x's 128 x 1 blocks.
+      (128, 128)  weights: s (..., ceil(m / 128), ceil(k / 128)).  qt is q^T byte for byte and st = s.transpose(-2, -1),
+                  a view of s.
+    q and qt are written in one launch that reads x once.  A blockwise FP8 linear layer y = x @ W.t() (W is (n, k)):
+      xq, xs, xqt, xst = quantize_fp8(x, transpose=True)
+      wq, ws, wqt, _ = quantize_fp8(W, block=(128, 128), transpose=True)
+      dyq, dys, dyqt, dyst = quantize_fp8(dy, transpose=True)
+      y  = scaled_mm(xq, wq.t(), xs, ws.t())             # forward
+      dx = scaled_mm(dyq, wqt.t(), dys, ws)              # dgrad: dy @ W
+      dw = scaled_mm(dyqt, xqt.t(), dyst, xst.t())       # wgrad: dy^T @ x, 128 x 1 blocks along the tokens
+    and a mixture-of-experts layer with expert weights W (G, n, k) and tokens grouped by offs:
+      wq, ws, wqt, _ = quantize_fp8(W, block=(128, 128), transpose=True)
+      y  = scaled_grouped_mm(xq, wq.transpose(-2, -1), xs, ws.transpose(-2, -1), offs)   # forward
+      dx = scaled_grouped_mm(dyq, wqt.transpose(-2, -1), dys, ws, offs)                 # dgrad
+    out (q) may be any FP8 tensor of x's shape and dtype whose rows (and entries) do not overlap; out_scale any float32
+    tensor of s's shape that is row-major or outer-dim-major in its last two dimensions (torch's layout for scale_a),
+    entries not overlapping.  New tensors are row-major.  The call never synchronises and can be captured in a CUDA graph.
+    An input or dtype of another type is a TypeError; another block, shape, layout, out or out_scale, or a CPU tensor, is
+    a ValueError."""
+    import torch
+    dtype = dtype or (out.dtype if out is not None else torch.float8_e4m3fn)
+    in_type = {torch.float32: OUT_F32, torch.bfloat16: OUT_BF16, torch.float16: OUT_F16}.get(x.dtype)
+    if in_type is None:
+        raise TypeError(f"x must be bfloat16, float16 or float32, not {x.dtype}")
+    if not _is_fp8(dtype):
+        raise TypeError(f"dtype must be float8_e4m3fn or float8_e5m2, not {dtype}")
+    block = tuple(block)
+    if block not in ((1, 128), (128, 128)):
+        raise ValueError(f"block must be (1, 128) or (128, 128), not {block}")
+    if x.dim() not in (2, 3):
+        raise ValueError(f"x must be 2-D or 3-D, not {x.dim()}-D")
+    lead, (m, k) = tuple(x.shape[:-2]), tuple(x.shape[-2:])
+    groups = lead[0] if lead else 1
+    if k > 1 and x.stride(-1) != 1:
+        raise ValueError(f"x must have a unit last stride, not strides {tuple(x.stride())}")
+    if m > 1 and x.stride(-2) < k:
+        raise ValueError(f"x's rows must not overlap: stride(-2) = {x.stride(-2)} < {k}")
+    qm, qk = -(-m // 128), -(-k // 128)
+    s_shape = lead + ((m if block[0] == 1 else qm), qk)
+    if out is not None:
+        if out.dtype != dtype or tuple(out.shape) != tuple(x.shape):
+            raise ValueError(f"out must be {dtype} of shape {tuple(x.shape)}, not {out.dtype} of shape {tuple(out.shape)}")
+        if (k > 1 and out.stride(-1) != 1) or (m > 1 and out.stride(-2) < k):
+            raise ValueError(f"out must be row-major with rows that do not overlap, not of strides {tuple(out.stride())}")
+        if lead and groups > 1 and m * k > 0 and out.stride(0) < (m - 1) * out.stride(-2) + k:
+            raise ValueError(f"the entries of out must not overlap (stride(0) = {out.stride(0)})")
+    if out_scale is not None:
+        if out_scale.dtype != torch.float32 or tuple(out_scale.shape) != s_shape:
+            raise ValueError(f"out_scale must be float32 of shape {s_shape}, not {out_scale.dtype} of shape "
+                             f"{tuple(out_scale.shape)}")
+        rows, blks = s_shape[-2:]
+        sr_, sb_ = out_scale.stride()[-2:]
+        if not _scale_layout_ok(rows, blks, sr_, sb_):
+            raise ValueError(f"out_scale must be row-major or outer-dim-major without overlap in its last two "
+                             f"dimensions, not of strides {tuple(out_scale.stride())}")
+        if lead and groups > 1 and rows * blks > 0 and out_scale.stride(0) < (rows - 1) * sr_ + (blks - 1) * sb_ + 1:
+            raise ValueError(f"the entries of out_scale must not overlap (stride(0) = {out_scale.stride(0)})")
+    if not all(t.is_cuda for t in (x, out, out_scale) if t is not None):
+        raise ValueError("x, out and out_scale must be CUDA tensors")
+    q = out if out is not None else torch.empty(x.shape, dtype=dtype, device=x.device)
+    s = out_scale if out_scale is not None else torch.empty(s_shape, dtype=torch.float32, device=x.device)
+    qt = st = None
+    if transpose:
+        qt = torch.empty(lead + (k, m), dtype=dtype, device=x.device)
+        st = torch.empty(lead + (k, qm), dtype=torch.float32, device=x.device) if block[0] == 1 else s.transpose(-2, -1)
+    if x.numel() > 0:
+        e = (lambda t: t.stride(0) if lead and groups > 1 else 0)
+        ld = (lambda t: t.stride(-2) if t.shape[-2] > 1 else t.shape[-1])
+        ct = FP8_E4M3 if dtype == torch.float8_e4m3fn else FP8_E5M2
+        t_args = (qt.data_ptr(), ld(qt), e(qt)) if transpose else (None, 0, 0)
+        st_args = (st.data_ptr(), *st.stride()[-2:], e(st)) if transpose and block[0] == 1 else (None, 0, 0, 0)
+        _check(lib.b200_fp8_quantize(in_type, ct, block[0], m, k, groups, x.data_ptr(), ld(x), e(x), q.data_ptr(),
+                                     ld(q), e(q), s.data_ptr(), *s.stride()[-2:], e(s), *t_args, *st_args,
+                                     _stream_ptr(stream)))
+    return (q, s, qt, st) if transpose else (q, s)
 
 
 def gemm_f32(A, B, out=None, mode=F32_AUTO, stream=None, accumulate=False):

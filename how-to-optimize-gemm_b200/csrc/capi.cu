@@ -20,6 +20,7 @@
 #include "gemm_generic.cuh"
 #include "gemm_mxf4.cuh"
 #include "gemm_tc.cuh"
+#include "fp8_quant.cuh"
 
 using namespace b200;
 
@@ -2323,6 +2324,120 @@ int b200_gemm_mxf4(int m, int n, int k, const uint8_t* dAq, const uint8_t* dSFA,
   if ((rc = last_launch_status())) return rc;
   Call c{st};
   return launch_tc<KIND_F16, 128, 6, float>(m, n, kpad, a16, kpad, m, 0, b16, npitch, kpad, 0, dC, ldc, "tc_mxf4_128x128", c);
+}
+
+// ---- blockwise FP8 quantisers (fp8_quant.cuh): the producers of b200_gemm_fp8_blockwise's operands ----------------
+extern "C++" {
+namespace {
+// The layout rule of b200_gemm_fp8_q8's dScaleC over (rows, blks): row-major or outer-dim-major, the stride of an
+// extent-1 dimension being free.
+bool scale_layout_ok(long long rows, long long blks, long long s_row, long long s_blk) {
+  const bool row_major = (blks == 1 || s_blk == 1) && (rows == 1 || s_row >= blks);
+  const bool col_major = (rows == 1 || s_row == 1) && (blks == 1 || s_blk >= rows);
+  return row_major || col_major;
+}
+
+template <typename In, typename OutT, int BLK, bool TRANS>
+int launch_fp8_quant(const Fp8QuantArgs& a, cudaStream_t st) {
+  auto kern = fp8_quant_kernel<In, OutT, BLK, TRANS>;
+  const int smem = TRANS ? quant_smem_bytes<In>() : 0;
+  int rc = smem > 48 * 1024 ? ensure_smem_attr(kern, smem) : 0;
+  if (rc) return rc;
+  int per_sm = 0;
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kQuantThreads, smem) != cudaSuccess || per_sm < 1) {
+    cudaGetLastError();
+    per_sm = 1;
+  }
+  const long long cap = (long long)t_ctx->sms * per_sm;
+  kern<<<(unsigned)(a.tiles < cap ? a.tiles : cap), kQuantThreads, smem, st>>>(a);
+  return 0;
+}
+
+template <typename In, typename OutT>
+int fp8_quant_recipe(const Fp8QuantArgs& a, int block, const char* const (&names)[4], cudaStream_t st) {
+  const int i = (block == 128 ? 2 : 0) + (a.qt ? 1 : 0);
+  t_last_kernel = names[i];
+  switch (i) {
+    case 0: return launch_fp8_quant<In, OutT, 1, false>(a, st);
+    case 1: return launch_fp8_quant<In, OutT, 1, true>(a, st);
+    case 2: return launch_fp8_quant<In, OutT, 128, false>(a, st);
+    default: return launch_fp8_quant<In, OutT, 128, true>(a, st);
+  }
+}
+
+template <typename In>
+int fp8_quant_in(const Fp8QuantArgs& a, int c_type, int block, const char* const (&e4)[4], const char* const (&e5)[4],
+                 cudaStream_t st) {
+  return c_type == B200_FP8_E4M3 ? fp8_quant_recipe<In, e4m3_out>(a, block, e4, st)
+                                 : fp8_quant_recipe<In, e5m2_out>(a, block, e5, st);
+}
+}  // namespace
+}  // extern "C++"
+
+int b200_fp8_quantize(int in_type, int c_type, int block, int rows, int cols, int batch,
+                      const void* dX, int ldx, long long stride_x,
+                      uint8_t* dQ, int ldq, long long stride_q,
+                      float* dScale, long long s_row, long long s_blk, long long s_entry,
+                      uint8_t* dQt, int ldqt, long long stride_qt,
+                      float* dScaleT, long long st_row, long long st_blk, long long st_entry, void* stream) {
+  if (in_type != B200_OUT_F32 && in_type != B200_OUT_BF16 && in_type != B200_OUT_F16) return B200_ERR_BAD_ARG;
+  if ((c_type != B200_FP8_E4M3 && c_type != B200_FP8_E5M2) || (block != 1 && block != 128)) return B200_ERR_BAD_ARG;
+  if (rows < 0 || cols < 0 || batch < 0 || stride_x < 0 || stride_q < 0 || s_row < 0 || s_blk < 0 || s_entry < 0 ||
+      stride_qt < 0 || st_row < 0 || st_blk < 0 || st_entry < 0)
+    return B200_ERR_BAD_ARG;
+  if (rows == 0 || cols == 0 || batch == 0) return 0;
+  const bool trans = dQt != nullptr;
+  if (ldx < cols || ldq < cols || (trans && ldqt < rows)) return B200_ERR_BAD_ARG;
+  if (!dX || !dQ || !dScale || (block == 1 && trans != (dScaleT != nullptr)) || (block == 128 && dScaleT))
+    return B200_ERR_BAD_ARG;
+  // scales: (rows, qc) for 1 x 128, (qr, qc) for 128 x 128; the transposed output's (cols, qr) for 1 x 128
+  const long long qr = (rows + 127LL) / 128, qc = (cols + 127LL) / 128, srows = block == 1 ? rows : qr;
+  if (!scale_layout_ok(srows, qc, s_row, s_blk) || (dScaleT && !scale_layout_ok(cols, qr, st_row, st_blk)))
+    return B200_ERR_BAD_ARG;
+  // batch entries of the outputs must not overlap; strides bounded as the stacked GEMMs' are
+  const long long in_bytes = in_type == B200_OUT_F32 ? 4 : 2;
+  const long long q_last = (rows - 1LL) * ldq + cols - 1, qt_last = trans ? (cols - 1LL) * ldqt + rows - 1 : 0;
+  const __int128 s_last = last_scale_index(1, 0, srows, qc, s_row, s_blk);
+  const __int128 st_last = dScaleT ? last_scale_index(1, 0, cols, qr, st_row, st_blk) : 0;
+  if (batch > 1) {
+    const long long max_stride = (1LL << 60) / (batch - 1);
+    if (stride_x > max_stride || stride_q > max_stride || s_entry > max_stride || stride_qt > max_stride ||
+        st_entry > max_stride)
+      return B200_ERR_BAD_ARG;
+    if (stride_q <= q_last || s_entry <= s_last || (trans && stride_qt <= qt_last) || (dScaleT && st_entry <= st_last))
+      return B200_ERR_BAD_ARG;
+  }
+  // the last element of every tensor has a byte offset that fits a signed 64-bit integer
+  const __int128 e_last = batch - 1;
+  if ((e_last * stride_x + (__int128)(rows - 1) * ldx + cols - 1) * in_bytes > INT64_MAX ||
+      e_last * stride_q + q_last > INT64_MAX || (e_last * s_entry + s_last) * 4 > INT64_MAX ||
+      (trans && e_last * stride_qt + qt_last > INT64_MAX) || (dScaleT && (e_last * st_entry + st_last) * 4 > INT64_MAX))
+    return B200_ERR_BAD_ARG;
+  int rc = ensure_device();
+  if (rc) return rc;
+  Fp8QuantArgs a{dX, ldx, batch > 1 ? stride_x : 0, dQ, ldq, batch > 1 ? stride_q : 0, dScale, s_row, s_blk,
+                 batch > 1 ? s_entry : 0, dQt, ldqt, batch > 1 ? stride_qt : 0, dScaleT, st_row, st_blk,
+                 batch > 1 ? st_entry : 0, rows, cols, (int)qc, qr * qc, qr * qc * batch, 0};
+  a.vec = aligned16(dX) && (ldx * in_bytes) % 16 == 0 && (batch == 1 || (stride_x * in_bytes) % 16 == 0);
+  cudaStream_t st = (cudaStream_t)stream;
+  static const char* const bf16_e4[4] = {"fp8_quant_bf16_e4m3_1x128", "fp8_quant_t_bf16_e4m3_1x128",
+                                         "fp8_quant_bf16_e4m3_128x128", "fp8_quant_t_bf16_e4m3_128x128"};
+  static const char* const bf16_e5[4] = {"fp8_quant_bf16_e5m2_1x128", "fp8_quant_t_bf16_e5m2_1x128",
+                                         "fp8_quant_bf16_e5m2_128x128", "fp8_quant_t_bf16_e5m2_128x128"};
+  static const char* const f16_e4[4] = {"fp8_quant_f16_e4m3_1x128", "fp8_quant_t_f16_e4m3_1x128",
+                                        "fp8_quant_f16_e4m3_128x128", "fp8_quant_t_f16_e4m3_128x128"};
+  static const char* const f16_e5[4] = {"fp8_quant_f16_e5m2_1x128", "fp8_quant_t_f16_e5m2_1x128",
+                                        "fp8_quant_f16_e5m2_128x128", "fp8_quant_t_f16_e5m2_128x128"};
+  static const char* const f32_e4[4] = {"fp8_quant_f32_e4m3_1x128", "fp8_quant_t_f32_e4m3_1x128",
+                                        "fp8_quant_f32_e4m3_128x128", "fp8_quant_t_f32_e4m3_128x128"};
+  static const char* const f32_e5[4] = {"fp8_quant_f32_e5m2_1x128", "fp8_quant_t_f32_e5m2_1x128",
+                                        "fp8_quant_f32_e5m2_128x128", "fp8_quant_t_f32_e5m2_128x128"};
+  if (in_type == B200_OUT_BF16) rc = fp8_quant_in<qin_bf16>(a, c_type, block, bf16_e4, bf16_e5, st);
+  else if (in_type == B200_OUT_F16) rc = fp8_quant_in<qin_f16>(a, c_type, block, f16_e4, f16_e5, st);
+  else rc = fp8_quant_in<qin_f32>(a, c_type, block, f32_e4, f32_e5, st);
+  if (rc) return rc;
+  g_launches++;
+  return last_launch_status();
 }
 
 int b200_convert_f32_to_bf16(const float* dSrc, uint16_t* dDst, size_t count, void* stream) {

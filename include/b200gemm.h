@@ -661,6 +661,41 @@ int b200_gemm_fp8_blockwise_batched_q8(int a_type, int b_type, int m, int n, int
                                        long long sc_row_stride, long long sc_blk_stride, long long sc_entry_stride,
                                        int batch, void* stream);
 
+/* ---- Blockwise FP8 quantisers (the operands of the blockwise FP8 GEMMs, with an optional transposed copy) ----------
+ * x is batch entries of a rows x cols row-major matrix of in_type (B200_OUT_F32, B200_OUT_BF16 or B200_OUT_F16 used as
+ * element-type codes), entry b at dX + b * stride_x with row pitch ldx >= cols elements, any base and any pitch.  Per
+ * block, amax = max |x| over the block's elements inside the matrix (NaN if one is NaN), and with F = 448 (c_type
+ * B200_FP8_E4M3) or 57344 (B200_FP8_E5M2):
+ *   d = rn(amax / F), 1 when that is 0, NaN when the block holds a NaN or an inf;   q = fp8(rn(x / d))
+ * fp8() round to nearest even with finite values saturated to +-F and NaN kept: exactly the dynamic 1 x 128 rule of
+ * b200_gemm_fp8_q8, whose (C, dScaleC) equals this call on its fp32 C.  Every input converts to fp32 exactly.
+ *   block = 1 (1 x 128: activations, gradients): one d per row i and 128-column block c, at dScale[i * s_row + c * s_blk]
+ *     over (rows, ceil(cols / 128)).  With dQt non-null, dQt (cols x rows, pitch ldqt >= rows bytes) is the 1 x 128
+ *     quantisation of x^T: dQt[j * ldqt + i] = fp8(rn(x[i, j] / dt)), dt = dScaleT[j * st_row + (i / 128) * st_blk]
+ *     over (cols, ceil(rows / 128)), one per column of x and 128-row block.  dScaleT is required with dQt.
+ *   block = 128 (128 x 128: weights): one d per 128 x 128 block (edge blocks clipped) at dScale[r * s_row + c * s_blk]
+ *     over (ceil(rows / 128), ceil(cols / 128)).  With dQt non-null, dQt is q^T byte for byte and shares the scales
+ *     (dScale transposed): dScaleT must be null.
+ * dQ holds q, rows x cols bytes at pitch ldq >= cols.  Entry b's q, scales, qt and transposed scales start at dQ + b *
+ * stride_q, dScale + b * s_entry, dQt + b * stride_qt and dScaleT + b * st_entry.  Nothing outside the matrices and
+ * their scale entries is written.  (q, dScale) with block = 1 is b200_gemm_fp8_blockwise's (A, scale_a) with
+ * scale_a_block = 1; with block = 128 it is a weight W (n x k) whose (B^T, scale_b^T) take scale_b_block = 128.
+ * rows == 0, cols == 0 or batch == 0 is a no-op, null pointers included.  One launch, no workspace, no host
+ * synchronisation: the call can be captured in a CUDA graph.
+ * Argument rules, all checked before the device is touched (B200_ERR_BAD_ARG): the type codes and block; negative
+ * sizes or strides; ldx, ldq or (with dQt) ldqt below its minimum; a null dX, dQ or dScale, or a dScaleT that is not
+ * given exactly with dQt (1 x 128) or is given (128 x 128); a scale layout that is neither row-major nor outer-dim-major
+ * (b200_gemm_fp8_q8's rule for dScaleC, the stride of an extent-1 dimension being free); batch > 1 with an output
+ * entry stride at or below its entry's last index (entries would overlap) or any entry stride above 2^60 / (batch - 1);
+ * a last element of any tensor whose byte offset does not fit a signed 64-bit integer.
+ * Kernels: "fp8_quant_bf16_e4m3_1x128", "fp8_quant_t_f32_e5m2_128x128", ... (_t: the transposed output is written). */
+int b200_fp8_quantize(int in_type, int c_type, int block, int rows, int cols, int batch,
+                      const void* dX, int ldx, long long stride_x,
+                      uint8_t* dQ, int ldq, long long stride_q,
+                      float* dScale, long long s_row, long long s_blk, long long s_entry,
+                      uint8_t* dQt, int ldqt, long long stride_qt,
+                      float* dScaleT, long long st_row, long long st_blk, long long st_entry, void* stream);
+
 /* Pre-split operands for the split-precision modes (AUTO = the library default): the reference
  * leaves its "packAB interface open" for callers that reuse one operand (README.md:85; PackMatrixA/B,
  * aarch64/MMult_4x4_13.cpp:259,361).  TMA needs no repacking of row-major operands, but the fp32 ->
