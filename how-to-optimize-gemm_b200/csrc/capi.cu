@@ -428,6 +428,10 @@ int launch_tc(int m, int n, int k, const void* A, long long lda, int a_rows_tota
   constexpr bool BLK = std::is_same<ScaleT, TcBlockScale>::value || std::is_same<ScaleT, TcStackBlockScale>::value ||
                       std::is_same<ScaleT, TcBlockScaleQ8>::value || std::is_same<ScaleT, TcStackBlockScaleQ8>::value;
   constexpr bool STACK_Q8 = std::is_same<ScaleT, TcStackScaleQ8>::value || std::is_same<ScaleT, TcStackBlockScaleQ8>::value;
+  // F16X2 (fp16 planes, several products): gemm_tc_split_kernel, whose epilogue runs behind the next tile's MMAs.
+  // BF16X3 / BF16X2 stay on gemm_tc_kernel (DESIGN.md §4.2).
+  constexpr bool SPLIT_F16 = KIND == KIND_FP16 && Prod::N > 1;
+  static_assert(!SPLIT_F16 || (std::is_same<OutT, float>::value && !EPI && STACK == STACK_NONE), "F16X2: fp32 C");
   constexpr int smem = Cfg::SMEM_BYTES + (BLK ? STAGES * kBlkScaleStageBytes : 0);
   constexpr CUtensorMapDataType dt = KIND == KIND_F16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
                                    : KIND == KIND_FP16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16
@@ -480,6 +484,7 @@ int launch_tc(int m, int n, int k, const void* A, long long lda, int a_rows_tota
     if constexpr (STACK_Q8) return gemm_tc_fp8_q8_stacked_kernel<KIND, BN, STAGES, OutT, Prod, BLK, STACK>;
     else if constexpr (FP8) return gemm_tc_fp8_kernel<KIND, BN, STAGES, OutT, Prod, BLK, STACK>;
     else if constexpr (STACK != STACK_NONE) return gemm_tc_stacked_kernel<KIND, BN, STAGES, OutT, AL, BL, STACK>;
+    else if constexpr (SPLIT_F16) return gemm_tc_split_kernel<KIND, BN, STAGES, Prod, A_ROW_BYTES, AL, BL>;
     else return gemm_tc_kernel<KIND, BN, STAGES, OutT, Prod, A_ROW_BYTES, AL, BL, EPI>;
   }();
   if (int arc = ensure_smem_attr(kern, smem)) return arc;

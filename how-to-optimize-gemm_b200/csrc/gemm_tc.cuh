@@ -599,6 +599,293 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   }
 }
 
+// ---- split-precision fp32 GEMM with the epilogue behind the next tile's MMAs (gemm_tc_split_kernel) -------------------
+// k-blocks of the next work item issued before a tile's store, which is cut into as many slices (2 .. 4, < STAGES)
+constexpr int kSplitEpiOverlap = 3;
+
+// wgmma.wait_group with an argument that is a constant after unrolling (0 .. 3)
+__device__ __forceinline__ void wgmma_wait_upto(int n) {
+  switch (n) {
+    case 0: wgmma_wait<0>(); break;
+    case 1: wgmma_wait<1>(); break;
+    case 2: wgmma_wait<2>(); break;
+    default: wgmma_wait<3>(); break;
+  }
+}
+
+// One k-block's plane products into acc (gemm_tc_kernel's chain): wait for stage s, issue, commit.  `first`: the first
+// k-block of a chunk, whose first product starts the accumulator from zero.
+template <class Cfg, class Prod>
+__device__ __forceinline__ void split_issue_kblock(float (&acc)[Cfg::ACC], uint32_t sA, uint32_t sB, uint32_t bar_full,
+                                                   int s, uint32_t ph, int cw, uint32_t b_lbo, uint32_t b_sbo,
+                                                   bool first) {
+  using MMA = typename Cfg::MMA;
+  mbar_wait(bar_full + 8 * s, ph);
+  const uint32_t a0 = sA + s * Cfg::A_STAGE + cw * Cfg::A_WG;
+  const uint32_t b0 = sB + s * Cfg::B_STAGE;
+  wgmma_fence();
+#pragma unroll
+  for (int pr = 0; pr < Prod::N; pr++) {
+#pragma unroll
+    for (int k = 0; k < Cfg::MMAS_PER_STAGE; k++) {
+      uint64_t ad, bd;
+      if constexpr (Cfg::A_MN)
+        ad = make_sdesc(a0 + Prod::ia(pr) * Cfg::A_PLANE + k * Cfg::A_KADV, Cfg::MN_BOX_BYTES, 1024, SWZ_128B);
+      else
+        ad = make_sdesc(a0 + Prod::ia(pr) * Cfg::A_PLANE + k * Cfg::A_KADV, 16, Cfg::A_SBO, Cfg::A_SWZ);
+      if constexpr (Cfg::B_MN)
+        bd = make_sdesc(b0 + Prod::ib(pr) * Cfg::B_PLANE + k * Cfg::B_KADV, b_lbo, b_sbo, SWZ_128B);
+      else
+        bd = make_sdesc(b0 + Prod::ib(pr) * Cfg::B_PLANE + k * Cfg::B_KADV, 16, Cfg::A_SBO, Cfg::A_SWZ);
+      MMA::mma(acc, ad, bd, ((first ? 0 : 1) | k | pr) != 0 ? 1u : 0u);
+    }
+  }
+  wgmma_commit();
+}
+
+// Whether work item w's tile is stored by split_store_plain: a whole tile (no K split) inside M x N whose C takes plain
+// 8-byte stores of the unscaled sum (no fold, alpha / beta or streaming).
+template <class Cfg>
+__device__ __forceinline__ bool split_tile_plain(const TcParams& p, int w, int num_kb) {
+  const WorkItem it = work_item(w, p, num_kb);
+  int mb, nb;
+  tile_coords(it.tile, p.tiles_m, p.tiles_n, p.group_m, mb, nb);
+  return w < p.full_tiles && (mb + 1) * Cfg::BM <= p.M && (nb + 1) * 128 <= p.N && p.vec_ok && !p.accumulate &&
+         !p.axpby && !p.stream_c && p.row_max != nullptr;
+}
+
+// One consumer warp's 16 rows of a split_tile_plain work item (its fp32 running sum `sum`) into C: per column pair
+// the two exponents, then the pair of both rows unscaled by mul_pow2 as store_pair does it and stored, with no per-pair
+// branch.  The 16 column groups go in kSplitEpiOverlap slices.  OVERLAP: the next item's first kSplitEpiOverlap
+// k-blocks are in flight from stage st0 on; after slice i the first i + 1 of them are retired and their stages
+// released, so a k-block stays queued on the tensor pipe while each slice is stored, and none is left after the last.
+template <class Cfg, int STAGES, bool OVERLAP>
+__device__ __forceinline__ void split_store_plain(const TcParams& p, const float (&sum)[Cfg::ACC], int w, int num_kb,
+                                                  int ew, int lane, int st0, uint32_t bar_empty, bool wg_leader) {
+  constexpr int J = 128 / 8, D = kSplitEpiOverlap;
+  const WorkItem it = work_item(w, p, num_kb);
+  int mb, nb;
+  tile_coords(it.tile, p.tiles_m, p.tiles_n, p.group_m, mb, nb);
+  const int row0 = mb * Cfg::BM + ew * 16 + (lane >> 2);
+  const int col0 = nb * 128 + 2 * (lane & 3);
+  const int re[2] = {pow2_exp(__ldg(p.row_max + row0)), pow2_exp(__ldg(p.row_max + row0 + 8))};
+  const float* const cmax = p.col_max + col0;
+  float* const c_row = reinterpret_cast<float*>(p.C) + (long long)row0 * p.ldc + col0;
+#pragma unroll
+  for (int i = 0; i < D; i++) {
+#pragma unroll
+    for (int j = J * i / D; j < J * (i + 1) / D; j++) {
+      const int ce0 = cmax != nullptr ? pow2_exp(__ldg(cmax + 8 * j)) : 0;
+      const int ce1 = cmax != nullptr ? pow2_exp(__ldg(cmax + 8 * j + 1)) : 0;
+#pragma unroll
+      for (int h = 0; h < 2; h++)
+        *reinterpret_cast<float2*>(c_row + 8 * h * p.ldc + 8 * j) =
+            make_float2(mul_pow2(sum[4 * j + 2 * h], re[h] + ce0), mul_pow2(sum[4 * j + 2 * h + 1], re[h] + ce1));
+    }
+    if constexpr (OVERLAP) {
+      wgmma_wait_upto(D - 1 - i);
+      if (wg_leader) mbar_arrive(bar_empty + 8 * ((st0 + i) % STAGES));
+    }
+  }
+}
+
+// Every other work item: gemm_tc_kernel's epilogue (K-split wait and publish, store_pair per column pair).
+template <class Cfg>
+__device__ __forceinline__ void split_store_general(const TcParams& p, const float (&sum)[Cfg::ACC], int w, int num_kb,
+                                                    int ew, int lane) {
+  const WorkItem it = work_item(w, p, num_kb);
+  int mb, nb;
+  tile_coords(it.tile, p.tiles_m, p.tiles_n, p.group_m, mb, nb);
+  int* flag = p.flags + (it.tile - p.full_tiles) * Cfg::EPI_WARPS + ew;
+  if (it.part > 0) {                               // K-split tail: wait until parts < it.part are in C
+    if (lane == 0) {
+      const long long t0 = clock64();
+      while (true) {
+        int v;
+        asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(flag) : "memory");
+        if (v == it.part) break;
+        if (clock64() - t0 > 4000000000LL) { asm volatile("trap;"); }
+      }
+    }
+    __syncwarp();
+  }
+  // beta * C is read by part 0 only; later K parts add alpha * partial to what is already there
+  const bool fold = p.accumulate != 0 || it.part > 0 || (p.axpby && p.beta != 0.f);
+  const float al = p.axpby ? p.alpha : 1.f;
+  const float be = (p.axpby && it.part == 0) ? p.beta : 1.f;
+  const int row0 = mb * Cfg::BM + ew * 16 + (lane >> 2);
+  const int col0 = nb * 128 + 2 * (lane & 3);
+  int re[2] = {0, 0};
+#pragma unroll
+  for (int h = 0; h < 2; h++)
+    if (row0 + 8 * h < p.M && p.row_max != nullptr) re[h] = pow2_exp(__ldg(p.row_max + row0 + 8 * h));
+#pragma unroll
+  for (int j = 0; j < 128 / 8; j++) {
+    const int col = col0 + 8 * j;
+    int ce[2] = {0, 0};
+    if (p.col_max != nullptr) {
+#pragma unroll
+      for (int e = 0; e < 2; e++)
+        if (col + e < p.N) ce[e] = pow2_exp(__ldg(p.col_max + col + e));
+    }
+#pragma unroll
+    for (int h = 0; h < 2; h++)
+      store_pair<float>(p, row0 + 8 * h, col, sum[4 * j + 2 * h], sum[4 * j + 2 * h + 1], fold, it.part > 0, al, be,
+                        re[h], ce, 0.f, 0.f);
+  }
+  if (w >= p.full_tiles && p.split > 1) {          // publish this part (the last one re-arms the flag)
+    __threadfence();
+    __syncwarp();
+    if (lane == 0) {
+      const int nv = it.part + 1 == p.split ? 0 : it.part + 1;
+      asm volatile("st.release.gpu.global.s32 [%0], %1;" ::"l"(flag), "r"(nv) : "memory");
+    }
+  }
+}
+
+// The split-precision fp32 kernel (F16X2): gemm_tc_kernel's producer, stage ring, descriptors, MMA chain, chunked fold
+// into the register running sum and K-split tail, for fp32 C in 128 x 128 tiles, with each work item's epilogue
+// run behind the next item's first k-blocks.  When item w's last chunk is folded into `sum`, the consumers issue the
+// CTA's next item's first kSplitEpiOverlap k-blocks into `acc` (its first chunk starts from zero, so acc holds nothing
+// of w) and store w from `sum` while the tensor cores run them.  The CTA's last item, and a tile that needs
+// store_pair's general store (edge tiles, fold, alpha / beta, streaming stores, K parts), are stored before any further
+// issue, as gemm_tc_kernel does.  Every product, fold and unscaling is gemm_tc_kernel's, so C is the same bit for bit.
+// A kernel of its own so that gemm_tc_kernel keeps its code (DESIGN.md §4.1, "Why a kernel of its own").
+template <int KIND, int BN, int STAGES, class Prod, int A_ROW_BYTES, int AL, int BL>
+__global__ void __launch_bounds__((TcConfig<KIND, BN, STAGES, Prod, A_ROW_BYTES, AL, BL>::THREADS), 1)
+gemm_tc_split_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                     const TcParams p) {
+  using Cfg = TcConfig<KIND, BN, STAGES, Prod, A_ROW_BYTES, AL, BL>;
+  constexpr int D = kSplitEpiOverlap;
+  static_assert(Cfg::REGACC && Prod::N > 1 && BN == 128, "split-precision modes: register running sum, 128-wide tiles");
+  static_assert(D >= 2 && D <= 4 && D < STAGES, "the deferred epilogue holds D stages while the producer refills the rest");
+
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;   // swizzle atoms need 1 KB
+  const uint32_t sA = smem_base;
+  const uint32_t sB = sA + STAGES * Cfg::A_STAGE;
+  const uint32_t bar_full = sB + STAGES * Cfg::B_STAGE;
+  const uint32_t bar_empty = bar_full + 8 * STAGES;
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmA);
+    tma_prefetch_desc(&tmB);
+    for (int i = 0; i < STAGES; i++) {
+      mbar_init(bar_full + 8 * i, 1);
+      mbar_init(bar_empty + 8 * i, Cfg::CONSUMERS);          // one arrive per consumer warpgroup
+    }
+    fence_barrier_init();
+  }
+  __syncthreads();
+  // PDL: everything above may overlap the tail of the previous kernel in the stream; nothing below may.
+  griddep_launch();
+  griddep_wait();
+
+  const int num_tiles = p.tiles_m * p.tiles_n;
+  const int num_items = p.full_tiles + (num_tiles - p.full_tiles) * p.split;
+  const int num_kb = (p.K + Cfg::BK - 1) / Cfg::BK;
+
+  if (warp < 4) {
+    // ===================== TMA producer (warpgroup 0), as in gemm_tc_kernel =====================
+    setmaxnreg_dec<40>();
+    if (warp == 0 && lane == 0) {
+      int s = 0;
+      uint32_t ph = 0;
+      for (int w = blockIdx.x; w < num_items; w += gridDim.x) {
+        const WorkItem it = work_item(w, p, num_kb);
+        int mb, nb;
+        tile_coords(it.tile, p.tiles_m, p.tiles_n, p.group_m, mb, nb);
+        const int m0 = mb * Cfg::BM, n0 = nb * BN;
+        for (int kb = it.kb0; kb < it.kb1; kb++) {
+          mbar_wait(bar_empty + 8 * s, ph ^ 1);
+          const uint32_t full = bar_full + 8 * s;
+          mbar_arrive_expect_tx(full, Cfg::STAGE_BYTES);
+          if constexpr (Cfg::A_MN) {
+#pragma unroll
+            for (int pa = 0; pa < Prod::NPA; pa++)
+#pragma unroll
+              for (int j = 0; j < Cfg::A_BOXES; j++)
+                tma_load_2d(sA + s * Cfg::A_STAGE + pa * Cfg::A_PLANE + j * Cfg::MN_BOX_BYTES, &tmA, full,
+                            m0 + j * Cfg::MN_BOX_COLS, pa * p.a_plane_rows + kb * Cfg::BK);
+          } else {
+#pragma unroll
+            for (int pa = 0; pa < Prod::NPA; pa++)
+              tma_load_2d(sA + s * Cfg::A_STAGE + pa * Cfg::A_PLANE, &tmA, full, kb * Cfg::BK, pa * p.a_plane_rows + m0);
+          }
+          if constexpr (!Cfg::B_MN) {
+#pragma unroll
+            for (int pb = 0; pb < Prod::NPB; pb++)
+              tma_load_2d(sB + s * Cfg::B_STAGE + pb * Cfg::B_PLANE, &tmB, full, kb * Cfg::BK, pb * p.b_plane_rows + n0);
+          } else {
+#pragma unroll
+            for (int pb = 0; pb < Prod::NPB; pb++)
+#pragma unroll
+              for (int j = 0; j < Cfg::B_BOXES; j++)
+                tma_load_2d(sB + s * Cfg::B_STAGE + pb * Cfg::B_PLANE + j * Cfg::B_BOX_BYTES, &tmB, full,
+                            n0 + j * Cfg::B_BOX_COLS, pb * p.b_plane_rows + kb * Cfg::BK);
+          }
+          if (++s == STAGES) { s = 0; ph ^= 1; }
+        }
+      }
+    }
+  } else {
+    // ===================== consumers (warpgroups 1 and 2): MMA chain + deferred epilogue =====================
+    setmaxnreg_inc<232>();
+    const int cw = warp / 4 - 1;                    // consumer warpgroup: rows [64 cw, 64 cw + 64) of the tile
+    const int ew = warp - 4;                        // consumer warp 0..7: 16 rows each
+    const bool wg_leader = (threadIdx.x & 127) == 0;
+    const uint32_t b_lbo = p.dbg_b_lbo ? (uint32_t)p.dbg_b_lbo : (uint32_t)Cfg::B_BOX_BYTES;
+    const uint32_t b_sbo = p.dbg_b_sbo ? (uint32_t)p.dbg_b_sbo : 1024u;
+    int s = 0;
+    uint32_t ph = 0;
+    float acc[Cfg::ACC];
+    float sum[Cfg::ACC];
+    // Every work item's first chunk is at least min(chunk_kb, num_kb / split) k-blocks long (a K part has at least
+    // num_kb / split), so this says whether each one has the D k-blocks a deferred store runs behind.
+    const bool hide = min(p.chunk_kb, num_kb / p.split) >= D;
+    int skip = 0;                                   // k-blocks of this item issued behind the previous item's store
+    for (int w = blockIdx.x; w < num_items; w += gridDim.x) {
+      const WorkItem it = work_item(w, p, num_kb);
+      for (int c0 = it.kb0; c0 < it.kb1; c0 += p.chunk_kb) {
+        const int c1 = min(c0 + p.chunk_kb, it.kb1);
+        int prev = -1;
+        for (int kb = c0 + skip; kb < c1; kb++) {
+          split_issue_kblock<Cfg, Prod>(acc, sA, sB, bar_full, s, ph, cw, b_lbo, b_sbo, kb == c0);
+          wgmma_wait<1>();                            // the previous k-block's products retired: its stage is free
+          if (prev >= 0 && wg_leader) mbar_arrive(bar_empty + 8 * prev);
+          prev = s;
+          if (++s == STAGES) { s = 0; ph ^= 1; }
+        }
+        skip = 0;
+        wgmma_wait<0>();
+        wgmma_fence_regs(acc);
+        if (prev >= 0 && wg_leader) mbar_arrive(bar_empty + 8 * prev);
+#pragma unroll
+        for (int i = 0; i < Cfg::ACC; i++) sum[i] = c0 == it.kb0 ? acc[i] : __fadd_rn(sum[i], acc[i]);
+      }
+      // ---- this warp's 16 rows of the tile into C: behind the next item's first D k-blocks where possible ----
+      if (split_tile_plain<Cfg>(p, w, num_kb)) {
+        if (hide && w + (int)gridDim.x < num_items) {
+          const int st0 = s;
+#pragma unroll
+          for (int i = 0; i < D; i++) {
+            split_issue_kblock<Cfg, Prod>(acc, sA, sB, bar_full, s, ph, cw, b_lbo, b_sbo, i == 0);
+            if (++s == STAGES) { s = 0; ph ^= 1; }
+          }
+          split_store_plain<Cfg, STAGES, true>(p, sum, w, num_kb, ew, lane, st0, bar_empty, wg_leader);
+          skip = D;
+        } else {
+          split_store_plain<Cfg, STAGES, false>(p, sum, w, num_kb, ew, lane, 0, bar_empty, wg_leader);
+        }
+      } else {
+        split_store_general<Cfg>(p, sum, w, num_kb, ew, lane);
+      }
+    }
+  }
+}
+
 // ---- the entry of a work tile of the stacked kernels (gemm_tc_stacked_kernel, gemm_tc_fp8_kernel with STACK) -----------
 struct StackEntry {
   int tile0, tiles_m;      // the entry's first work tile and its tile rows (tile_coords)
